@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — CTR examples/sec of the Wide&Deep train step on N B200 (BASELINE.json metric).
+"""bench.py — CTR examples/sec of the Wide&Deep train step on N H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torch.distributed.run)
     python bench.py --impl reference ...                      (optimised CPU restatement of the reference step, host cores)
     python bench.py --workload criteo|multihot|wide           (default criteo = BASELINE.json configs[1] / [2])
+    python bench.py --dump-outputs DIR ...                    (what the last timed step left behind, as DIR/<name>.npy)
 
 Workloads (config.workload), one "step" = ids + forward + sum-reduced sigmoid-CE + backward + all optimizers:
   criteo    configs[1] (N = 1) / configs[2] (N > 1): synthetic Criteo shape, 13 dense + 26 categorical (Criteo-Kaggle
@@ -15,7 +16,7 @@ Workloads (config.workload), one "step" = ids + forward + sum-reduced sigmoid-CE
             FTRL, 131072 examples per GPU (1 M at N = 8).
 N > 1: the batch is split by example; every table larger than 16384 rows is ROW-SHARDED over the ranks and exchanged through peer
 memory by the library's own kernels (wide_deep_b200/csrc/shard.cu), smaller tables are replicated and their gradients travel with
-the dense gradients in one two-shot all-reduce over peer memory.  WD_DP_MODE=lists selects round 1's replicated-table path
+the dense gradients in one two-shot all-reduce over peer memory.  WD_DP_MODE=lists selects the replicated-table path
 (NCCL all-gather of (row, gradient) lists) instead.
 
 JSON keys beyond the base contract:
@@ -25,14 +26,20 @@ JSON keys beyond the base contract:
             alternating slots on the upload stream (the copy of step i+1 overlaps step i, like dataset.prefetch in the reference),
             then the step, then a device -> host read of its loss — all inside the timed region
   roofline  the dominant kernel group, timed live with CUDA events on the model stream (a few profiled steps, N = 1): criteo = the
-            nine MLP GEMM launches vs the measured bf16 tensor peak; multihot = embedding gather + pool vs measured HBM bandwidth;
-            wide = the wide-table kernels vs HBM bandwidth.  `kernels` carries the per-phase times and the gather's HBM figure.
+            nine MLP GEMM launches vs the bf16 tensor peak; multihot = embedding gather + pool vs HBM bandwidth; wide = the wide-table
+            kernels vs HBM bandwidth (peaks: MEASURED_PEAKS.json when present, else the H100 SXM data sheet, named in `peak_source`).  `kernels` carries the per-phase times and the gather's HBM figure.
   dtype     arithmetic of the MLP GEMMs ("bf16x3" = fp32 operands split into bf16 hi + lo, three tensor-core products, fp32
             accumulation); `parity` re-checks the engine against the oracle in this run, `strict_engine` = the same step on tf32x3
   cpu_baseline  the optimised CPU restatement (oracle/fast.py) on the host cores, same workload, bounded sample
 Before the W warm-up steps every ring slot is visited three times untimed (two eager steps + the CUDA-graph capture of that slot), so
 the timed K steps replay graphs only.  WD_STEP_TRACE=1 (N = 1) / WD_SHARD_TRACE=1 (N > 1) print a stream / flag-barrier timeline of
-one replayed step to stderr (profiles/r2_step_timelines.md).
+one replayed step to stderr.
+--dump-outputs DIR: after the K timed steps (before anything else runs) the loss of the last timed step and every trained
+parameter tensor are written as float32 DIR/<name>.npy ('/' in a tensor name becomes '__'); a tensor above the per-tensor budget
+is stored as a sample of its rows (fixed: drawn from a generator seeded by the tensor's name), the whole dump stays under 64 MB.
+At N > 1 only rank 0 writes: of a row-sharded tensor its own rows (global rows 0, N, 2N, ...) under the tensor's name, and no
+loss.npy (the sharded step reduces the loss only when asked for it).  Inputs and initial
+parameters are seeded, so two builds run with the same arguments can be compared file by file.
 """
 import argparse
 import json
@@ -60,7 +67,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_burst=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source="fallback")
+    # NVIDIA's data sheet for the H100 SXM at 700 W: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 (ceilings, not measurements)
+    return dict(hbm_gbs=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source="H100 SXM data sheet")
 
 
 def usable_cores():
@@ -87,24 +95,8 @@ def usable_cores():
     return max(1, n)
 
 
-def gemm_traffic_from_profile(engine, batch):
-    """DRAM bytes of the GEMM launches of one step, from the newest committed ncu capture that matches (engine, batch):
-    profiles/*_gemm_traffic.json = {"engine", "batch", "dram_bytes_per_step", "command", "source"} written by
-    tools/ncu_summary.py --traffic from the `ncu --set full` raw CSV.  (None, reason) when no capture matches — never a constant."""
-    import glob
-    best = None
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "*_gemm_traffic.json"))):
-        try:
-            d = json.load(open(path))
-        except Exception:
-            continue
-        if d.get("engine") == engine and int(d.get("batch", -1)) == int(batch):
-            best = (float(d["dram_bytes_per_step"]), os.path.relpath(path, ROOT))
-    return best if best else (None, "no committed ncu capture for engine=%s batch=%d" % (engine, batch))
-
-
 class ClockSampler(object):
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe).
+    """SM clock / throttle reasons sampled DURING the timed region.
 
     A step is ~1 ms, so `nvidia-smi -lms` (>= 100 ms per sample) would miss short runs: NVML is polled in-process every 2 ms from a
     thread (same counters nvidia-smi reads); nvidia-smi is the fallback when the NVML binding is missing."""
@@ -203,7 +195,7 @@ class Workload(object):
             self.P = (n_cat * self.emb + self.n_dense) * 1024 + 1024 * 512 + 512 * 256 + 256
             self.desc = ("synthetic Criteo shape: 13 dense + 26 categorical (Criteo-Kaggle cardinalities, 33.76M rows), emb 32, "
                          "wide 26 hash + 13 bucketized + 8 crosses@1M, MLP 1024-512-256 relu+BN, Adagrad/FTRL; train step")
-            self.l2 = "ring of %d distinct resident batches; touched rows per step ~60 MB, tables 8.6 GB >> 126 MB L2" % RING
+            self.l2 = "ring of %d distinct resident batches; touched rows per step ~60 MB, tables 8.6 GB >> 50 MB L2" % RING
         elif name == "multihot":
             self.rows = 12_500_000 * self.world
             self.fc, self.cross, self.model, self.emb = synthetic.multihot_conf(rows=self.rows)
@@ -212,7 +204,7 @@ class Workload(object):
             self.P = 64 * 512 + (512 + 64) * 512 + (1024 + 64) * 512 + (1536 + 64) * 512 + (2048 + 64)
             self.desc = ("one hashed multihot slot, Poisson(30) ids per example clipped to [1,128], %d rows (12.5M per GPU) x 64, mean "
                          "pooling, ResDnn 4x512 (resnet concatenations) relu+BN, Adagrad; train step" % self.rows)
-            self.l2 = "ring of %d distinct resident batches; ~246K random 256-byte rows per step of a 6.4 GB table >> 126 MB L2" % RING
+            self.l2 = "ring of %d distinct resident batches; ~246K random 256-byte rows per step of a 6.4 GB table >> 50 MB L2" % RING
         elif name == "wide":
             self.rows = 125_000_000 * self.world
             self.fc, self.cross, self.model, self.emb = synthetic.wide_conf(total_cross_rows=self.rows)
@@ -223,7 +215,7 @@ class Workload(object):
             self.P = 0
             self.desc = ("wide-only: 9 hashed key fields + 32 hashed pairwise crosses into %d buckets (125M per GPU), FTRL(0.1, l1 0.5, "
                          "l2 1); train step" % self.rows)
-            self.l2 = "ring of %d distinct resident batches; 4.2M random 16-byte records per step of a 2 GB table >> 126 MB L2" % RING
+            self.l2 = "ring of %d distinct resident batches; 4.2M random 16-byte records per step of a 2 GB table >> 50 MB L2" % RING
         else:
             raise SystemExit("unknown workload %r" % name)
 
@@ -410,6 +402,28 @@ def parity_check(engine, rows=2048):
 
 
 # ------------------------------------------------------------------------------------------------ our arm
+DUMP_BYTES = 56 << 20          # budget of --dump-outputs (the limit is 64 MB, .npy headers included)
+
+
+def dump_outputs(out_dir, model, loss):
+    """What the last timed step left behind: its loss (single GPU) and every trained tensor, float32 .npy files.  A tensor above
+    an equal share of DUMP_BYTES is stored as a sample of its rows drawn by a generator seeded from the tensor's name."""
+    import zlib
+    os.makedirs(out_dir, exist_ok=True)
+    if loss is not None:
+        np.save(os.path.join(out_dir, "loss.npy"), np.asarray([loss], dtype=np.float32))
+    names = model.tensor_names()
+    share = DUMP_BYTES // 4 // max(len(names), 1)                 # elements per tensor
+    for name in names:
+        t = model.get_tensor(name)
+        t = t.reshape(t.shape[0], -1) if t.ndim > 1 else t.reshape(-1, 1)
+        stem = os.path.join(out_dir, name.replace("/", "__"))
+        if t.size > share:
+            rows = np.sort(np.random.default_rng(zlib.crc32(name.encode())).choice(t.shape[0], max(1, share // t.shape[1]), replace=False))
+            t = t[rows]
+        np.save(stem + ".npy", np.ascontiguousarray(t, dtype=np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -419,9 +433,11 @@ def main():
     ap.add_argument("--workload", default=os.environ.get("WD_WORKLOAD", "criteo"), choices=["criteo", "multihot", "wide"])
     ap.add_argument("--batch", type=int, default=None, help="examples per GPU per step (default: the workload's)")
     ap.add_argument("--engine", default=os.environ.get("WD_GEMM_ENGINE", "bf16x3"),
-                    help="MLP GEMM engine: bf16x3 (tcgen05 kind::f16 on bf16 hi/lo copies, 2^-16 products; re-checked against the "
-                         "oracle in this run) | tc3x (tcgen05 kind::tf32 3-pass, 2^-21, the library default) | ffma (fp32 CUDA cores)")
+                    help="MLP GEMM engine: bf16x3 (wgmma on bf16 hi/lo copies, 2^-16 products; re-checked against the "
+                         "oracle in this run) | tc3x (wgmma tf32 3-pass, 2^-21, the library default) | ffma (fp32 CUDA cores)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss of the last timed step and the trained tensors (sampled above a size budget) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -521,6 +537,8 @@ def main():
     if rank == 0:
         clocks.start()
     ms = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, None if trainer else model.last_loss())
     model.prefetch_slot(E2E0, host[0][0])
     for i in range(8):                                   # both e2e slots past their eager steps (graphs captured)
         step_e2e(i)
@@ -593,16 +611,13 @@ def main():
             gemm_ms = sum(v for k, v in phases.items() if k.startswith("gemm_"))
             flops = 6.0 * B * wl.P                                # 2BP forward + 4BP backward (SURVEY 8d)
             ach = flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
-            traffic, traffic_src = gemm_traffic_from_profile(args.engine, B)
             out["roofline"] = {"kernel": "mlp gemm (fwd+dgrad+wgrad)", "bound": "tensor", "achieved": ach, "peak": peaks["bf16_sustained"],
                                "unit": "TFLOP/s", "frac": ach / peaks["bf16_sustained"],
                                # the GEMMs run inside a long step, back to back with the rest of it: the SUSTAINED peak applies; the
                                # fraction against the burst figure (a kernel timed alone) is given beside it
                                "peak_burst": peaks["bf16_burst"], "frac_burst": ach / peaks["bf16_burst"], "peak_applies": "sustained",
-                               # dram__bytes_read.sum + dram__bytes_write.sum summed over the GEMM launches of one step, read from the
-                               # committed ncu capture of this engine / batch size (profiles/*_gemm_traffic.json); null when there is none
-                               "traffic": traffic, "traffic_unit": "bytes per step (all GEMM launches of one step)", "traffic_source": traffic_src,
-                               "peak_source": peaks["source"] + " dense bf16.  achieved = algorithmic fp32 FLOPs (6*B*P) / GEMM time; "
+                               "traffic": None,
+                               "peak_source": peaks["source"] + ", dense bf16.  achieved = algorithmic fp32 FLOPs (6*B*P) / GEMM time; "
                                               "both split engines issue 3 tensor-core products per algorithmic one, so the fp32-"
                                               "equivalent ceiling is 1/3 of the bf16 peak for bf16x3 and 1/6 for tc3x",
                                "tensor_pipe_frac": 3.0 * ach / peaks["bf16_sustained"] * (2.0 if args.engine == "tc3x" else 1.0),
@@ -620,7 +635,7 @@ def main():
                 u = min(nnz_avg * B, wl.rows)
                 bwd_bytes = 4 * B * wl.emb + 4 * nnz_avg * B + 16 * u * wl.emb
                 b_ms = phases.get("emb_grad_sum", 0.0) + phases.get("sparse_apply", 0.0)
-                out["roofline"] = dict(gk, kernel="emb gather + mean pool (forward)", traffic=None, peak_source=peaks["source"] + " HBM copy bandwidth",
+                out["roofline"] = dict(gk, kernel="emb gather + mean pool (forward)", traffic=None, peak_source=peaks["source"] + ", HBM bandwidth",
                                        share_of_step=g_ms / phases.get("total", 1.0))
                 out["kernels"]["emb_grad_sum_apply_bwd"] = {"bound": "hbm", "achieved": bwd_bytes / (b_ms * 1e-3) / 1e9 if b_ms > 0 else 0.0,
                                                             "peak": peaks["hbm_gbs"], "unit": "GB/s", "algorithmic_bytes": bwd_bytes, "ms": b_ms}
@@ -631,7 +646,7 @@ def main():
             ach = w_bytes / (w_ms * 1e-3) / 1e9 if w_ms > 0 else 0.0
             out["roofline"] = {"kernel": "wide logit gather + gradient sums + FTRL (excludes the id hashing and the sort)", "bound": "hbm",
                                "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": ach / peaks["hbm_gbs"], "traffic": None,
-                               "algorithmic_bytes": w_bytes, "ms": w_ms, "peak_source": peaks["source"] + " HBM copy bandwidth",
+                               "algorithmic_bytes": w_bytes, "ms": w_ms, "peak_source": peaks["source"] + ", HBM bandwidth",
                                "share_of_step": w_ms / phases.get("total", 1.0)}
             out["kernels"] = {"phases_ms": {k: round(v, 4) for k, v in phases.items()}}
         if not args.no_cpu_baseline and world == 1 and args.engine != "tc3x" and wl.name == "criteo":

@@ -1,5 +1,5 @@
 /*
- * wd_b200.h — C-ABI of libwd_b200.so: the B200-native Wide&Deep CTR train/eval step.
+ * wd_b200.h — C-ABI of libwd_b200.so: the H100-native (sm_90a) Wide&Deep CTR train/eval step.
  *
  * The reference (Lapis-Hong/wide_deep) has no native plugin/FFI boundary: its seam is the Python-level
  * estimator object built by build_custom_estimator (reference python/lib/build_estimator.py:264-294) whose
@@ -45,9 +45,9 @@ enum { WD_ACT_RELU = 0, WD_ACT_RELU6, WD_ACT_SIGMOID, WD_ACT_TANH, WD_ACT_LEAKY_
 /* dnn_connected_mode (reference python/lib/dnn.py:92-193) */
 enum { WD_MODE_SIMPLE = 0, WD_MODE_FIRST_DENSE, WD_MODE_LAST_DENSE, WD_MODE_DENSE, WD_MODE_RESNET };
 /* GEMM engine for the MLP */
-enum { WD_GEMM_AUTO = 0, WD_GEMM_FFMA = 1, WD_GEMM_TC3X = 2 /* tcgen05 kind::tf32, 3-pass split */,
-       WD_GEMM_TC1X = 3 /* tcgen05 kind::tf32 single pass: fast, NOT within the 1e-4 parity bar */,
-       WD_GEMM_BF16X3 = 4 /* tcgen05 kind::f16 on bf16 hi/lo copies written by the producing kernels, 3 passes */ };
+enum { WD_GEMM_AUTO = 0, WD_GEMM_FFMA = 1, WD_GEMM_TC3X = 2 /* wgmma tf32, 3-pass split */,
+       WD_GEMM_TC1X = 3 /* wgmma tf32 single pass: fast, NOT within the 1e-4 parity bar */,
+       WD_GEMM_BF16X3 = 4 /* wgmma on bf16 hi/lo copies written by the producing kernels, 3 passes */ };
 
 typedef struct WdOptimizer {
     int32_t kind;        /* WD_OPT_* */
@@ -259,7 +259,7 @@ int wd_debug_hidden(WdModel *m, int tower, int layer, float *out, int64_t cap);
 /* Kernel launch counter (launches of this library's kernels since creation). */
 int64_t wd_launch_count(WdModel *m);
 /* How many MLP GEMMs of a tensor-core engine (tc3x / tc1x) were handed to the fp32 FFMA kernel because their shape is not
- * covered by the tcgen05 kernel.  0 for every plan the library builds itself (all widths are padded to whole k-blocks); the
+ * covered by the wgmma kernel.  0 for every plan the library builds itself (all widths are padded to whole k-blocks); the
  * tests assert 0 so a silent downgrade cannot hide. */
 int64_t wd_gemm_fallback_count(WdModel *m);
 /* Per-phase device timings of the last synchronised step in milliseconds (CUDA events recorded on the model

@@ -25,7 +25,7 @@ parser.add_argument("--checkpoint_path", type=str, default=CONFIG["checkpoint_pa
 
 
 def main():
-    print("Using wide_deep_b200 (CUDA sm_100a) in place of TensorFlow")
+    print("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow")
     print("Model type: {}".format(FLAGS.model_type))
     model_dir = os.path.join(FLAGS.model_dir, FLAGS.model_type)
     print("Model directory: {}".format(model_dir))

@@ -119,7 +119,7 @@ def main():
     rank, world, local = distributed_env()
     if world > 1:
         return main_distributed(rank, world, local)
-    print("Using wide_deep_b200 (CUDA sm_100a) in place of TensorFlow")
+    print("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow")
     print("\nModel Type: {}".format(FLAGS.model_type))
     model_dir = os.path.join(FLAGS.model_dir, FLAGS.model_type)
     print("\nModel Directory: {}".format(model_dir))
@@ -151,7 +151,7 @@ def main_distributed(rank, world, local):
     torch.cuda.set_device(local)
     dist.init_process_group("gloo")                    # plumbing only (IPC handles, checkpoint gather); data moves over NVLink
     log = print if rank == 0 else (lambda *a, **k: None)
-    log("Using wide_deep_b200 (CUDA sm_100a) in place of TensorFlow: rank {} of {}".format(rank, world))
+    log("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow: rank {} of {}".format(rank, world))
     model_dir = os.path.join(FLAGS.model_dir, FLAGS.model_type)
     if not FLAGS.keep_train and rank == 0:
         shutil.rmtree(model_dir, ignore_errors=True)

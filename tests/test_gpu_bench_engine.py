@@ -7,14 +7,14 @@ seconds — the towers, the kernels and the tile shapes are the benchmark's.
   1. identical parameters: |gpu - oracle| <= 1e-4 * max(|oracle|, 1) on the logits of 3 x 2048 examples.
   2. 50 training steps in the settled regime ("warm": the oracle alone walks through the first ten steps, its state is copied
      to the GPU model, then both train 50 steps on the same batches): the loss of EVERY step within 1e-4 relative and the
-     logits of a fresh batch after the run within 5e-4.  Measured on B200: 6e-8 / 2e-7 for all engines (bf16x3 included).
+     logits of a fresh batch after the run within 5e-4.
   3. 50 training steps from the TF initialisers ("init").  With the reference's SUM-reduced loss and Adagrad(0.05) the first
      steps of this synthetic configuration are a violent transient (oracle losses 1.5e3 -> 4.2e5 -> 1.6e4 -> 4.9e2 -> 4.7e3
      ...) that amplifies ANY rounding difference by three orders of magnitude: the exact-fp32 FFMA engine — which differs
-     from the float64-accumulating oracle only in summation order — already drifts to 3e-4 on a step loss and 3.6e-3 on
-     fresh logits (tests/engine_drift_report.py).  No fp32 implementation can hold 1e-4 there, so the bound asserted for
+     from the float64-accumulating oracle only in summation order — already drifts past 1e-4 on a step loss and on
+     fresh logits (tests/engine_drift_report.py prints both).  No fp32 implementation can hold 1e-4 there, so the bound asserted for
      the tensor-core engines is relative to that floor: within 10x the drift the FFMA engine shows on the same run
-     (measured: tc3x 2.1x, bf16x3 6.3x on the worst step loss; 1.3x and 3.9x on the final logits) — bounded, not waived.
+     (the test prints both ratios) — bounded, not waived.
 Both engines also assert that no GEMM fell back to the FFMA kernel."""
 import numpy as np
 import pytest
@@ -123,7 +123,7 @@ def test_bench_shape_50_step_drift_from_init_is_within_the_fp32_envelope():
 
 
 def test_bench_shape_parameters_after_two_steps():
-    """Every trained tensor of the bf16x3 engine on the benchmark towers (B = 2048: the CTA-pair kernel, the fused logits-layer /
+    """Every trained tensor of the bf16x3 engine on the benchmark towers (B = 2048: the fused logits-layer /
     activation backward and — in the WD_FUSE_DACT=1 subprocess of the next test — the activation / batch-norm backward fused into
     the data-gradient epilogues) against the oracle: bias / gamma / beta gradients come from column partials, so a wrong partial
     shows up here at once."""
@@ -148,7 +148,7 @@ def test_bench_shape_parameters_after_two_steps():
 
 @pytest.mark.parametrize("fuse", ["1", "0"])
 def test_pair_kernel_on_a_ragged_batch(fuse):
-    """The CTA-pair kernel forced onto a small ragged problem (B = 700: the last pair's second CTA holds 60 valid rows), with and
+    """The 128 x 256 tiles forced onto a small ragged problem (B = 300: the last row tile holds 44 valid rows), with and
     without the fused activation-backward epilogue: the environment switches are read once per process, hence the subprocess."""
     import os
     import subprocess

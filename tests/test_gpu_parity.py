@@ -325,7 +325,7 @@ def test_eval_metrics():
         assert abs(got[k] - exp[k]) <= 2e-4 * max(abs(exp[k]), 1.0), "%s: %g vs %g" % (k, got[k], exp[k])
 
 
-# ------------------------------------------------------------------------------------ tcgen05 engine
+# ------------------------------------------------------------------------------------ wgmma engines
 def _engine_pair(engine, hidden, mode, B, seed):
     fc, cross, model = small_conf(hidden=hidden, mode=mode)
     om = OM.OracleModel(fc, cross, model, "wide_deep").init(seed)
@@ -338,10 +338,9 @@ def _engine_pair(engine, hidden, mode, B, seed):
 @pytest.mark.parametrize("engine", ["tc3x", "bf16x3"])
 @pytest.mark.parametrize("mode", ["simple", "dense", "first_dense"])
 def test_tc3x_engine_train_parity(mode, engine):
-    """tcgen05 with the 3-pass hi/lo split.  tc3x (kind::tf32, 2^-21 products) must meet the same bars as the fp32 FFMA
-    engine.  bf16x3 (kind::f16 on bf16 hi/lo copies written by the producing kernels, 2^-16 products) is the fast mode: its
-    loss must still agree to 1e-4 and its logits to 5e-4 on these small, badly conditioned towers (measured 1.2e-4 worst, 5e-6
-    on the benchmark shape).  A 1e-5 pre-activation error flips the occasional relu gate (about one of the ~10^5
+    """wgmma with the 3-pass hi/lo split.  tc3x (tf32, 2^-21 products) must meet the same bars as the fp32 FFMA
+    engine.  bf16x3 (bf16 hi/lo copies written by the producing kernels, 2^-16 products) is the fast mode: its
+    loss must still agree to 1e-4 and its logits to 5e-4 on these small, badly conditioned towers.  A 1e-5 pre-activation error flips the occasional relu gate (about one of the ~10^5
     activations of a step), which moves a handful of weight-gradient elements by a finite amount, so for bf16x3 the
     trained parameters are compared robustly (a flipped unit moves its whole weight column): 98 % of every tensor within
     2e-3 of its scale, nothing beyond 10 %."""

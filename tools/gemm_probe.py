@@ -20,7 +20,7 @@ for it in range(4):
     lib.wd_debug_gemm_probe(out)
 a = np.array(out[:], dtype=np.int64).reshape(32, 8)
 names = ["fwd0", "fwd1", "fwd2", "dg2", "wg2", "dg1", "wg1", "dg0", "wg0"]
-print("slot  first_data  mma_t1_done  mma_last_done  epi1_start epi1_end  epiL_start epiL_end   (us from kernel start)")
+print("slot  first_data  mma_first_done  mma_last_done  epi_first_done  epi_last_done   (us from kernel start, CTA 0)")
 for i in range(9):
     r = a[i]; t0 = r[0]
-    print(names[i], " ".join("%8.1f" % ((x - t0) / 1e3) if x > 0 else "       -" for x in r[1:]))
+    print(names[i], " ".join("%8.1f" % ((x - t0) / 1e3) if x > 0 else "       -" for x in r[1:6]))

@@ -103,7 +103,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(SO_PATH):
-            raise NativeError(ESTATE, "%s not found: run `python build_native.py` (nvcc, sm_100a)" % SO_PATH)
+            raise NativeError(ESTATE, "%s not found: run `python build_native.py` (nvcc, sm_90a)" % SO_PATH)
         L = ctypes.CDLL(SO_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(L, name)

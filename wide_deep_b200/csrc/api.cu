@@ -427,11 +427,11 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
                     // split-K factor of the weight gradient: enough (tile x split) work items to fill one wave of SMs,
                     // each split still at least 512 batch rows long
                     {
-                        // (the 3xBF16 engine covers N in 256-wide tiles when N allows it)
-                        const int tn = (m->gemm_engine == WD_GEMM_BF16X3 && L.N_phys % 256 == 0) ? 256 : 128;
-                        const int tiles = ((L.K_phys + 127) / 128) * ((L.N_phys + tn - 1) / tn);
+                        const int tiles = ((L.K_phys + 127) / 128) * ((L.N_phys + 127) / 128);     // both engines: 128 x 128 tiles
+                        int num_sms = kNumSms;
+                        cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device);
                         int sp = m->wgrad_splits;
-                        while (sp < 32 && tiles * sp * 2 <= 148 && m->max_batch_pad / (sp * 2) >= 512) sp *= 2;   // double only while one wave still holds it
+                        while (sp < 32 && tiles * sp * 2 <= num_sms && m->max_batch_pad / (sp * 2) >= 512) sp *= 2;   // double only while one wave still holds it
                         L.wgrad_splits = sp;
                     }
                     L.t_kernel = add_dense(L.K_phys, L.N_phys, L.wgrad_splits, 0, (int64_t)L.K_phys * L.N_phys, true);

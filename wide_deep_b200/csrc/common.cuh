@@ -26,6 +26,7 @@ void set_error(const char* fmt, ...);
 
 constexpr uint32_t kInvalidRow = 0xFFFFFFFFu;
 constexpr int kMaxSegs = 8;      // sources concatenated into one MLP layer input
+constexpr int kNumSms = 132;     // SMs of an H100 SXM: the grid caps of the grid-stride kernels are sized by it
 constexpr int kMaxDims = 8;      // distinct embedding widths per model
 // sort / unique-row scratch sets ("lists"): 0 embedding rows and 1 wide rows of the replicated tables; row-sharded tables add
 // 2 / 3 = rows this rank OWNS that were touched by any rank this step (embedding / wide) and 4 / 5 = this rank's own ids
@@ -452,7 +453,7 @@ inline void mark(WdModel* m, const char* name) {
     t.n++;
 }
 
-inline int grid_for(int64_t n, int block, int cap = 148 * 16) {
+inline int grid_for(int64_t n, int block, int cap = kNumSms * 16) {
     int64_t g = (n + block - 1) / block;
     if (g < 1) g = 1;
     if (g > cap) g = cap;

@@ -1,4 +1,4 @@
-// Shared GEMM interface of the MLP engines (FFMA in mlp.cu, tcgen05 in gemm_tc.cu and gemm_bf16.cu): operand descriptions,
+// Shared GEMM interface of the MLP engines (FFMA in mlp.cu, wgmma in gemm_tc.cu and gemm_bf16.cu): operand descriptions,
 // epilogue description and the activation functions (reference python/lib/utils/model_util.py:28-59).
 #pragma once
 #include <cuda_bf16.h>
@@ -47,7 +47,7 @@ struct GemmA {                         // A operand: up to kMaxSegs K-contiguous
     const __nv_bfloat16* hi[kMaxSegs]; // 3xBF16 engine: the same segments pre-split into bf16 hi / lo copies (same ld)
     const __nv_bfloat16* lo[kMaxSegs];
 };
-// EPI_DACT (3xBF16 pair kernel only): a data-gradient GEMM whose epilogue is the activation / batch-norm backward of the layer
+// EPI_DACT (3xBF16 engine only): a data-gradient GEMM whose epilogue is the activation / batch-norm backward of the layer
 // it feeds — dH never reaches memory: dZ = dH * gamma' * act'(A) leaves as bf16 hi / lo copies and the 128-row column partials of
 // the bias / gamma / beta gradients go to the partial arena (what act_bn_bwd_q_kernel does in a separate pass otherwise)
 enum { EPI_FWD = 0, EPI_STORE = 1, EPI_WGRAD = 2, EPI_DACT = 3 };

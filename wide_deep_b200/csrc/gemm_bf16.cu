@@ -1,36 +1,38 @@
-// 3xBF16 tcgen05 engine for the MLP GEMMs on sm_100a (the default engine).
+// 3xBF16 wgmma engine for the MLP GEMMs on sm_90a (the engine bench.py runs).
 //
-//   C[M,N] = sum_k A[M,k] * B[N,k]      fp32 values, both operands K-contiguous, fp32 accumulation in TMEM
+//   C[M,N] = sum_k A[M,k] * B[N,k]      fp32 values, fp32 accumulation in registers
 //
 // Every fp32 operand exists in HBM as two bf16 copies, hi = bf16_rn(x) and lo = bf16_rn(x - hi), written by the kernel that
 // PRODUCED the operand (forward epilogue, act_bn_bwd_kernel, x0_split_kernel, dense_apply_kernel), so this kernel moves and
 // multiplies bf16 only: per 64-element k-block four TMA tiles (A_hi, A_lo, B_hi, B_lo; 128-byte swizzle) and
-// 4 k-steps x 3 tcgen05.mma.kind::f16 (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi) into one fp32 accumulator.  hi + lo represents x to
-// 2^-17 and the dropped a_lo*b_lo term is below 2^-16, so one product carries ~1e-5 relative error (rms ~8e-6; random signs, so a
-// long dot product does better): measured 5e-6 on the logits of the benchmark shape, up to ~1e-4 on small ill-conditioned
-// towers (tests/test_gpu_parity.py, tests/engine_error_report.py).  That is a FAST mode: it meets the 1e-4 logit bar on the
-// benchmarked configuration (bench.py re-checks it against the oracle in the same run) but is not fp32-faithful the way the
-// 3xTF32 engine (gemm_tc.cu, 2^-21) is; it costs half the shared-memory bytes per flop, runs at twice the tensor-pipe rate and
-// needs no in-kernel splitting pass.  (Keeping the residual in fp16 would give 19 bits, but tcgen05.mma.kind::f16 traps with an
-// illegal-instruction fault on sm_100a when the A and B formats differ — tried, reverted.)
+// 4 k-steps x 3 wgmma.mma_async (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi) into one fp32 accumulator.  hi + lo represents x to
+// 2^-17 and the dropped a_lo*b_lo term is below 2^-16, so one product carries ~1e-5 relative error (random signs, so a long dot
+// product does better).  That is a FAST mode: it is held to the 1e-4 logit bar on the benchmarked configuration (bench.py
+// re-checks it against the oracle in the same run, tests/test_gpu_bench_engine.py under pytest) but is not fp32-faithful the way
+// the 3xTF32 engine (gemm_tc.cu, 2^-21) is; it moves half the shared-memory bytes per flop and needs no in-kernel splitting pass.
 //
 // Operand majors.  Forward: A = activations [m][k] (K-major), B = weights W[k][n] (MN-major: n contiguous) — no transposed weight
 // copy exists.  Data gradient: A = dZ [m][n] and B = W[k_in][n], both K-major over n.  Weight gradient: A = layer input [b][k_in]
 // and B = dZ [b][n], both MN-major with the batch as the reduction dimension — no transposed activation copies exist either,
 // and TMA zero-fills the batch tail.  An MN-major operand is fetched as 64-column boxes (64 k-rows x 128 B, 128-byte swizzle);
-// its UMMA descriptor uses LBO = one box (8 KB) between 64-wide column groups and SBO = 1 KB between 8-row k groups.
+// its descriptor uses LBO = one box (8 KB) between 64-wide column groups and SBO = 1 KB between 8-row k groups.
 //
-// One persistent CTA per SM, ten warps: 0 = TMA producer, 1 = MMA issuer (one elected lane), 2-9 = epilogue (TMEM lane quarter
-// = warp % 4, two warps per quarter splitting the columns).  The TMEM accumulator is double buffered (2 x TBN columns) so the epilogue's global stores of tile i overlap the
-// MMAs of tile i+1.  Forward epilogue = bias + activation + BN-affine; it stores the post-activation values (fp32, for the
-// backward), the layer output as bf16 hi/lo copies (what the next layer and the weight gradient read) and, only for layers the
-// logits layer reads, the fp32 layer output.
+// One persistent CTA per SM, three warp groups: group 0 = TMA producer (one elected thread, registers handed over with
+// setmaxnreg), groups 1-2 = consumers, each owning 64 rows of the 128 x TBN tile in registers (TBN / 2 accumulators per thread).
+// A consumer releases a pipeline stage once the wgmma batch that read it has retired (wait_group 1: the next batch is already
+// queued), and the producer runs ahead into the next tile while the consumers store the current one.  Forward epilogue = bias +
+// activation + BN-affine straight from the accumulator fragment; it stores the post-activation values (fp32, for the backward),
+// the layer output as bf16 hi/lo copies (what the next layer and the weight gradient read) and, only for layers the logits layer
+// reads, the fp32 layer output.  A quad of lanes owns 8 consecutive columns of a row, so every fp32 store instruction writes
+// whole 32-byte sectors.
 #include <cuda.h>
 #include <stdlib.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "gemm.cuh"
-#include "tc_ptx.cuh"
+#include "wgmma_ptx.cuh"
 
 namespace wd {
 
@@ -38,27 +40,9 @@ int tc_make_map_bf16(CUtensorMap* map, const void* ptr, int rows, int cols, int 
 
 namespace {
 
-// explicit shared-window accesses: the staging tiles are carved out of the dynamic shared memory through integer arithmetic, so
-// the compiler cannot prove the address space and would emit generic LD / ST (long-scoreboard, slower) for them
-__device__ __forceinline__ void sts128(uint32_t a, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t a) {
-    uint4 v;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ void sts32f(uint32_t a, float x) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(x) : "memory"); }
-__device__ __forceinline__ float4 lds128f(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ float lds32f(uint32_t a) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory"); return v; }
-
-constexpr int QBM = 128;         // UMMA M
+constexpr int QBM = 128;         // tile rows: two warp groups x wgmma M = 64
 constexpr int QBK = 64;          // bf16 elements per k-block = one 128-byte swizzle row
-constexpr int Q_THREADS = 320;       // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue
+constexpr int Q_THREADS = 384;   // warp group 0 TMA, warp groups 1-2 MMA + epilogue
 
 struct QMaps {
     CUtensorMap a_hi[kMaxSegs], a_lo[kMaxSegs];
@@ -66,10 +50,18 @@ struct QMaps {
 };
 struct QSegs { int n; int k[kMaxSegs]; int koff[kMaxSegs]; };
 
-// optional timeline probe of CTA 0 (WD_GEMM_PROBE=1): globaltimer stamps per launch slot, read back by wd_debug_gemm_probe
+// optional timeline probe of CTA 0 (WD_GEMM_PROBE=1): globaltimer stamps per launch slot, read back by wd_debug_gemm_probe.
+// 0 kernel start, 1 first operands landed, 2 / 3 main loop of the first / last tile done, 4 / 5 epilogue of the first / last tile done
 __device__ unsigned long long g_probe[32 * 8];
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define PROBE(i) do { if (probe >= 0 && blockIdx.x == 0 && lane == 0) g_probe[probe * 8 + (i)] = gtime(); } while (0)
+#define PROBE(i) do { if (probe >= 0 && blockIdx.x == 0 && (threadIdx.x & 127) == 0) g_probe[probe * 8 + (i)] = gtime(); } while (0)
+
+__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {    // packed bf16 pairs of the hi / lo copies
+    const __nv_bfloat162 hp = __floats2bfloat162_rn(x0, x1);
+    hi = *reinterpret_cast<const uint32_t*>(&hp);
+    const __nv_bfloat162 lp = __floats2bfloat162_rn(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
+    lo = *reinterpret_cast<const uint32_t*>(&lp);
+}
 
 template <int TBN, int MODE>
 __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid_constant__ QMaps maps, const QSegs segs, int M, int N, int ktot,
@@ -77,22 +69,19 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
     extern __shared__ uint8_t smem_raw[];
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr bool A_MN = MODE == EPI_WGRAD;                       // operand stored with its M / N index contiguous
-    constexpr bool B_MN = MODE != EPI_STORE;
+    constexpr bool B_MN = MODE == EPI_FWD || MODE == EPI_WGRAD;
     constexpr int A_BYTES = QBM * 128, B_BYTES = TBN * 128;
     constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);
-    constexpr int NST = TBN == 256 ? 2 : 3;
+    constexpr int NST = TBN == 256 ? 2 : 3;                        // 96 KB / 64 KB stages: 192 KB of the 227 KB a block may use
     auto a_hi = [&](int s) { return base + s * STAGE_BYTES; };
     auto a_lo = [&](int s) { return base + s * STAGE_BYTES + A_BYTES; };
     auto b_hi = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES; };
     auto b_lo = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES + B_BYTES; };
-    uint8_t* stage_out = base + NST * STAGE_BYTES;                 // 8 epilogue warps x 2 KB store staging (1024-byte aligned)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stage_out + 16384);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(base + NST * STAGE_BYTES);
     uint64_t* full = bars; uint64_t* empty = bars + NST;
-    uint64_t* tmem_full = bars + 2 * NST; uint64_t* tmem_empty = bars + 2 * NST + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * NST + 4);
-    float* epi_params = reinterpret_cast<float*>(bars + 16);      // [8 epilogue warps][bias | scale | shift][32]
+    float* colsum = reinterpret_cast<float*>(bars + 16);           // EPI_DACT: [3 sums][8 consumer warps][TBN columns]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + QBM - 1) / QBM;
     const int ntiles = tiles_n * tiles_m * nsplit;
     // k-blocks of one tile: FWD / STORE walk the segments (each padded to whole k-blocks by TMA zero fill), WGRAD walks its split
@@ -113,23 +102,16 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 256); }
+        for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }       // empty: one arrival per consumer warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * TBN)));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    if (warp == 0) PROBE(0);
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
+        reg_dealloc<40>();
+        PROBE(0);
+        if (warp == 0 && lane == 0) {
             int g = 0;
             for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
                 int m0, n0, z, kbeg, nkb;
@@ -169,649 +151,139 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        // instruction descriptor: D = f32, A = B = bf16, both K-major, N >> 3, M >> 4
-        constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                                   ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(QBM >> 4) << 24);
+    } else {
+        // ------------------------------------------------------------------ consumers: warp group cw owns rows [64 cw, 64 cw + 64)
+        reg_alloc<232>();
+        const int cw = wg - 1, cwarp = warp - 4;
         constexpr uint32_t a_step = A_MN ? 2048u : 32u, b_step = B_MN ? 2048u : 32u;   // bytes per 16-element k-step
+        constexpr int TA = A_MN ? 1 : 0, TB = B_MN ? 1 : 0;
+        float d[TBN / 2];
         int g = 0, use = 0;
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             int m0, n0, z, kbeg, nkb;
             tile_range(tile, m0, n0, z, kbeg, nkb);
-            if (nkb == 0) continue;
-            const int a = use & 1, au = use >> 1;
-            if (au > 0) mbar_wait(&tmem_empty[a], (au - 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tacc = tmem_base + (uint32_t)(a * TBN);
+            if (nkb == 0) {
+#pragma unroll
+                for (int i = 0; i < TBN / 2; ++i) d[i] = 0.f;
+            }
+            int prev = -1;
             for (int kb = 0; kb < nkb; ++kb, ++g) {
                 const int s = g % NST, it = g / NST;
                 mbar_wait(&full[s], it & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
                 if (g == 0) PROBE(1);
-                if (lane == 0) {
-                    const uint32_t sa_hi = smem_u32(a_hi(s)), sb_hi = smem_u32(b_hi(s));
-                    const uint32_t sa_lo = smem_u32(a_lo(s)), sb_lo = smem_u32(b_lo(s));
+                const uint32_t sa_hi = smem_u32(a_hi(s)) + cw * 8192, sa_lo = smem_u32(a_lo(s)) + cw * 8192;   // 64 rows (or one 64-column box) per group
+                const uint32_t sb_hi = smem_u32(b_hi(s)), sb_lo = smem_u32(b_lo(s));
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < QBK / 16; ++k) {
-                        const uint64_t da_hi = A_MN ? make_desc_mn(sa_hi + k * a_step) : make_desc(sa_hi + k * a_step);
-                        const uint64_t da_lo = A_MN ? make_desc_mn(sa_lo + k * a_step) : make_desc(sa_lo + k * a_step);
-                        const uint64_t db_hi = B_MN ? make_desc_mn(sb_hi + k * b_step) : make_desc(sb_hi + k * b_step);
-                        const uint64_t db_lo = B_MN ? make_desc_mn(sb_lo + k * b_step) : make_desc(sb_lo + k * b_step);
-                        umma_bf16(tacc, da_lo, db_hi, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                        umma_bf16(tacc, da_hi, db_lo, idesc, 1u);
-                        umma_bf16(tacc, da_hi, db_hi, idesc, 1u);
-                    }
-                    umma_commit(&empty[s]);
-                    if (kb == nkb - 1) umma_commit(&tmem_full[a]);
+                for (int k = 0; k < QBK / 16; ++k) {
+                    const uint64_t da_hi = A_MN ? make_desc_mn(sa_hi + k * a_step) : make_desc(sa_hi + k * a_step);
+                    const uint64_t da_lo = A_MN ? make_desc_mn(sa_lo + k * a_step) : make_desc(sa_lo + k * a_step);
+                    const uint64_t db_hi = B_MN ? make_desc_mn(sb_hi + k * b_step) : make_desc(sb_hi + k * b_step);
+                    const uint64_t db_lo = B_MN ? make_desc_mn(sb_lo + k * b_step) : make_desc(sb_lo + k * b_step);
+                    wgmma_bf16<TA, TB>(d, da_lo, db_hi, (kb > 0 || k > 0) ? 1u : 0u);
+                    wgmma_bf16<TA, TB>(d, da_hi, db_lo, 1u);
+                    wgmma_bf16<TA, TB>(d, da_hi, db_hi, 1u);
                 }
-                __syncwarp();
-            }
-            PROBE(use == 0 ? 2 : 3);
-            ++use;
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue: warps 2..9
-        // TMEM lane quarter = warp % 4 (hardware rule), so two warps share a quarter and split the tile's columns in halves.
-        // A thread owns one accumulator row (tcgen05.ld 32x32b); storing straight from registers would touch 32 different
-        // 128-byte lines per instruction, so every 32-row x 64-byte piece goes through a 2 KB swizzled (conflict-free) staging
-        // tile: lane = row writes it, then 4 lanes x 16 B cover a row and one store instruction writes 8 rows — whole sectors,
-        // fire-and-forget.  (A TMA-store epilogue was measured no faster; the epilogue is bound by its instruction count, hence
-        // eight warps, packed bf16 conversions and a predicate-free relu path.)
-        const int ew = warp - 2, q = warp & 3, half = ew >> 2;
-        const uint32_t stg_s = smem_u32(stage_out + ew * 2048);
-        int use = 0;
-        auto put64 = [&](const uint32_t* x) {                         // 16 words per lane -> [32 rows][64 B], 64-byte swizzle
-            __syncwarp();                                             // earlier readers of the staging tile are done
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-                sts128(stg_s + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4), x[4 * c], x[4 * c + 1], x[4 * c + 2], x[4 * c + 3]);
-            __syncwarp();
-        };
-        // rows [mw, mw + 32) of a row-major matrix, 64 bytes per row starting at dst (byte pointer of row mw); accumulate: fp32 +=
-        auto flush64 = [&](uint8_t* __restrict__ dst, int64_t ld_bytes, int mw, bool accumulate) {
-            // all four staged pieces (and, when accumulating, the four previous values) are fetched into DISTINCT registers before
-            // the first store: a store holds its source registers until the data has left for L1, so re-using one register quad per
-            // piece (what a load-store-load-store order compiles to) serialises the warp on that hand-off
-            const int c = lane & 3, r0 = lane >> 2;
-            uint4 v[4], p[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = i * 8 + r0;
-                v[i] = lds128(stg_s + r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
-            }
-            if (accumulate) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = i * 8 + r0;
-                    p[i] = *reinterpret_cast<const uint4*>(dst + (int64_t)min(r, M - 1 - mw < 0 ? 0 : M - 1 - mw) * ld_bytes + c * 16);
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();                              // the batch that read stage `prev` has retired
+                    if (lane == 0) mbar_arrive(&empty[prev]);
                 }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    v[i].x = __float_as_uint(__uint_as_float(v[i].x) + __uint_as_float(p[i].x)); v[i].y = __float_as_uint(__uint_as_float(v[i].y) + __uint_as_float(p[i].y));
-                    v[i].z = __float_as_uint(__uint_as_float(v[i].z) + __uint_as_float(p[i].z)); v[i].w = __float_as_uint(__uint_as_float(v[i].w) + __uint_as_float(p[i].w));
-                }
+                prev = s;
             }
+            wgmma_wait<0>();                                      // the accumulator is final
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            if (cwarp == 0) PROBE(use == 0 ? 2 : 3);
+
+            // ---- epilogue from the accumulator fragment: rows r0 and r0 + 8, columns n0 + 8 j + 2 (lane % 4) + {0, 1}
+            const int r0 = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+            const int cq = 2 * (lane & 3);
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = i * 8 + r0;
-                if (mw + r < M) *reinterpret_cast<uint4*>(dst + (int64_t)r * ld_bytes + c * 16) = v[i];
-            }
-        };
-        auto store_f32 = [&](float* __restrict__ dst, int64_t ld, int mw, int nb, const uint32_t* x, bool accumulate) {   // 32 x 32 fp32
-            uint8_t* d = reinterpret_cast<uint8_t*>(dst + (int64_t)mw * ld + nb);
-            put64(x); flush64(d, ld * 4, mw, accumulate);
-            put64(x + 16); flush64(d + 64, ld * 4, mw, accumulate);
-        };
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            int m0, n0, z, kbeg, nkb;
-            tile_range(tile, m0, n0, z, kbeg, nkb);
-            const int mw = m0 + q * 32;                        // first row of this warp's chunks
-            const int m = mw + lane;
-            const int a = use & 1, au = use >> 1;
-            const int c_beg = half * (TBN / 64), c_end = c_beg + TBN / 64;
-            // bias / BN scale / BN shift of column nb + lane: fetched one chunk ahead (the first chunk's before the wait for the
-            // accumulator), so their global-load latency never sits on the epilogue's critical path
-            float pb = 0.f, pg = 1.f, pe = 0.f;
-            auto load_params = [&](int nbx, float& b_, float& g_, float& e_) {
-                const int gn = nbx + lane;
-                const bool in = gn < ep.n_logical;
-                b_ = in ? ep.bias[gn] : 0.f;
-                g_ = (in && ep.bn) ? ep.gamma[gn] * 0.99950037468777f : 1.f;
-                e_ = (in && ep.bn) ? ep.beta[gn] : 0.f;
-            };
-            if (MODE == EPI_FWD && n0 + c_beg * 32 < N) load_params(n0 + c_beg * 32, pb, pg, pe);
-            if (nkb > 0) {
-                mbar_wait(&tmem_full[a], au & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            }
-            if (ew == 0) PROBE(use == 0 ? 4 : 6);
-#pragma unroll 1
-            for (int c = c_beg; c < c_end; ++c) {
-                const int nb = n0 + c * 32;
-                if (nb >= N) break;
-                float qb = 0.f, qg = 1.f, qe = 0.f;
-                if (MODE == EPI_FWD && c + 1 < c_end && nb + 32 < N) load_params(nb + 32, qb, qg, qe);
-                uint32_t v[32];
-                if (nkb > 0) tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * TBN + c * 32), v);
-                else {
+            for (int j = 0; j < TBN / 8; ++j) {
+                const int c = n0 + 8 * j + cq;
+                if (n0 + 8 * j < N) {
+                    if (MODE == EPI_FWD) {
+                        const bool in0 = c < ep.n_logical, in1 = c + 1 < ep.n_logical;
+                        const float b0 = in0 ? __ldg(ep.bias + c) : 0.f, b1 = in1 ? __ldg(ep.bias + c + 1) : 0.f;
+                        const float g0 = (in0 && ep.bn) ? __ldg(ep.gamma + c) * 0.99950037468777f : 1.f;
+                        const float g1 = (in1 && ep.bn) ? __ldg(ep.gamma + c + 1) * 0.99950037468777f : 1.f;
+                        const float e0 = (in0 && ep.bn) ? __ldg(ep.beta + c) : 0.f, e1 = (in1 && ep.bn) ? __ldg(ep.beta + c + 1) : 0.f;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 0u;
-                }
-                if (MODE == EPI_FWD) {
-                    const uint32_t wp = smem_u32(epi_params + ew * 96);
-                    __syncwarp();
-                    sts32f(wp + 4 * lane, pb); sts32f(wp + 4 * (32 + lane), pg); sts32f(wp + 4 * (64 + lane), pe);
-                    pb = qb; pg = qg; pe = qe;
-                    __syncwarp();
-                    uint32_t h[32];
-                    const bool rv = m < ep.m_valid;
-                    if (ep.act == WD_ACT_RELU) {
-                        // warp-uniform fast path, no per-column predicate: padded columns have zero weights, bias 0, scale 1,
-                        // shift 0, and relu(0) = 0 keeps them zero
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 b4 = lds128f(wp + 16 * j4);
-                            const float4 g4 = lds128f(wp + 128 + 16 * j4);
-                            const float4 e4 = lds128f(wp + 256 + 16 * j4);
-                            const float a0 = fmaxf(__uint_as_float(v[4 * j4]) + b4.x, 0.f), a1 = fmaxf(__uint_as_float(v[4 * j4 + 1]) + b4.y, 0.f);
-                            const float a2 = fmaxf(__uint_as_float(v[4 * j4 + 2]) + b4.z, 0.f), a3 = fmaxf(__uint_as_float(v[4 * j4 + 3]) + b4.w, 0.f);
-                            v[4 * j4] = __float_as_uint(a0); v[4 * j4 + 1] = __float_as_uint(a1); v[4 * j4 + 2] = __float_as_uint(a2); v[4 * j4 + 3] = __float_as_uint(a3);
-                            h[4 * j4] = __float_as_uint(fmaf(a0, g4.x, e4.x)); h[4 * j4 + 1] = __float_as_uint(fmaf(a1, g4.y, e4.y));
-                            h[4 * j4 + 2] = __float_as_uint(fmaf(a2, g4.z, e4.z)); h[4 * j4 + 3] = __float_as_uint(fmaf(a3, g4.w, e4.w));
+                        for (int hh = 0; hh < 2; ++hh) {
+                            const int r = r0 + 8 * hh;
+                            if (r >= M) continue;
+                            const bool rv = r < ep.m_valid;          // rows past the batch: zeros
+                            float a0 = 0.f, a1 = 0.f, h0 = 0.f, h1 = 0.f;
+                            if (rv && in0) { a0 = ep.act == WD_ACT_RELU ? fmaxf(d[4 * j + 2 * hh] + b0, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh] + b0); h0 = fmaf(a0, g0, e0); }
+                            if (rv && in1) { a1 = ep.act == WD_ACT_RELU ? fmaxf(d[4 * j + 2 * hh + 1] + b1, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh + 1] + b1); h1 = fmaf(a1, g1, e1); }
+                            const int64_t o = (int64_t)r * ep.ldh + c;
+                            if (ep.A_out != ep.H_out) *reinterpret_cast<float2*>(ep.A_out + o) = make_float2(a0, a1);
+                            if (ep.H_out) *reinterpret_cast<float2*>(ep.H_out + o) = make_float2(h0, h1);   // fp32 copy only where something reads it
+                            uint32_t ph, pl;
+                            split_pair(h0, h1, ph, pl);
+                            *reinterpret_cast<uint32_t*>(ep.Hs_hi + o) = ph;
+                            *reinterpret_cast<uint32_t*>(ep.Hs_lo + o) = pl;
                         }
-                        if (nb + 32 > ep.n_logical) {                 // chunk straddling the logical width: BN shift must not leak into padding
+                    } else if (MODE == EPI_DACT) {
+                        // d = dH of the fed layer; never stored.  dZ = dH * gamma' * act'(A) leaves as bf16 hi / lo copies, the column
+                        // sums of dZ (bias), dH * A (gamma) and dH (beta) over this warp's 16 rows go to shared memory
+                        const bool in0 = c < ep.n_logical, in1 = c + 1 < ep.n_logical;
+                        const float g0 = (in0 && ep.bn) ? __ldg(ep.gamma + c) * 0.99950037468777f : 1.f;
+                        const float g1 = (in1 && ep.bn) ? __ldg(ep.gamma + c + 1) * 0.99950037468777f : 1.f;
+                        float sb0 = 0.f, sb1 = 0.f, sg0 = 0.f, sg1 = 0.f, se0 = 0.f, se1 = 0.f;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) if (nb + j >= ep.n_logical) { v[j] = 0u; h[j] = 0u; }
+                        for (int hh = 0; hh < 2; ++hh) {
+                            const int r = r0 + 8 * hh;
+                            if (r >= M) continue;
+                            const int64_t o = (int64_t)r * ep.ldh + c;
+                            const float2 av = __ldg(reinterpret_cast<const float2*>(ep.Aact + o));
+                            const float dh0 = in0 ? d[4 * j + 2 * hh] : 0.f, dh1 = in1 ? d[4 * j + 2 * hh + 1] : 0.f;
+                            const float aa0 = in0 ? av.x : 0.f, aa1 = in1 ? av.y : 0.f;
+                            const float dz0 = dh0 * g0 * act_bwd(ep.act, aa0), dz1 = dh1 * g1 * act_bwd(ep.act, aa1);
+                            uint32_t ph, pl;
+                            split_pair(dz0, dz1, ph, pl);
+                            *reinterpret_cast<uint32_t*>(ep.Hs_hi + o) = ph;
+                            *reinterpret_cast<uint32_t*>(ep.Hs_lo + o) = pl;
+                            sb0 += dz0; sb1 += dz1;
+                            sg0 += dh0 * aa0 * 0.99950037468777f; sg1 += dh1 * aa1 * 0.99950037468777f;
+                            se0 += dh0; se1 += dh1;
+                        }
+#pragma unroll
+                        for (int o = 4; o <= 16; o <<= 1) {           // over the 8 row pairs of the warp, fixed order
+                            sb0 += __shfl_xor_sync(0xffffffffu, sb0, o); sb1 += __shfl_xor_sync(0xffffffffu, sb1, o);
+                            sg0 += __shfl_xor_sync(0xffffffffu, sg0, o); sg1 += __shfl_xor_sync(0xffffffffu, sg1, o);
+                            se0 += __shfl_xor_sync(0xffffffffu, se0, o); se1 += __shfl_xor_sync(0xffffffffu, se1, o);
+                        }
+                        if (lane < 4) {
+                            float* cs = colsum + cwarp * TBN + 8 * j + cq;
+                            cs[0] = sb0; cs[1] = sb1;
+                            cs[8 * TBN] = sg0; cs[8 * TBN + 1] = sg1;
+                            cs[16 * TBN] = se0; cs[16 * TBN + 1] = se1;
                         }
                     } else {
+                        float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const bool ok = (nb + j) < ep.n_logical;
-                            const float av = ok ? act_fwd(ep.act, __uint_as_float(v[j]) + lds32f(wp + 4 * j)) : 0.f;
-                            v[j] = __float_as_uint(av);
-                            h[j] = __float_as_uint(ok ? fmaf(av, lds32f(wp + 4 * (32 + j)), lds32f(wp + 4 * (64 + j))) : 0.f);
-                        }
-                    }
-                    if (!rv) {                                        // rows past the batch: zeros (only in the last row tile)
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) { v[j] = 0u; h[j] = 0u; }
-                    }
-                    if (ep.A_out != ep.H_out) store_f32(ep.A_out, ep.ldh, mw, nb, v, false);
-                    if (ep.H_out) store_f32(ep.H_out, ep.ldh, mw, nb, h, false);      // fp32 copy only where something reads it
-                    uint32_t hh[16], hl[16];                           // packed bf16 pairs of the hi / lo copies
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float x0 = __uint_as_float(h[2 * j]), x1 = __uint_as_float(h[2 * j + 1]);
-                        const __nv_bfloat162 hp = __floats2bfloat162_rn(x0, x1);
-                        const uint32_t hb = *reinterpret_cast<const uint32_t*>(&hp);
-                        const __nv_bfloat162 lp = __floats2bfloat162_rn(x0 - __uint_as_float(hb << 16), x1 - __uint_as_float(hb & 0xFFFF0000u));
-                        hh[j] = hb;
-                        hl[j] = *reinterpret_cast<const uint32_t*>(&lp);
-                    }
-                    uint8_t* dh = reinterpret_cast<uint8_t*>(ep.Hs_hi + (int64_t)mw * ep.ldh + nb);
-                    uint8_t* dl = reinterpret_cast<uint8_t*>(ep.Hs_lo + (int64_t)mw * ep.ldh + nb);
-                    put64(hh); flush64(dh, (int64_t)ep.ldh * 2, mw, false);
-                    put64(hl); flush64(dl, (int64_t)ep.ldh * 2, mw, false);
-                } else {
-                    store_f32(ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0), ep.ldc, mw, nb, v, MODE == EPI_STORE && ep.accumulate);
-                }
-            }
-            if (nkb > 0) {
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(&tmem_empty[a]);                   // accumulator buffer a may be overwritten
-                if (ew == 0) PROBE(use == 0 ? 5 : 7);
-                ++use;
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * TBN)));
-}
-
-// ================================================================================================================================
-// CTA-PAIR variant (tcgen05 cta_group::2): two CTAs of a cluster (the two SMs of a TPC) compute one 256 x 256 tile.  CTA r stages
-// rows [128 r, 128 r + 128) of A and columns [128 r, 128 r + 128) of B; the pair's tensor cores read the two B halves from both
-// shared memories, so each SM reads 4 KB (A) + 4 KB (its B half) per UMMA instead of 4 + 8 KB and fills 64 KB instead of 96 KB per
-// k-block: 160 KB over the 128 B/clk shared-memory port per 1536 tensor clocks (the single-CTA tile needs 240 KB = 1920 clocks), and
-// the freed shared memory holds a third pipeline stage.  One thread of the LEADER CTA (cluster rank 0) issues the UMMAs for both;
-// every TMA load of either CTA signals the leader's `full` barrier; tcgen05.commit multicasts the `empty` / `tmem_full` arrivals to
-// both CTAs; the epilogue warps of both CTAs read their own TMEM halves and release the accumulator on the leader's barrier.
-// Every barrier wait carries a watchdog (trap instead of a hung device).
-__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t map_to_cta(uint32_t smem_addr, uint32_t rank) {       // shared::cluster address of the same offset in CTA `rank`
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity) {
-    const uint32_t a = smem_u32(bar);
-    for (uint32_t spin = 0;; ++spin) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-        if (ok) return;
-        if (spin > (1u << 27)) { printf("libwd_b200: 2-CTA GEMM barrier watchdog (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
-    }
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {          // arrives on the barrier at this offset in BOTH CTAs
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-
-// Sum of x[j] over the 32 lanes for every j, transposed: lane j returns the sum of column j.  Five exchange rounds that halve
-// the live values (16 + 8 + 4 + 2 + 1 shuffles), fixed order.
-__device__ __forceinline__ float colsum32(float (&x)[32], int lane) {
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) {
-        const bool up = (lane & o) != 0;
-#pragma unroll
-        for (int i = 0; i < o; ++i) {
-            const float keep = up ? x[i + o] : x[i];
-            const float send = up ? x[i] : x[i + o];
-            x[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-        }
-    }
-    return x[0];
-}
-
-constexpr bool kPairDefault = true;  // validated on B200 (tests green, +7 % on the layer-0 GEMMs); WD_GEMM_2CTA=0 selects the single-CTA kernel
-constexpr int P_TBN = 256;           // tile columns of the pair (each CTA stages 128 of them)
-constexpr int P_NST = 3;
-
-template <int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(Q_THREADS, 1)
-tc_gemm_bf16_pair_kernel(const __grid_constant__ QMaps maps, const QSegs segs, int M, int N, int ktot, int ksplit_len, int nsplit, Epi ep) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    constexpr bool A_MN = MODE == EPI_WGRAD;
-    constexpr bool B_MN = MODE == EPI_FWD || MODE == EPI_WGRAD;
-    constexpr int A_BYTES = QBM * 128, B_BYTES = (P_TBN / 2) * 128;          // per CTA: 128 rows of A, 128 columns of B, 64 k each
-    constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);                     // 64 KB
-    auto a_hi = [&](int s) { return base + s * STAGE_BYTES; };
-    auto a_lo = [&](int s) { return base + s * STAGE_BYTES + A_BYTES; };
-    auto b_hi = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES; };
-    auto b_lo = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES + B_BYTES; };
-    uint8_t* stage_out = base + P_NST * STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stage_out + 16384);
-    uint64_t* full = bars; uint64_t* empty = bars + P_NST;
-    uint64_t* tmem_full = bars + 2 * P_NST; uint64_t* tmem_empty = bars + 2 * P_NST + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * P_NST + 4);
-    float* epi_params = reinterpret_cast<float*>(bars + 16);
-    float* colsum = epi_params + 8 * 96;                           // EPI_DACT: [8 epilogue warps][3 sums][128 columns]
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_rank();
-    const bool leader = rank == 0;
-    const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-    const int tiles_n = (N + P_TBN - 1) / P_TBN, tiles_m = (M + 2 * QBM - 1) / (2 * QBM);
-    const int ntiles = tiles_n * tiles_m * nsplit;
-    int nkb_all = 0;
-    for (int s = 0; s < segs.n; ++s) nkb_all += (segs.k[s] + QBK - 1) / QBK;
-    auto tile_range = [&](int tile, int& m0, int& n0, int& z, int& kbeg, int& nkb) {
-        z = tile / (tiles_n * tiles_m);
-        int r = tile % (tiles_n * tiles_m);
-        m0 = (r / tiles_n) * (2 * QBM) + (int)rank * QBM;         // this CTA's 128 rows
-        n0 = (r % tiles_n) * P_TBN;
-        kbeg = 0;
-        nkb = nkb_all;
-        if (MODE == EPI_WGRAD) {
-            kbeg = z * ksplit_len;
-            int kend = min(ktot, kbeg + ksplit_len);
-            nkb = kend > kbeg ? (kend - kbeg + QBK - 1) / QBK : 0;
-        }
-    };
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < P_NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 16); }       // 8 epilogue warps x 2 CTAs
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * P_TBN)));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();                                            // both CTAs' barriers exist before anything arrives remotely
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer (both CTAs)
-        if (lane == 0) {
-            int g = 0;
-            for (int tile = pair; tile < ntiles; tile += npairs) {
-                int m0, n0, z, kbeg, nkb;
-                tile_range(tile, m0, n0, z, kbeg, nkb);
-                const int nh = n0 + (int)rank * (P_TBN / 2);       // this CTA's half of the B tile
-                int seg = 0, kin = 0;
-                for (int kb = 0; kb < nkb; ++kb, ++g) {
-                    const int s = g % P_NST, it = g / P_NST;
-                    if (it > 0) mbar_wait_wd(&empty[s], (it - 1) & 1);
-                    int ka, kbcoord;
-                    if (MODE == EPI_WGRAD) { ka = kbeg + kb * QBK; kbcoord = ka; }
-                    else {
-                        if (kin >= segs.k[seg]) { ++seg; kin = 0; }
-                        ka = kin; kbcoord = segs.koff[seg] + kin;
-                        kin += QBK;
-                    }
-                    const uint32_t lbar = map_to_cta(smem_u32(&full[s]), 0);
-                    if (leader) mbar_expect_tx(&full[s], 2 * STAGE_BYTES);             // the bytes of both CTAs land on this barrier
-                    if (!A_MN) {
-                        tma_load_2d_pair(a_hi(s), &maps.a_hi[seg], lbar, ka, m0);
-                        tma_load_2d_pair(a_lo(s), &maps.a_lo[seg], lbar, ka, m0);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < QBM / 64; ++i) {
-                            tma_load_2d_pair(a_hi(s) + i * 8192, &maps.a_hi[seg], lbar, m0 + 64 * i, ka);
-                            tma_load_2d_pair(a_lo(s) + i * 8192, &maps.a_lo[seg], lbar, m0 + 64 * i, ka);
-                        }
-                    }
-                    if (!B_MN) {
-                        tma_load_2d_pair(b_hi(s), &maps.b_hi, lbar, kbcoord, nh);
-                        tma_load_2d_pair(b_lo(s), &maps.b_lo, lbar, kbcoord, nh);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < P_TBN / 128; ++i) {
-                            tma_load_2d_pair(b_hi(s) + i * 8192, &maps.b_hi, lbar, nh + 64 * i, kbcoord);
-                            tma_load_2d_pair(b_lo(s) + i * 8192, &maps.b_lo, lbar, nh + 64 * i, kbcoord);
+                        for (int hh = 0; hh < 2; ++hh) {
+                            const int r = r0 + 8 * hh;
+                            if (r >= M) continue;
+                            float2* pc = reinterpret_cast<float2*>(Cb + (int64_t)r * ep.ldc + c);
+                            float2 o = make_float2(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1]);
+                            if (MODE == EPI_STORE && ep.accumulate) { const float2 p = *pc; o.x += p.x; o.y += p.y; }
+                            *pc = o;
                         }
                     }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (leader CTA only)
-        if (leader) {
-            constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((A_MN ? 1u : 0u) << 15) | ((B_MN ? 1u : 0u) << 16) |
-                                       ((uint32_t)(P_TBN >> 3) << 17) | ((uint32_t)((2 * QBM) >> 4) << 24);
-            constexpr uint32_t a_step = A_MN ? 2048u : 32u, b_step = B_MN ? 2048u : 32u;
-            int g = 0, use = 0;
-            for (int tile = pair; tile < ntiles; tile += npairs) {
-                int m0, n0, z, kbeg, nkb;
-                tile_range(tile, m0, n0, z, kbeg, nkb);
-                if (nkb == 0) continue;
-                const int a = use & 1, au = use >> 1;
-                if (au > 0) mbar_wait_wd(&tmem_empty[a], (au - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t tacc = tmem_base + (uint32_t)(a * P_TBN);
-                for (int kb = 0; kb < nkb; ++kb, ++g) {
-                    const int s = g % P_NST, it = g / P_NST;
-                    mbar_wait_wd(&full[s], it & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    if (lane == 0) {
-                        const uint32_t sa_hi = smem_u32(a_hi(s)), sb_hi = smem_u32(b_hi(s));
-                        const uint32_t sa_lo = smem_u32(a_lo(s)), sb_lo = smem_u32(b_lo(s));
-#pragma unroll
-                        for (int k = 0; k < QBK / 16; ++k) {
-                            const uint64_t da_hi = A_MN ? make_desc_mn(sa_hi + k * a_step) : make_desc(sa_hi + k * a_step);
-                            const uint64_t da_lo = A_MN ? make_desc_mn(sa_lo + k * a_step) : make_desc(sa_lo + k * a_step);
-                            const uint64_t db_hi = B_MN ? make_desc_mn(sb_hi + k * b_step) : make_desc(sb_hi + k * b_step);
-                            const uint64_t db_lo = B_MN ? make_desc_mn(sb_lo + k * b_step) : make_desc(sb_lo + k * b_step);
-                            umma_bf16_pair(tacc, da_lo, db_hi, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                            umma_bf16_pair(tacc, da_hi, db_lo, idesc, 1u);
-                            umma_bf16_pair(tacc, da_hi, db_hi, idesc, 1u);
-                        }
-                        umma_commit_pair(&empty[s]);
-                        if (kb == nkb - 1) umma_commit_pair(&tmem_full[a]);
-                    }
-                    __syncwarp();
-                }
-                ++use;
-            }
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue: warps 2..9 of both CTAs (own TMEM half)
-        const int ew = warp - 2, q = warp & 3, half = ew >> 2;
-        const uint32_t stg_s = smem_u32(stage_out + ew * 2048);
-        int use = 0;
-        auto put64 = [&](const uint32_t* x) {
-            __syncwarp();
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-                sts128(stg_s + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4), x[4 * c], x[4 * c + 1], x[4 * c + 2], x[4 * c + 3]);
-            __syncwarp();
-        };
-        auto flush64 = [&](uint8_t* __restrict__ dst, int64_t ld_bytes, int mw, bool accumulate) {
-            // all four staged pieces (and, when accumulating, the four previous values) are fetched into DISTINCT registers before
-            // the first store: a store holds its source registers until the data has left for L1, so re-using one register quad per
-            // piece (what a load-store-load-store order compiles to) serialises the warp on that hand-off
-            const int c = lane & 3, r0 = lane >> 2;
-            uint4 v[4], p[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = i * 8 + r0;
-                v[i] = lds128(stg_s + r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
-            }
-            if (accumulate) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = i * 8 + r0;
-                    p[i] = *reinterpret_cast<const uint4*>(dst + (int64_t)min(r, M - 1 - mw < 0 ? 0 : M - 1 - mw) * ld_bytes + c * 16);
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    v[i].x = __float_as_uint(__uint_as_float(v[i].x) + __uint_as_float(p[i].x)); v[i].y = __float_as_uint(__uint_as_float(v[i].y) + __uint_as_float(p[i].y));
-                    v[i].z = __float_as_uint(__uint_as_float(v[i].z) + __uint_as_float(p[i].z)); v[i].w = __float_as_uint(__uint_as_float(v[i].w) + __uint_as_float(p[i].w));
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = i * 8 + r0;
-                if (mw + r < M) *reinterpret_cast<uint4*>(dst + (int64_t)r * ld_bytes + c * 16) = v[i];
-            }
-        };
-        auto store_f32 = [&](float* __restrict__ dst, int64_t ld, int mw, int nb, const uint32_t* x, bool accumulate) {
-            uint8_t* d = reinterpret_cast<uint8_t*>(dst + (int64_t)mw * ld + nb);
-            put64(x); flush64(d, ld * 4, mw, accumulate);
-            put64(x + 16); flush64(d + 64, ld * 4, mw, accumulate);
-        };
-        // the reverse path (EPI_DACT): rows [mw, mw + 32) x 64 bytes of a row-major matrix, fetched with whole-sector loads (8 rows x
-        // 64 B per instruction), staged, and handed out one row per lane
-        auto fetch64 = [&](const uint8_t* __restrict__ src, int64_t ld_bytes, int mw, uint4 (&r)[4]) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int rr = min(mw + i * 8 + (lane >> 2), M - 1);
-                r[i] = __ldg(reinterpret_cast<const uint4*>(src + (int64_t)(rr - mw) * ld_bytes + (lane & 3) * 16));
-            }
-        };
-        auto take64 = [&](const uint4 (&r)[4], float* x) {
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int rr = i * 8 + (lane >> 2), c = lane & 3;
-                sts128(stg_s + rr * 64 + ((c ^ ((rr >> 1) & 3)) << 4), r[i].x, r[i].y, r[i].z, r[i].w);
-            }
-            __syncwarp();
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const uint4 t = lds128(stg_s + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4));
-                x[4 * c] = __uint_as_float(t.x); x[4 * c + 1] = __uint_as_float(t.y); x[4 * c + 2] = __uint_as_float(t.z); x[4 * c + 3] = __uint_as_float(t.w);
-            }
-        };
-        const uint32_t lead_empty[2] = {map_to_cta(smem_u32(&tmem_empty[0]), 0), map_to_cta(smem_u32(&tmem_empty[1]), 0)};
-        for (int tile = pair; tile < ntiles; tile += npairs) {
-            int m0, n0, z, kbeg, nkb;
-            tile_range(tile, m0, n0, z, kbeg, nkb);
-            const int mw = m0 + q * 32;
-            const int m = mw + lane;
-            const int a = use & 1, au = use >> 1;
-            const int c_beg = half * (P_TBN / 64), c_end = c_beg + P_TBN / 64;
-            float pb = 0.f, pg = 1.f, pe = 0.f;
-            auto load_params = [&](int nbx, float& b_, float& g_, float& e_) {
-                const int gn = nbx + lane;
-                const bool in = gn < ep.n_logical;
-                b_ = (in && MODE == EPI_FWD) ? ep.bias[gn] : 0.f;
-                g_ = (in && ep.bn) ? ep.gamma[gn] * 0.99950037468777f : 1.f;
-                e_ = (in && ep.bn && MODE == EPI_FWD) ? ep.beta[gn] : 0.f;
-            };
-            if ((MODE == EPI_FWD || MODE == EPI_DACT) && n0 + c_beg * 32 < N) load_params(n0 + c_beg * 32, pb, pg, pe);
-            if (nkb > 0) {
-                mbar_wait_wd(&tmem_full[a], au & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            }
-#pragma unroll 1
-            for (int c = c_beg; c < c_end; ++c) {
-                const int nb = n0 + c * 32;
-                if (nb >= N) break;
-                float qb = 0.f, qg = 1.f, qe = 0.f;
-                if ((MODE == EPI_FWD || MODE == EPI_DACT) && c + 1 < c_end && nb + 32 < N) load_params(nb + 32, qb, qg, qe);
-                uint4 ar0[4], ar1[4];                                  // EPI_DACT: the fed layer's activations of this chunk, in flight
-                if (MODE == EPI_DACT) {
-                    const uint8_t* asrc = reinterpret_cast<const uint8_t*>(ep.Aact + (int64_t)mw * ep.ldh + nb);
-                    fetch64(asrc, (int64_t)ep.ldh * 4, mw, ar0);
-                    fetch64(asrc + 64, (int64_t)ep.ldh * 4, mw, ar1);
-                }
-                uint32_t v[32];
-                if (nkb > 0) tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * P_TBN + c * 32), v);
-                else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 0u;
-                }
-                if (MODE == EPI_FWD) {
-                    const uint32_t wp = smem_u32(epi_params + ew * 96);
-                    __syncwarp();
-                    sts32f(wp + 4 * lane, pb); sts32f(wp + 4 * (32 + lane), pg); sts32f(wp + 4 * (64 + lane), pe);
-                    pb = qb; pg = qg; pe = qe;
-                    __syncwarp();
-                    uint32_t h[32];
-                    const bool rv = m < ep.m_valid;
-                    if (ep.act == WD_ACT_RELU) {
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 b4 = lds128f(wp + 16 * j4);
-                            const float4 g4 = lds128f(wp + 128 + 16 * j4);
-                            const float4 e4 = lds128f(wp + 256 + 16 * j4);
-                            const float a0 = fmaxf(__uint_as_float(v[4 * j4]) + b4.x, 0.f), a1 = fmaxf(__uint_as_float(v[4 * j4 + 1]) + b4.y, 0.f);
-                            const float a2 = fmaxf(__uint_as_float(v[4 * j4 + 2]) + b4.z, 0.f), a3 = fmaxf(__uint_as_float(v[4 * j4 + 3]) + b4.w, 0.f);
-                            v[4 * j4] = __float_as_uint(a0); v[4 * j4 + 1] = __float_as_uint(a1); v[4 * j4 + 2] = __float_as_uint(a2); v[4 * j4 + 3] = __float_as_uint(a3);
-                            h[4 * j4] = __float_as_uint(fmaf(a0, g4.x, e4.x)); h[4 * j4 + 1] = __float_as_uint(fmaf(a1, g4.y, e4.y));
-                            h[4 * j4 + 2] = __float_as_uint(fmaf(a2, g4.z, e4.z)); h[4 * j4 + 3] = __float_as_uint(fmaf(a3, g4.w, e4.w));
-                        }
-                        if (nb + 32 > ep.n_logical) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) if (nb + j >= ep.n_logical) { v[j] = 0u; h[j] = 0u; }
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const bool ok = (nb + j) < ep.n_logical;
-                            const float av = ok ? act_fwd(ep.act, __uint_as_float(v[j]) + lds32f(wp + 4 * j)) : 0.f;
-                            v[j] = __float_as_uint(av);
-                            h[j] = __float_as_uint(ok ? fmaf(av, lds32f(wp + 4 * (32 + j)), lds32f(wp + 4 * (64 + j))) : 0.f);
-                        }
-                    }
-                    if (!rv) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) { v[j] = 0u; h[j] = 0u; }
-                    }
-                    if (ep.A_out != ep.H_out) store_f32(ep.A_out, ep.ldh, mw, nb, v, false);
-                    if (ep.H_out) store_f32(ep.H_out, ep.ldh, mw, nb, h, false);
-                    uint32_t hh[16], hl[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float x0 = __uint_as_float(h[2 * j]), x1 = __uint_as_float(h[2 * j + 1]);
-                        const __nv_bfloat162 hp = __floats2bfloat162_rn(x0, x1);
-                        const uint32_t hb = *reinterpret_cast<const uint32_t*>(&hp);
-                        const __nv_bfloat162 lp = __floats2bfloat162_rn(x0 - __uint_as_float(hb << 16), x1 - __uint_as_float(hb & 0xFFFF0000u));
-                        hh[j] = hb;
-                        hl[j] = *reinterpret_cast<const uint32_t*>(&lp);
-                    }
-                    uint8_t* dh = reinterpret_cast<uint8_t*>(ep.Hs_hi + (int64_t)mw * ep.ldh + nb);
-                    uint8_t* dl = reinterpret_cast<uint8_t*>(ep.Hs_lo + (int64_t)mw * ep.ldh + nb);
-                    put64(hh); flush64(dh, (int64_t)ep.ldh * 2, mw, false);
-                    put64(hl); flush64(dl, (int64_t)ep.ldh * 2, mw, false);
-                } else if (MODE == EPI_DACT) {
-                    // v = dH of the fed layer (row m, columns nb .. nb + 31); never stored
-                    const uint32_t wp = smem_u32(epi_params + ew * 96);
-                    __syncwarp();
-                    sts32f(wp + 4 * lane, pg);                        // gamma * 1/sqrt(1 + eps) of column nb + lane (1 without batch norm)
-                    pg = qg;
-                    __syncwarp();
-                    float gs[32];
-#pragma unroll
-                    for (int j4 = 0; j4 < 8; ++j4) {
-                        const float4 t = lds128f(wp + 16 * j4);
-                        gs[4 * j4] = t.x; gs[4 * j4 + 1] = t.y; gs[4 * j4 + 2] = t.z; gs[4 * j4 + 3] = t.w;
-                    }
-                    const bool rv = m < M;
-                    float av[32], dz[32];
-                    take64(ar0, av);
-                    take64(ar1, av + 16);
-                    const bool relu = ep.act == WD_ACT_RELU;
-                    float te[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const bool ok = rv && (nb + j) < ep.n_logical;
-                        const float dh = ok ? __uint_as_float(v[j]) : 0.f;
-                        const float aj = ok ? av[j] : 0.f;
-                        dz[j] = relu ? (aj > 0.f ? dh * gs[j] : 0.f) : dh * gs[j] * act_bwd(ep.act, aj);
-                        av[j] = dh * aj * 0.99950037468777f;           // gamma-gradient term
-                        te[j] = dh;                                   // beta-gradient term
-                    }
-                    // column sums over the warp's 32 rows (fixed butterfly order): lane j ends with the sum of column nb + j
-                    const uint32_t cs = smem_u32(colsum + ew * 384 + (c - c_beg) * 32 + lane);
-                    if (ep.bn) {
-                        sts32f(cs + 512, colsum32(av, lane));
-                        sts32f(cs + 1024, colsum32(te, lane));
-                    }
-                    {
-                        uint32_t hh[16], hl[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const float x0 = dz[2 * j], x1 = dz[2 * j + 1];
-                            const __nv_bfloat162 hp = __floats2bfloat162_rn(x0, x1);
-                            const uint32_t hb = *reinterpret_cast<const uint32_t*>(&hp);
-                            const __nv_bfloat162 lp = __floats2bfloat162_rn(x0 - __uint_as_float(hb << 16), x1 - __uint_as_float(hb & 0xFFFF0000u));
-                            hh[j] = hb;
-                            hl[j] = *reinterpret_cast<const uint32_t*>(&lp);
-                        }
-                        uint8_t* dh_ = reinterpret_cast<uint8_t*>(ep.Hs_hi + (int64_t)mw * ep.ldh + nb);
-                        uint8_t* dl_ = reinterpret_cast<uint8_t*>(ep.Hs_lo + (int64_t)mw * ep.ldh + nb);
-                        put64(hh); flush64(dh_, (int64_t)ep.ldh * 2, mw, false);
-                        put64(hl); flush64(dl_, (int64_t)ep.ldh * 2, mw, false);
-                    }
-                    sts32f(cs, colsum32(dz, lane));
-                } else {
-                    store_f32(ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0), ep.ldc, mw, nb, v, MODE == EPI_STORE && ep.accumulate);
-                }
-            }
-            if (nkb > 0) {
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(lead_empty[a]);          // this warp is done with accumulator buffer a (of its CTA)
-                ++use;
             }
             if (MODE == EPI_DACT) {
-                // 128-row partials of this CTA's row tile: the four lane quarters summed in quarter order, one column per thread
+                // 128-row partials of this row tile: the eight consumer warps summed in warp order, one column per thread
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int t = threadIdx.x - 64, hcol = t >> 7, col = t & 127;
-                const int n = n0 + hcol * 128 + col;
-                if (n < N && m0 < M) {
+                const int col = threadIdx.x - 128, n = n0 + col;
+                if (col < TBN && n < N) {
                     float sb = 0.f, sg = 0.f, se = 0.f;
 #pragma unroll
-                    for (int qq = 0; qq < 4; ++qq) {
-                        const uint32_t src = smem_u32(colsum + (hcol * 4 + ((qq + 2) & 3)) * 384 + col);   // warp 2 + 4 h + i serves quarter (i + 2) & 3
-                        sb += lds32f(src);
-                        if (ep.bn) { sg += lds32f(src + 512); se += lds32f(src + 1024); }
+                    for (int w = 0; w < 8; ++w) {
+                        sb += colsum[w * TBN + col];
+                        if (ep.bn) { sg += colsum[(8 + w) * TBN + col]; se += colsum[(16 + w) * TBN + col]; }
                     }
                     const int64_t o = (int64_t)(m0 / QBM) * ep.pstride + n;
                     ep.p_bias[o] = sb;
@@ -819,31 +291,10 @@ tc_gemm_bf16_pair_kernel(const __grid_constant__ QMaps maps, const QSegs segs, i
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
+            if (cwarp == 0) PROBE(use == 0 ? 4 : 5);
+            ++use;
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();                                            // the peer may still be reading this CTA's B half / signalling its barriers
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * P_TBN)));
-}
-
-template <int MODE>
-int launch_pair(WdModel* m, const QMaps& maps, const QSegs& segs, int M, int N, int ktot, int splits, int ksplit_len, const Epi& ep) {
-    constexpr int smem = P_NST * 2 * (QBM * 128 + (P_TBN / 2) * 128) + 16384 + 1024 + 128 + 3072 + (MODE == EPI_DACT ? 8 * 384 * 4 : 0);
-    static bool configured = false;
-    static int num_sms = 0;
-    if (!configured) {
-        WD_CUDA(cudaFuncSetAttribute(tc_gemm_bf16_pair_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        WD_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device));
-        configured = true;
-    }
-    const int nsplit = MODE == EPI_WGRAD ? splits : 1;
-    const int ntiles = ((N + P_TBN - 1) / P_TBN) * ((M + 2 * QBM - 1) / (2 * QBM)) * nsplit;
-    const int pairs = std::min(ntiles, num_sms / 2);
-    tc_gemm_bf16_pair_kernel<MODE><<<2 * pairs, Q_THREADS, smem, m->stream>>>(maps, segs, M, N, ktot, ksplit_len, nsplit, ep);
-    m->launches++;
-    WD_CUDA(cudaGetLastError());
-    return WD_OK;
 }
 
 int g_probe_slot = 0;
@@ -851,7 +302,7 @@ int g_probe_slot = 0;
 template <int TBN, int MODE>
 int launch_q(WdModel* m, const QMaps& maps, const QSegs& segs, int M, int N, int ktot, int splits, int ksplit_len, const Epi& ep) {
     constexpr int NST = TBN == 256 ? 2 : 3;
-    constexpr int smem = NST * 2 * (QBM * 128 + TBN * 128) + 16384 + 1024 + 128 + 3072;
+    constexpr int smem = NST * 2 * (QBM * 128 + TBN * 128) + 1024 + 128 + (MODE == EPI_DACT ? 3 * 8 * TBN * 4 : 0);
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {
@@ -879,30 +330,17 @@ extern "C" int wd_debug_gemm_probe(unsigned long long* out) {
     return e == cudaSuccess ? 0 : -1;
 }
 
-// whether the engine uses 128 x 256 output tiles for this problem (also consulted when the split-K factor is chosen)
-bool tc_bf16_wide_tile(int mode, int M, int N, int splits, int num_sms) {
-    static const bool no_wide = getenv("WD_TC_N128") != nullptr;
-    static const bool force_wide = getenv("WD_TC_FORCE_WIDE") != nullptr;       // tests: take the 128x256 / pair path whenever N allows
-    if (no_wide || N <= 128) return false;
-    if (force_wide) return true;
-    // rounds of the persistent grid x cost of one k-block (shared-memory bytes per k-block: 160 KB vs 240 KB, see DESIGN.md)
-    const int64_t tm = (M + QBM - 1) / QBM, sp = mode == EPI_WGRAD ? splits : 1;
-    const int64_t t128 = tm * ((N + 127) / 128) * sp, t256 = tm * ((N + 255) / 256) * sp;
-    const int64_t c128 = (t128 + num_sms - 1) / num_sms * 1250, c256 = (t256 + num_sms - 1) / num_sms * 1920;
-    return c256 < c128;
-}
-
-// whether this problem runs on the CTA-pair kernel (cta_group::2): WD_GEMM_2CTA=0 keeps the single-CTA kernel everywhere
-bool tc_bf16_uses_pair(int mode, int M, int N, int splits, int num_sms) {
-    static const bool pair_on = getenv("WD_GEMM_2CTA") ? atoi(getenv("WD_GEMM_2CTA")) != 0 : kPairDefault;
-    return pair_on && M >= 256 && tc_bf16_wide_tile(mode == EPI_DACT ? EPI_STORE : mode, M, N, splits, num_sms);
+// 128 x 128 output tiles: on the benchmark towers (H100 80GB HBM3, 700 W) the step ran at 8.75 M examples/s with them and at
+// 7.63 M with 128 x 256 tiles (BASELINE.md section 4).  The 256-wide instantiations are kept for WD_TC_FORCE_WIDE=1 only, which the tests set to run the
+// two-stage ring and the m64n256k16 MMA on small problems; nothing selects them otherwise.
+static bool wide_tile(int N) {
+    static const bool force_wide = getenv("WD_TC_FORCE_WIDE") != nullptr;
+    return force_wide && N > 128;
 }
 
 int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, int M, int N,
                  const Epi& ep, int splits, int ksplit_len) {
     if (N % 32 != 0 || A.n > kMaxSegs || !B_hi || !B_lo) { set_error("bf16 GEMM engine: unsupported operands"); return WD_EUNSUPPORTED; }
-    static int num_sms = 0;
-    if (!num_sms) cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device);
     QMaps maps;
     QSegs segs{};
     segs.n = A.n;
@@ -922,25 +360,22 @@ int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi
         ktot += A.k[s];
     }
     for (int s = A.n; s < kMaxSegs; ++s) { maps.a_hi[s] = maps.a_hi[0]; maps.a_lo[s] = maps.a_lo[0]; }
-    const bool wide = tc_bf16_wide_tile(mode, M, N, splits, num_sms);
-    const bool pair = tc_bf16_uses_pair(mode, M, N, splits, num_sms);
-    if (mode == EPI_DACT && !pair) { set_error("bf16 GEMM engine: the fused activation-backward epilogue exists only in the pair kernel"); return WD_EUNSUPPORTED; }
+    const bool wide = wide_tile(N);
     const int tbn = wide ? 256 : 128;
     if (!b_mn) {
-        if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, N, ktot, ldb, pair ? 128 : tbn))) return rc;      // a pair's CTA stages half of the tile's columns
-        if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, N, ktot, ldb, pair ? 128 : tbn))) return rc;
+        if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, N, ktot, ldb, tbn))) return rc;
+        if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, N, ktot, ldb, tbn))) return rc;
     } else {
         if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, ktot, N, ldb, 64))) return rc;
         if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, ktot, N, ldb, 64))) return rc;
     }
     if (mode == EPI_WGRAD) ksplit_len = (ksplit_len + QBK - 1) / QBK * QBK;
-    if (mode == EPI_FWD && (!ep.Hs_hi || !ep.Hs_lo)) { set_error("bf16 GEMM engine: forward without hi/lo outputs"); return WD_EINVAL; }
+    if ((mode == EPI_FWD || mode == EPI_DACT) && (!ep.Hs_hi || !ep.Hs_lo)) { set_error("bf16 GEMM engine: epilogue without hi/lo outputs"); return WD_EINVAL; }
 #define WD_Q_LAUNCH(MODE_) \
-    if (pair) return launch_pair<MODE_>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep); \
     return wide ? launch_q<256, MODE_>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep) : launch_q<128, MODE_>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep)
     if (mode == EPI_FWD) { WD_Q_LAUNCH(EPI_FWD); }
     if (mode == EPI_STORE) { WD_Q_LAUNCH(EPI_STORE); }
-    if (mode == EPI_DACT) return launch_pair<EPI_DACT>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep);
+    if (mode == EPI_DACT) { WD_Q_LAUNCH(EPI_DACT); }
     WD_Q_LAUNCH(EPI_WGRAD);
 #undef WD_Q_LAUNCH
 }

@@ -1,23 +1,24 @@
-// tcgen05 (5th-generation tensor core) engine for the MLP GEMMs on sm_100a.
+// wgmma (Hopper warp-group tensor core) engine for the MLP GEMMs on sm_90a.
 //
-//   C[M,N] = sum_k A[M,k] * B[N,k]     fp32 operands, both K-contiguous ("TN"), fp32 accumulate in TMEM
+//   C[M,N] = sum_k A[M,k] * B[N,k]     fp32 operands, both K-contiguous ("TN"), fp32 accumulate in registers
 //
 // fp32-faithful products on the tf32 pipe (3xTF32): every operand tile is split in shared memory into
 //   hi = x with the low 13 mantissa bits cleared (exactly representable in tf32)     lo = x - hi (exact)
-// and three UMMAs accumulate  a_lo*b_hi + a_hi*b_lo + a_hi*b_hi  into the same TMEM accumulator; the dropped
+// and three MMAs accumulate  a_lo*b_hi + a_hi*b_lo + a_hi*b_hi  into the same accumulator; the dropped
 // a_lo*b_lo term is below 2^-22 relative, i.e. at fp32 rounding level, which is what the 1e-4 logit parity bar
-// (BASELINE.json) needs and what a single tf32 pass (2^-11, measured ~1e-3 on the logits) cannot give.
+// (BASELINE.json) needs and what a single tf32 pass (2^-11) cannot give.
 //
-// Structure of one CTA (one 128 x TBN output tile, K loop over 32-float = 128-byte blocks):
-//   warp 0      TMA producer: cp.async.bulk.tensor.2d of the raw fp32 A / B blocks (128B-swizzled) into the
-//               "hi" buffers of a 3-stage ring, completion on mbarrier full[s]
-//   warps 2-5   splitters: wait full[s], rewrite the block in place as hi and write lo beside it (element-wise,
+// One persistent CTA per SM loops over 128 x TBN output tiles, K loop over 32-float = 128-byte blocks.  Four warp groups:
+//   group 0     TMA producer (one elected thread): cp.async.bulk.tensor.2d of the raw fp32 A / B blocks (128B-swizzled)
+//               into the "hi" buffers of a stage ring, completion on mbarrier full[s]
+//   group 1     splitters: wait full[s], rewrite the block in place as hi and write lo beside it (element-wise,
 //               so the swizzle never has to be decoded), fence.proxy.async, arrive split[s]
-//   warp 1      MMA issuer (one elected lane): wait split[s], 4 k-steps x 3 tcgen05.mma.kind::tf32 (UMMA 128xTBNx8),
-//               tcgen05.commit -> empty[s] (frees the stage), last block also -> accum_full
-//   warps 2-5   epilogue: tcgen05.ld 32x32b of the accumulator, fused bias + activation + BN-affine (+ transposed
-//               copy) or plain / accumulating / split-K store
-// Inputs that run past M, N or K are zero-filled by TMA (tensor maps carry the true extents).
+//   groups 2-3  consumers, 64 tile rows each: wait split[s], 4 k-steps x 3 wgmma.mma_async m64nTBNk8 tf32, release the stage
+//               on empty[s] once that batch has retired; then the epilogue straight from the accumulator fragment: fused
+//               bias + activation + BN-affine (+ transposed copy) or plain / accumulating / split-K store
+// The producer and the splitters hand registers to the consumers (setmaxnreg) and run ahead into the next tile while the
+// consumers store the current one.  Inputs that run past M, N or K are zero-filled by TMA (tensor maps carry the true
+// extents).
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -26,14 +27,14 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
-#include "tc_ptx.cuh"
+#include "wgmma_ptx.cuh"
 
 namespace wd {
 
-constexpr int TBM = 128;        // UMMA M
+constexpr int TBM = 128;        // tile rows: two consumer warp groups x wgmma M = 64
 constexpr int TBK = 32;         // floats per k-block = one 128-byte swizzle row
 constexpr int TSTAGES = 3;
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 512;
 
 struct TcMaps {
     CUtensorMap a[kMaxSegs];
@@ -42,209 +43,23 @@ struct TcMaps {
 };
 
 // ---------------------------------------------------------------------------------------------- kernel
-template <int TBN, int MODE, bool SPLIT3>
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_kernel(const __grid_constant__ TcMaps maps, int nseg, int4 segk01, int4 segk23,
-                                                               int M, int N, int ktot, int ksplit_len, Epi ep) {
-    extern __shared__ uint8_t smem_raw[];
-    // carve: 1024-byte aligned operand ring, then barriers
-    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    constexpr int A_BYTES = TBM * 128, B_BYTES = TBN * 128;
-    constexpr int STAGE_BYTES = (SPLIT3 ? 2 : 1) * (A_BYTES + B_BYTES);
-    uint8_t* a_hi[TSTAGES]; uint8_t* a_lo[TSTAGES]; uint8_t* b_hi[TSTAGES]; uint8_t* b_lo[TSTAGES];
-#pragma unroll
-    for (int s = 0; s < TSTAGES; ++s) {
-        uint8_t* st = base + s * STAGE_BYTES;
-        a_hi[s] = st; b_hi[s] = st + A_BYTES;
-        a_lo[s] = st + A_BYTES + B_BYTES; b_lo[s] = a_lo[s] + A_BYTES;
-    }
-    uint64_t* bars = reinterpret_cast<uint64_t*>(base + TSTAGES * STAGE_BYTES);
-    uint64_t* full = bars; uint64_t* split = bars + TSTAGES; uint64_t* empty = bars + 2 * TSTAGES; uint64_t* accum_full = bars + 3 * TSTAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * TSTAGES + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.y * TBM, n0 = blockIdx.x * TBN;
-    int kbeg = 0, kend = ktot;
-    if (MODE == EPI_WGRAD) { kbeg = blockIdx.z * ksplit_len; kend = min(ktot, kbeg + ksplit_len); }
-    const int nkb = kend > kbeg ? (kend - kbeg + TBK - 1) / TBK : 0;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < TSTAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 1); }
-        mbar_init(accum_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {        // TMEM allocation: TBN fp32 accumulator columns (power of two >= 32)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)TBN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
-            const int segk[kMaxSegs] = {segk01.x, segk01.y, segk01.z, segk01.w, segk23.x, segk23.y, segk23.z, segk23.w};
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % TSTAGES, it = kb / TSTAGES;
-                if (it > 0) mbar_wait(&empty[s], (it - 1) & 1);
-                int kg = kbeg + kb * TBK;
-                int seg = 0, kk = kg;
-                while (seg < nseg - 1 && kk >= segk[seg]) { kk -= segk[seg]; ++seg; }
-                mbar_expect_tx(&full[s], A_BYTES + B_BYTES);
-                tma_load_2d(a_hi[s], &maps.a[seg], &full[s], kk, m0);
-                tma_load_2d(b_hi[s], &maps.b, &full[s], kg, n0);
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int s = kb % TSTAGES, it = kb / TSTAGES;
-            mbar_wait(SPLIT3 ? &split[s] : &full[s], it & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (lane == 0) {
-                const uint32_t sa_hi = smem_u32(a_hi[s]), sb_hi = smem_u32(b_hi[s]);
-                const uint32_t sa_lo = smem_u32(a_lo[s]), sb_lo = smem_u32(b_lo[s]);
-#pragma unroll
-                for (int k = 0; k < TBK / 8; ++k) {
-                    const uint32_t off = k * 32;          // 8 tf32 = 32 bytes inside the 128-byte swizzle row
-                    uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
-                    if (SPLIT3) {
-                        umma_tf32(tmem_base, make_desc(sa_lo + off), make_desc(sb_hi + off), idesc, acc);
-                        umma_tf32(tmem_base, make_desc(sa_hi + off), make_desc(sb_lo + off), idesc, 1u);
-                        umma_tf32(tmem_base, make_desc(sa_hi + off), make_desc(sb_hi + off), idesc, 1u);
-                    } else {
-                        umma_tf32(tmem_base, make_desc(sa_hi + off), make_desc(sb_hi + off), idesc, acc);
-                    }
-                }
-                umma_commit(&empty[s]);
-                if (kb == nkb - 1) umma_commit(accum_full);
-            }
-            __syncwarp();
-        }
-    } else {
-        // ------------------------------------------------------------------ splitters, then epilogue
-        const int t = threadIdx.x - 64;                     // 0..127
-        if (SPLIT3) {
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % TSTAGES, it = kb / TSTAGES;
-                mbar_wait(&full[s], it & 1);
-                float4* ah = reinterpret_cast<float4*>(a_hi[s]); float4* al = reinterpret_cast<float4*>(a_lo[s]);
-                float4* bh = reinterpret_cast<float4*>(b_hi[s]); float4* bl = reinterpret_cast<float4*>(b_lo[s]);
-                auto split4 = [](float4 x, float4& hi, float4& lo) {
-                    hi.x = __uint_as_float(__float_as_uint(x.x) & 0xFFFFE000u); lo.x = x.x - hi.x;
-                    hi.y = __uint_as_float(__float_as_uint(x.y) & 0xFFFFE000u); lo.y = x.y - hi.y;
-                    hi.z = __uint_as_float(__float_as_uint(x.z) & 0xFFFFE000u); lo.z = x.z - hi.z;
-                    hi.w = __uint_as_float(__float_as_uint(x.w) & 0xFFFFE000u); lo.w = x.w - hi.w;
-                };
-#pragma unroll
-                for (int i = 0; i < A_BYTES / 16 / 128; ++i) {
-                    float4 x = ah[t + i * 128], hi, lo;
-                    split4(x, hi, lo);
-                    ah[t + i * 128] = hi; al[t + i * 128] = lo;
-                }
-#pragma unroll
-                for (int i = 0; i < B_BYTES / 16 / 128; ++i) {
-                    float4 x = bh[t + i * 128], hi, lo;
-                    split4(x, hi, lo);
-                    bh[t + i * 128] = hi; bl[t + i * 128] = lo;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to UMMA
-                mbar_arrive(&split[s]);
-            }
-        }
-        // ---- epilogue: this warp reads TMEM lanes [32*(warp%4), +32)
-        const int q = warp & 3;
-        const int m = m0 + q * 32 + lane;
-        if (nkb > 0) {
-            mbar_wait(accum_full, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-#pragma unroll 1
-        for (int c = 0; c < TBN / 32; ++c) {
-            const int nb = n0 + c * 32;
-            if (nb >= N) break;
-            uint32_t v[32];
-            if (nkb > 0) tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-            else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = 0u;
-            }
-            if (MODE == EPI_FWD) {
-                float h[32];
-                const bool rv = m < ep.m_valid;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int gn = nb + j;
-                    float a = 0.f, hh = 0.f;
-                    if (rv && gn < ep.n_logical) {
-                        a = act_fwd(ep.act, __uint_as_float(v[j]) + ep.bias[gn]);
-                        hh = ep.bn ? a * (ep.gamma[gn] * 0.99950037468777f) + ep.beta[gn] : a;
-                    }
-                    v[j] = __float_as_uint(a);
-                    h[j] = hh;
-                }
-                if (m < M) {
-                    if (ep.A_out != ep.H_out) {
-                        float4* pa = reinterpret_cast<float4*>(ep.A_out + (int64_t)m * ep.ldh + nb);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) pa[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                    }
-                    float4* ph = reinterpret_cast<float4*>(ep.H_out + (int64_t)m * ep.ldh + nb);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) ph[j] = make_float4(h[4 * j], h[4 * j + 1], h[4 * j + 2], h[4 * j + 3]);
-                }
-                if (ep.HT) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) ep.HT[(int64_t)(nb + j) * ep.ldt + m] = h[j];   // lanes = consecutive m: coalesced
-                }
-            } else {
-                if (m < M) {
-                    float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)blockIdx.z * ep.split_stride : 0);
-                    float4* pc = reinterpret_cast<float4*>(Cb + (int64_t)m * ep.ldc + nb);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                        if (MODE == EPI_STORE && ep.accumulate) { float4 p = pc[j]; o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w; }
-                        pc[j] = o;
-                    }
-                }
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TBN));
-}
-
-// ------------------------------------------------------------------------------------- persistent kernel (v2)
-// One CTA per SM loops over output tiles.  Ten warps: 0 TMA producer, 1 MMA issuer, 2-5 splitters, 6-9 epilogue.
-// The TMEM accumulator is double buffered (2 x TBN columns): the MMA warp fills buffer a^1 for the next tile
-// while the epilogue warps drain buffer a, so tensor-core work is no longer serialised with the epilogue's global
-// stores (and barrier init / TMEM allocation / tensor-map fetch are paid once per SM instead of once per tile).
-constexpr int TC2_THREADS = 320;
-
 // BPRE: the B operand (weights) arrives already split into hi / lo copies (two tensor maps), only A is split here.
 template <int TBN, int MODE, bool SPLIT3, bool BPRE>
-__global__ void __launch_bounds__(TC2_THREADS, 1) tc_gemm_kernel_v2(const __grid_constant__ TcMaps maps, int nseg, int4 segk01, int4 segk23,
-                                                                   int M, int N, int ktot, int ksplit_len, int nsplit, Epi ep) {
+__global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_kernel(const __grid_constant__ TcMaps maps, int nseg, int4 segk01, int4 segk23,
+                                                               int M, int N, int ktot, int ksplit_len, int nsplit, Epi ep) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int A_BYTES = TBM * 128, B_BYTES = TBN * 128;
     constexpr int STAGE_BYTES = (SPLIT3 ? 2 : 1) * (A_BYTES + B_BYTES);
-    constexpr int NST = (SPLIT3 && TBN == 256) ? 2 : TSTAGES;       // 96 KB stages: two fit in shared memory
+    constexpr int NST = TSTAGES;
     auto a_hi = [&](int s) { return base + s * STAGE_BYTES; };
     auto b_hi = [&](int s) { return base + s * STAGE_BYTES + A_BYTES; };
     auto a_lo = [&](int s) { return base + s * STAGE_BYTES + A_BYTES + B_BYTES; };
     auto b_lo = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES + B_BYTES; };
     uint64_t* bars = reinterpret_cast<uint64_t*>(base + NST * STAGE_BYTES);
     uint64_t* full = bars; uint64_t* split = bars + NST; uint64_t* empty = bars + 2 * NST;
-    uint64_t* tmem_full = bars + 3 * NST; uint64_t* tmem_empty = bars + 3 * NST + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * NST + 4);
-    float* epi_params = reinterpret_cast<float*>(bars + 16);      // [4 epilogue warps][bias | scale | shift][32]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
     const int ntiles = tiles_n * tiles_m * nsplit;
     auto tile_range = [&](int tile, int& m0, int& n0, int& z, int& kbeg, int& nkb) {
@@ -259,22 +74,15 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) tc_gemm_kernel_v2(const __grid
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 128); }
+        for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 8); }   // empty: one arrival per consumer warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * TBN)));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
+        reg_dealloc<40>();
+        if (warp == 0 && lane == 0) {
             const int segk[kMaxSegs] = {segk01.x, segk01.y, segk01.z, segk01.w, segk23.x, segk23.y, segk23.z, segk23.w};
             int g = 0;
             for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -293,48 +101,11 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) tc_gemm_kernel_v2(const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-        int g = 0, use = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            int m0, n0, z, kbeg, nkb;
-            tile_range(tile, m0, n0, z, kbeg, nkb);
-            if (nkb == 0) continue;
-            const int a = use & 1, au = use >> 1;              // accumulator buffer, how often it was used before
-            if (au > 0) mbar_wait(&tmem_empty[a], (au - 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tacc = tmem_base + (uint32_t)(a * TBN);
-            for (int kb = 0; kb < nkb; ++kb, ++g) {
-                const int s = g % NST, it = g / NST;
-                mbar_wait(SPLIT3 ? &split[s] : &full[s], it & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) {
-                    const uint32_t sa_hi = smem_u32(a_hi(s)), sb_hi = smem_u32(b_hi(s));
-                    const uint32_t sa_lo = smem_u32(a_lo(s)), sb_lo = smem_u32(b_lo(s));
-#pragma unroll
-                    for (int k = 0; k < TBK / 8; ++k) {
-                        const uint32_t off = k * 32;
-                        uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
-                        if (SPLIT3) {
-                            umma_tf32(tacc, make_desc(sa_lo + off), make_desc(sb_hi + off), idesc, acc);
-                            umma_tf32(tacc, make_desc(sa_hi + off), make_desc(sb_lo + off), idesc, 1u);
-                            umma_tf32(tacc, make_desc(sa_hi + off), make_desc(sb_hi + off), idesc, 1u);
-                        } else {
-                            umma_tf32(tacc, make_desc(sa_hi + off), make_desc(sb_hi + off), idesc, acc);
-                        }
-                    }
-                    umma_commit(&empty[s]);
-                    if (kb == nkb - 1) umma_commit(&tmem_full[a]);
-                }
-                __syncwarp();
-            }
-            ++use;
-        }
-    } else if (warp < 6) {
+    } else if (wg == 1) {
         // ------------------------------------------------------------------ splitters
+        reg_dealloc<72>();
         if (SPLIT3) {
-            const int t = threadIdx.x - 64;                     // 0..127
+            const int t = threadIdx.x - 128;                    // 0..127
             int g = 0;
             for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
                 int m0, n0, z, kbeg, nkb;
@@ -364,110 +135,98 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) tc_gemm_kernel_v2(const __grid
                             bh[t + i * 128] = hi; bl[t + i * 128] = lo;
                         }
                     }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
                     mbar_arrive(&split[s]);
                 }
             }
         }
     } else {
-        // ------------------------------------------------------------------ epilogue (warps 6..9 -> TMEM lane quarters 2,3,0,1)
-        const int q = warp & 3;
-        int use = 0;
+        // ------------------------------------------------------------------ consumers: warp group cw owns rows [64 cw, 64 cw + 64)
+        reg_alloc<200>();
+        const int cw = wg - 2;
+        float d[TBN / 2];
+        int g = 0;
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             int m0, n0, z, kbeg, nkb;
             tile_range(tile, m0, n0, z, kbeg, nkb);
-            const int m = m0 + q * 32 + lane;
-            const int a = use & 1, au = use >> 1;
-            if (nkb > 0) {
-                mbar_wait(&tmem_full[a], au & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            if (nkb == 0) {
+#pragma unroll
+                for (int i = 0; i < TBN / 2; ++i) d[i] = 0.f;
             }
-#pragma unroll 1
-            for (int c = 0; c < TBN / 32; ++c) {
-                const int nb = n0 + c * 32;
-                if (nb >= N) break;
-                uint32_t v[32];
-                if (nkb > 0) tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * TBN + c * 32), v);
-                else {
+            int prev = -1;
+            for (int kb = 0; kb < nkb; ++kb, ++g) {
+                const int s = g % NST, it = g / NST;
+                mbar_wait(SPLIT3 ? &split[s] : &full[s], it & 1);
+                const uint32_t sa_hi = smem_u32(a_hi(s)) + cw * 8192, sa_lo = smem_u32(a_lo(s)) + cw * 8192;   // 64 rows x 128 B per group
+                const uint32_t sb_hi = smem_u32(b_hi(s)), sb_lo = smem_u32(b_lo(s));
+                wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 0u;
-                }
-                if (MODE == EPI_FWD) {
-                    // stage this chunk's bias / BN scale / BN shift once per warp (coalesced), read back as smem broadcasts
-                    float* wp = epi_params + (warp - 6) * 96;
-                    {
-                        const int gn = nb + lane;
-                        const bool in = gn < ep.n_logical;
-                        wp[lane] = in ? ep.bias[gn] : 0.f;
-                        wp[32 + lane] = (in && ep.bn) ? ep.gamma[gn] * 0.99950037468777f : 1.f;
-                        wp[64 + lane] = (in && ep.bn) ? ep.beta[gn] : 0.f;
-                    }
-                    __syncwarp();
-                    float h[32];
-                    const bool rv = m < ep.m_valid;
-                    if (ep.act == WD_ACT_RELU) {                      // warp-uniform fast path
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 bb = *reinterpret_cast<const float4*>(wp + 4 * j4);
-                            const float4 gg = *reinterpret_cast<const float4*>(wp + 32 + 4 * j4);
-                            const float4 be = *reinterpret_cast<const float4*>(wp + 64 + 4 * j4);
-                            const float b4[4] = {bb.x, bb.y, bb.z, bb.w}, g4[4] = {gg.x, gg.y, gg.z, gg.w}, e4[4] = {be.x, be.y, be.z, be.w};
-#pragma unroll
-                            for (int jj = 0; jj < 4; ++jj) {
-                                const int j = 4 * j4 + jj;
-                                const bool ok = rv && (nb + j) < ep.n_logical;
-                                const float av = ok ? fmaxf(__uint_as_float(v[j]) + b4[jj], 0.f) : 0.f;
-                                v[j] = __float_as_uint(av);
-                                h[j] = ok ? fmaf(av, g4[jj], e4[jj]) : 0.f;
-                            }
-                        }
+                for (int k = 0; k < TBK / 8; ++k) {
+                    const uint32_t off = k * 32;          // 8 tf32 = 32 bytes inside the 128-byte swizzle row
+                    const uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
+                    if (SPLIT3) {
+                        wgmma_tf32(d, make_desc(sa_lo + off), make_desc(sb_hi + off), acc);
+                        wgmma_tf32(d, make_desc(sa_hi + off), make_desc(sb_lo + off), 1u);
+                        wgmma_tf32(d, make_desc(sa_hi + off), make_desc(sb_hi + off), 1u);
                     } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const bool ok = rv && (nb + j) < ep.n_logical;
-                            const float av = ok ? act_fwd(ep.act, __uint_as_float(v[j]) + wp[j]) : 0.f;
-                            v[j] = __float_as_uint(av);
-                            h[j] = ok ? fmaf(av, wp[32 + j], wp[64 + j]) : 0.f;
-                        }
+                        wgmma_tf32(d, make_desc(sa_hi + off), make_desc(sb_hi + off), acc);
                     }
-                    __syncwarp();
-                    if (m < M) {
-                        if (ep.A_out != ep.H_out) {
-                            float4* pa = reinterpret_cast<float4*>(ep.A_out + (int64_t)m * ep.ldh + nb);
+                }
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();                              // the batch that read stage `prev` has retired
+                    if (lane == 0) mbar_arrive(&empty[prev]);
+                }
+                prev = s;
+            }
+            wgmma_wait<0>();                                      // the accumulator is final
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+            // ---- epilogue from the accumulator fragment: rows r0 and r0 + 8, columns n0 + 8 j + 2 (lane % 4) + {0, 1}
+            const int r0 = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+            const int cq = 2 * (lane & 3);
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) pa[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
+            for (int j = 0; j < TBN / 8; ++j) {
+                const int c = n0 + 8 * j + cq;
+                if (n0 + 8 * j >= N) continue;
+                if (MODE == EPI_FWD) {
+                    const bool in0 = c < ep.n_logical, in1 = c + 1 < ep.n_logical;
+                    const float b0 = in0 ? __ldg(ep.bias + c) : 0.f, b1 = in1 ? __ldg(ep.bias + c + 1) : 0.f;
+                    const float g0 = (in0 && ep.bn) ? __ldg(ep.gamma + c) * 0.99950037468777f : 1.f;
+                    const float g1 = (in1 && ep.bn) ? __ldg(ep.gamma + c + 1) * 0.99950037468777f : 1.f;
+                    const float e0 = (in0 && ep.bn) ? __ldg(ep.beta + c) : 0.f, e1 = (in1 && ep.bn) ? __ldg(ep.beta + c + 1) : 0.f;
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const int r = r0 + 8 * hh;
+                        const bool rv = r < ep.m_valid;              // rows >= m_valid are written as zero (transposed padding)
+                        float a0 = 0.f, a1 = 0.f, h0 = 0.f, h1 = 0.f;
+                        if (rv && in0) { a0 = ep.act == WD_ACT_RELU ? fmaxf(d[4 * j + 2 * hh] + b0, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh] + b0); h0 = fmaf(a0, g0, e0); }
+                        if (rv && in1) { a1 = ep.act == WD_ACT_RELU ? fmaxf(d[4 * j + 2 * hh + 1] + b1, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh + 1] + b1); h1 = fmaf(a1, g1, e1); }
+                        if (r < M) {
+                            const int64_t o = (int64_t)r * ep.ldh + c;
+                            if (ep.A_out != ep.H_out) *reinterpret_cast<float2*>(ep.A_out + o) = make_float2(a0, a1);
+                            *reinterpret_cast<float2*>(ep.H_out + o) = make_float2(h0, h1);
                         }
-                        float4* ph = reinterpret_cast<float4*>(ep.H_out + (int64_t)m * ep.ldh + nb);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) ph[j] = make_float4(h[4 * j], h[4 * j + 1], h[4 * j + 2], h[4 * j + 3]);
-                    }
-                    if (ep.HT) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) ep.HT[(int64_t)(nb + j) * ep.ldt + m] = h[j];
+                        if (ep.HT) {                                 // 8 lanes = 8 consecutive m: whole 32-byte sectors
+                            ep.HT[(int64_t)c * ep.ldt + r] = h0;
+                            ep.HT[(int64_t)(c + 1) * ep.ldt + r] = h1;
+                        }
                     }
                 } else {
-                    if (m < M) {
-                        float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0);
-                        float4* pc = reinterpret_cast<float4*>(Cb + (int64_t)m * ep.ldc + nb);
+                    float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0);
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                            if (MODE == EPI_STORE && ep.accumulate) { float4 p = pc[j]; o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w; }
-                            pc[j] = o;
-                        }
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const int r = r0 + 8 * hh;
+                        if (r >= M) continue;
+                        float2* pc = reinterpret_cast<float2*>(Cb + (int64_t)r * ep.ldc + c);
+                        float2 o = make_float2(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1]);
+                        if (MODE == EPI_STORE && ep.accumulate) { const float2 p = *pc; o.x += p.x; o.y += p.y; }
+                        *pc = o;
                     }
                 }
-            }
-            if (nkb > 0) {
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(&tmem_empty[a]);                   // accumulator buffer a may be overwritten
-                ++use;
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * TBN)));
 }
 
 // ---------------------------------------------------------------------------------------------- host
@@ -558,36 +317,21 @@ int tc_make_map_bf16(CUtensorMap* map, const void* ptr, int rows, int cols, int 
 template <int TBN, int MODE, bool SPLIT3, bool BPRE>
 static int launch_tc(WdModel* m, const TcMaps& maps, int nseg, const int* segk, int M, int N, int ktot, int splits, int ksplit_len, const Epi& ep) {
     constexpr int A_BYTES = TBM * 128, B_BYTES = TBN * 128;
-    constexpr int NST = (SPLIT3 && TBN == 256) ? 2 : TSTAGES;
-    constexpr int smem = NST * (SPLIT3 ? 2 : 1) * (A_BYTES + B_BYTES) + 1024 + 256 + 1536;
-    dim3 grid((N + TBN - 1) / TBN, (M + TBM - 1) / TBM, MODE == EPI_WGRAD ? splits : 1);
+    constexpr int NST = TSTAGES;
+    constexpr int smem = NST * (SPLIT3 ? 2 : 1) * (A_BYTES + B_BYTES) + 1024 + 128;
     int4 s01 = make_int4(segk[0], segk[1], segk[2], segk[3]), s23 = make_int4(segk[4], segk[5], segk[6], segk[7]);
-    static const bool use_v1 = getenv("WD_TC_V1") != nullptr;
-    if (!use_v1 || BPRE || TBN != 128) {
-        static bool configured2 = false;
-        static int num_sms = 0;
-        if (!configured2) {
-            WD_CUDA(cudaFuncSetAttribute(tc_gemm_kernel_v2<TBN, MODE, SPLIT3, BPRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            WD_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device));
-            configured2 = true;
-        }
-        const int nsplit = MODE == EPI_WGRAD ? splits : 1;
-        const int ntiles = (int)(grid.x * grid.y) * nsplit;
-        tc_gemm_kernel_v2<TBN, MODE, SPLIT3, BPRE><<<ntiles < num_sms ? ntiles : num_sms, TC2_THREADS, smem, m->stream>>>(maps, nseg, s01, s23, M, N, ktot, ksplit_len, nsplit, ep);
-        m->launches++;
-        WD_CUDA(cudaGetLastError());
-        return WD_OK;
+    static bool configured = false;
+    static int num_sms = 0;
+    if (!configured) {
+        WD_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TBN, MODE, SPLIT3, BPRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        WD_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device));
+        configured = true;
     }
-    if constexpr (!BPRE && TBN == 128) {
-        static bool configured = false;
-        if (!configured) {
-            WD_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TBN, MODE, SPLIT3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            configured = true;
-        }
-        tc_gemm_kernel<TBN, MODE, SPLIT3><<<grid, TC_THREADS, smem, m->stream>>>(maps, nseg, s01, s23, M, N, ktot, ksplit_len, ep);
-        m->launches++;
-        WD_CUDA(cudaGetLastError());
-    }
+    const int nsplit = MODE == EPI_WGRAD ? splits : 1;
+    const int ntiles = ((N + TBN - 1) / TBN) * ((M + TBM - 1) / TBM) * nsplit;
+    tc_gemm_kernel<TBN, MODE, SPLIT3, BPRE><<<ntiles < num_sms ? ntiles : num_sms, TC_THREADS, smem, m->stream>>>(maps, nseg, s01, s23, M, N, ktot, ksplit_len, nsplit, ep);
+    m->launches++;
+    WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 
@@ -608,14 +352,9 @@ int tc_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M
     for (int s = A.n; s < kMaxSegs; ++s) maps.a[s] = maps.a[0];
     const bool split3 = m->gemm_engine == WD_GEMM_TC3X;
     const bool bpre = split3 && B_hi && B_lo && mode != EPI_WGRAD;
-    static const bool no_wide = getenv("WD_TC_N128") != nullptr;
-    static int num_sms_h = 0;
-    if (!num_sms_h) cudaDeviceGetAttribute(&num_sms_h, cudaDevAttrMultiProcessorCount, m->device);
-    // 128x256 tiles (less shared-memory traffic per flop) when the weights are pre-split and the grid still fills the SMs
-    const bool wide = bpre && (N % 256 == 0) && !no_wide && ((int64_t)((M + TBM - 1) / TBM) * (N / 256) >= num_sms_h);
-    const int tbn = wide ? 256 : 128;
-    if ((rc = make_map(&maps.b, bpre ? B_hi : B, N, ktot, ldb, tbn))) return rc;
-    if (bpre) { if ((rc = make_map(&maps.b_lo, B_lo, N, ktot, ldb, tbn))) return rc; }
+    // 128 x 128 tiles only: 64 accumulator registers per consumer thread is what four warp groups leave room for
+    if ((rc = make_map(&maps.b, bpre ? B_hi : B, N, ktot, ldb, 128))) return rc;
+    if (bpre) { if ((rc = make_map(&maps.b_lo, B_lo, N, ktot, ldb, 128))) return rc; }
     else maps.b_lo = maps.b;
     if (mode == EPI_WGRAD) ksplit_len = (ksplit_len + TBK - 1) / TBK * TBK;
     if (mode == EPI_WGRAD)
@@ -624,7 +363,6 @@ int tc_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M
 #define WD_TC_LAUNCH(MODE_)                                                                                                     \
     if (!split3) return launch_tc<128, MODE_, false, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep);             \
     if (!bpre) return launch_tc<128, MODE_, true, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep);                \
-    if (wide) return launch_tc<256, MODE_, true, true>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep);                  \
     return launch_tc<128, MODE_, true, true>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep)
     if (mode == EPI_FWD) { WD_TC_LAUNCH(EPI_FWD); }
     WD_TC_LAUNCH(EPI_STORE);

@@ -56,18 +56,18 @@ int init_sparse_tables(WdModel* m, uint64_t seed, int random_w) {
     for (size_t t = 0; t < m->tables.size(); ++t) {
         auto& tb = m->tables[t];
         // (a shard draws from its own stream: rank r of a sharded table uses seed + 7919 * r)
-        emb_init_kernel<<<grid_for(tb.arows * tb.stride, 256, 148 * 32), 256, 0, m->stream>>>(tb.data, tb.arows, tb.dim, tb.dim_logical, tb.stride, s_dnn,
+        emb_init_kernel<<<grid_for(tb.arows * tb.stride, 256, kNumSms * 32), 256, 0, m->stream>>>(tb.data, tb.arows, tb.dim, tb.dim_logical, tb.stride, s_dnn,
                                                                                            splitmix64_host(seed + 1000 + t + (tb.sharded ? 7919ull * m->shard.rank : 0ull)), random_w);
         m->launches++;
     }
     if (m->use_wide && m->wide_rows > 0) {
         float s_lin = slot1_init(m->lin_opt);
-        wide_init_kernel<<<grid_for(m->wide_rows, 256, 148 * 32), 256, 0, m->stream>>>(m->d_wide, m->wide_rows, s_lin);
+        wide_init_kernel<<<grid_for(m->wide_rows, 256, kNumSms * 32), 256, 0, m->stream>>>(m->d_wide, m->wide_rows, s_lin);
         m->launches++;
     }
     if (m->use_wide && m->shard.sp[1].on) {
         float s_lin = slot1_init(m->lin_opt);
-        wide_init_kernel<<<grid_for(m->shard.sp[1].local_rows, 256, 148 * 32), 256, 0, m->stream>>>(m->shard.sp[1].d_wide, m->shard.sp[1].local_rows, s_lin);
+        wide_init_kernel<<<grid_for(m->shard.sp[1].local_rows, 256, kNumSms * 32), 256, 0, m->stream>>>(m->shard.sp[1].d_wide, m->shard.sp[1].local_rows, s_lin);
         m->launches++;
     }
     WD_CUDA(cudaGetLastError());
@@ -122,7 +122,7 @@ int metrics_setup() {
 }
 
 int metrics_accumulate(WdModel* m) {
-    metrics_kernel<<<grid_for(m->dbatch.B, 256, 148), 256, 0, m->stream>>>(m->dbatch.B, m->d_logits, m->d_label, m->dbatch.weight, m->d_metrics);
+    metrics_kernel<<<grid_for(m->dbatch.B, 256, kNumSms), 256, 0, m->stream>>>(m->dbatch.B, m->d_logits, m->d_label, m->dbatch.weight, m->d_metrics);
     m->launches++;
     m->eval_batches++;
     WD_CUDA(cudaGetLastError());

@@ -11,7 +11,7 @@
 //   dgrad     A = dZ [batch, N],                    B = W  [K, N] rows of one input segment
 //   wgrad     A = inputT [K, batch],                B = dZT [N, batch]     (split over the batch)
 // which is why activations and gradients are also kept transposed.  This file holds the fp32 CUDA-core
-// (FFMA) engine — exact fp32 products, used as the parity engine and as the reference the tcgen05 engine
+// (FFMA) engine — exact fp32 products, used as the parity engine and as the reference the wgmma engine
 // (gemm_tc.cu) is validated against.
 #include <stdlib.h>
 
@@ -158,11 +158,10 @@ static void launch_gemm(WdModel* m, int mode, const GemmA& A, const float* B, in
     m->launches++;
 }
 
-// tcgen05 engine (gemm_tc.cu); returns WD_EUNSUPPORTED when the shape is not covered
+// wgmma tf32 engine (gemm_tc.cu); returns WD_EUNSUPPORTED when the shape is not covered
 int tc_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M, int N, const Epi& ep, int splits, int ksplit_len,
             const float* B_hi, const float* B_lo);
-// 3xBF16 tcgen05 engine (gemm_bf16.cu): operands are the bf16 hi / lo copies (GemmA::hi/lo, Bq_hi/Bq_lo)
-bool tc_bf16_uses_pair(int mode, int M, int N, int splits, int num_sms);
+// 3xBF16 wgmma engine (gemm_bf16.cu): operands are the bf16 hi / lo copies (GemmA::hi/lo, Bq_hi/Bq_lo)
 int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, int M, int N,
                  const Epi& ep, int splits, int ksplit_len);
 
@@ -184,7 +183,7 @@ static int run_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ld
         if (rc != WD_EUNSUPPORTED) { mark(m, kNames[mode]); return rc; }
         m->gemm_fallbacks++;                              // loud: counted, reported by wd_gemm_fallback_count, asserted 0 in the tests
         static bool warned = false;
-        if (!warned) { fprintf(stderr, "libwd_b200: tcgen05 engine does not cover a GEMM (M=%d N=%d segs=%d): running it on the FFMA kernel\n", M, N, A.n); warned = true; }
+        if (!warned) { fprintf(stderr, "libwd_b200: wgmma engine does not cover a GEMM (M=%d N=%d segs=%d): running it on the FFMA kernel\n", M, N, A.n); warned = true; }
     }
     launch_gemm(m, mode, A, B, ldb, M, N, ep, splits, ksplit_len);
     mark(m, kNames[mode]);
@@ -1028,13 +1027,10 @@ int mlp_backward(WdModel* m) {
     const __nv_bfloat16* Wq = reinterpret_cast<const __nv_bfloat16*>(m->d_Wsplit);
     // 3xBF16 engine: a hidden layer read by exactly one later HIDDEN layer (every layer but the last of `simple` towers) gets its
     // activation / batch-norm backward inside the epilogue of that consumer's data-gradient GEMM (EPI_DACT): its dH is never
-    // stored and act_bn_bwd_q_kernel is not launched for it.  Opt-in (WD_FUSE_DACT=1): measured on B200 the fused epilogue
-    // (1400 instructions per 32 x 32 chunk on eight epilogue warps) costs more than the separate pass saves (0.534 vs 0.520 ms per
-    // step, profiles/r2_*); the logits-layer fusion below (logits_act_bwd_q_kernel) is always on.
+    // stored and act_bn_bwd_q_kernel is not launched for it.  Opt-in (WD_FUSE_DACT=1); the logits-layer fusion below
+    // (logits_act_bwd_q_kernel) is always on.
     static const bool fuse_dact_on = getenv("WD_FUSE_DACT") ? atoi(getenv("WD_FUSE_DACT")) != 0 : false;
     static const bool fuse_logits_on = getenv("WD_FUSE_LOGITS_BWD") ? atoi(getenv("WD_FUSE_LOGITS_BWD")) != 0 : true;
-    static int num_sms = 0;
-    if (!num_sms) cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device);
     for (auto& tw : m->towers) {
         std::vector<char> written(tw.n_hidden, 0);
         std::vector<int> readers(tw.n_hidden, 0);
@@ -1116,8 +1112,7 @@ int mlp_backward(WdModel* m) {
                 Epi e2{};
                 e2.C = dst; e2.ldc = dld; e2.accumulate = acc;
                 int mode2 = EPI_STORE;
-                if (q && fuse_dact_on && sg.src >= 0 && readers[sg.src] == 1 && m->dropout_rate <= 0.f && sg.width_phys == tw.layers[sg.src].N_phys &&
-                    tc_bf16_uses_pair(EPI_DACT, B, sg.width_phys, 1, num_sms)) {
+                if (q && fuse_dact_on && sg.src >= 0 && readers[sg.src] == 1 && m->dropout_rate <= 0.f && sg.width_phys == tw.layers[sg.src].N_phys) {
                     Layer& S = tw.layers[sg.src];
                     mode2 = EPI_DACT;
                     fused[sg.src] = 1;

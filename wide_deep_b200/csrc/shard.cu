@@ -583,10 +583,10 @@ static int shard_serve(WdModel* m, int s) {
     if (!sp.on) return WD_OK;
     const ShardPeer& me = sp.peers[S.rank];
     if (s == 0)
-        shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, 148 * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
+        shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
             sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_peers, sp.nbags_cap, sp.width);
     else
-        shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, 148 * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
+        shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
             sp.d_wide, sp.d_peers, sp.nbags_cap);
     m->launches++;
     WD_CUDA(cudaGetLastError());
@@ -613,7 +613,7 @@ static int shard_combine(WdModel* m, int s) {
     const int B = m->dbatch.B;
     const ShardPeer& me = sp.peers[S.rank];
     if (s == 0)
-        shard_combine_emb_kernel<<<grid_for((int64_t)B * sp.n_slots * 8, 256, 148 * 8), 256, 0, m->stream>>>(B, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0,
+        shard_combine_emb_kernel<<<grid_for((int64_t)B * sp.n_slots * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(B, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0,
             sp.d_bagmask, me.bagscale, me.recv, S.world, sp.nbags_cap, sp.width, m->d_X0, m->d0_phys);
     else
         shard_combine_wide_kernel<<<grid_for(B, 256), 256, 0, m->stream>>>(B, sp.d_bagmask, me.recv, S.world, sp.nbags_cap, m->d_wide_logit);

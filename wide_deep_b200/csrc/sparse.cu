@@ -343,7 +343,7 @@ static void launch_emb_fwd(WdModel* m, int di, bool widebag) {
                 cudaFuncSetAttribute(emb_pool_fwd_tma_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                 configured[di] = true;
             }
-            int grid = grid_for((int64_t)m->dbatch.B * 32, 256, 148 * 3);
+            int grid = grid_for((int64_t)m->dbatch.B * 32, 256, kNumSms * 3);
             emb_pool_fwd_tma_kernel<G><<<grid, 256, smem, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_desc[di], m->d_col_offs, m->d_e_emb,
                                                                    m->d_X0, m->d0_phys, buf_bytes, nbuf, contiguous);
             m->launches++;
@@ -352,7 +352,7 @@ static void launch_emb_fwd(WdModel* m, int di, bool widebag) {
     }
     if (!widebag) {
         constexpr int RMAX = 4;                       // 4 rounds in flight per lane group at <= 64 registers: 32 warps per SM
-        int grid = grid_for((int64_t)m->dbatch.B * 32, 256, 148 * 8);
+        int grid = grid_for((int64_t)m->dbatch.B * 32, 256, kNumSms * 8);
         emb_pool_fwd_rows_kernel<G, RMAX><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_desc[di], m->d_col_offs,
                                                                         m->d_e_emb, m->d_X0, m->d0_phys);
         m->launches++;
@@ -360,7 +360,7 @@ static void launch_emb_fwd(WdModel* m, int di, bool widebag) {
     }
     int64_t nbags = (int64_t)m->dbatch.B * ntab;
     int64_t warps = widebag ? nbags : (nbags + (32 / G) - 1) / (32 / G);
-    int grid = grid_for(warps * 32, 256, 148 * 8);
+    int grid = grid_for(warps * 32, 256, kNumSms * 8);
     if (widebag)
         emb_pool_fwd_kernel<G, true><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_tables[di],
             m->d_tab_data, m->d_tab_stride, m->d_tab_x0, m->d_tab_col, m->d_tab_row_base, m->d_col_offs, m->d_e_emb, m->d_X0, m->d0_phys);
@@ -920,12 +920,12 @@ int small_scatter(WdModel* m, int which) {
     float* block = m->d_G + m->dense_count;
     if (which == 0) {
         if (m->n_small_tab == 0 || !(m->use_deep && !m->tables.empty())) return WD_OK;
-        small_scatter_emb_kernel<<<grid_for(m->max_nnz * 8, 256, 148 * 8), 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], m->d_ugrad[0], m->emb_max_dim,
+        small_scatter_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], m->d_ugrad[0], m->emb_max_dim,
             (uint32_t)m->small_base[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_dim, m->d_rtab_gs_off, block,
             block + m->gs_touch_off[0], m->d_nubig[0]);
     } else {
         if (!m->use_wide || m->small_base[1] >= m->wide_rows) return WD_OK;
-        small_scatter_wide_kernel<<<grid_for(m->max_nnz, 256, 148 * 8), 256, 0, m->stream>>>(m->d_nuniq[1], m->d_urow[1], m->d_ugrad[1],
+        small_scatter_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(m->d_nuniq[1], m->d_urow[1], m->d_ugrad[1],
             (uint32_t)m->small_base[1], block + m->gs_emb_floats, block + m->gs_touch_off[1], m->d_nubig[1]);
     }
     copy_count_kernel<<<1, 1, 0, m->stream>>>(m->d_nuniq[which], m->d_nubig[which]);

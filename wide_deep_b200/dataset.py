@@ -264,7 +264,7 @@ def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=N
     the per-batch parsing is lazy, so the returned iterator may be drained from a prefetch thread."""
     assert mode in ("train", "eval", "pred"), "mode must in `train`, `eval`, or `pred`, found {}".format(mode)
     if img_data_file:
-        raise ValueError("image inputs are not supported by the B200 path (cnn_use_flag: 0)")
+        raise ValueError("image inputs are not supported by this library (cnn_use_flag: 0)")
     reader = TsvReader(config, plan, is_pred=(mode == "pred"))
     lib = _native.lib()
     # one image of all files + an index of its non-empty lines (wd_tsv_index_lines): sharding and shuffling permute INDICES, the

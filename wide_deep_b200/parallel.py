@@ -1,7 +1,7 @@
 """Data-parallel training over the GPUs of one box (one process per GPU, torch.distributed for plumbing).
 
 The reference trains with an asynchronous TensorFlow parameter server (reference python/lib/build_estimator.py:
-172-198, python/train.py:209-217; per-worker input shard python/lib/dataset.py:173-174).  On B200 the batch is
+172-198, python/train.py:209-217; per-worker input shard python/lib/dataset.py:173-174).  Here the batch is
 row-sharded over ranks and every step is synchronous and EXACT: the G-rank result equals the 1-rank result on
 the concatenated batch (up to fp32 summation order), because
 
