@@ -92,8 +92,8 @@ typedef struct WdPlanDesc {
     int32_t d0_phys;                /* physical width of the deep input (multiple of 32; padding columns stay 0) */
     int64_t wide_rows;              /* total rows of the wide weight table */
 
-    int32_t n_towers;
-    const int32_t *tower_nlayers;   /* hidden layers per tower */
+    int32_t n_towers;               /* at most 8 (WD_EUNSUPPORTED otherwise) */
+    const int32_t *tower_nlayers;  /* hidden layers per tower */
     const int32_t *tower_mode;      /* WD_MODE_* */
     const int32_t *hidden_units;    /* concatenated over towers */
     int32_t activation;             /* WD_ACT_* */

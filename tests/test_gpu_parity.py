@@ -220,6 +220,26 @@ def test_multi_tower():
     _train_compare(fc, cross, model, "wide_deep", steps=2, seed=13)
 
 
+def test_six_towers():
+    """More towers than the four the head kernel once took: the logits layers of all six run in the one head kernel."""
+    fc, cross, model = small_conf()
+    model["dnn_hidden_units"] = [[64, 32], [48, 16, 8], [32], [40, 24], [16, 16], [24]]
+    model["dnn_connected_mode"] = ["simple", "dense", "simple", "dense", "simple", "dense"]
+    _train_compare(fc, cross, model, "wide_deep", steps=2, seed=13)
+
+
+def test_more_than_eight_towers_is_rejected():
+    from wide_deep_b200 import _native
+    fc, cross, model = small_conf()
+    model["dnn_hidden_units"] = [[16]] * 9
+    model["dnn_connected_mode"] = "simple"
+    plan = Plan(fc, cross, model, "wide_deep", max_batch=64, max_nnz=64 * 64, max_keys=64 * 64, gemm_engine="ffma")
+    with pytest.raises(_native.NativeError) as e:
+        WideDeepModel(plan)
+    assert e.value.code == _native.EUNSUPPORTED
+    assert "towers" in str(e.value)
+
+
 def test_weighted_examples_and_ragged_batch():
     fc, cross, model = small_conf()
     _train_compare(fc, cross, model, "wide_deep", steps=2, seed=17, weighted=True, B=77, max_batch=128)
@@ -393,8 +413,9 @@ def test_tc1x_engine_is_close_but_not_parity_grade():
 
 
 @pytest.mark.parametrize("engine", ["tc3x", "bf16x3"])
-def test_tc3x_wide_tiles_and_presplit_weights(engine):
-    """Hidden widths that are multiples of 256 take the 128x256-tile path with pre-split (hi/lo) weights."""
+def test_hidden_widths_over_128_with_presplit_weights(engine):
+    """Hidden widths of 512 and 256: several 128 x 128 output tiles per layer, and the forward and data-gradient GEMMs read the
+    weights as pre-split hi / lo copies; B = 700 leaves a ragged last row tile."""
     B = 700
     ptol = 2e-4 if engine == "tc3x" else 2e-3
     fc, om, plan, pm = _engine_pair(engine, (512, 256), "simple", B, seed=53)
@@ -413,8 +434,8 @@ def test_tc3x_wide_tiles_and_presplit_weights(engine):
 
 def test_criteo_shape_scaled_down():
     """The benchmark configuration (BASELINE.json configs[1]) with every table scaled by 1e-3: single-valued 32-wide
-    embedding bags adjacent in the deep input -> exercises the TMA-staged gather with its single-bulk-store fast path,
-    the pre-split-weight GEMMs and the chunked hot-row gradient sums, against the oracle."""
+    embedding bags -> exercises the short-bag gather (emb_pool_fwd_rows_kernel), the pre-split-weight GEMMs and the chunked
+    hot-row gradient sums, against the oracle."""
     from wide_deep_b200 import synthetic
     from wide_deep_b200.model import Batch
     fc, cross, model, emb = synthetic.criteo_conf(scale=1e-3, hidden=(256, 128, 64))

@@ -390,6 +390,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             }
 
         // towers
+        if (d->n_towers > kMaxTowers) { set_error("more than %d towers", kMaxTowers); return WD_EUNSUPPORTED; }
         int hu_off = 0, did = 0;
         for (int t = 0; t < d->n_towers; ++t) {
             Tower tw{};

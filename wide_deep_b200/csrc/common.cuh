@@ -26,6 +26,7 @@ void set_error(const char* fmt, ...);
 
 constexpr uint32_t kInvalidRow = 0xFFFFFFFFu;
 constexpr int kMaxSegs = 8;      // sources concatenated into one MLP layer input
+constexpr int kMaxTowers = 8;    // deep towers per model: the head kernel takes all of their logits layers as one parameter block
 constexpr int kNumSms = 132;     // SMs of an H100 SXM: the grid caps of the grid-stride kernels are sized by it
 constexpr int kMaxDims = 8;      // distinct embedding widths per model
 // sort / unique-row scratch sets ("lists"): 0 embedding rows and 1 wide rows of the replicated tables; row-sharded tables add
@@ -349,7 +350,7 @@ struct WdModel {
     float* d_loss_part = nullptr;            // per-block partials
     float* d_loss = nullptr;                 // scalar
     unsigned long long* d_step_trace = nullptr;   // WD_STEP_TRACE=1: globaltimer stamps of the last step (wd_debug_step_trace)
-    int32_t* d_head_counter = nullptr;       // blocks of the fused head kernel that have finished (last one sums the loss)
+    int32_t* d_head_counter = nullptr;       // blocks of the head kernel that have finished (last one sums the loss)
     float* d_bpow = nullptr;                 // Adam: {linear beta1^t, linear beta2^t, dnn beta1^t, dnn beta2^t}, multiplied in fp32 after every step (AdamOptimizer._finish)
     float* h_loss_pinned = nullptr;
 

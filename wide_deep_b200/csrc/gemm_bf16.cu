@@ -3,8 +3,8 @@
 //   C[M,N] = sum_k A[M,k] * B[N,k]      fp32 values, fp32 accumulation in registers
 //
 // Every fp32 operand exists in HBM as two bf16 copies, hi = bf16_rn(x) and lo = bf16_rn(x - hi), written by the kernel that
-// PRODUCED the operand (forward epilogue, act_bn_bwd_kernel, x0_split_kernel, dense_apply_kernel), so this kernel moves and
-// multiplies bf16 only: per 64-element k-block four TMA tiles (A_hi, A_lo, B_hi, B_lo; 128-byte swizzle) and
+// PRODUCED the operand (forward epilogue, x0_split_kernel, act_bn_bwd_q_kernel, logits_act_bwd_q_kernel, dense_vec_kernel), so
+// this kernel moves and multiplies bf16 only: per 64-element k-block four TMA tiles (A_hi, A_lo, B_hi, B_lo; 128-byte swizzle) and
 // 4 k-steps x 3 wgmma.mma_async (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi) into one fp32 accumulator.  hi + lo represents x to
 // 2^-17 and the dropped a_lo*b_lo term is below 2^-16, so one product carries ~1e-5 relative error (random signs, so a long dot
 // product does better).  That is a FAST mode: it is held to the 1e-4 logit bar on the benchmarked configuration (bench.py
@@ -18,7 +18,7 @@
 // its descriptor uses LBO = one box (8 KB) between 64-wide column groups and SBO = 1 KB between 8-row k groups.
 //
 // One persistent CTA per SM, three warp groups: group 0 = TMA producer (one elected thread, registers handed over with
-// setmaxnreg), groups 1-2 = consumers, each owning 64 rows of the 128 x TBN tile in registers (TBN / 2 accumulators per thread).
+// setmaxnreg), groups 1-2 = consumers, each owning 64 rows of the 128 x 128 tile in registers (64 accumulators per thread).
 // A consumer releases a pipeline stage once the wgmma batch that read it has retired (wait_group 1: the next batch is already
 // queued), and the producer runs ahead into the next tile while the consumers store the current one.  Forward epilogue = bias +
 // activation + BN-affine straight from the accumulator fragment; it stores the post-activation values (fp32, for the backward),
@@ -41,6 +41,8 @@ int tc_make_map_bf16(CUtensorMap* map, const void* ptr, int rows, int cols, int 
 namespace {
 
 constexpr int QBM = 128;         // tile rows: two warp groups x wgmma M = 64
+constexpr int QBN = 128;         // tile columns (wgmma N)
+constexpr int QNST = 3;          // pipeline stages of 64 KB: 192 KB of the 227 KB a block may use
 constexpr int QBK = 64;          // bf16 elements per k-block = one 128-byte swizzle row
 constexpr int Q_THREADS = 384;   // warp group 0 TMA, warp groups 1-2 MMA + epilogue
 
@@ -56,33 +58,24 @@ __device__ unsigned long long g_probe[32 * 8];
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #define PROBE(i) do { if (probe >= 0 && blockIdx.x == 0 && (threadIdx.x & 127) == 0) g_probe[probe * 8 + (i)] = gtime(); } while (0)
 
-__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {    // packed bf16 pairs of the hi / lo copies
-    const __nv_bfloat162 hp = __floats2bfloat162_rn(x0, x1);
-    hi = *reinterpret_cast<const uint32_t*>(&hp);
-    const __nv_bfloat162 lp = __floats2bfloat162_rn(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
-    lo = *reinterpret_cast<const uint32_t*>(&lp);
-}
-
-template <int TBN, int MODE>
+template <int MODE>
 __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid_constant__ QMaps maps, const QSegs segs, int M, int N, int ktot,
                                                                    int ksplit_len, int nsplit, Epi ep, int probe) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr bool A_MN = MODE == EPI_WGRAD;                       // operand stored with its M / N index contiguous
     constexpr bool B_MN = MODE == EPI_FWD || MODE == EPI_WGRAD;
-    constexpr int A_BYTES = QBM * 128, B_BYTES = TBN * 128;
+    constexpr int A_BYTES = QBM * 128, B_BYTES = QBN * 128;
     constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);
-    constexpr int NST = TBN == 256 ? 2 : 3;                        // 96 KB / 64 KB stages: 192 KB of the 227 KB a block may use
     auto a_hi = [&](int s) { return base + s * STAGE_BYTES; };
     auto a_lo = [&](int s) { return base + s * STAGE_BYTES + A_BYTES; };
     auto b_hi = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES; };
     auto b_lo = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES + B_BYTES; };
-    uint64_t* bars = reinterpret_cast<uint64_t*>(base + NST * STAGE_BYTES);
-    uint64_t* full = bars; uint64_t* empty = bars + NST;
-    float* colsum = reinterpret_cast<float*>(bars + 16);           // EPI_DACT: [3 sums][8 consumer warps][TBN columns]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(base + QNST * STAGE_BYTES);
+    uint64_t* full = bars; uint64_t* empty = bars + QNST;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
-    const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + QBM - 1) / QBM;
+    const int tiles_n = (N + QBN - 1) / QBN, tiles_m = (M + QBM - 1) / QBM;
     const int ntiles = tiles_n * tiles_m * nsplit;
     // k-blocks of one tile: FWD / STORE walk the segments (each padded to whole k-blocks by TMA zero fill), WGRAD walks its split
     int nkb_all = 0;
@@ -91,7 +84,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
         z = tile / (tiles_n * tiles_m);
         int r = tile % (tiles_n * tiles_m);
         m0 = (r / tiles_n) * QBM;
-        n0 = (r % tiles_n) * TBN;
+        n0 = (r % tiles_n) * QBN;
         kbeg = 0;
         nkb = nkb_all;
         if (MODE == EPI_WGRAD) {
@@ -102,7 +95,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
     };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }       // empty: one arrival per consumer warp
+        for (int s = 0; s < QNST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }       // empty: one arrival per consumer warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -118,7 +111,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
                 tile_range(tile, m0, n0, z, kbeg, nkb);
                 int seg = 0, kin = 0;                            // current segment, k offset inside it
                 for (int kb = 0; kb < nkb; ++kb, ++g) {
-                    const int s = g % NST, it = g / NST;
+                    const int s = g % QNST, it = g / QNST;
                     if (it > 0) mbar_wait(&empty[s], (it - 1) & 1);
                     int ka, kbcoord;
                     if (MODE == EPI_WGRAD) { ka = kbeg + kb * QBK; kbcoord = ka; }
@@ -143,7 +136,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
                         tma_load_2d(b_lo(s), &maps.b_lo, &full[s], kbcoord, n0);
                     } else {
 #pragma unroll
-                        for (int i = 0; i < TBN / 64; ++i) {
+                        for (int i = 0; i < QBN / 64; ++i) {
                             tma_load_2d(b_hi(s) + i * 8192, &maps.b_hi, &full[s], n0 + 64 * i, kbcoord);
                             tma_load_2d(b_lo(s) + i * 8192, &maps.b_lo, &full[s], n0 + 64 * i, kbcoord);
                         }
@@ -157,18 +150,18 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
         const int cw = wg - 1, cwarp = warp - 4;
         constexpr uint32_t a_step = A_MN ? 2048u : 32u, b_step = B_MN ? 2048u : 32u;   // bytes per 16-element k-step
         constexpr int TA = A_MN ? 1 : 0, TB = B_MN ? 1 : 0;
-        float d[TBN / 2];
+        float d[QBN / 2];
         int g = 0, use = 0;
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
             int m0, n0, z, kbeg, nkb;
             tile_range(tile, m0, n0, z, kbeg, nkb);
             if (nkb == 0) {
 #pragma unroll
-                for (int i = 0; i < TBN / 2; ++i) d[i] = 0.f;
+                for (int i = 0; i < QBN / 2; ++i) d[i] = 0.f;
             }
             int prev = -1;
             for (int kb = 0; kb < nkb; ++kb, ++g) {
-                const int s = g % NST, it = g / NST;
+                const int s = g % QNST, it = g / QNST;
                 mbar_wait(&full[s], it & 1);
                 if (g == 0) PROBE(1);
                 const uint32_t sa_hi = smem_u32(a_hi(s)) + cw * 8192, sa_lo = smem_u32(a_lo(s)) + cw * 8192;   // 64 rows (or one 64-column box) per group
@@ -199,7 +192,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
             const int r0 = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
             const int cq = 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < TBN / 8; ++j) {
+            for (int j = 0; j < QBN / 8; ++j) {
                 const int c = n0 + 8 * j + cq;
                 if (n0 + 8 * j < N) {
                     if (MODE == EPI_FWD) {
@@ -224,42 +217,6 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
                             *reinterpret_cast<uint32_t*>(ep.Hs_hi + o) = ph;
                             *reinterpret_cast<uint32_t*>(ep.Hs_lo + o) = pl;
                         }
-                    } else if (MODE == EPI_DACT) {
-                        // d = dH of the fed layer; never stored.  dZ = dH * gamma' * act'(A) leaves as bf16 hi / lo copies, the column
-                        // sums of dZ (bias), dH * A (gamma) and dH (beta) over this warp's 16 rows go to shared memory
-                        const bool in0 = c < ep.n_logical, in1 = c + 1 < ep.n_logical;
-                        const float g0 = (in0 && ep.bn) ? __ldg(ep.gamma + c) * 0.99950037468777f : 1.f;
-                        const float g1 = (in1 && ep.bn) ? __ldg(ep.gamma + c + 1) * 0.99950037468777f : 1.f;
-                        float sb0 = 0.f, sb1 = 0.f, sg0 = 0.f, sg1 = 0.f, se0 = 0.f, se1 = 0.f;
-#pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            const int r = r0 + 8 * hh;
-                            if (r >= M) continue;
-                            const int64_t o = (int64_t)r * ep.ldh + c;
-                            const float2 av = __ldg(reinterpret_cast<const float2*>(ep.Aact + o));
-                            const float dh0 = in0 ? d[4 * j + 2 * hh] : 0.f, dh1 = in1 ? d[4 * j + 2 * hh + 1] : 0.f;
-                            const float aa0 = in0 ? av.x : 0.f, aa1 = in1 ? av.y : 0.f;
-                            const float dz0 = dh0 * g0 * act_bwd(ep.act, aa0), dz1 = dh1 * g1 * act_bwd(ep.act, aa1);
-                            uint32_t ph, pl;
-                            split_pair(dz0, dz1, ph, pl);
-                            *reinterpret_cast<uint32_t*>(ep.Hs_hi + o) = ph;
-                            *reinterpret_cast<uint32_t*>(ep.Hs_lo + o) = pl;
-                            sb0 += dz0; sb1 += dz1;
-                            sg0 += dh0 * aa0 * 0.99950037468777f; sg1 += dh1 * aa1 * 0.99950037468777f;
-                            se0 += dh0; se1 += dh1;
-                        }
-#pragma unroll
-                        for (int o = 4; o <= 16; o <<= 1) {           // over the 8 row pairs of the warp, fixed order
-                            sb0 += __shfl_xor_sync(0xffffffffu, sb0, o); sb1 += __shfl_xor_sync(0xffffffffu, sb1, o);
-                            sg0 += __shfl_xor_sync(0xffffffffu, sg0, o); sg1 += __shfl_xor_sync(0xffffffffu, sg1, o);
-                            se0 += __shfl_xor_sync(0xffffffffu, se0, o); se1 += __shfl_xor_sync(0xffffffffu, se1, o);
-                        }
-                        if (lane < 4) {
-                            float* cs = colsum + cwarp * TBN + 8 * j + cq;
-                            cs[0] = sb0; cs[1] = sb1;
-                            cs[8 * TBN] = sg0; cs[8 * TBN + 1] = sg1;
-                            cs[16 * TBN] = se0; cs[16 * TBN + 1] = se1;
-                        }
                     } else {
                         float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0);
 #pragma unroll
@@ -274,23 +231,6 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
                     }
                 }
             }
-            if (MODE == EPI_DACT) {
-                // 128-row partials of this row tile: the eight consumer warps summed in warp order, one column per thread
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int col = threadIdx.x - 128, n = n0 + col;
-                if (col < TBN && n < N) {
-                    float sb = 0.f, sg = 0.f, se = 0.f;
-#pragma unroll
-                    for (int w = 0; w < 8; ++w) {
-                        sb += colsum[w * TBN + col];
-                        if (ep.bn) { sg += colsum[(8 + w) * TBN + col]; se += colsum[(16 + w) * TBN + col]; }
-                    }
-                    const int64_t o = (int64_t)(m0 / QBM) * ep.pstride + n;
-                    ep.p_bias[o] = sb;
-                    if (ep.bn) { ep.p_gamma[o] = sg; ep.p_beta[o] = se; }
-                }
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-            }
             if (cwarp == 0) PROBE(use == 0 ? 4 : 5);
             ++use;
         }
@@ -299,22 +239,21 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
 
 int g_probe_slot = 0;
 
-template <int TBN, int MODE>
+template <int MODE>
 int launch_q(WdModel* m, const QMaps& maps, const QSegs& segs, int M, int N, int ktot, int splits, int ksplit_len, const Epi& ep) {
-    constexpr int NST = TBN == 256 ? 2 : 3;
-    constexpr int smem = NST * 2 * (QBM * 128 + TBN * 128) + 1024 + 128 + (MODE == EPI_DACT ? 3 * 8 * TBN * 4 : 0);
+    constexpr int smem = QNST * 2 * (QBM * 128 + QBN * 128) + 1024 + 128;
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {
-        WD_CUDA(cudaFuncSetAttribute(tc_gemm_bf16_kernel<TBN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        WD_CUDA(cudaFuncSetAttribute(tc_gemm_bf16_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         WD_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device));
         configured = true;
     }
     const int nsplit = MODE == EPI_WGRAD ? splits : 1;
-    const int ntiles = ((N + TBN - 1) / TBN) * ((M + QBM - 1) / QBM) * nsplit;
+    const int ntiles = ((N + QBN - 1) / QBN) * ((M + QBM - 1) / QBM) * nsplit;
     static const bool probe_on = getenv("WD_GEMM_PROBE") != nullptr;
     const int probe = probe_on ? (g_probe_slot++ & 31) : -1;
-    tc_gemm_bf16_kernel<TBN, MODE><<<ntiles < num_sms ? ntiles : num_sms, Q_THREADS, smem, m->stream>>>(maps, segs, M, N, ktot, ksplit_len, nsplit, ep, probe);
+    tc_gemm_bf16_kernel<MODE><<<ntiles < num_sms ? ntiles : num_sms, Q_THREADS, smem, m->stream>>>(maps, segs, M, N, ktot, ksplit_len, nsplit, ep, probe);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -328,14 +267,6 @@ extern "C" int wd_debug_gemm_probe(unsigned long long* out) {
     cudaError_t e = cudaMemcpyFromSymbol(out, g_probe, sizeof(unsigned long long) * 32 * 8);
     g_probe_slot = 0;
     return e == cudaSuccess ? 0 : -1;
-}
-
-// 128 x 128 output tiles: on the benchmark towers (H100 80GB HBM3, 700 W) the step ran at 8.75 M examples/s with them and at
-// 7.63 M with 128 x 256 tiles (BASELINE.md section 4).  The 256-wide instantiations are kept for WD_TC_FORCE_WIDE=1 only, which the tests set to run the
-// two-stage ring and the m64n256k16 MMA on small problems; nothing selects them otherwise.
-static bool wide_tile(int N) {
-    static const bool force_wide = getenv("WD_TC_FORCE_WIDE") != nullptr;
-    return force_wide && N > 128;
 }
 
 int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, int M, int N,
@@ -360,24 +291,18 @@ int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi
         ktot += A.k[s];
     }
     for (int s = A.n; s < kMaxSegs; ++s) { maps.a_hi[s] = maps.a_hi[0]; maps.a_lo[s] = maps.a_lo[0]; }
-    const bool wide = wide_tile(N);
-    const int tbn = wide ? 256 : 128;
     if (!b_mn) {
-        if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, N, ktot, ldb, tbn))) return rc;
-        if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, N, ktot, ldb, tbn))) return rc;
+        if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, N, ktot, ldb, QBN))) return rc;
+        if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, N, ktot, ldb, QBN))) return rc;
     } else {
         if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, ktot, N, ldb, 64))) return rc;
         if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, ktot, N, ldb, 64))) return rc;
     }
     if (mode == EPI_WGRAD) ksplit_len = (ksplit_len + QBK - 1) / QBK * QBK;
-    if ((mode == EPI_FWD || mode == EPI_DACT) && (!ep.Hs_hi || !ep.Hs_lo)) { set_error("bf16 GEMM engine: epilogue without hi/lo outputs"); return WD_EINVAL; }
-#define WD_Q_LAUNCH(MODE_) \
-    return wide ? launch_q<256, MODE_>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep) : launch_q<128, MODE_>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep)
-    if (mode == EPI_FWD) { WD_Q_LAUNCH(EPI_FWD); }
-    if (mode == EPI_STORE) { WD_Q_LAUNCH(EPI_STORE); }
-    if (mode == EPI_DACT) { WD_Q_LAUNCH(EPI_DACT); }
-    WD_Q_LAUNCH(EPI_WGRAD);
-#undef WD_Q_LAUNCH
+    if (mode == EPI_FWD && (!ep.Hs_hi || !ep.Hs_lo)) { set_error("bf16 GEMM engine: epilogue without hi/lo outputs"); return WD_EINVAL; }
+    if (mode == EPI_FWD) return launch_q<EPI_FWD>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep);
+    if (mode == EPI_STORE) return launch_q<EPI_STORE>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep);
+    return launch_q<EPI_WGRAD>(m, maps, segs, M, N, ktot, splits, ksplit_len, ep);
 }
 
 }  // namespace wd

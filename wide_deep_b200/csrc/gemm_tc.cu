@@ -8,12 +8,12 @@
 // a_lo*b_lo term is below 2^-22 relative, i.e. at fp32 rounding level, which is what the 1e-4 logit parity bar
 // (BASELINE.json) needs and what a single tf32 pass (2^-11) cannot give.
 //
-// One persistent CTA per SM loops over 128 x TBN output tiles, K loop over 32-float = 128-byte blocks.  Four warp groups:
+// One persistent CTA per SM loops over 128 x 128 output tiles, K loop over 32-float = 128-byte blocks.  Four warp groups:
 //   group 0     TMA producer (one elected thread): cp.async.bulk.tensor.2d of the raw fp32 A / B blocks (128B-swizzled)
 //               into the "hi" buffers of a stage ring, completion on mbarrier full[s]
 //   group 1     splitters: wait full[s], rewrite the block in place as hi and write lo beside it (element-wise,
 //               so the swizzle never has to be decoded), fence.proxy.async, arrive split[s]
-//   groups 2-3  consumers, 64 tile rows each: wait split[s], 4 k-steps x 3 wgmma.mma_async m64nTBNk8 tf32, release the stage
+//   groups 2-3  consumers, 64 tile rows each: wait split[s], 4 k-steps x 3 wgmma.mma_async m64n128k8 tf32, release the stage
 //               on empty[s] once that batch has retired; then the epilogue straight from the accumulator fragment: fused
 //               bias + activation + BN-affine (+ transposed copy) or plain / accumulating / split-K store
 // The producer and the splitters hand registers to the consumers (setmaxnreg) and run ahead into the next tile while the
@@ -32,6 +32,7 @@
 namespace wd {
 
 constexpr int TBM = 128;        // tile rows: two consumer warp groups x wgmma M = 64
+constexpr int TBN = 128;        // tile columns: 64 accumulator registers per consumer thread is what four warp groups leave room for
 constexpr int TBK = 32;         // floats per k-block = one 128-byte swizzle row
 constexpr int TSTAGES = 3;
 constexpr int TC_THREADS = 512;
@@ -43,12 +44,14 @@ struct TcMaps {
 };
 
 // ---------------------------------------------------------------------------------------------- kernel
-// BPRE: the B operand (weights) arrives already split into hi / lo copies (two tensor maps), only A is split here.
-template <int TBN, int MODE, bool SPLIT3, bool BPRE>
+// SPLIT3: three products (3xTF32), else one (tc1x).  The forward and data-gradient GEMMs of 3xTF32 (BPRE) read the weights
+// already split into hi / lo copies (two tensor maps) and split only A here.
+template <int MODE, bool SPLIT3>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_gemm_kernel(const __grid_constant__ TcMaps maps, int nseg, int4 segk01, int4 segk23,
                                                                int M, int N, int ktot, int ksplit_len, int nsplit, Epi ep) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    constexpr bool BPRE = SPLIT3 && MODE != EPI_WGRAD;
     constexpr int A_BYTES = TBM * 128, B_BYTES = TBN * 128;
     constexpr int STAGE_BYTES = (SPLIT3 ? 2 : 1) * (A_BYTES + B_BYTES);
     constexpr int NST = TSTAGES;
@@ -314,7 +317,7 @@ int tc_make_map_bf16(CUtensorMap* map, const void* ptr, int rows, int cols, int 
     return WD_OK;
 }
 
-template <int TBN, int MODE, bool SPLIT3, bool BPRE>
+template <int MODE, bool SPLIT3>
 static int launch_tc(WdModel* m, const TcMaps& maps, int nseg, const int* segk, int M, int N, int ktot, int splits, int ksplit_len, const Epi& ep) {
     constexpr int A_BYTES = TBM * 128, B_BYTES = TBN * 128;
     constexpr int NST = TSTAGES;
@@ -323,13 +326,13 @@ static int launch_tc(WdModel* m, const TcMaps& maps, int nseg, const int* segk, 
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {
-        WD_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<TBN, MODE, SPLIT3, BPRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        WD_CUDA(cudaFuncSetAttribute(tc_gemm_kernel<MODE, SPLIT3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         WD_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, m->device));
         configured = true;
     }
     const int nsplit = MODE == EPI_WGRAD ? splits : 1;
     const int ntiles = ((N + TBN - 1) / TBN) * ((M + TBM - 1) / TBM) * nsplit;
-    tc_gemm_kernel<TBN, MODE, SPLIT3, BPRE><<<ntiles < num_sms ? ntiles : num_sms, TC_THREADS, smem, m->stream>>>(maps, nseg, s01, s23, M, N, ktot, ksplit_len, nsplit, ep);
+    tc_gemm_kernel<MODE, SPLIT3><<<ntiles < num_sms ? ntiles : num_sms, TC_THREADS, smem, m->stream>>>(maps, nseg, s01, s23, M, N, ktot, ksplit_len, nsplit, ep);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -351,21 +354,18 @@ int tc_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M
     }
     for (int s = A.n; s < kMaxSegs; ++s) maps.a[s] = maps.a[0];
     const bool split3 = m->gemm_engine == WD_GEMM_TC3X;
-    const bool bpre = split3 && B_hi && B_lo && mode != EPI_WGRAD;
-    // 128 x 128 tiles only: 64 accumulator registers per consumer thread is what four warp groups leave room for
-    if ((rc = make_map(&maps.b, bpre ? B_hi : B, N, ktot, ldb, 128))) return rc;
-    if (bpre) { if ((rc = make_map(&maps.b_lo, B_lo, N, ktot, ldb, 128))) return rc; }
+    const bool bpre = split3 && mode != EPI_WGRAD;                     // (tc_gemm_kernel's BPRE)
+    if (bpre && (!B_hi || !B_lo)) { set_error("3xTF32 GEMM engine: weights without hi/lo copies"); return WD_EINVAL; }
+    if ((rc = make_map(&maps.b, bpre ? B_hi : B, N, ktot, ldb, TBN))) return rc;
+    if (bpre) { if ((rc = make_map(&maps.b_lo, B_lo, N, ktot, ldb, TBN))) return rc; }
     else maps.b_lo = maps.b;
     if (mode == EPI_WGRAD) ksplit_len = (ksplit_len + TBK - 1) / TBK * TBK;
-    if (mode == EPI_WGRAD)
-        return split3 ? launch_tc<128, EPI_WGRAD, true, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep)
-                      : launch_tc<128, EPI_WGRAD, false, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep);
-#define WD_TC_LAUNCH(MODE_)                                                                                                     \
-    if (!split3) return launch_tc<128, MODE_, false, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep);             \
-    if (!bpre) return launch_tc<128, MODE_, true, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep);                \
-    return launch_tc<128, MODE_, true, true>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep)
-    if (mode == EPI_FWD) { WD_TC_LAUNCH(EPI_FWD); }
-    WD_TC_LAUNCH(EPI_STORE);
+#define WD_TC_LAUNCH(MODE_)                                                                                      \
+    return split3 ? launch_tc<MODE_, true>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep)              \
+                  : launch_tc<MODE_, false>(m, maps, A.n, segk, M, N, ktot, splits, ksplit_len, ep)
+    if (mode == EPI_FWD) WD_TC_LAUNCH(EPI_FWD);
+    if (mode == EPI_STORE) WD_TC_LAUNCH(EPI_STORE);
+    WD_TC_LAUNCH(EPI_WGRAD);
 #undef WD_TC_LAUNCH
 }
 

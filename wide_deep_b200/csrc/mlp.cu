@@ -13,8 +13,6 @@
 // which is why activations and gradients are also kept transposed.  This file holds the fp32 CUDA-core
 // (FFMA) engine — exact fp32 products, used as the parity engine and as the reference the wgmma engine
 // (gemm_tc.cu) is validated against.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "gemm.cuh"
 
@@ -175,7 +173,7 @@ static int run_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ld
     mark(m, "mlp_other");
     if (m->gemm_engine == WD_GEMM_BF16X3) {
         int rc = tc_gemm_bf16(m, mode, A, Bq_hi, Bq_lo, ldb, M, N, ep, splits, ksplit_len);
-        mark(m, kNames[mode == EPI_DACT ? EPI_STORE : mode]);
+        mark(m, kNames[mode]);
         return rc;
     }
     if (m->gemm_engine == WD_GEMM_TC3X || m->gemm_engine == WD_GEMM_TC1X) {
@@ -210,15 +208,7 @@ __global__ void transpose_kernel(const float* __restrict__ in, int ld_in, int M,
 __global__ void x0_split_kernel(const float* __restrict__ in, int64_t n4, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
         const float4 x = reinterpret_cast<const float4*>(in)[i];
-        __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
-        split_bf16(x.x, h0, l0); split_bf16(x.y, h1, l1); split_bf16(x.z, h2, l2); split_bf16(x.w, h3, l3);
-        uint2 ph, pl;
-        ph.x = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-        ph.y = (uint32_t)__bfloat16_as_ushort(h2) | ((uint32_t)__bfloat16_as_ushort(h3) << 16);
-        pl.x = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-        pl.y = (uint32_t)__bfloat16_as_ushort(l2) | ((uint32_t)__bfloat16_as_ushort(l3) << 16);
-        reinterpret_cast<uint2*>(hi)[i] = ph;
-        reinterpret_cast<uint2*>(lo)[i] = pl;
+        store_split4(hi + 4 * i, lo + 4 * i, x.x, x.y, x.z, x.w);
     }
 }
 
@@ -248,114 +238,12 @@ __global__ void __launch_bounds__(256) dropout_fwd_kernel(int B, int N, int n_lo
     }
 }
 
-// logits layer forward: one warp per example, dot over the concatenated sources
+// input segments of a tower's logits layer
 struct GemvSegs { int n; const float* ptr[kMaxSegs]; int ld[kMaxSegs]; int k[kMaxSegs]; int koff[kMaxSegs]; };
-__global__ void __launch_bounds__(256) logits_fwd_kernel(GemvSegs S, const float* __restrict__ kernel, const float* __restrict__ bias,
-                                                        int B, float* __restrict__ out) {
-    int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    int nw = (gridDim.x * blockDim.x) >> 5;
-    for (int b = warp; b < B; b += nw) {
-        float acc = 0.f;
-        for (int s = 0; s < S.n; ++s) {
-            const float* row = S.ptr[s] + (int64_t)b * S.ld[s];
-            const float* kw = kernel + S.koff[s];
-            for (int k = lane * 4; k < S.k[s]; k += 128) {
-                float4 x = *reinterpret_cast<const float4*>(row + k);
-                float4 w = *reinterpret_cast<const float4*>(kw + k);
-                acc = fmaf(x.x, w.x, acc); acc = fmaf(x.y, w.y, acc); acc = fmaf(x.z, w.z, acc); acc = fmaf(x.w, w.w, acc);
-            }
-        }
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
-        if (lane == 0) out[b] = acc + bias[0];
-    }
-}
 
-// head: logits = wide + sum of towers; per-example loss; dlogit = (sigmoid(x) - y) * w; block partial sums
-struct TowerLogits { int n; const float* p[8]; };
-__global__ void __launch_bounds__(256) head_kernel(int B, const float* __restrict__ wide_logit, TowerLogits T,
-                                                  const float* __restrict__ label, const float* __restrict__ weight,
-                                                  float* __restrict__ logits, float* __restrict__ dlogit, float* __restrict__ loss_part) {
-    __shared__ float red[8];
-    float lsum = 0.f;
-    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < B; b += gridDim.x * blockDim.x) {
-        float x = wide_logit ? wide_logit[b] : 0.f;
-        for (int t = 0; t < T.n; ++t) x += T.p[t][b];
-        logits[b] = x;
-        if (label) {
-            float y = label[b], w = weight ? weight[b] : 1.f;
-            // sigmoid cross entropy with logits: max(x,0) - x*y + log1p(exp(-|x|))   (SURVEY A.10)
-            float l = fmaxf(x, 0.f) - x * y + log1pf(expf(-fabsf(x)));
-            lsum += w * l;
-            if (dlogit) dlogit[b] = (1.f / (1.f + expf(-x)) - y) * w;
-        }
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, d);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = lsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float s = 0.f;
-        for (int i = 0; i < 8; ++i) s += red[i];
-        loss_part[blockIdx.x] = s;
-    }
-}
-__global__ void loss_final_kernel(const float* __restrict__ part, int n, float* out) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) {
-        double s = 0.0;
-        for (int i = 0; i < n; ++i) s += (double)part[i];
-        *out = (float)s;
-    }
-}
-
-// logits layer backward, data part: dsrc[b, k] (+)= dlogit[b] * kernel[koff + k]
-__global__ void logits_dgrad_kernel(int B, int K, const float* __restrict__ dlogit, const float* __restrict__ kw,
-                                    float* __restrict__ dst, int ld, int accumulate) {
-    int64_t total = (int64_t)B * (K / 4);
-    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-        int b = (int)(t / (K / 4)), k = (int)(t % (K / 4)) * 4;
-        float g = dlogit[b];
-        float4 w = *reinterpret_cast<const float4*>(kw + k);
-        float4* d = reinterpret_cast<float4*>(dst + (int64_t)b * ld + k);
-        float4 v = make_float4(g * w.x, g * w.y, g * w.z, g * w.w);
-        if (accumulate) { float4 o = *d; v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w; }
-        *d = v;
-    }
-}
-// logits layer backward, weight part: gpart[rt][koff + k] = sum_{b in row tile} src[b,k] * dlogit[b]; bias likewise
-// block = 64 columns x 4 row groups of 32 rows (one 128-row tile); partial sums combined through shared memory
-__global__ void __launch_bounds__(256) logits_wgrad_kernel(int B, int K, const float* __restrict__ src, int ld,
-                                                          const float* __restrict__ dlogit, float* __restrict__ gpart,
-                                                          int64_t gstride, float* __restrict__ bias_part, int64_t bias_stride) {
-    __shared__ float red[4][64];
-    __shared__ float dl[128];
-    const int rt = blockIdx.y, kx = threadIdx.x & 63, ry = threadIdx.x >> 6;
-    const int k = blockIdx.x * 64 + kx;
-    const int b0 = rt * 128;
-    if (threadIdx.x < 128) dl[threadIdx.x] = (b0 + threadIdx.x < B) ? dlogit[b0 + threadIdx.x] : 0.f;
-    __syncthreads();
-    float acc = 0.f;
-    if (k < K) {
-        const int r0 = b0 + ry * 32;
-#pragma unroll 8
-        for (int i = 0; i < 32; ++i)
-            if (r0 + i < B) acc = fmaf(src[(int64_t)(r0 + i) * ld + k], dl[ry * 32 + i], acc);
-    }
-    red[ry][kx] = acc;
-    __syncthreads();
-    if (ry == 0 && k < K) gpart[(int64_t)rt * gstride + k] = red[0][kx] + red[1][kx] + red[2][kx] + red[3][kx];
-    if (bias_part && blockIdx.x == 0 && threadIdx.x == 0) {
-        float s = 0.f;
-        for (int i = 0; i < 128; ++i) s += dl[i];
-        bias_part[(int64_t)rt * bias_stride] = s;
-    }
-}
-
-// ---- fused head: logits layers of all towers (one warp per example) + wide logit + sigmoid cross entropy + dlogit + the batch
-// loss (block partials, summed in block order by the last block to finish) — one launch instead of logits_fwd per tower, head
-// and loss_final
-constexpr int kFusedTowers = 4;
-struct HeadIn { int n; GemvSegs S[kFusedTowers]; const float* kernel[kFusedTowers]; const float* bias[kFusedTowers]; float* tower_logit[kFusedTowers]; };
+// ---- head: logits layers of all towers (one warp per example) + wide logit + sigmoid cross entropy + dlogit + the batch loss
+// (block partials, summed in block order by the last block to finish), in one launch
+struct HeadIn { int n; GemvSegs S[kMaxTowers]; const float* kernel[kMaxTowers]; const float* bias[kMaxTowers]; float* tower_logit[kMaxTowers]; };
 __global__ void __launch_bounds__(256) logits_head_kernel(HeadIn in, int B, const float* __restrict__ wide_logit, const float* __restrict__ label,
                                                         const float* __restrict__ weight, float* __restrict__ logits, float* __restrict__ dlogit,
                                                         float* __restrict__ loss_part, int32_t* __restrict__ counter, float* __restrict__ loss_out) {
@@ -484,7 +372,7 @@ __global__ void __launch_bounds__(256) act_bn_bwd_kernel(int B, int N, int n_log
                                                         int ld, const float* __restrict__ gamma, int act, int bn,
                                                         float* __restrict__ dZ, float* __restrict__ dZT, int ldt,
                                                         float* __restrict__ p_bias, float* __restrict__ p_gamma, float* __restrict__ p_beta,
-                                                        int64_t pstride, __nv_bfloat16* __restrict__ q_hi, __nv_bfloat16* __restrict__ q_lo, DropArgs dr) {
+                                                        int64_t pstride, DropArgs dr) {
     __shared__ float tile[32][33];
     const unsigned long long dkey = dr.rate > 0.f ? drop_key(dr) : 0ull;
     const float inv_keep = dr.rate > 0.f ? 1.f / (1.f - dr.rate) : 1.f;
@@ -506,16 +394,9 @@ __global__ void __launch_bounds__(256) act_bn_bwd_kernel(int B, int N, int n_log
                 dz = dh * gsc * dm * act_bwd(act, a);
                 sb += dz; sg += dh * (a * dm) * inv; sbe += dh;
             }
-            if (q_hi) {                                           // 3xBF16 engine: the GEMMs read bf16 hi / lo copies only
-                if (mm < B && n < N) {
-                    __nv_bfloat16 h, l;
-                    split_bf16(dz, h, l);
-                    q_hi[(int64_t)mm * ld + n] = h; q_lo[(int64_t)mm * ld + n] = l;
-                }
-            } else if (mm < B && n < N) dZ[(int64_t)mm * ld + n] = dz;
+            if (mm < B && n < N) dZ[(int64_t)mm * ld + n] = dz;
             tile[ty * 4 + i][tx] = dz;
         }
-        if (q_hi) continue;                                       // (uniform) the 3xBF16 engine needs no transposed copy
         __syncthreads();
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -573,15 +454,7 @@ __global__ void __launch_bounds__(256) act_bn_bwd_q_kernel(int B, int N, int n_l
                     sb[j] += dz[j]; sg[j] += dh[j] * (a[j] * dm) * inv; sbe[j] += dh[j];
                 }
             }
-            __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
-            split_bf16(dz[0], h0, l0); split_bf16(dz[1], h1, l1); split_bf16(dz[2], h2, l2); split_bf16(dz[3], h3, l3);
-            uint2 ph, pl;
-            ph.x = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-            ph.y = (uint32_t)__bfloat16_as_ushort(h2) | ((uint32_t)__bfloat16_as_ushort(h3) << 16);
-            pl.x = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-            pl.y = (uint32_t)__bfloat16_as_ushort(l2) | ((uint32_t)__bfloat16_as_ushort(l3) << 16);
-            *reinterpret_cast<uint2*>(q_hi + (int64_t)mm * ld + n0) = ph;
-            *reinterpret_cast<uint2*>(q_lo + (int64_t)mm * ld + n0) = pl;
+            store_split4(q_hi + (int64_t)mm * ld + n0, q_lo + (int64_t)mm * ld + n0, dz[0], dz[1], dz[2], dz[3]);
         }
     }
 #pragma unroll
@@ -647,15 +520,7 @@ __global__ void __launch_bounds__(256) logits_act_bwd_q_kernel(int B, int N, int
                     sb[j] += dz[j]; sg[j] += dh * a[j] * inv; sbe[j] += dh;
                 }
             }
-            __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
-            split_bf16(dz[0], h0, l0); split_bf16(dz[1], h1, l1); split_bf16(dz[2], h2, l2); split_bf16(dz[3], h3, l3);
-            uint2 ph, pl;
-            ph.x = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-            ph.y = (uint32_t)__bfloat16_as_ushort(h2) | ((uint32_t)__bfloat16_as_ushort(h3) << 16);
-            pl.x = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-            pl.y = (uint32_t)__bfloat16_as_ushort(l2) | ((uint32_t)__bfloat16_as_ushort(l3) << 16);
-            *reinterpret_cast<uint2*>(q_hi + (int64_t)mm * ld + n0) = ph;
-            *reinterpret_cast<uint2*>(q_lo + (int64_t)mm * ld + n0) = pl;
+            store_split4(q_hi + (int64_t)mm * ld + n0, q_lo + (int64_t)mm * ld + n0, dz[0], dz[1], dz[2], dz[3]);
         }
     }
 #pragma unroll
@@ -747,7 +612,6 @@ __device__ __forceinline__ void opt_update_d(const OptParamsD& o, float g, float
         w -= o.lr * g;
     }
 }
-// applies the optimizer over the dense arena; kernels also refresh their transposed copy Wt[n][k]
 // hi/lo split of a weight for the 3xTF32 engine (same split the GEMM applies to activations in shared memory)
 __device__ __forceinline__ void store_split(float* __restrict__ Wsplit, int64_t wt_count, int64_t wt_off, int64_t e, int64_t et, float w) {
     float hi = __uint_as_float(__float_as_uint(w) & 0xFFFFE000u), lo = w - hi;
@@ -764,9 +628,11 @@ __device__ __forceinline__ void store_split_bf16(float* __restrict__ Wsplit, int
     q[wt_off + e] = hi;
     q[wt_count + wt_off + e] = lo;
 }
+// applies the optimizer over the dense arena (every engine but 3xBF16); kernels also refresh their transposed copy Wt[n][k] and
+// its hi / lo split
 __global__ void dense_apply_kernel(const DenseTensor* __restrict__ T, int nt, int64_t total, const float* __restrict__ G,
                                    float* __restrict__ P, float* __restrict__ S1, float* __restrict__ S2, float* __restrict__ Wt,
-                                   float* __restrict__ Wsplit, int64_t wt_count, OptParamsD dnn, OptParamsD lin, int lin_tensor, int bf16) {
+                                   float* __restrict__ Wsplit, int64_t wt_count, OptParamsD dnn, OptParamsD lin, int lin_tensor) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         int lo = 0, hi = nt - 1;
         while (lo < hi) {
@@ -781,11 +647,8 @@ __global__ void dense_apply_kernel(const DenseTensor* __restrict__ T, int nt, in
         if (t.wt_off >= 0) {
             int64_t e = i - t.off;
             int k = (int)(e / t.cols), n = (int)(e % t.cols);
-            if (bf16) store_split_bf16(Wsplit, wt_count, t.wt_off, e, w);
-            else {
-                Wt[t.wt_off + (int64_t)n * t.rows + k] = w;
-                store_split(Wsplit, wt_count, t.wt_off, e, (int64_t)n * t.rows + k, w);
-            }
+            Wt[t.wt_off + (int64_t)n * t.rows + k] = w;
+            store_split(Wsplit, wt_count, t.wt_off, e, (int64_t)n * t.rows + k, w);
         }
     }
 }
@@ -854,15 +717,7 @@ __global__ void __launch_bounds__(256) dense_vec_kernel(const DenseTensor* __res
         reinterpret_cast<float4*>(S2)[i4] = s2;
         if (t.wt_off >= 0) {                                              // bf16 hi / lo copies of W [K, N] (what the GEMMs read)
             __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(Wsplit);
-            __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
-            split_bf16(w.x, h0, l0); split_bf16(w.y, h1, l1); split_bf16(w.z, h2, l2); split_bf16(w.w, h3, l3);
-            uint2 ph, pl;
-            ph.x = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-            ph.y = (uint32_t)__bfloat16_as_ushort(h2) | ((uint32_t)__bfloat16_as_ushort(h3) << 16);
-            pl.x = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-            pl.y = (uint32_t)__bfloat16_as_ushort(l2) | ((uint32_t)__bfloat16_as_ushort(l3) << 16);
-            *reinterpret_cast<uint2*>(q + t.wt_off + e) = ph;
-            *reinterpret_cast<uint2*>(q + wt_count + t.wt_off + e) = pl;
+            store_split4(q + t.wt_off + e, q + wt_count + t.wt_off + e, w.x, w.y, w.z, w.w);
         }
     }
 }
@@ -958,19 +813,6 @@ int mlp_forward(WdModel* m, bool train) {
                 m->launches++;
             }
         }
-        Layer& LL = tw.layers[tw.n_hidden];
-        GemvSegs S{};
-        S.n = LL.n_in_segs;
-        for (int s = 0; s < LL.n_in_segs; ++s) {
-            S.ptr[s] = src_ptr(m, tw, LL.segs[s].src, false);
-            S.ld[s] = src_ld(m, tw, LL.segs[s].src, false);
-            S.k[s] = LL.segs[s].width_phys;
-            S.koff[s] = LL.segs[s].k_off;
-        }
-        if ((int)m->towers.size() <= kFusedTowers) continue;            // logits layers run inside the fused head kernel (loss_forward)
-        logits_fwd_kernel<<<grid_for((int64_t)B * 32, 256), 256, 0, m->stream>>>(S, m->d_P + m->dense[LL.t_kernel].off,
-                                                                                m->d_P + m->dense[LL.t_bias].off, B, tw.logit);
-        m->launches++;
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -978,40 +820,28 @@ int mlp_forward(WdModel* m, bool train) {
 
 int loss_forward(WdModel* m, bool need_grad) {
     const int B = m->dbatch.B;
-    const int ntow = m->use_deep ? (int)m->towers.size() : 0;
-    if (ntow <= kFusedTowers) {
-        HeadIn in{};
-        in.n = ntow;
-        for (int t = 0; t < ntow; ++t) {
-            Tower& tw = m->towers[t];
-            Layer& LL = tw.layers[tw.n_hidden];
-            in.S[t].n = LL.n_in_segs;
-            for (int s = 0; s < LL.n_in_segs; ++s) {
-                in.S[t].ptr[s] = src_ptr(m, tw, LL.segs[s].src, false);
-                in.S[t].ld[s] = src_ld(m, tw, LL.segs[s].src, false);
-                in.S[t].k[s] = LL.segs[s].width_phys;
-                in.S[t].koff[s] = LL.segs[s].k_off;
-            }
-            in.kernel[t] = m->d_P + m->dense[LL.t_kernel].off;
-            in.bias[t] = m->d_P + m->dense[LL.t_bias].off;
-            in.tower_logit[t] = tw.logit;
+    const int ntow = m->use_deep ? (int)m->towers.size() : 0;      // <= kMaxTowers (wd_model_create)
+    HeadIn in{};
+    in.n = ntow;
+    for (int t = 0; t < ntow; ++t) {
+        Tower& tw = m->towers[t];
+        Layer& LL = tw.layers[tw.n_hidden];
+        in.S[t].n = LL.n_in_segs;
+        for (int s = 0; s < LL.n_in_segs; ++s) {
+            in.S[t].ptr[s] = src_ptr(m, tw, LL.segs[s].src, false);
+            in.S[t].ld[s] = src_ld(m, tw, LL.segs[s].src, false);
+            in.S[t].k[s] = LL.segs[s].width_phys;
+            in.S[t].koff[s] = LL.segs[s].k_off;
         }
-        const int blocks = grid_for((int64_t)B * 8, 256, 512);           // eight lanes per example (loss_part holds 512 block partials)
-        logits_head_kernel<<<blocks, 256, 0, m->stream>>>(in, B, m->use_wide ? m->d_wide_logit : nullptr, m->batch_has_label ? m->d_label : nullptr,
-                                                         m->dbatch.weight, m->d_logits, need_grad ? m->d_dlogit : nullptr, m->d_loss_part,
-                                                         m->d_head_counter, m->d_loss);
-        m->launches++;
-        WD_CUDA(cudaGetLastError());
-        return WD_OK;
+        in.kernel[t] = m->d_P + m->dense[LL.t_kernel].off;
+        in.bias[t] = m->d_P + m->dense[LL.t_bias].off;
+        in.tower_logit[t] = tw.logit;
     }
-    TowerLogits T{};
-    T.n = m->use_deep ? (int)m->towers.size() : 0;
-    for (int t = 0; t < T.n; ++t) T.p[t] = m->towers[t].logit;
-    int blocks = grid_for(B, 256, 256);
-    head_kernel<<<blocks, 256, 0, m->stream>>>(B, m->use_wide ? m->d_wide_logit : nullptr, T, m->batch_has_label ? m->d_label : nullptr,
-                                              m->dbatch.weight, m->d_logits, need_grad ? m->d_dlogit : nullptr, m->d_loss_part);
-    loss_final_kernel<<<1, 32, 0, m->stream>>>(m->d_loss_part, blocks, m->d_loss);
-    m->launches += 2;
+    const int blocks = grid_for((int64_t)B * 8, 256, 512);               // eight lanes per example (loss_part holds 512 block partials)
+    logits_head_kernel<<<blocks, 256, 0, m->stream>>>(in, B, m->use_wide ? m->d_wide_logit : nullptr, m->batch_has_label ? m->d_label : nullptr,
+                                                     m->dbatch.weight, m->d_logits, need_grad ? m->d_dlogit : nullptr, m->d_loss_part,
+                                                     m->d_head_counter, m->d_loss);
+    m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
@@ -1025,12 +855,6 @@ int mlp_backward(WdModel* m) {
     const bool need_dx0 = !m->tables.empty();
     const bool q = m->gemm_engine == WD_GEMM_BF16X3;
     const __nv_bfloat16* Wq = reinterpret_cast<const __nv_bfloat16*>(m->d_Wsplit);
-    // 3xBF16 engine: a hidden layer read by exactly one later HIDDEN layer (every layer but the last of `simple` towers) gets its
-    // activation / batch-norm backward inside the epilogue of that consumer's data-gradient GEMM (EPI_DACT): its dH is never
-    // stored and act_bn_bwd_q_kernel is not launched for it.  Opt-in (WD_FUSE_DACT=1); the logits-layer fusion below
-    // (logits_act_bwd_q_kernel) is always on.
-    static const bool fuse_dact_on = getenv("WD_FUSE_DACT") ? atoi(getenv("WD_FUSE_DACT")) != 0 : false;
-    static const bool fuse_logits_on = getenv("WD_FUSE_LOGITS_BWD") ? atoi(getenv("WD_FUSE_LOGITS_BWD")) != 0 : true;
     for (auto& tw : m->towers) {
         std::vector<char> written(tw.n_hidden, 0);
         std::vector<int> readers(tw.n_hidden, 0);
@@ -1055,7 +879,9 @@ int mlp_backward(WdModel* m) {
             if (!(sg.src < 0 && !need_dx0)) grad_dst(sg.src, &dst, &dld, &acc);
             // (the first segment of the first tower also leaves the wide bias's gradient partials: both are tile sums of dlogit)
             const bool wb = m->use_wide && s == 0 && &tw == &m->towers.front();
-            if (q && fuse_logits_on && LL.n_in_segs == 1 && sg.src >= 0 && readers[sg.src] == 2 && m->dropout_rate <= 0.f &&
+            // 3xBF16 engine, a hidden layer read by the logits layer alone: its activation / batch-norm backward runs in the same
+            // pass (logits_act_bwd_q_kernel), so its dH is never stored and act_bn_bwd_q_kernel is not launched for it
+            if (q && LL.n_in_segs == 1 && sg.src >= 0 && readers[sg.src] == 2 && m->dropout_rate <= 0.f &&
                 sg.width_phys == tw.layers[sg.src].N_phys) {
                 Layer& S = tw.layers[sg.src];
                 logits_act_bwd_q_kernel<<<dim3((S.N_phys + 63) / 64, rts), 256, 0, m->stream>>>(B, S.N_phys, S.N, src, ld, S.A, S.N_phys, m->d_dlogit,
@@ -1088,7 +914,7 @@ int mlp_backward(WdModel* m) {
             dim3 g((L.N_phys + 31) / 32, rts);
             const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l};
             if (fused[l]) {
-                // dZ and the partials of this layer were written by the data-gradient GEMM of the layer above
+                // dZ and the partials of this layer were written by logits_act_bwd_q_kernel
             } else if (q)
                 act_bn_bwd_q_kernel<<<dim3((L.N_phys + 63) / 64, rts), 256, 0, m->stream>>>(B, L.N_phys, L.N, L.dH, L.A, L.N_phys,
                     L.t_gamma >= 0 ? m->d_P + m->dense[L.t_gamma].off : nullptr, m->activation, m->batch_norm, pb, pg, pbe,
@@ -1096,8 +922,7 @@ int mlp_backward(WdModel* m) {
             else
             act_bn_bwd_kernel<<<g, 256, 0, m->stream>>>(B, L.N_phys, L.N, L.dH, L.A, L.N_phys,
                                                        L.t_gamma >= 0 ? m->d_P + m->dense[L.t_gamma].off : nullptr, m->activation,
-                                                       m->batch_norm, L.dZ, L.dZT, m->ldt, pb, pg, pbe, m->dense[L.t_bias].gstride,
-                                                       q ? L.dZs[0] : nullptr, q ? L.dZs[1] : nullptr, dr);
+                                                       m->batch_norm, L.dZ, L.dZT, m->ldt, pb, pg, pbe, m->dense[L.t_bias].gstride, dr);
             if (!fused[l]) m->launches++;
             // data gradients first: the deep-input gradient dX0 is what the embedding backward waits for, so it is
             // produced before this layer's weight gradients (which then overlap the sparse backward on the side stream)
@@ -1111,21 +936,8 @@ int mlp_backward(WdModel* m) {
                 A2.hi[0] = L.dZs[0]; A2.lo[0] = L.dZs[1];
                 Epi e2{};
                 e2.C = dst; e2.ldc = dld; e2.accumulate = acc;
-                int mode2 = EPI_STORE;
-                if (q && fuse_dact_on && sg.src >= 0 && readers[sg.src] == 1 && m->dropout_rate <= 0.f && sg.width_phys == tw.layers[sg.src].N_phys) {
-                    Layer& S = tw.layers[sg.src];
-                    mode2 = EPI_DACT;
-                    fused[sg.src] = 1;
-                    e2.Aact = S.A; e2.ldh = S.N_phys; e2.Hs_hi = S.dZs[0]; e2.Hs_lo = S.dZs[1];
-                    e2.gamma = S.t_gamma >= 0 ? m->d_P + m->dense[S.t_gamma].off : nullptr;
-                    e2.n_logical = S.N; e2.act = m->activation; e2.bn = m->batch_norm;
-                    e2.p_bias = m->d_gpart + m->dense[S.t_bias].gpart_off;
-                    e2.p_gamma = S.t_gamma >= 0 ? m->d_gpart + m->dense[S.t_gamma].gpart_off : nullptr;
-                    e2.p_beta = S.t_beta >= 0 ? m->d_gpart + m->dense[S.t_beta].gpart_off : nullptr;
-                    e2.pstride = m->dense[S.t_bias].gstride;
-                }
                 const int64_t woff = tkn.wt_off + (int64_t)sg.k_off * L.N_phys;
-                int rc = run_gemm(m, mode2, A2, m->d_P + tkn.off + (int64_t)sg.k_off * L.N_phys, L.N_phys, B, sg.width_phys, e2, 1, 0,
+                int rc = run_gemm(m, EPI_STORE, A2, m->d_P + tkn.off + (int64_t)sg.k_off * L.N_phys, L.N_phys, B, sg.width_phys, e2, 1, 0,
                                   m->d_Wsplit + woff, m->d_Wsplit + m->wt_count + woff, Wq + woff, Wq + m->wt_count + woff);
                 if (rc) return rc;
             }
@@ -1262,7 +1074,7 @@ static int dense_apply_plain(WdModel* m) {
         return WD_OK;
     }
     dense_apply_kernel<<<grid_for(m->dense_count, 256), 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), m->dense_count, m->d_G,
-                                                                            m->d_P, m->d_S1, m->d_S2, m->d_Wt, m->d_Wsplit, m->wt_count, d, l, lin_tensor, m->gemm_engine == WD_GEMM_BF16X3);
+                                                                            m->d_P, m->d_S1, m->d_S2, m->d_Wt, m->d_Wsplit, m->wt_count, d, l, lin_tensor);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;

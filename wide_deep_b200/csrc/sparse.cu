@@ -10,8 +10,6 @@
 // HBM-bound kernels: 16-byte vector loads through the read-only path, several rows in flight per lane
 // group, rows are 16..256 B records {w | optimizer slots} so forward touches one line and backward one
 // contiguous record.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "sparse_dev.cuh"
 
@@ -39,11 +37,9 @@ __global__ void __launch_bounds__(256) wide_fwd_kernel(int B, int C, const int32
 }
 
 // --------------------------------------------------------------------------------------- embedding forward
-// All tables of one width D (G = D/4 lanes per bag, float4 per lane).  Bag = (example b, table k).
-// NARROW: one G-lane group per bag, 32/G bags per warp in flight (single-valued / short bags).
-// WIDE (full warp per bag): the 32/G groups take interleaved ids, then a shuffle tree combines them
-// (long multihot bags).
-template <int G, bool WIDEBAG>
+// All tables of one width D (G = D/4 lanes per bag, float4 per lane).  Bag = (example b, table k).  Long multihot bags: a full
+// warp per bag, the 32/G lane groups take interleaved ids, then a shuffle tree combines them.
+template <int G>
 __global__ void __launch_bounds__(256) emb_pool_fwd_kernel(int B, int C, int ntab, const int32_t* __restrict__ tab_ids,
                                                            float* const* __restrict__ tab_data,
                                                            const int32_t* __restrict__ tab_stride,
@@ -56,85 +52,52 @@ __global__ void __launch_bounds__(256) emb_pool_fwd_kernel(int B, int C, int nta
     const int64_t nbags = (int64_t)B * ntab;
     const int64_t gwarp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarp = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    if (!WIDEBAG) {
-        for (int64_t bag = gwarp * GROUPS + grp; bag < nbags; bag += nwarp * GROUPS) {
-            int b = (int)(bag / ntab), t = tab_ids[bag % ntab];
-            int c = tab_col[t];
-            int s = offs[(int64_t)b * C + c], e = offs[(int64_t)b * C + c + 1];
-            const float* base = tab_data[t] + lig * 4;
-            const int stride = tab_stride[t];
-            const int64_t rb = tab_row_base[t];
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-            int j = s;
-            for (; j + 4 <= e; j += 4) {                         // 4 rows in flight per group
-                float4 v0 = ldg_nc_f4(base + (int64_t)(e_emb[j] - rb) * stride);
-                float4 v1 = ldg_nc_f4(base + (int64_t)(e_emb[j + 1] - rb) * stride);
-                float4 v2 = ldg_nc_f4(base + (int64_t)(e_emb[j + 2] - rb) * stride);
-                float4 v3 = ldg_nc_f4(base + (int64_t)(e_emb[j + 3] - rb) * stride);
-                acc.x += v0.x; acc.y += v0.y; acc.z += v0.z; acc.w += v0.w;
-                acc.x += v1.x; acc.y += v1.y; acc.z += v1.z; acc.w += v1.w;
-                acc.x += v2.x; acc.y += v2.y; acc.z += v2.z; acc.w += v2.w;
-                acc.x += v3.x; acc.y += v3.y; acc.z += v3.z; acc.w += v3.w;
-            }
-            for (; j < e; ++j) {
-                float4 v = ldg_nc_f4(base + (int64_t)(e_emb[j] - rb) * stride);
-                acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-            }
-            int n = e - s;
-            if (n > 1) {
-                float inv = 1.f / (float)n;                      // combiner='mean'
-                acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
-            }
-            *reinterpret_cast<float4*>(X0 + (int64_t)b * ld + tab_x0[t] + lig * 4) = acc;
-        }
-    } else {
-        for (int64_t bag = gwarp; bag < nbags; bag += nwarp) {
-            int b = (int)(bag / ntab), t = tab_ids[bag % ntab];
-            int c = tab_col[t];
-            int s = offs[(int64_t)b * C + c], e = offs[(int64_t)b * C + c + 1];
-            const float* base = tab_data[t] + lig * 4;
-            const int stride = tab_stride[t];
-            const int64_t rb = tab_row_base[t];
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-            // 32 ids of the bag per round trip (one per lane), then the rows of the chunk that belong to this lane group eight at a
-            // time back to back: the chain offsets -> ids -> rows is 2 + ceil(rows / (8 GROUPS)) dependent round trips per 32 ids
-            // instead of one per four rows.  (Sixteen in flight was measured slower: 120 registers -> 2 blocks per SM -> 3.5 waves
-            // of the 8192 bags, 25.6 us against 20 us.)  Group grp still sums rows grp, grp + GROUPS, ... in that order (the result
-            // is bit-identical to the sequential walk).
-            constexpr int STEPS = 32 / GROUPS, RND = STEPS < 8 ? STEPS : 8;
-            for (int j0 = s; j0 < e; j0 += 32) {
-                const int cnt = min(32, e - j0);
-                const uint32_t my = lane < cnt ? e_emb[j0 + lane] : 0u;
+    for (int64_t bag = gwarp; bag < nbags; bag += nwarp) {
+        int b = (int)(bag / ntab), t = tab_ids[bag % ntab];
+        int c = tab_col[t];
+        int s = offs[(int64_t)b * C + c], e = offs[(int64_t)b * C + c + 1];
+        const float* base = tab_data[t] + lig * 4;
+        const int stride = tab_stride[t];
+        const int64_t rb = tab_row_base[t];
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        // 32 ids of the bag per round trip (one per lane), then the rows of the chunk that belong to this lane group eight at a
+        // time back to back: the chain offsets -> ids -> rows is 2 + ceil(rows / (8 GROUPS)) dependent round trips per 32 ids
+        // instead of one per four rows.  (Sixteen in flight was measured slower: 120 registers -> 2 blocks per SM -> 3.5 waves
+        // of the 8192 bags, 25.6 us against 20 us.)  Group grp still sums rows grp, grp + GROUPS, ... in that order (the result
+        // is bit-identical to the sequential walk).
+        constexpr int STEPS = 32 / GROUPS, RND = STEPS < 8 ? STEPS : 8;
+        for (int j0 = s; j0 < e; j0 += 32) {
+            const int cnt = min(32, e - j0);
+            const uint32_t my = lane < cnt ? e_emb[j0 + lane] : 0u;
 #pragma unroll
-                for (int k0 = 0; k0 < STEPS; k0 += RND) {
-                    if (k0 * GROUPS >= cnt) break;
-                    float4 v[RND];
+            for (int k0 = 0; k0 < STEPS; k0 += RND) {
+                if (k0 * GROUPS >= cnt) break;
+                float4 v[RND];
 #pragma unroll
-                    for (int u = 0; u < RND; ++u) {
-                        const int r = (k0 + u) * GROUPS + grp;
-                        const uint32_t id = __shfl_sync(0xffffffffu, my, r & 31);
-                        v[u] = r < cnt ? ldg_nc_f4(base + (int64_t)(id - rb) * stride) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
+                for (int u = 0; u < RND; ++u) {
+                    const int r = (k0 + u) * GROUPS + grp;
+                    const uint32_t id = __shfl_sync(0xffffffffu, my, r & 31);
+                    v[u] = r < cnt ? ldg_nc_f4(base + (int64_t)(id - rb) * stride) : make_float4(0.f, 0.f, 0.f, 0.f);
+                }
 #pragma unroll
-                    for (int u = 0; u < RND; ++u) {
-                        if ((k0 + u) * GROUPS + grp < cnt) { acc.x += v[u].x; acc.y += v[u].y; acc.z += v[u].z; acc.w += v[u].w; }
-                    }
+                for (int u = 0; u < RND; ++u) {
+                    if ((k0 + u) * GROUPS + grp < cnt) { acc.x += v[u].x; acc.y += v[u].y; acc.z += v[u].z; acc.w += v[u].w; }
                 }
             }
-#pragma unroll
-            for (int d = G; d < 32; d <<= 1) {                  // segmented (per lane-in-group) shuffle reduction
-                acc.x += __shfl_xor_sync(0xffffffffu, acc.x, d);
-                acc.y += __shfl_xor_sync(0xffffffffu, acc.y, d);
-                acc.z += __shfl_xor_sync(0xffffffffu, acc.z, d);
-                acc.w += __shfl_xor_sync(0xffffffffu, acc.w, d);
-            }
-            int n = e - s;
-            if (n > 1) {
-                float inv = 1.f / (float)n;
-                acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
-            }
-            if (grp == 0) *reinterpret_cast<float4*>(X0 + (int64_t)b * ld + tab_x0[t] + lig * 4) = acc;
         }
+#pragma unroll
+        for (int d = G; d < 32; d <<= 1) {                  // segmented (per lane-in-group) shuffle reduction
+            acc.x += __shfl_xor_sync(0xffffffffu, acc.x, d);
+            acc.y += __shfl_xor_sync(0xffffffffu, acc.y, d);
+            acc.z += __shfl_xor_sync(0xffffffffu, acc.z, d);
+            acc.w += __shfl_xor_sync(0xffffffffu, acc.w, d);
+        }
+        int n = e - s;
+        if (n > 1) {
+            float inv = 1.f / (float)n;
+            acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
+        }
+        if (grp == 0) *reinterpret_cast<float4*>(X0 + (int64_t)b * ld + tab_x0[t] + lig * 4) = acc;
     }
 }
 
@@ -189,184 +152,20 @@ __global__ void __launch_bounds__(256, 4) emb_pool_fwd_rows_kernel(int B, int C,
     }
 }
 
-// --------------------------------------------------------------------------------- TMA-staged gather (short bags)
-// Warp per example, rows staged in shared memory by 1-D TMA bulk copies (cp.async.bulk.shared::cluster.global with
-// mbarrier complete_tx): every lane issues the copies of "its" table's rows, so a warp has the whole example (e.g.
-// 26 x 128 B) in flight with a handful of instructions and no registers tied up; a ring of NBUF staging buffers per
-// warp keeps several examples in flight.  Single-valued bags whose columns are adjacent in the deep input (the
-// Criteo shape) are written back with ONE bulk store (cp.async.bulk.global.shared::cta) straight from the staging
-// buffer; otherwise lane groups pool the staged rows (mean) and store float4s.
-__device__ __forceinline__ uint32_t sm_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(sm_u32(dst)), "l"(src), "r"(bytes), "r"(sm_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void bulk_s2g(void* dst, const void* src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(sm_u32(src)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_parity(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "W_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra W_DONE;\n\t"
-        "bra W_LOOP;\n\t"
-        "W_DONE:\n\t}" ::"r"(sm_u32(bar)), "r"(parity) : "memory");
-}
-
-template <int G>
-__global__ void __launch_bounds__(256) emb_pool_fwd_tma_kernel(int B, int C, int ntab, const TabDesc* __restrict__ desc,
-                                                               const int32_t* __restrict__ offs, const uint32_t* __restrict__ e_emb,
-                                                               float* __restrict__ X0, int ld, int buf_bytes, int nbuf, int contiguous) {
-    extern __shared__ __align__(128) uint8_t tsm[];
-    constexpr int ROWB = G * 16;                         // bytes per embedding row
-    constexpr int GROUPS = 32 / G;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int slots = buf_bytes / ROWB;
-    uint8_t* wbase = tsm + (size_t)warp * nbuf * buf_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(tsm + (size_t)8 * nbuf * buf_bytes) + warp * 8;      // up to 8 buffers per warp
-    if (lane == 0)
-        for (int i = 0; i < nbuf; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sm_u32(&bars[i])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
-    const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarp = (gridDim.x * blockDim.x) >> 5;
-    const int nex = gwarp < B ? (B - gwarp + nwarp - 1) / nwarp : 0;   // examples of this warp
-
-    // per-lane state of an in-flight example (tables lane, lane+32, ... only the first 32 tables use the TMA path)
-    auto issue = [&](int i) -> int {                 // stage example i of this warp; returns total entries (or -1: too many)
-        const int b = gwarp + i * nwarp;
-        const int buf = i % nbuf;
-        const int32_t* orow = offs + (int64_t)b * C;
-        int s = 0, n = 0;
-        TabDesc d{};
-        if (lane < ntab) { d = desc[lane]; s = orow[d.col]; n = orow[d.col + 1] - s; }
-        int pos = n;                                   // exclusive prefix of n over lanes
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, pos, o); if (lane >= o) pos += t; }
-        const int total = __shfl_sync(0xffffffffu, pos, 31);
-        pos -= n;
-        if (total > slots) {                           // does not fit the staging buffer: keep the barrier phase in step, drain with direct loads
-            if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sm_u32(&bars[buf])), "r"(0u) : "memory");
-            return -1;
-        }
-        uint8_t* bbase = wbase + (size_t)buf * buf_bytes;
-        for (int j = 0; j < n; ++j) {
-            const float* src = d.data + (int64_t)(e_emb[s + j] - d.row_base) * d.stride;
-            bulk_g2s(bbase + (size_t)(pos + j) * ROWB, src, ROWB, &bars[buf]);
-        }
-        if (lane == 0)
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sm_u32(&bars[buf])), "r"((uint32_t)(total * ROWB)) : "memory");
-        return total;
-    };
-
-    const int depth = nbuf - 1 > 0 ? nbuf - 1 : 1;      // examples in flight ahead of the one being drained
-    for (int i = 0; i < nex && i < depth; ++i) {
-        if (issue(i) < 0) { /* handled when drained (falls back to direct loads) */ }
-    }
-    for (int i = 0; i < nex; ++i) {
-        const int b = gwarp + i * nwarp;
-        const int buf = i % nbuf;
-        const int32_t* orow = offs + (int64_t)b * C;
-        float* xrow = X0 + (int64_t)b * ld;
-        // recompute this example's layout (cheap, L1/L2 hits) instead of carrying it across the pipeline
-        int s = 0, n = 0;
-        TabDesc d{};
-        if (lane < ntab) { d = desc[lane]; s = orow[d.col]; n = orow[d.col + 1] - s; }
-        int pos = n;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, pos, o); if (lane >= o) pos += t; }
-        const int total = __shfl_sync(0xffffffffu, pos, 31);
-        pos -= n;
-        const bool staged = total <= slots;
-        uint8_t* bbase = wbase + (size_t)buf * buf_bytes;
-        mbar_wait_parity(&bars[buf], (uint32_t)((i / nbuf) & 1));
-        const bool all_single = __all_sync(0xffffffffu, lane >= ntab || n == 1);
-        if (staged && all_single && contiguous) {
-            // the staging buffer already is the example's slice of the deep input
-            if (lane == 0) {
-                bulk_s2g(xrow + desc[0].x0, bbase, (uint32_t)(ntab * ROWB));
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-        } else {
-            const int lig = lane % G, grp = lane / G;
-            for (int k0 = 0; k0 < ntab; k0 += GROUPS) {
-                const int k = k0 + grp;
-                const int kk = k < ntab ? k : 0;
-                const int pk = __shfl_sync(0xffffffffu, pos, kk), nk = __shfl_sync(0xffffffffu, n, kk), sk = __shfl_sync(0xffffffffu, s, kk);
-                if (k < ntab) {
-                    const TabDesc dk = desc[k];
-                    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-                    for (int j = 0; j < nk; ++j) {
-                        float4 v = staged ? *reinterpret_cast<const float4*>(bbase + (size_t)(pk + j) * ROWB + lig * 16)
-                                          : ldg_nc_f4(dk.data + (int64_t)(e_emb[sk + j] - dk.row_base) * dk.stride + lig * 4);
-                        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-                    }
-                    if (nk > 1) { const float inv = 1.f / (float)nk; acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv; }
-                    *reinterpret_cast<float4*>(xrow + dk.x0 + lig * 4) = acc;
-                }
-            }
-        }
-        __syncwarp();
-        // refill: example i + depth goes into buffer (i + depth) % nbuf == the buffer drained one iteration ago (or this
-        // one when nbuf == depth + 1 ... ) -> wait until its bulk store has finished reading shared memory
-        const int nxt = i + depth;
-        if (nxt < nex) {
-            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            __syncwarp();
-            issue(nxt);
-        }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-
 template <int G>
 static void launch_emb_fwd(WdModel* m, int di, bool widebag) {
-    int ntab = m->dim_ntables[di];
-    static const int gather_mode = getenv("WD_GATHER") ? atoi(getenv("WD_GATHER")) : 0;     // 0: LDG kernel (default: measured faster), 1: TMA-staged kernel
-    if (!widebag && gather_mode == 1 && ntab <= 32) {
-        const int rowb = G * 16;
-        int buf_bytes = ((ntab * rowb * 5 / 4 + 1023) / 1024) * 1024;             // 25% head-room for multihot bags (larger ones use direct loads)
-        if (buf_bytes < 1024) buf_bytes = 1024;
-        int nbuf = 2;                                  // two staging buffers per warp: ~3 blocks (24 warps) per SM at 5 KB buffers
-        if (nbuf >= 2) {
-            // tables of this width adjacent in the deep input, in descriptor order?  (host check once per model would do; cheap here)
-            int contiguous = 1;
-            int prev = -1;
-            for (auto& tb : m->tables)
-                if (tb.dim == m->dims[di]) {
-                    if (prev >= 0 && tb.x0_off != prev + tb.dim) contiguous = 0;
-                    prev = tb.x0_off;
-                }
-            size_t smem = (size_t)8 * nbuf * buf_bytes + 8 * 8 * sizeof(uint64_t);
-            static bool configured[wd::kMaxDims] = {false};
-            if (!configured[di]) {
-                cudaFuncSetAttribute(emb_pool_fwd_tma_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                configured[di] = true;
-            }
-            int grid = grid_for((int64_t)m->dbatch.B * 32, 256, kNumSms * 3);
-            emb_pool_fwd_tma_kernel<G><<<grid, 256, smem, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_desc[di], m->d_col_offs, m->d_e_emb,
-                                                                   m->d_X0, m->d0_phys, buf_bytes, nbuf, contiguous);
-            m->launches++;
-            return;
-        }
-    }
+    const int ntab = m->dim_ntables[di];
     if (!widebag) {
         constexpr int RMAX = 4;                       // 4 rounds in flight per lane group at <= 64 registers: 32 warps per SM
         int grid = grid_for((int64_t)m->dbatch.B * 32, 256, kNumSms * 8);
         emb_pool_fwd_rows_kernel<G, RMAX><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_desc[di], m->d_col_offs,
                                                                         m->d_e_emb, m->d_X0, m->d0_phys);
-        m->launches++;
-        return;
+    } else {
+        const int64_t nbags = (int64_t)m->dbatch.B * ntab;            // one warp per bag
+        int grid = grid_for(nbags * 32, 256, kNumSms * 8);
+        emb_pool_fwd_kernel<G><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_tables[di],
+            m->d_tab_data, m->d_tab_stride, m->d_tab_x0, m->d_tab_col, m->d_tab_row_base, m->d_col_offs, m->d_e_emb, m->d_X0, m->d0_phys);
     }
-    int64_t nbags = (int64_t)m->dbatch.B * ntab;
-    int64_t warps = widebag ? nbags : (nbags + (32 / G) - 1) / (32 / G);
-    int grid = grid_for(warps * 32, 256, kNumSms * 8);
-    if (widebag)
-        emb_pool_fwd_kernel<G, true><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_tables[di],
-            m->d_tab_data, m->d_tab_stride, m->d_tab_x0, m->d_tab_col, m->d_tab_row_base, m->d_col_offs, m->d_e_emb, m->d_X0, m->d0_phys);
-    else
-        emb_pool_fwd_kernel<G, false><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_tables[di],
-            m->d_tab_data, m->d_tab_stride, m->d_tab_x0, m->d_tab_col, m->d_tab_row_base, m->d_col_offs, m->d_e_emb, m->d_X0, m->d0_phys);
     m->launches++;
 }
 
@@ -817,8 +616,7 @@ int sparse_group(WdModel* m) {
 // but Adam, whose moments decay over whole tables): the rows are updated inside these two launches and sparse_apply_which has
 // nothing left to launch for the list (m->list_apply_fused).
 static bool fuse_row_apply(const WdModel* m, const WdOptimizer& o) {
-    static const bool no_fuse = getenv("WD_NO_FUSED_ROW_APPLY") != nullptr;              // A/B switch (bench only)
-    return m->fuse_dense && o.kind != WD_OPT_ADAM && m->gs_count == 0 && !no_fuse;
+    return m->fuse_dense && o.kind != WD_OPT_ADAM && m->gs_count == 0;
 }
 int sparse_reduce_emb(WdModel* m) {
     const int g = grid_for(m->max_nnz, 256);
