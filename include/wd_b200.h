@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define WD_API_VERSION 2
+#define WD_API_VERSION 3
 
 enum { WD_OK = 0, WD_EINVAL = -1, WD_ENODEVICE = -2, WD_ECUDA = -3, WD_ENOMEM = -4, WD_EUNSUPPORTED = -5, WD_ESTATE = -6 };
 
@@ -48,6 +48,9 @@ enum { WD_MODE_SIMPLE = 0, WD_MODE_FIRST_DENSE, WD_MODE_LAST_DENSE, WD_MODE_DENS
 enum { WD_GEMM_AUTO = 0, WD_GEMM_FFMA = 1, WD_GEMM_TC3X = 2 /* wgmma tf32, 3-pass split */,
        WD_GEMM_TC1X = 3 /* wgmma tf32 single pass: fast, NOT within the 1e-4 parity bar */,
        WD_GEMM_BF16X3 = 4 /* wgmma on bf16 hi/lo copies written by the producing kernels, 3 passes */ };
+/* where an embedding table's records live (WdPlanDesc::table_placement) */
+enum { WD_PLACE_HBM = 0, WD_PLACE_HOST = 1 /* mapped, page-locked host memory */,
+       WD_PLACE_AUTO = 2 /* HBM if it fits, else host memory (resolved once by wd_model_create) */ };
 
 typedef struct WdOptimizer {
     int32_t kind;        /* WD_OPT_* */
@@ -128,6 +131,15 @@ typedef struct WdPlanDesc {
      * csrc/gemm.cuh — so runs are reproducible and the oracle can apply the same mask; 0 = no dropout. */
     float dropout_rate;
     uint64_t dropout_seed;
+    /* Embedding-table placement, [n_tables] WD_PLACE_* (NULL: every table in HBM).  The reference keeps its tables in host RAM:
+     * it trains on the CPU or spreads them over parameter servers (reference python/lib/build_estimator.py:211-214,
+     * python/lib/joint.py:141-143).  A host-placed table keeps its [w | slots] records in mapped, page-locked host memory; every
+     * step copies the records of the rows it touches into an HBM staging buffer, runs the same kernels on them and writes them
+     * back, so results are bit-identical to the table in HBM.  WD_PLACE_AUTO: wd_model_create allocates the auto tables largest
+     * first and moves to host memory only a table whose HBM allocation fails (with room kept for the buffers allocated after
+     * creation).  Host placement is refused (WD_EUNSUPPORTED) with shard_world > 1, dense_exchange_max_rows > 0 or Adam as the
+     * dnn optimizer; auto tables stay in HBM in those cases. */
+    const uint8_t *table_placement;
 } WdPlanDesc;
 
 /* One batch in HOST memory (pinned for async copies).  Replaces the feature dict produced by input_fn
@@ -165,6 +177,10 @@ int wd_set_opt_step(WdModel *m, int64_t steps);
  * (Adagrad: acc; FTRL: n, z).  Logical (unpadded) shapes; kernels are [in, out] like tf.layers.dense. */
 int wd_tensor_io(WdModel *m, int kind, int index, int sub, int slot, void *host, int64_t count, int to_device);
 int64_t wd_tensor_size(WdModel *m, int kind, int index, int sub);
+/* Memory the model holds: device_bytes = HBM it allocated, host_bytes = page-locked host memory of its host-placed embedding
+ * tables (WdPlanDesc::table_placement).  Either pointer may be NULL.  (The reference's parameters sit in host RAM on the CPU
+ * or on the parameter servers, reference python/lib/build_estimator.py:211-214.) */
+int wd_memory_usage(WdModel *m, int64_t *device_bytes, int64_t *host_bytes);
 
 /* One training step: H2D copy, ids, forward, loss, backward, optimizers.  Replaces one
  * sess.run(train_op) of Estimator.train (reference python/train.py:128-133; joint.py:224-262).

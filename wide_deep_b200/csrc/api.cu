@@ -119,6 +119,7 @@ extern "C" int wd_model_destroy(WdModel* m) {
     for (auto& g : m->merge_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (m->ev_bwd_done) cudaEventDestroy(m->ev_bwd_done);
     for (void* p : m->allocs) cudaFree(p);
+    for (void* p : m->host_allocs) cudaFreeHost(p);
     if (m->h_loss_pinned) cudaFreeHost(m->h_loss_pinned);
     for (auto& e : m->timer.ev) if (e) cudaEventDestroy(e);
     if (m->shard.aux) { cudaStreamSynchronize(m->shard.aux); cudaStreamDestroy(m->shard.aux); }
@@ -301,7 +302,9 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             if (tb.dim % 4 || tb.x0_off % 4) { set_error("table %d: dim and deep-input offset must be multiples of 4", t); return WD_EINVAL; }
             for (int c = 0; c < C; ++c) if (d->col_emb_table[c] == t) tb.col = c;
             if (tb.col < 0) { set_error("table %d has no producing column", t); return WD_EINVAL; }
-            if ((rc = dev_alloc(m, &tb.data, tb.arows * tb.stride, true))) return rc;
+            tb.place = d->table_placement ? d->table_placement[t] : WD_PLACE_HBM;
+            if (tb.place < WD_PLACE_HBM || tb.place > WD_PLACE_AUTO) { set_error("table %d: placement %d is not a WD_PLACE_*", t, tb.place); return WD_EINVAL; }
+            tb.data = nullptr;                                       // allocated by place_tables, after every other buffer of the model
             for (int i = 0; i < tb.dim_logical; ++i) x->x0_real[tb.x0_off + i] = 1;
             m->emb_max_dim = std::max(m->emb_max_dim, tb.dim);
             m->tables.push_back(tb);
@@ -333,6 +336,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             }
             m->gs_emb_floats = off;
             m->n_rtab = (int)row_order.size();
+            m->rtab_order = row_order;
             { const int64_t* t_; if ((rc = upload_vec(m, rb.data(), m->n_rtab, &t_))) return rc; m->d_rtab_row_base = (int64_t*)t_; }
             { const int64_t* t_; if ((rc = upload_vec(m, go.data(), m->n_rtab, &t_))) return rc; m->d_rtab_gs_off = (int64_t*)t_; }
             { float* const* t_; if ((rc = upload_vec<float*>(m, dt.data(), m->n_rtab, (float* const**)&t_))) return rc; m->d_rtab_data = (float**)t_; }
@@ -515,6 +519,21 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     }
     m->sort_hist_cap = 1024 * ((m->max_nnz + kSortTile - 1) / kSortTile + 1) + 4 * 1024 + 64;
     for (int k = 0; k < 4; ++k) if ((rc = dev_alloc(m, &m->d_sort_hist_s[k], m->sort_hist_cap))) return rc;
+    if (m->use_deep) {
+        // Embedding tables come last, so an auto-placed table competes only with what is allocated after wd_model_create returns.
+        // HBM kept free while the auto tables are allocated (see ensure_slot, place_tables and the step graphs):
+        //   kReserveSlots batch slots beyond slot 0 (cat offsets, keys, dense, label, weight each; bench.py and the estimator use
+        //   at most 10),
+        //   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table) and their descriptors,
+        //   kGraphReserve for the instantiated step graphs (one train and one backward graph per slot) and the runtime's growth.
+        constexpr int kReserveSlots = 16;
+        constexpr int64_t kGraphReserve = 256ll << 20;
+        const int64_t slot_bytes = (Bm * std::max(d->n_cat_fields, 1) + 1) * 4 + m->keys_cap * 8 + Bm * std::max(d->n_dense_fields, 1) * 4 + 2 * Bm * 4;
+        int max_stride = 0;
+        for (auto& tb : m->tables) max_stride = std::max(max_stride, tb.stride);
+        const int64_t stage_bytes = m->max_nnz * ((int64_t)max_stride + 1) * 4 + 64 * (int64_t)m->tables.size() + 4096;
+        if ((rc = place_tables(m, kReserveSlots * slot_bytes + stage_bytes + kGraphReserve))) return rc;
+    }
     if (G > 1) {
         if ((rc = shard_build(m, d))) return rc;
         DevPlan& dp = m->dplan;
@@ -651,6 +670,13 @@ extern "C" int64_t wd_tensor_size(WdModel* m, int kind, int index, int sub) {
     return WD_EINVAL;
 }
 
+extern "C" int wd_memory_usage(WdModel* m, int64_t* device_bytes, int64_t* host_bytes) {
+    if (!m) { set_error("null model"); return WD_EINVAL; }
+    if (device_bytes) *device_bytes = m->bytes_allocated;
+    if (host_bytes) *host_bytes = m->host_bytes;
+    return WD_OK;
+}
+
 extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, void* host, int64_t count, int to_device) {
     if (!m || !host) { set_error("null argument"); return WD_EINVAL; }
     WD_CUDA(cudaSetDevice(m->device));
@@ -675,6 +701,7 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         if (slot * tb.dim >= tb.stride) { set_error("table has no optimizer slot %d", slot); return WD_EINVAL; }
         float* dev = tb.data + slot * tb.dim;
         const size_t lw = (size_t)tb.dim_logical * 4;
+        const cudaMemcpyKind dir = tb.host ? cudaMemcpyDefault : (to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost);
         if (to_device) WD_CUDA(cudaMemcpy2DAsync(dev, (size_t)tb.stride * 4, host, lw, lw, tb.arows, dir, m->stream));
         else WD_CUDA(cudaMemcpy2DAsync(host, lw, dev, (size_t)tb.stride * 4, lw, tb.arows, dir, m->stream));
         WD_CUDA(cudaStreamSynchronize(m->stream));
@@ -942,6 +969,13 @@ static int forward_core(WdModel* m, bool train) {
     }
     if (train && (rc = group_async(m))) return rc;
     if (!wide_aside && (rc = sparse_forward_wide(m))) return rc;
+    if (m->n_host_tab > 0) {
+        // host tables: the gather reads the step's unique host rows from the staging buffer, so the embedding list is grouped first
+        // (on side stream 0 when the train step put it there, else here; the backward then groups it once more only when profiling)
+        if (m->side_pending[0]) WD_CUDA(cudaStreamWaitEvent(m->stream, m->ev_grouped[0], 0));
+        else if ((rc = sparse_group_which(m, 0))) return rc;
+        if ((rc = host_tables_stage_in(m))) return rc;
+    }
     if ((rc = sparse_forward_emb(m))) return rc;
     stamp(m, ST_GATHER);
     if ((rc = mlp_forward(m, train))) return rc;

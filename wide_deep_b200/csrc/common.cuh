@@ -85,6 +85,8 @@ struct EmbTable {
     int stride;              // dim * (1 + nslots)
     bool sharded;            // row-sharded over the ranks: this rank holds rows r with r mod G == rank at local index r / G
     int64_t arows;           // rows allocated on this rank (= rows unless sharded); row_base then counts in the shard's row space
+    int place;               // requested placement WD_PLACE_*
+    bool host;               // records live in mapped page-locked host memory (staged through HBM every step, host_tables.cu)
 };
 
 struct TabDesc {            // per-table descriptor grouped by width (one 32-byte load in the gather kernels)
@@ -289,6 +291,22 @@ struct WdModel {
     wd::DevPlan dplan{};
     std::vector<void*> allocs;               // everything cudaMalloc'ed (freed in destroy)
     int64_t bytes_allocated = 0;
+    // ---- host-placed embedding tables (host_tables.cu)
+    std::vector<void*> host_allocs;          // cudaHostAlloc'ed table records (freed in destroy)
+    int64_t host_bytes = 0;
+    int n_host_tab = 0;
+    std::vector<int> rtab_order;             // table ids in global row order (the d_rtab_* arrays)
+    float* d_stage = nullptr;                // [max_nnz][stage_stride] records of the step's unique host rows, row u at u * stage_stride
+    int stage_stride = 0;                    // largest stride of the host tables
+    uint32_t* d_g_emb = nullptr;             // [max_nnz] ids the gather reads: e_emb, host-table entries replaced by their unique index u
+    // what the gather kernels and the fused row updates address: the tables' own arrays, or for host tables the staging buffer
+    // (data = d_stage, row base 0, stride stage_stride); all alias the arrays above when no table is on the host
+    float** d_gtab_data = nullptr;           // [n_tables] data (gather, RowApply)
+    int32_t* d_gtab_stride = nullptr;        // [n_tables] stride (gather)
+    int64_t* d_gtab_row_base = nullptr;      // [n_tables] row base (gather)
+    int32_t* d_tab_stage = nullptr;          // [n_tables] 0: record in place; stage_stride: staged (RowApply); null without host tables
+    float** d_rtab_gdata = nullptr;          // [n_rtab] data in row order, d_stage for host tables (HotApply)
+    int32_t* d_rtab_stage = nullptr;         // [n_rtab] 0 / stage_stride in row order (HotApply, stage-in / write-back); null without host tables
 
     // numeric deep columns (device arrays)
     int32_t *d_num_field = nullptr, *d_num_norm_kind = nullptr, *d_num_x0_off = nullptr;
@@ -416,6 +434,9 @@ int loss_forward(WdModel* m, bool need_grad);                    // mlp.cu: logi
 int model_init_params(WdModel* m, uint64_t seed);                // init.cu
 int step_tick(WdModel* m);                                       // misc.cu: train-step counter on the device (dropout)
 int adam_tick(WdModel* m);                                       // misc.cu: beta powers advance (after every optimizer of the step)
+int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host), descriptors
+int host_tables_stage_in(WdModel* m);                            // host_tables.cu: host rows -> staging buffer, gather ids
+int host_tables_write_back(WdModel* m);                          // host_tables.cu: staging buffer -> host rows
 int metrics_accumulate(WdModel* m);                              // metrics.cu
 int metrics_finish(WdModel* m, double* out10);
 

@@ -159,12 +159,12 @@ static void launch_emb_fwd(WdModel* m, int di, bool widebag) {
         constexpr int RMAX = 4;                       // 4 rounds in flight per lane group at <= 64 registers: 32 warps per SM
         int grid = grid_for((int64_t)m->dbatch.B * 32, 256, kNumSms * 8);
         emb_pool_fwd_rows_kernel<G, RMAX><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_desc[di], m->d_col_offs,
-                                                                        m->d_e_emb, m->d_X0, m->d0_phys);
+                                                                        m->d_g_emb, m->d_X0, m->d0_phys);
     } else {
         const int64_t nbags = (int64_t)m->dbatch.B * ntab;            // one warp per bag
         int grid = grid_for(nbags * 32, 256, kNumSms * 8);
         emb_pool_fwd_kernel<G><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_tables[di],
-            m->d_tab_data, m->d_tab_stride, m->d_tab_x0, m->d_tab_col, m->d_tab_row_base, m->d_col_offs, m->d_e_emb, m->d_X0, m->d0_phys);
+            m->d_gtab_data, m->d_gtab_stride, m->d_tab_x0, m->d_tab_col, m->d_gtab_row_base, m->d_col_offs, m->d_g_emb, m->d_X0, m->d0_phys);
     }
     m->launches++;
 }
@@ -234,7 +234,10 @@ __global__ void sort_keys_kernel(const int32_t* __restrict__ d_nnz, const uint32
 // the hot rows (summed into cpart, combined afterwards by chunk_combine_kernel).
 // APPLY (single-GPU step, row-local optimizer): the optimizer update of a directly summed row follows its sum in the same thread —
 // the summed gradient never reaches memory; the hot rows are updated by chunk_combine_kernel<1>.
-struct RowApply { const uint32_t* urow; float* const* tab_data; const int32_t* tab_stride; const int64_t* tab_row_base; OptParams o; };
+// tab_stage (null without host tables): per table 0 = record in place, else the table is staged — the record of unique row `it`
+// is at tab_data[t] (the staging buffer) + it * tab_stage[t].
+struct RowApply { const uint32_t* urow; float* const* tab_data; const int32_t* tab_stride; const int64_t* tab_row_base; OptParams o;
+                  const int32_t* tab_stage; };
 template <bool APPLY>
 __global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ d_nchunks,
                                                            const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff,
@@ -293,7 +296,8 @@ __global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __rest
             if (APPLY && direct) {
                 if (q * 4 < dim) {
                     const int stride = ra.tab_stride[t];
-                    float* rec = ra.tab_data[t] + ((int64_t)ra.urow[it] - ra.tab_row_base[t]) * stride;
+                    const int sst = ra.tab_stage ? ra.tab_stage[t] : 0;
+                    float* rec = ra.tab_data[t] + (sst ? it * sst : ((int64_t)ra.urow[it] - ra.tab_row_base[t]) * stride);
                     const int nslots = stride / dim - 1;
                     float4 w = *reinterpret_cast<float4*>(rec + q * 4);
                     float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + q * 4) : make_float4(0, 0, 0, 0);
@@ -325,6 +329,7 @@ struct HotApply {
     const uint32_t* urow; int ntab; const int64_t* tab_row_base; float* const* tab_data; const int32_t* tab_dim; const int32_t* tab_stride;   // KIND 1 (tables in row order)
     float4* wide;                                                                                                                          // KIND 2
     OptParams o;
+    const int32_t* tab_stage;     // KIND 1, as RowApply::tab_stage (tables in row order): staged record of unique row uu at tab_data + uu * tab_stage
 };
 template <int KIND>
 __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ choff,
@@ -377,7 +382,8 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
                         }
                         const int dim = ha.tab_dim[lo], stride = ha.tab_stride[lo];
                         if (lq * 4 < dim) {
-                            float* rec = ha.tab_data[lo] + (row - ha.tab_row_base[lo]) * stride;
+                            const int sst = ha.tab_stage ? ha.tab_stage[lo] : 0;
+                            float* rec = ha.tab_data[lo] + (sst ? uu * sst : (row - ha.tab_row_base[lo]) * stride);
                             const int nslots = stride / dim - 1;
                             float4 w = *reinterpret_cast<float4*>(rec + lq * 4);
                             float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + lq * 4) : make_float4(0, 0, 0, 0);
@@ -625,8 +631,10 @@ int sparse_reduce_emb(WdModel* m) {
         const int ge = grid_for((m->max_nnz + m->cpart_cap) * 8, 256);
         // the hot rows' update lives in the lane-group branch of chunk_combine_kernel: widths 4, 8, ..., 128
         const bool fused = fuse_row_apply(m, m->dnn_opt) && width >= 4 && (G4 & (G4 - 1)) == 0 && G4 <= 32;
-        const RowApply ra{m->d_urow[0], m->d_tab_data, m->d_tab_stride, m->d_tab_row_base, make_opt(m->dnn_opt)};
-        const HotApply ha{m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride, nullptr, make_opt(m->dnn_opt)};
+        // (host tables: the fused updates go to the staged records, host_tables_write_back copies them home after the list's apply)
+        const RowApply ra{m->d_urow[0], m->d_gtab_data, m->d_tab_stride, m->d_tab_row_base, make_opt(m->dnn_opt), m->d_tab_stage};
+        const HotApply ha{m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_gdata, m->d_rtab_dim, m->d_rtab_stride, nullptr, make_opt(m->dnn_opt),
+                          m->d_rtab_stage};
         if (fused) {
             emb_grad_sum_kernel<true><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], m->d_sv[0],
                 m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->d_tab_dim, m->d_tab_x0, m->d_dX0, m->d0_phys, m->d_ugrad[0], m->d_cpart[0], width, ra);
@@ -830,7 +838,9 @@ int sparse_apply_which(WdModel* m, int which) {
     // rows already updated by the gradient-sum / combine launches of this step (single-GPU step), unless a caller replaced the list since
     const bool done = m->list_apply_fused[which] && !m->sparse_overridden[which];
     m->list_apply_fused[which] = false;
-    if (done) return WD_OK;
+    // the fused updates of host-table rows went to their staged copies: copy those home (the unfused kernels below update host
+    // records in place, through the mapped pointers of d_rtab_data)
+    if (done) return (which == 0 && m->n_host_tab > 0) ? host_tables_write_back(m) : WD_OK;
     if (which == 0 && m->use_deep && !m->tables.empty()) {
         const bool adam = m->dnn_opt.kind == WD_OPT_ADAM;
         if (adam && (rc = adam_dense_pass(m, 0, false))) return rc;

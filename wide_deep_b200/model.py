@@ -99,6 +99,12 @@ class WideDeepModel(object):
     def tensor_names(self):
         return list(self.plan.tensor_names.keys())
 
+    def memory_usage(self):
+        """(device bytes, host bytes): HBM the model allocated, page-locked host memory of its host-placed embedding tables."""
+        dev, host = ctypes.c_int64(), ctypes.c_int64()
+        check(self._lib.wd_memory_usage(self._h, ctypes.byref(dev), ctypes.byref(host)))
+        return dev.value, host.value
+
     def n_slots(self, name):
         o = self.plan.lin_opt if name.startswith("linear/") else self.plan.dnn_opt
         return {"sgd": 0, "adagrad": 1, "ftrl": 2, "adam": 2, "rmsprop": 2}[o["kind"]]

@@ -36,6 +36,9 @@ MODES = ["simple", "first_dense", "last_dense", "dense", "resnet"]
 T_WIDE_COL, T_EMB_TABLE, T_DENSE, T_WIDE_BIAS = range(4)
 D_KERNEL, D_BIAS, D_GAMMA, D_BETA = range(4)
 GEMM = {"auto": 0, "ffma": 1, "tc3x": 2, "tc1x": 3, "bf16x3": 4}
+PLACE_HBM, PLACE_HOST, PLACE_AUTO = range(3)      # WD_PLACE_*
+PLACE_NAMES = {PLACE_HBM: "hbm", PLACE_HOST: "host", PLACE_AUTO: "auto"}
+API_VERSION = 3                                   # WD_API_VERSION
 
 
 def embedding_dim(n):
@@ -118,6 +121,7 @@ class PlanDescC(ctypes.Structure):
         ("table_sharded", _P), ("col_wide_sharded", _P),
         ("shard_capacity", ctypes.c_int64), ("shard_slack", ctypes.c_float),
         ("dropout_rate", ctypes.c_float), ("dropout_seed", ctypes.c_uint64),
+        ("table_placement", _P),
     ]
 
 
@@ -135,7 +139,7 @@ class Plan(object):
     """Compiled model description.  Attributes of interest:
       cat_fields / dense_fields : ordered input field names (batch layout)
       columns                   : list[Column] in evaluation order
-      tables                    : list of dict(name, column, rows, dim, x0_off)
+      tables                    : list of dict(name, column, rows, dim, x0_off, sharded, placement = PLACE_*)
       numerics                  : list of dict(name, field, norm, x0_off)
       deep_layout               : OrderedDict column name -> (logical offset, physical offset, width)
       towers                    : list of dict(hidden, mode)
@@ -144,7 +148,7 @@ class Plan(object):
 
     def __init__(self, feature_conf, cross_conf, model_conf, model_type="wide_deep", max_batch=8192,
                  embedding_dim_override=None, tf_compat_pad=False, gemm_engine="auto", max_nnz=0, max_keys=0,
-                 dense_exchange_max_rows=0, shard_world=1, shard_rank=0, shard_capacity=0, shard_slack=2.0):
+                 dense_exchange_max_rows=0, shard_world=1, shard_rank=0, shard_capacity=0, shard_slack=2.0, host_tables=None):
         if model_type not in ("wide", "deep", "wide_deep"):
             raise ValueError("Invalid model type: {}, must be one of `wide`, `deep`, `wide_deep`".format(model_type))
         self.model_type, self.max_batch, self.tf_compat_pad = model_type, int(max_batch), bool(tf_compat_pad)
@@ -308,6 +312,25 @@ class Plan(object):
                 po += width
         self.d0, self.d0_phys = lo, max(32, _pad(po, 32)) if self.use_deep else 0
 
+        # ---- table placement (WD_PLACE_*).  None: auto — the library keeps every table in HBM that fits there and moves only the
+        # tables whose HBM allocation fails to page-locked host memory.  "all" / a list of table names: exactly those tables in host
+        # memory, every other one in HBM.
+        self.host_tables = host_tables
+        names = [t["name"] for t in self.tables]
+        if host_tables is None:
+            want = None
+        elif isinstance(host_tables, str):
+            if host_tables != "all":
+                raise ValueError("host_tables must be None, 'all' or a list of embedding table names, got {!r}".format(host_tables))
+            want = set(names)
+        else:
+            want = set(host_tables)
+            unknown = sorted(want - set(names))
+            if unknown:
+                raise ValueError("host_tables: no embedding table named {} (tables: {})".format(unknown, names))
+        for t in self.tables:
+            t["placement"] = PLACE_AUTO if want is None else (PLACE_HOST if t["name"] in want else PLACE_HBM)
+
         # ---- MLP
         hu = model_conf.get("dnn_hidden_units") or []
         towers = [list(h) for h in hu] if hu and isinstance(hu[0], (list, tuple)) else [list(hu)]
@@ -433,7 +456,8 @@ class Plan(object):
                     tables=len(self.tables), table_rows=sum(t["rows"] for t in self.tables),
                     table_params=sum(t["rows"] * t["dim"] for t in self.tables),
                     deep_dim=self.d0, deep_dim_phys=self.d0_phys,
-                    towers=[(t["hidden"], t["mode"]) for t in self.towers])
+                    towers=[(t["hidden"], t["mode"]) for t in self.towers],
+                    placement=OrderedDict((t["name"], PLACE_NAMES[t["placement"]]) for t in self.tables))
 
     # ------------------------------------------------------------------ C image
     def to_c(self):
@@ -464,7 +488,7 @@ class Plan(object):
                 aux_off.append(0)
                 aux_n.append(0)
         d = PlanDescC()
-        d.api_version = 2
+        d.api_version = API_VERSION
         d.model_type = (1 if self.use_wide else 0) | (2 if self.use_deep else 0)
         d.n_cat_fields, d.n_dense_fields = len(self.cat_fields), len(self.dense_fields)
         d.cat_field_is_string = arr(self.cat_is_string, np.uint8)
@@ -512,6 +536,7 @@ class Plan(object):
         d.shard_capacity, d.shard_slack = self.shard_capacity, self.shard_slack
         d.dropout_rate, d.dropout_seed = self.dropout, self.dropout_seed
         d.wide_small_base = self.wide_small_base if self.wide_small_base is not None else self.wide_rows
+        d.table_placement = arr([t["placement"] for t in self.tables], np.uint8)
         return d, keep
 
 
