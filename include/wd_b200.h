@@ -181,6 +181,18 @@ int64_t wd_tensor_size(WdModel *m, int kind, int index, int sub);
  * tables (WdPlanDesc::table_placement).  Either pointer may be NULL.  (The reference's parameters sit in host RAM on the CPU
  * or on the parameter servers, reference python/lib/build_estimator.py:211-214.) */
 int wd_memory_usage(WdModel *m, int64_t *device_bytes, int64_t *host_bytes);
+/* HBM cache of host-placed table records: an 8-way set-associative, write-back cache of whole [w | slots] records, with LRU
+ * replacement inside a set.  Rows a step touches that are cached are neither fetched nor written home; results stay
+ * bit-identical to the uncached model.  Call after wd_model_create and before the first step or forward (WD_ESTATE after).
+ * `bytes` is the HBM budget of the records: it is rounded down to 8 x 2^k slots of the widest host record; the slot metadata
+ * (9 bytes per slot) comes on top.  A no-op (capacity 0) when no table is on the host.  WD_ENOMEM when the cache would leave less
+ * free HBM than the model keeps in reserve for its later allocations (batch slots, step graphs).  The cache is opt-in:
+ * wd_step_backward(_slot) is refused (WD_EUNSUPPORTED) on a model with a cache. */
+int wd_host_cache_enable(WdModel *m, int64_t bytes);
+/* Cumulative cache counters: out[0] capacity in slots, [1] hits, [2] misses loaded into a slot, [3] overflow rows (staged
+ * without a slot: more misses in a set than it has ways), [4] dirty evictions written home.  Copies the first min(n, 5);
+ * reset != 0 zeroes the counters [1..4] after the copy.  Synchronises the model stream. */
+int wd_host_cache_stats(WdModel *m, int64_t *out, int32_t n, int32_t reset);
 
 /* One training step: H2D copy, ids, forward, loss, backward, optimizers.  Replaces one
  * sess.run(train_op) of Estimator.train (reference python/train.py:128-133; joint.py:224-262).

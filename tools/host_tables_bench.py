@@ -1,17 +1,22 @@
 """Host-placed embedding tables against the same tables in HBM, on one GPU.
 
-For each workload (the Criteo and multihot shapes of wide_deep_b200/synthetic.py, as bench.py builds them) two models live in
-one process: A with every table in HBM, B with every table larger than --host-min-rows rows in page-locked host memory
-(Plan(host_tables=[...])).  Both start from the same init seed and train on the same seeded resident batches; the timed windows
-alternate A / B / A / B, so both models take the same sequence of steps.  Reported per workload:
+For each workload (the Criteo and multihot shapes of wide_deep_b200/synthetic.py, as bench.py builds them) up to three models
+live in one process: A with every table in HBM, B with every table larger than --host-min-rows rows in page-locked host memory
+(Plan(host_tables=[...])), and with --cache-bytes N > 0 also C, which is B plus an HBM cache of N bytes for the host records
+(Plan(host_cache_bytes=N)).  All start from the same init seed and train on the same seeded resident batches (a ring of --ring
+distinct batches, so a cache sees as many distinct rows as --ring steps of a real stream); the timed windows alternate
+A / B / C / A / B / C, so every model takes the same sequence of steps.  --zipf ALPHA draws the Criteo ids from a Zipf
+distribution (synthetic.criteo_batch_arrays(zipf=...)); multihot ids stay uniform.  Reported per workload:
   * examples/s of each model (host clock around windows that end in a device synchronise);
+  * for C, from its cache counters over the timed windows: hit rate, and PCIe records and bytes per step in each direction
+    (in: loads + overflow rows; out: dirty evictions + overflow rows);
   * unique host-table rows per step (U_host, counted from the column ids of the ring's batches), unique embedding rows per
     step (d_nuniq), and the PCIe bytes per step, U_host x record bytes in each direction;
   * pinned host->device / device->host copy bandwidth measured in the same run, and the PCIe floor of the extra step time;
   * GPU name, power limit and max SM clock (read-only nvidia-smi query).
-Afterwards every parameter and optimizer slot of B is compared byte for byte with A's.
+Afterwards every parameter and optimizer slot of B and C is compared byte for byte with A's.
 
-    python tools/host_tables_bench.py [--workloads criteo,multihot] [--steps 50] [--warmup 12] [--out FILE]
+    python tools/host_tables_bench.py [--workloads criteo,multihot] [--steps 50] [--ring 64] [--zipf 1.05] [--cache-bytes N] [--out FILE]
 """
 import argparse
 import json
@@ -26,7 +31,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-RING = 4
 
 
 def gpu_info():
@@ -59,20 +63,21 @@ def copy_bandwidth(nbytes=1 << 30, reps=10):
     return out
 
 
-def build(wl, B, host_tables):
+def build(wl, B, host_tables, cache_bytes=0):
     from wide_deep_b200.plan import Plan
     return Plan(wl["fc"], wl["cross"], wl["model"], wl["model_type"], max_batch=B, embedding_dim_override=wl["emb"],
-                gemm_engine="bf16x3", max_keys=B * wl["keys_per_row"], max_nnz=B * wl["ids_per_row"], host_tables=host_tables)
+                gemm_engine="bf16x3", max_keys=B * wl["keys_per_row"], max_nnz=B * wl["ids_per_row"], host_tables=host_tables,
+                host_cache_bytes=cache_bytes)
 
 
-def workload(name):
+def workload(name, zipf=None):
     from wide_deep_b200 import synthetic
     if name == "criteo":
         fc, cross, model, emb = synthetic.criteo_conf()
         n_cat = sum(1 for c in fc.values() if c["type"] == "category")
         return dict(fc=fc, cross=cross, model=model, emb=emb, model_type="wide_deep", ids_per_row=len(fc) + len(cross),
                     keys_per_row=n_cat, batch=8192,
-                    arrays=lambda B, s: synthetic.criteo_batch_arrays(fc, B, step=s))
+                    arrays=lambda B, s: synthetic.criteo_batch_arrays(fc, B, step=s, zipf=zipf))
     if name == "multihot":
         fc, cross, model, emb = synthetic.multihot_conf()
         return dict(fc=fc, cross=cross, model=model, emb=emb, model_type="deep", ids_per_row=128, keys_per_row=128, batch=8192,
@@ -97,20 +102,22 @@ def all_equal(a, b):
     return True, None
 
 
-def run(name, steps, warmup, host_min_rows, seed=7):
+def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed=7):
     from wide_deep_b200.model import WideDeepModel
-    wl = workload(name)
+    wl = workload(name, zipf)
     B = wl["batch"]
     plan_a = build(wl, B, [])
     host = [t["name"] for t in plan_a.tables if t["rows"] > host_min_rows]
-    plan_b = build(wl, B, host)
-    batches = [batch_of(name, wl["arrays"](B, s), B) for s in range(RING)]
+    plans = {"hbm": plan_a, "host": build(wl, B, host)}
+    if cache_bytes > 0:
+        plans["cache"] = build(wl, B, host, cache_bytes)
+    batches = [batch_of(name, wl["arrays"](B, s), B) for s in range(ring)]
     t0 = time.time()
-    a = WideDeepModel(plan_a).init(seed)
-    b = WideDeepModel(plan_b).init(seed)
+    models = {k: WideDeepModel(p).init(seed) for k, p in plans.items()}
     setup_s = time.time() - t0
-    for m in (a, b):
-        for s in range(RING):
+    a = models["hbm"]
+    for m in models.values():
+        for s in range(ring):
             m.upload_slot(s, batches[s])
     # U_host: unique ids of the host tables' columns in each ring batch
     by_table = {i: t for i, t in enumerate(plan_a.tables)}
@@ -122,10 +129,10 @@ def run(name, steps, warmup, host_min_rows, seed=7):
         rec_bytes[ci] = ((t["dim"] + 3) // 4 * 4) * (1 + nslots) * 4
     u_host, bytes_way, nuniq = [], [], []
     step = 0
-    for i in range(warmup):                      # same steps on both models; the first RING steps also count the rows
-        for m in (a, b):
-            m.train_step_slot(step % RING, want_loss=True)
-        if i < RING:
+    for i in range(warmup):                      # same steps on every model; the first steps also count the rows
+        for m in models.values():
+            m.train_step_slot(step % ring, want_loss=True)
+        if i < min(ring, 8):
             offs, ids = a.column_ids()
             C = len(plan_a.columns)
             u, by = 0, 0
@@ -138,37 +145,66 @@ def run(name, steps, warmup, host_min_rows, seed=7):
             bytes_way.append(by)
             nuniq.append(a.sparse_grads(0)[2])
         step += 1
-    times = {"hbm": [], "host": []}
-    for w in range(4):                            # A / B / A / B
-        m, key = (a, "hbm") if w % 2 == 0 else (b, "host")
-        s0 = step - (steps if w % 2 else 0)
-        m.sync()
-        t = time.perf_counter()
-        for i in range(steps):
-            m.train_step_slot((s0 + i) % RING, want_loss=False)
-        m.sync()
-        times[key].append(time.perf_counter() - t)
-        if w % 2 == 0:
-            step += steps
+    if "cache" in models:
+        models["cache"].host_cache_stats(reset=True)
+    times = {k: [] for k in models}
+    for w in range(2):                            # A / B / C / A / B / C, each window on the same steps
+        for key, m in models.items():
+            m.sync()
+            t = time.perf_counter()
+            for i in range(steps):
+                m.train_step_slot((step + i) % ring, want_loss=False)
+            m.sync()
+            times[key].append(time.perf_counter() - t)
+        step += steps
     rate = {k: B * steps / min(v) for k, v in times.items()}
-    same, where = all_equal(a, b)
-    dev_b, host_b = b.memory_usage()
-    dev_a, _ = a.memory_usage()
-    a.close()
-    b.close()
-    return dict(workload=name, batch=B, steps_per_window=steps, host_tables=len(host), host_table_bytes=host_b,
-                hbm_bytes_hbm_model=dev_a, hbm_bytes_host_model=dev_b, setup_s=round(setup_s, 1),
-                examples_per_s_hbm=rate["hbm"], examples_per_s_host=rate["host"],
-                step_ms_hbm=1e3 * min(times["hbm"]) / steps, step_ms_host=1e3 * min(times["host"]) / steps,
-                window_s=times, unique_rows_per_step=float(np.mean(nuniq)), unique_host_rows_per_step=float(np.mean(u_host)),
-                pcie_bytes_per_step_each_way=float(np.mean(bytes_way)), byte_identical=same, first_difference=where)
+    phases = {}
+    for key, m in models.items():                 # one profiled (eager) step per model, the same step on each: phase times in ms
+        m.set_profile(True)
+        m.train_step_slot(step % ring, want_loss=True)
+        phases[key] = {n: round(v, 4) for n, v in m.last_timings().items()}
+        m.set_profile(False)
+    step += 1
+    res = dict(workload=name, zipf=zipf, ring=ring, batch=B, steps_per_window=steps, host_tables=len(host), setup_s=round(setup_s, 1),
+               unique_rows_per_step=float(np.mean(nuniq)), unique_host_rows_per_step=float(np.mean(u_host)),
+               pcie_bytes_per_step_each_way=float(np.mean(bytes_way)), window_s=times, phase_ms=phases)
+    for k, m in models.items():
+        dev, hb = m.memory_usage()
+        res["examples_per_s_" + k] = rate[k]
+        res["step_ms_" + k] = 1e3 * min(times[k]) / steps
+        res["hbm_bytes_" + k] = dev
+        res["host_bytes_" + k] = hb
+    if "cache" in models:
+        c = models["cache"].host_cache_stats()
+        n = 2 * steps
+        rec = float(np.mean(bytes_way)) / max(float(np.mean(u_host)), 1.0)       # mean record bytes of the host rows
+        looked_up = c["hits"] + c["loads"] + c["overflow"]
+        res.update(cache_bytes=cache_bytes, cache_slots=c["capacity"], cache_counters=c,
+                   hit_rate=c["hits"] / looked_up if looked_up else None,
+                   pcie_records_in_per_step=(c["loads"] + c["overflow"]) / n,
+                   pcie_records_out_per_step=(c["evictions"] + c["overflow"]) / n,
+                   pcie_bytes_in_per_step=(c["loads"] + c["overflow"]) / n * rec,
+                   pcie_bytes_out_per_step=(c["evictions"] + c["overflow"]) / n * rec)
+    for k in models:
+        if k == "hbm":
+            continue
+        same, where = all_equal(a, models[k])
+        res["byte_identical_" + k] = same
+        res["first_difference_" + k] = where
+    res["byte_identical"] = all(res["byte_identical_" + k] for k in models if k != "hbm")
+    for m in models.values():
+        m.close()
+    return res
 
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--workloads", default="criteo,multihot")
     ap.add_argument("--steps", type=int, default=50)
-    ap.add_argument("--warmup", type=int, default=12, help="steps before timing (3 per ring slot: two eager, then the graph)")
+    ap.add_argument("--ring", type=int, default=64, help="distinct resident batches the steps cycle through (at most 64)")
+    ap.add_argument("--warmup", type=int, default=None, help="steps before timing (default 3 per ring slot: two eager, then the graph)")
+    ap.add_argument("--zipf", type=float, default=None, help="Criteo ids from Zipf(ALPHA) instead of uniform")
+    ap.add_argument("--cache-bytes", type=int, default=0, help="also run the host model with an HBM cache of this many bytes")
     ap.add_argument("--host-min-rows", type=int, default=16384, help="tables with more rows than this go to host memory")
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
     args = ap.parse_args()
@@ -177,7 +213,8 @@ def main():
     print(json.dumps(dict(info, **bw)), flush=True)
     ok = True
     for name in args.workloads.split(","):
-        r = run(name, args.steps, args.warmup, args.host_min_rows)
+        r = run(name, args.steps, 3 * args.ring if args.warmup is None else args.warmup, args.host_min_rows, args.ring,
+                zipf=args.zipf, cache_bytes=args.cache_bytes)
         extra = (r["step_ms_host"] - r["step_ms_hbm"]) / 1e3
         by = r["pcie_bytes_per_step_each_way"]
         r.update(info)

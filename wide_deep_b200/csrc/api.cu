@@ -521,18 +521,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     for (int k = 0; k < 4; ++k) if ((rc = dev_alloc(m, &m->d_sort_hist_s[k], m->sort_hist_cap))) return rc;
     if (m->use_deep) {
         // Embedding tables come last, so an auto-placed table competes only with what is allocated after wd_model_create returns.
-        // HBM kept free while the auto tables are allocated (see ensure_slot, place_tables and the step graphs):
-        //   kReserveSlots batch slots beyond slot 0 (cat offsets, keys, dense, label, weight each; bench.py and the estimator use
-        //   at most 10),
-        //   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table) and their descriptors,
-        //   kGraphReserve for the instantiated step graphs (one train and one backward graph per slot) and the runtime's growth.
-        constexpr int kReserveSlots = 16;
-        constexpr int64_t kGraphReserve = 256ll << 20;
-        const int64_t slot_bytes = (Bm * std::max(d->n_cat_fields, 1) + 1) * 4 + m->keys_cap * 8 + Bm * std::max(d->n_dense_fields, 1) * 4 + 2 * Bm * 4;
-        int max_stride = 0;
-        for (auto& tb : m->tables) max_stride = std::max(max_stride, tb.stride);
-        const int64_t stage_bytes = m->max_nnz * ((int64_t)max_stride + 1) * 4 + 64 * (int64_t)m->tables.size() + 4096;
-        if ((rc = place_tables(m, kReserveSlots * slot_bytes + stage_bytes + kGraphReserve))) return rc;
+        if ((rc = place_tables(m, hbm_reserve_bytes(m)))) return rc;
     }
     if (G > 1) {
         if ((rc = shard_build(m, d))) return rc;
@@ -588,6 +577,24 @@ extern "C" int wd_model_create(const WdPlanDesc* d, int device, WdModel** out) {
     *out = m;
     return WD_OK;
 }
+
+namespace wd {
+// HBM kept free for what is allocated after the embedding tables (see ensure_slot, place_tables and the step graphs): the auto
+// tables are placed with it held back, and wd_host_cache_enable refuses a cache that would eat into it.
+//   kReserveSlots batch slots beyond slot 0 (cat offsets, keys, dense, label, weight each; bench.py and the estimator use at most 10),
+//   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table) and their descriptors,
+//   kGraphReserve for the instantiated step graphs (one train and one backward graph per slot) and the runtime's growth.
+int64_t hbm_reserve_bytes(const WdModel* m) {
+    constexpr int kReserveSlots = 16;
+    constexpr int64_t kGraphReserve = 256ll << 20;
+    const int64_t Bm = m->max_batch;
+    const int64_t slot_bytes = (Bm * std::max(m->n_cat_fields, 1) + 1) * 4 + m->keys_cap * 8 + Bm * std::max(m->n_dense_fields, 1) * 4 + 2 * Bm * 4;
+    int max_stride = 0;
+    for (auto& tb : m->tables) max_stride = std::max(max_stride, tb.stride);
+    const int64_t stage_bytes = m->max_nnz * ((int64_t)max_stride + 1) * 4 + 64 * (int64_t)m->tables.size() + 4096;
+    return kReserveSlots * slot_bytes + stage_bytes + kGraphReserve;
+}
+}  // namespace wd
 
 // glorot-uniform kernels / zero biases / gamma 1 / beta 0 built on the host (dense part is ~1.5M floats)
 static int init_dense(WdModel* m, WdModelExtra* x, uint64_t seed) {
@@ -701,6 +708,11 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         if (slot * tb.dim >= tb.stride) { set_error("table has no optimizer slot %d", slot); return WD_EINVAL; }
         float* dev = tb.data + slot * tb.dim;
         const size_t lw = (size_t)tb.dim_logical * 4;
+        // host records cached in HBM: dirty slots go home before either direction; a write then empties the cache
+        if (tb.host && m->cache_slots > 0) {
+            const int rc = host_cache_sync(m, true, to_device != 0);
+            if (rc) return rc;
+        }
         const cudaMemcpyKind dir = tb.host ? cudaMemcpyDefault : (to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost);
         if (to_device) WD_CUDA(cudaMemcpy2DAsync(dev, (size_t)tb.stride * 4, host, lw, lw, tb.arows, dir, m->stream));
         else WD_CUDA(cudaMemcpy2DAsync(host, lw, dev, (size_t)tb.stride * 4, lw, tb.arows, dir, m->stream));
@@ -955,6 +967,7 @@ static int group_async(WdModel* m) {
 
 static int forward_core(WdModel* m, bool train) {
     int rc;
+    m->stepped = true;
     stamp(m, ST_START);
     if ((rc = ids_prepare(m))) return rc;
     mark(m, "ids");
@@ -974,7 +987,7 @@ static int forward_core(WdModel* m, bool train) {
         // (on side stream 0 when the train step put it there, else here; the backward then groups it once more only when profiling)
         if (m->side_pending[0]) WD_CUDA(cudaStreamWaitEvent(m->stream, m->ev_grouped[0], 0));
         else if ((rc = sparse_group_which(m, 0))) return rc;
-        if ((rc = host_tables_stage_in(m))) return rc;
+        if ((rc = host_tables_stage_in(m, train))) return rc;
     }
     if ((rc = sparse_forward_emb(m))) return rc;
     stamp(m, ST_GATHER);
@@ -1204,12 +1217,21 @@ static int backward_eager(WdModel* m, bool join) {
 // is ~65 launches on three streams: like the full step it is captured per batch slot after two eager runs and replayed.  Inside
 // the graph the streams overlap as in the eager schedule; after it the sparse lists continue on their side streams, which wait for
 // the graph through ev_bwd_done.
+// The split step applies the embedding rows with the unfused kernels, which update host records through their mapped pointers:
+// with an HBM cache in front of those records the update would bypass it.
+static int refuse_split_step_with_cache(WdModel* m) {
+    if (m->cache_slots == 0) return WD_OK;
+    set_error("the split step (wd_step_backward / wd_step_apply) is not supported on a model with a host-table cache");
+    return WD_EUNSUPPORTED;
+}
+
 extern "C" int wd_step_backward_slot(WdModel* m, int slot, float* loss_out) {
     int rc = check_ready(m);
     if (rc) return rc;
     if ((rc = select_slot(m, slot))) return rc;
     if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
+    if ((rc = refuse_split_step_with_cache(m))) return rc;
     timer_begin(m);
     BatchSlot& sl = m->slots[slot];
     const bool can_graph = m->graphs_enabled && !m->timer.enabled;
@@ -1270,8 +1292,10 @@ extern "C" int wd_last_loss(WdModel* m, float* loss_out) {
 }
 
 extern "C" int wd_step_backward(WdModel* m, const WdBatch* b, float* loss_out) {
-    int rc = b ? wd_batch_upload(m, b) : check_ready(m);
+    int rc = check_ready(m);
     if (rc) return rc;
+    if ((rc = refuse_split_step_with_cache(m))) return rc;
+    if (b && (rc = wd_batch_upload(m, b))) return rc;
     timer_begin(m);
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     if ((rc = forward_core(m, true))) return rc;

@@ -307,6 +307,19 @@ struct WdModel {
     int32_t* d_tab_stage = nullptr;          // [n_tables] 0: record in place; stage_stride: staged (RowApply); null without host tables
     float** d_rtab_gdata = nullptr;          // [n_rtab] data in row order, d_stage for host tables (HotApply)
     int32_t* d_rtab_stage = nullptr;         // [n_rtab] 0 / stage_stride in row order (HotApply, stage-in / write-back); null without host tables
+    // HBM cache of host records (wd_host_cache_enable): d_stage is then [cache_slots slots | max_nnz overflow rows]
+    int64_t cache_slots = 0;                 // C = 8 x 2^cache_set_bits; 0: no cache (every staged row is an overflow row)
+    int cache_set_bits = 0;
+    uint32_t* d_ctag = nullptr;              // [C] global row held by the slot, kInvalidRow: empty
+    uint32_t* d_cstamp = nullptr;            // [C] stamp of the last call that used the slot (0: empty)
+    uint8_t* d_cdirty = nullptr;             // [C] 1: the slot is newer than its host record
+    uint32_t* d_cnow = nullptr;              // device counter, bumped once per stage-in (the stamp of that call)
+    unsigned long long* d_cstats = nullptr;  // [4] hits, loads, overflow rows, dirty evictions
+    int32_t* d_uslot = nullptr;              // [max_nnz] staging row of unique row u; null without a cache (row u)
+    uint32_t* d_uvict = nullptr;             // [max_nnz] row the slot of u held before u was loaded into it
+    uint8_t* d_uflag = nullptr;              // [max_nnz] kLoad / kVictimDirty (host_tables.cu)
+    uint32_t *d_ck[2] = {}, *d_cv[2] = {};   // (set, u) pairs and their sort ping-pong buffers
+    bool stepped = false;                    // a forward or train step was issued (step graphs may exist)
 
     // numeric deep columns (device arrays)
     int32_t *d_num_field = nullptr, *d_num_norm_kind = nullptr, *d_num_x0_off = nullptr;
@@ -435,12 +448,16 @@ int model_init_params(WdModel* m, uint64_t seed);                // init.cu
 int step_tick(WdModel* m);                                       // misc.cu: train-step counter on the device (dropout)
 int adam_tick(WdModel* m);                                       // misc.cu: beta powers advance (after every optimizer of the step)
 int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host), descriptors
-int host_tables_stage_in(WdModel* m);                            // host_tables.cu: host rows -> staging buffer, gather ids
-int host_tables_write_back(WdModel* m);                          // host_tables.cu: staging buffer -> host rows
+int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
+int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
+int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
+int64_t hbm_reserve_bytes(const WdModel* m);                     // api.cu: HBM the model keeps free for its later allocations
 int metrics_accumulate(WdModel* m);                              // metrics.cu
 int metrics_finish(WdModel* m, double* out10);
 
-int radix_sort_pairs(WdModel* m, int which, int bits, const int32_t* d_n);   // sort.cu
+// sorts (*keys, *vals) of length *d_n by the low `bits` bits of the key, with (*keys2, *vals2) as ping-pong buffers; the
+// pointers are swapped so that the sorted pairs end in (*keys, *vals)
+int radix_sort_pairs(WdModel* m, uint32_t** keys, uint32_t** vals, uint32_t** keys2, uint32_t** vals2, int bits, const int32_t* d_n);   // sort.cu
 int exclusive_scan_i32(WdModel* m, int32_t* data, int64_t n, int32_t* total_out);   // sort.cu (in place, n known on host)
 int seg_heads(WdModel* m, const int32_t* d_n, const uint32_t* keys, uint32_t invalid, int32_t* pos, int64_t cap, int32_t* ustart, uint32_t* urow,
               int32_t* d_nuniq);                                                    // sort.cu: unique rows of sorted keys (2 launches)

@@ -9,6 +9,8 @@
 //               gather kernels see the host tables as (data = staging buffer, row base 0, stride = staging stride)
 //   apply       the fused updates (RowApply / HotApply in sparse.cu) address the staged record of u
 //   write-back  host_rows_kernel<false>: staging buffer row u -> host record, after the list's apply, on its stream
+// With the opt-in HBM cache (wd_host_cache_enable, below) row u is staged in a cache slot that outlives the step, and only the
+// rows that miss are moved.
 // Every kernel downstream of the stage-in runs on bit-identical values in the same order, so the result equals the HBM-resident
 // model's bit for bit.  Updates that do not go through the fused kernels (data-parallel lists: wd_step_backward + wd_step_apply)
 // address the host records directly through their mapped pointers.
@@ -29,61 +31,242 @@ __device__ __forceinline__ int rtab_of(const int64_t* __restrict__ rtab_row_base
     return lo;
 }
 
-// IN: host record of unique row u -> stage + u * S; !IN: the reverse.  One thread per float4 of a staged record, consecutive
-// threads on consecutive float4 of a record (the PCIe transfers are whole records); each thread keeps kInFlight float4 in flight.
+// ---------------------------------------------------------------------------------------------------------- HBM cache
+// wd_host_cache_enable turns the front of the staging buffer into an 8-way set-associative, write-back cache of host records:
+//   d_stage = [C cache slots | max_nnz overflow rows], stride stage_stride; slot s * 8 + w is way w of set s
+//   set of a row  Fibonacci hash of the global row (the hot rows of skewed id streams are the low ids of every table: a plain
+//                 modulo would put them into neighbouring sets)
+//   stage-in      keys (set of every unique host row) -> stable radix sort by set -> assign (one thread per run of one set: hits
+//                 keep their slot, misses take the other ways by (last use, way index), empty ways first, and rows beyond the
+//                 ways overflow to staging row C + u) -> transfer (dirty victim home, then the new record in) -> remap
+//   write-back    after the list's apply, overflow rows only; cached records stay dirty until they are evicted or flushed
+// Train calls mark every slot they use dirty; forward-only calls mark nothing dirty.  Without a cache (C = 0) every row is an
+// overflow row at staging row u, uslot is null and the key / sort / assign launches are skipped.
+constexpr int kWays = 8;
+constexpr uint8_t kLoad = 1, kVictimDirty = 2;      // d_uflag bits
+
+__device__ __forceinline__ uint32_t cache_set_of(uint32_t row, int set_bits) {
+    return set_bits ? (row * 0x9E3779B1u) >> (32 - set_bits) : 0u;
+}
+
+// key = set of unique row u (host rows) or nsets (HBM rows: sorted last, never assigned), value = u; bumps the call's stamp
+__global__ void __launch_bounds__(256) cache_keys_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, int ntab,
+                                                         const int64_t* __restrict__ rtab_row_base, const int32_t* __restrict__ rtab_stage,
+                                                         int set_bits, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                         uint32_t* __restrict__ now) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) ++*now;
+    const int nu = *d_nuniq;
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) {
+        const uint32_t row = urow[u];
+        keys[u] = rtab_stage[rtab_of(rtab_row_base, ntab, row)] != 0 ? cache_set_of(row, set_bits) : (1u << set_bits);
+        vals[u] = (uint32_t)u;
+    }
+}
+
+struct CacheMeta { uint32_t* tag; uint32_t* stamp; uint8_t* dirty; const uint32_t* now; unsigned long long* stats; };
+
+// One thread per run of equal sets in the sorted (set, u) pairs; a run lists its rows in ascending row order (stable sort of the
+// ascending unique rows).  Writes uslot / uvict / uflag of the run's rows and the set's metadata; counters: hits, loads, overflow
+// rows, dirty evictions.
+__global__ void __launch_bounds__(256) cache_assign_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ keys,
+                                                           const uint32_t* __restrict__ vals, const uint32_t* __restrict__ urow, int set_bits,
+                                                           int64_t C, int train, CacheMeta cm, int32_t* __restrict__ uslot,
+                                                           uint32_t* __restrict__ uvict, uint8_t* __restrict__ uflag) {
+    const int n = *d_nuniq;
+    const uint32_t nsets = 1u << set_bits, now = *cm.now;
+    unsigned nhit = 0, nload = 0, nover = 0, nevict = 0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t s = keys[i];
+        if (s >= nsets || (i > 0 && keys[i - 1] == s)) continue;
+        int e = i + 1;
+        while (e < n && keys[e] == s) ++e;
+        const int64_t base = (int64_t)s * kWays;
+        uint32_t tag[kWays], st[kWays];
+        uint8_t dty[kWays];
+#pragma unroll
+        for (int w = 0; w < kWays; ++w) { tag[w] = cm.tag[base + w]; st[w] = cm.stamp[base + w]; dty[w] = cm.dirty[base + w]; }
+        unsigned used = 0;
+        for (int j = i; j < e; ++j) {                                   // hits keep their slot
+            const uint32_t u = vals[j], row = urow[u];
+#pragma unroll
+            for (int w = 0; w < kWays; ++w)
+                if (tag[w] == row) { used |= 1u << w; uslot[u] = (int32_t)(base + w); uflag[u] = 0; uvict[u] = kInvalidRow; ++nhit; }
+        }
+        // the other ways by (last use, way index); an empty way has stamp 0, every used one a stamp >= 1
+        int order[kWays], nfree = 0;
+        for (int w = 0; w < kWays; ++w) {
+            if ((used >> w) & 1) continue;
+            const uint32_t k = tag[w] == kInvalidRow ? 0u : st[w];
+            int p = nfree++;
+            for (; p > 0 && (tag[order[p - 1]] == kInvalidRow ? 0u : st[order[p - 1]]) > k; --p) order[p] = order[p - 1];
+            order[p] = w;
+        }
+        int next = 0;
+        for (int j = i; j < e; ++j) {                                   // misses, in row order
+            const uint32_t u = vals[j], row = urow[u];
+            bool hit = false;
+#pragma unroll
+            for (int w = 0; w < kWays; ++w) hit |= tag[w] == row;      // (a way loaded below holds a row of this run: never equal)
+            if (hit) continue;
+            if (next < nfree) {
+                const int w = order[next++];
+                const bool vd = tag[w] != kInvalidRow && dty[w];
+                uslot[u] = (int32_t)(base + w);
+                uvict[u] = tag[w];
+                uflag[u] = kLoad | (vd ? kVictimDirty : 0);
+                nevict += vd;
+                ++nload;
+                tag[w] = row;
+                dty[w] = 0;
+                used |= 1u << w;
+            } else {                                                    // the set is full: staged without a slot
+                uslot[u] = (int32_t)(C + u);
+                uvict[u] = kInvalidRow;
+                uflag[u] = kLoad;
+                ++nover;
+            }
+        }
+#pragma unroll
+        for (int w = 0; w < kWays; ++w) {
+            if ((used >> w) & 1) { st[w] = now; if (train) dty[w] = 1; }
+            cm.tag[base + w] = tag[w]; cm.stamp[base + w] = st[w]; cm.dirty[base + w] = dty[w];
+        }
+    }
+    nhit = __reduce_add_sync(0xffffffffu, nhit); nload = __reduce_add_sync(0xffffffffu, nload);
+    nover = __reduce_add_sync(0xffffffffu, nover); nevict = __reduce_add_sync(0xffffffffu, nevict);
+    if ((threadIdx.x & 31) == 0) {
+        if (nhit) atomicAdd(&cm.stats[0], (unsigned long long)nhit);
+        if (nload) atomicAdd(&cm.stats[1], (unsigned long long)nload);
+        if (nover) atomicAdd(&cm.stats[2], (unsigned long long)nover);
+        if (nevict) atomicAdd(&cm.stats[3], (unsigned long long)nevict);
+    }
+}
+
+// Transfer between the host records of the step's unique host rows and their staging rows (uslot[u], or u without a cache).
+// IN: the record of every row to load -> its staging row; a dirty victim's record goes home first (uvict[u], the row the slot
+// held).  !IN: overflow staging rows (>= C) -> host records.  One thread per float4 of a staged record, consecutive threads on
+// consecutive float4 of a record (the PCIe transfers are whole records); each thread keeps kInFlight float4 in flight.  The thread
+// that writes float4 q of a slot has read the victim's float4 q before, so the eviction needs no barrier; a victim is never a row
+// of the current call (that row would have been a hit).
 constexpr int kInFlight = 4;
+struct StageMap { const int32_t* uslot; const uint32_t* uvict; const uint8_t* uflag; int64_t C; };
 template <bool IN>
 __global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, int ntab,
                                                         const int64_t* __restrict__ rtab_row_base, float* const* __restrict__ rtab_data,
                                                         const int32_t* __restrict__ rtab_stride, const int32_t* __restrict__ rtab_stage,
-                                                        float* __restrict__ stage, int S) {
+                                                        float* __restrict__ stage, int S, StageMap sm) {
     const int q4 = S >> 2;
     const int64_t total = (int64_t)*d_nuniq * q4;
     const int64_t T = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < total; i0 += T * kInFlight) {
-        float4 v[kInFlight];
-        float* dst[kInFlight];
+        float4 v[kInFlight], vv[kInFlight];
+        float *dst[kInFlight], *vdst[kInFlight];
 #pragma unroll
         for (int k = 0; k < kInFlight; ++k) {
-            dst[k] = nullptr;
+            dst[k] = vdst[k] = nullptr;
             const int64_t i = i0 + k * T;
             if (i >= total) continue;
             const int64_t u = i / q4;
             const int q = (int)(i - u * q4);
             const int64_t row = urow[u];
             const int lo = rtab_of(rtab_row_base, ntab, row);
+            if (rtab_stage[lo] == 0) continue;                           // HBM table
+            int64_t srow = u;
+            if (sm.uslot) {
+                srow = sm.uslot[u];
+                if (IN) {
+                    const uint8_t f = sm.uflag[u];
+                    if (!(f & kLoad)) continue;                              // hit: the slot holds the record
+                    if (f & kVictimDirty) {
+                        const int64_t vr = sm.uvict[u];
+                        const int vlo = rtab_of(rtab_row_base, ntab, vr);
+                        const int vstride = rtab_stride[vlo];
+                        if (q * 4 < vstride) {
+                            vv[k] = *reinterpret_cast<const float4*>(stage + srow * S + q * 4);
+                            vdst[k] = rtab_data[vlo] + (vr - rtab_row_base[vlo]) * vstride + q * 4;
+                        }
+                    }
+                } else if (srow < sm.C) continue;                            // cached: stays in its slot
+            }
             const int stride = rtab_stride[lo];
-            if (rtab_stage[lo] == 0 || q * 4 >= stride) continue;          // HBM table / beyond this table's record
+            if (q * 4 >= stride) continue;                                   // beyond this table's record
             float* rec = rtab_data[lo] + (row - rtab_row_base[lo]) * stride + q * 4;
-            float* st = stage + u * S + q * 4;
+            float* st = stage + srow * S + q * 4;
             if (IN) { v[k] = *reinterpret_cast<const float4*>(rec); dst[k] = st; }
             else { v[k] = *reinterpret_cast<const float4*>(st); dst[k] = rec; }
         }
 #pragma unroll
-        for (int k = 0; k < kInFlight; ++k)
+        for (int k = 0; k < kInFlight; ++k) {
+            if (IN && vdst[k]) *reinterpret_cast<float4*>(vdst[k]) = vv[k];
             if (dst[k]) *reinterpret_cast<float4*>(dst[k]) = v[k];
+        }
     }
 }
 
-// gather ids: e_emb, with the entries of host tables replaced by their unique-row index u (urow[0..nu) is sorted ascending)
+// gather ids: e_emb, with the entries of host tables replaced by the staging row of their unique row u (uslot[u], or u without a
+// cache; urow[0..nu) is sorted ascending)
 __global__ void __launch_bounds__(256) host_remap_kernel(const int32_t* __restrict__ d_nnz, const uint32_t* __restrict__ e_emb,
                                                          const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, int ntab,
                                                          const int64_t* __restrict__ rtab_row_base, const int32_t* __restrict__ rtab_stage,
-                                                         uint32_t* __restrict__ g_emb) {
+                                                         const int32_t* __restrict__ uslot, uint32_t* __restrict__ g_emb) {
     const int n = *d_nnz, nu = *d_nuniq;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t r = e_emb[i];
         uint32_t g = r;
-        if (r != kInvalidRow && rtab_stage[rtab_of(rtab_row_base, ntab, r)] != 0) g = (uint32_t)lower_bound_u32(urow, nu, r);
+        if (r != kInvalidRow && rtab_stage[rtab_of(rtab_row_base, ntab, r)] != 0) {
+            const int u = lower_bound_u32(urow, nu, r);
+            g = uslot ? (uint32_t)uslot[u] : (uint32_t)u;
+        }
         g_emb[i] = g;
     }
 }
 
-int host_tables_stage_in(WdModel* m) {
+// dirty slots -> host records (one thread per float4 of a slot)
+__global__ void __launch_bounds__(256) cache_flush_kernel(int64_t C, int S, const uint32_t* __restrict__ tag, const uint8_t* __restrict__ dirty,
+                                                          int ntab, const int64_t* __restrict__ rtab_row_base, float* const* __restrict__ rtab_data,
+                                                          const int32_t* __restrict__ rtab_stride, const float* __restrict__ stage) {
+    const int q4 = S >> 2;
+    const int64_t total = C * q4;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t slot = i / q4;
+        const int q = (int)(i - slot * q4);
+        if (!dirty[slot] || tag[slot] == kInvalidRow) continue;
+        const int64_t row = tag[slot];
+        const int lo = rtab_of(rtab_row_base, ntab, row);
+        const int stride = rtab_stride[lo];
+        if (q * 4 >= stride) continue;
+        *reinterpret_cast<float4*>(rtab_data[lo] + (row - rtab_row_base[lo]) * stride + q * 4) =
+            *reinterpret_cast<const float4*>(stage + slot * S + q * 4);
+    }
+}
+__global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32_t* __restrict__ stamp, uint8_t* __restrict__ dirty, int invalidate) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < C; i += (int64_t)gridDim.x * blockDim.x) {
+        dirty[i] = 0;
+        if (invalidate) { tag[i] = kInvalidRow; stamp[i] = 0; }
+    }
+}
+
+int host_tables_stage_in(WdModel* m, bool train) {
+    const int64_t C = m->cache_slots;
+    const int g = grid_for(m->max_nnz, 256);
+    if (C > 0) {
+        cache_keys_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_stage, m->cache_set_bits,
+                                                   m->d_ck[0], m->d_cv[0], m->d_cnow);
+        m->launches++;
+        int rc = radix_sort_pairs(m, &m->d_ck[0], &m->d_cv[0], &m->d_ck[1], &m->d_cv[1], m->cache_set_bits + 1, m->d_nuniq[0]);
+        if (rc) return rc;
+        mark(m, "cache_sort");
+        const CacheMeta cm{m->d_ctag, m->d_cstamp, m->d_cdirty, m->d_cnow, m->d_cstats};
+        cache_assign_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_ck[0], m->d_cv[0], m->d_urow[0], m->cache_set_bits, C, train ? 1 : 0, cm,
+                                                     m->d_uslot, m->d_uvict, m->d_uflag);
+        m->launches++;
+        mark(m, "cache_assign");
+    }
+    const StageMap sm{m->d_uslot, m->d_uvict, m->d_uflag, C};
     host_rows_kernel<true><<<grid_for(m->max_nnz * (m->stage_stride / 4) / kInFlight, 256), 256, 0, m->stream>>>(
-        m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_rtab_stage, m->d_stage, m->stage_stride);
-    host_remap_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], m->n_rtab,
-                                                                        m->d_rtab_row_base, m->d_rtab_stage, m->d_g_emb);
+        m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_rtab_stage, m->d_stage, m->stage_stride, sm);
+    host_remap_kernel<<<g, 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], m->n_rtab,
+                                                m->d_rtab_row_base, m->d_rtab_stage, m->d_uslot, m->d_g_emb);
     m->launches += 2;
     mark(m, "stage_in");
     WD_CUDA(cudaGetLastError());
@@ -91,10 +274,27 @@ int host_tables_stage_in(WdModel* m) {
 }
 
 int host_tables_write_back(WdModel* m) {
+    const StageMap sm{m->d_uslot, m->d_uvict, m->d_uflag, m->cache_slots};
     host_rows_kernel<false><<<grid_for(m->max_nnz * (m->stage_stride / 4) / kInFlight, 256), 256, 0, m->stream>>>(
-        m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_rtab_stage, m->d_stage, m->stage_stride);
+        m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_rtab_stage, m->d_stage, m->stage_stride, sm);
     m->launches++;
     mark(m, "write_back");
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+
+// Everything that reads or writes host records outside the step: flush = dirty slots home (they stay cached, now clean),
+// invalidate = empty every slot (after the host records were rewritten).  Enqueued on the model stream.
+int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
+    const int64_t C = m->cache_slots;
+    if (C == 0) return WD_OK;
+    if (flush) {
+        cache_flush_kernel<<<grid_for(C * (m->stage_stride / 4), 256), 256, 0, m->stream>>>(C, m->stage_stride, m->d_ctag, m->d_cdirty, m->n_rtab,
+                                                                                          m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_stage);
+        m->launches++;
+    }
+    cache_clear_kernel<<<grid_for(C, 256), 256, 0, m->stream>>>(C, m->d_ctag, m->d_cstamp, m->d_cdirty, invalidate ? 1 : 0);
+    m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
@@ -109,6 +309,52 @@ static int upload(WdModel* m, T** dst, const std::vector<T>& h) {
 template <typename T>
 static int overwrite(WdModel* m, T* dst, const std::vector<T>& h) {
     WD_CUDA(cudaMemcpyAsync(dst, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, m->stream));
+    return WD_OK;
+}
+
+// What the gather kernels and the fused updates address: host tables through the staging buffer (data = d_stage, row base 0,
+// stride stage_stride), every other table in place.  alloc: upload the descriptor arrays (place_tables); else overwrite the ones
+// that carry the staging buffer's address (wd_host_cache_enable replaces the buffer).
+static int stage_descriptors(WdModel* m, bool alloc) {
+    const int nt = (int)m->tables.size();
+    int rc;
+    std::vector<float*> gdata(nt), rgdata;
+    std::vector<int32_t> gstride(nt), stage(nt, 0), rstage;
+    std::vector<int64_t> grb(nt);
+    for (int t = 0; t < nt; ++t) {
+        const EmbTable& tb = m->tables[t];
+        gdata[t] = tb.host ? m->d_stage : tb.data;
+        gstride[t] = tb.host ? m->stage_stride : tb.stride;
+        grb[t] = tb.host ? 0 : tb.row_base;
+        stage[t] = tb.host ? m->stage_stride : 0;
+    }
+    for (int t : m->rtab_order) {
+        const EmbTable& tb = m->tables[t];
+        rgdata.push_back(tb.host ? m->d_stage : tb.data);
+        rstage.push_back(tb.host ? m->stage_stride : 0);
+    }
+    if (m->n_host_tab > 0) {
+        if (alloc) {
+            if ((rc = upload(m, &m->d_gtab_data, gdata))) return rc;
+            if ((rc = upload(m, &m->d_gtab_stride, gstride))) return rc;
+            if ((rc = upload(m, &m->d_gtab_row_base, grb))) return rc;
+            if ((rc = upload(m, &m->d_tab_stage, stage))) return rc;
+            if ((rc = upload(m, &m->d_rtab_gdata, rgdata))) return rc;
+            if ((rc = upload(m, &m->d_rtab_stage, rstage))) return rc;
+        } else {
+            if ((rc = overwrite(m, m->d_gtab_data, gdata))) return rc;
+            if (!rgdata.empty() && (rc = overwrite(m, m->d_rtab_gdata, rgdata))) return rc;
+        }
+    }
+    for (int i = 0; i < m->n_dims; ++i) {    // per-width descriptors of the short-bag gather (table ids ascending, as build_model)
+        std::vector<TabDesc> descs;
+        for (int t = 0; t < nt; ++t) {
+            const EmbTable& tb = m->tables[t];
+            if (tb.dim != m->dims[i] || tb.sharded) continue;
+            descs.push_back(TabDesc{gdata[t], grb[t], gstride[t], tb.x0_off, tb.col, tb.dim});
+        }
+        if ((rc = overwrite(m, m->d_dim_desc[i], descs))) return rc;
+    }
     return WD_OK;
 }
 
@@ -169,46 +415,90 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
     for (int t : m->rtab_order) rdata.push_back(m->tables[t].data);
     if ((rc = overwrite(m, m->d_tab_data, data))) return rc;
     if (!rdata.empty() && (rc = overwrite(m, m->d_rtab_data, rdata))) return rc;
-    // what the gather kernels / fused updates address: host tables through the staging buffer
-    std::vector<float*> gdata(data), rgdata(rdata);
-    std::vector<int32_t> gstride(nt), stage(nt, 0), rstage;
-    std::vector<int64_t> grb(nt);
-    for (int t = 0; t < nt; ++t) {
-        const EmbTable& tb = m->tables[t];
-        gstride[t] = tb.host ? m->stage_stride : tb.stride;
-        grb[t] = tb.host ? 0 : tb.row_base;
-        stage[t] = tb.host ? m->stage_stride : 0;
-    }
-    for (size_t i = 0; i < m->rtab_order.size(); ++i) {
-        const bool h = m->tables[m->rtab_order[i]].host;
-        rstage.push_back(h ? m->stage_stride : 0);
-    }
     if (m->n_host_tab > 0) {
         if ((rc = dev_alloc(m, &m->d_stage, m->max_nnz * (int64_t)m->stage_stride, true))) return rc;
         if ((rc = dev_alloc(m, &m->d_g_emb, m->max_nnz, true))) return rc;
-        for (int t = 0; t < nt; ++t) if (m->tables[t].host) gdata[t] = m->d_stage;
-        for (size_t i = 0; i < m->rtab_order.size(); ++i) if (rstage[i]) rgdata[i] = m->d_stage;
-        if ((rc = upload(m, &m->d_gtab_data, gdata))) return rc;
-        if ((rc = upload(m, &m->d_gtab_stride, gstride))) return rc;
-        if ((rc = upload(m, &m->d_gtab_row_base, grb))) return rc;
-        if ((rc = upload(m, &m->d_tab_stage, stage))) return rc;
-        if ((rc = upload(m, &m->d_rtab_gdata, rgdata))) return rc;
-        if ((rc = upload(m, &m->d_rtab_stage, rstage))) return rc;
     } else {                                 // nothing on the host: the step addresses the tables' own arrays
         m->d_g_emb = m->d_e_emb;
         m->d_gtab_data = m->d_tab_data; m->d_gtab_stride = m->d_tab_stride; m->d_gtab_row_base = m->d_tab_row_base;
         m->d_rtab_gdata = m->d_rtab_data;
     }
-    for (int i = 0; i < m->n_dims; ++i) {    // per-width descriptors of the short-bag gather (table ids ascending, as build_model)
-        std::vector<TabDesc> descs;
-        for (int t = 0; t < nt; ++t) {
-            const EmbTable& tb = m->tables[t];
-            if (tb.dim != m->dims[i] || tb.sharded) continue;
-            descs.push_back(TabDesc{gdata[t], grb[t], gstride[t], tb.x0_off, tb.col, tb.dim});
-        }
-        if ((rc = overwrite(m, m->d_dim_desc[i], descs))) return rc;
-    }
+    if ((rc = stage_descriptors(m, true))) return rc;
     WD_CUDA(cudaStreamSynchronize(m->stream));
+    return WD_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------ C-ABI
+extern "C" int wd_host_cache_enable(WdModel* m, int64_t bytes) {
+    if (!m) { set_error("null model"); return WD_EINVAL; }
+    if (bytes < 0) { set_error("host cache: negative budget %lld", (long long)bytes); return WD_EINVAL; }
+    WD_CUDA(cudaSetDevice(m->device));
+    if (m->stepped) { set_error("wd_host_cache_enable after the first step or forward: the step graphs are already captured"); return WD_ESTATE; }
+    if (m->cache_slots > 0) { set_error("wd_host_cache_enable: the cache is already enabled"); return WD_ESTATE; }
+    if (m->n_host_tab == 0) return WD_OK;                                // nothing on the host: capacity 0
+    const int64_t S = m->stage_stride, slot_bytes = S * 4;
+    const int64_t sets = bytes / (kWays * slot_bytes);
+    if (sets < 1) return WD_OK;
+    int bits = 0;
+    while (((int64_t)2 << bits) <= sets) ++bits;
+    const int64_t C = (int64_t)kWays << bits;
+    if (C + m->max_nnz >= ((int64_t)1 << 31)) {
+        set_error("host cache: %lld slots + %lld overflow rows do not fit 31-bit staging rows", (long long)C, (long long)m->max_nnz);
+        return WD_EINVAL;
+    }
+    // HBM the cache adds: its slots, per-slot tag / stamp / dirty, and per unique row uslot / uvict / uflag + the (set, u) sort pairs
+    const int64_t meta = C * 9 + 4 + 4 * 8 + m->max_nnz * 9 + 4 * (m->max_nnz + 8) * 4;
+    size_t free_b = 0, total_b = 0;
+    WD_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const int64_t reserve = hbm_reserve_bytes(m);
+    if ((int64_t)free_b - (C * slot_bytes + meta) < reserve) {
+        set_error("host cache of %lld bytes would leave %lld bytes of HBM free, less than the %lld the model keeps for its later allocations",
+                  (long long)(C * slot_bytes), (long long)((int64_t)free_b - C * slot_bytes - meta), (long long)reserve);
+        return WD_ENOMEM;
+    }
+    // the staging buffer grows to [C slots | max_nnz overflow rows]: the old one is freed and every descriptor re-pointed
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    auto it = std::find(m->allocs.begin(), m->allocs.end(), (void*)m->d_stage);
+    if (it != m->allocs.end()) {
+        WD_CUDA(cudaFree(m->d_stage));
+        m->allocs.erase(it);
+        m->bytes_allocated -= m->max_nnz * slot_bytes;
+    }
+    m->d_stage = nullptr;
+    int rc;
+    if ((rc = dev_alloc(m, &m->d_stage, (C + m->max_nnz) * S, false))) return rc;
+    if ((rc = dev_alloc(m, &m->d_ctag, C, false))) return rc;
+    WD_CUDA(cudaMemsetAsync(m->d_ctag, 0xFF, C * 4, m->stream));       // kInvalidRow
+    if ((rc = dev_alloc(m, &m->d_cstamp, C))) return rc;
+    if ((rc = dev_alloc(m, &m->d_cdirty, C))) return rc;
+    if ((rc = dev_alloc(m, &m->d_cnow, 1))) return rc;
+    if ((rc = dev_alloc(m, &m->d_cstats, 4))) return rc;
+    if ((rc = dev_alloc(m, &m->d_uslot, m->max_nnz))) return rc;
+    if ((rc = dev_alloc(m, &m->d_uvict, m->max_nnz))) return rc;
+    if ((rc = dev_alloc(m, &m->d_uflag, m->max_nnz))) return rc;
+    for (int k = 0; k < 2; ++k) {
+        if ((rc = dev_alloc(m, &m->d_ck[k], m->max_nnz + 8))) return rc;
+        if ((rc = dev_alloc(m, &m->d_cv[k], m->max_nnz + 8))) return rc;
+    }
+    m->cache_slots = C;
+    m->cache_set_bits = bits;
+    if ((rc = stage_descriptors(m, false))) return rc;
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    return WD_OK;
+}
+
+extern "C" int wd_host_cache_stats(WdModel* m, int64_t* out, int32_t n, int32_t reset) {
+    if (!m || n < 0 || (n > 0 && !out)) { set_error("null argument"); return WD_EINVAL; }
+    WD_CUDA(cudaSetDevice(m->device));
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    unsigned long long h[4] = {0, 0, 0, 0};
+    if (m->d_cstats) WD_CUDA(cudaMemcpy(h, m->d_cstats, sizeof(h), cudaMemcpyDeviceToHost));
+    const int64_t v[5] = {m->cache_slots, (int64_t)h[0], (int64_t)h[1], (int64_t)h[2], (int64_t)h[3]};
+    for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
+    if (reset && m->d_cstats) {
+        WD_CUDA(cudaMemsetAsync(m->d_cstats, 0, sizeof(h), m->stream));
+        WD_CUDA(cudaStreamSynchronize(m->stream));
+    }
     return WD_OK;
 }
 

@@ -71,7 +71,7 @@ int init_sparse_tables(WdModel* m, uint64_t seed, int random_w) {
         m->launches++;
     }
     WD_CUDA(cudaGetLastError());
-    return WD_OK;
+    return host_cache_sync(m, false, true);                     // the host records were rewritten: cached copies are stale
 }
 
 // ----------------------------------------------------------------------------------------------- metrics

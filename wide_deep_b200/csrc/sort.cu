@@ -411,9 +411,9 @@ __global__ void __launch_bounds__(RS_THREADS) rs_scatter_kernel(const uint32_t* 
     }
 }
 
-// Sort pairs (m->d_sk[which], m->d_sv[which]) of length *d_n by the low `bits` bits of the key.
-// On return the sorted pairs are in d_sk/d_sv (buffers are swapped as needed).
-int radix_sort_pairs(WdModel* m, int which, int bits, const int32_t* d_n) {
+// Sort pairs (*keys, *vals) of length *d_n by the low `bits` bits of the key, with (*keys2, *vals2) as the ping-pong buffers.
+// On return the sorted pairs are in (*keys, *vals) (the pointers are swapped as needed).  Scratch: the current stream's set.
+int radix_sort_pairs(WdModel* m, uint32_t** keys, uint32_t** vals, uint32_t** keys2, uint32_t** vals2, int bits, const int32_t* d_n) {
     if (bits < 1) bits = 1;
     // Lists of millions of keys (the wide-only workload: 5.4 M keys per step): 4096-key tiles reordered in shared memory before
     // they are written (rs_scatter_kernel<.., true>; on an H100 80GB HBM3 at 700 W the wide workload trains at 89 M examples/s
@@ -447,19 +447,19 @@ int radix_sort_pairs(WdModel* m, int which, int bits, const int32_t* d_n) {
                 WD_CUDA(cudaFuncSetAttribute(rs_scatter_kernel<RS_BIG_TILE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
                 m->sort_smem_opt_in = true;
             }
-            rs_hist_kernel<RS_BIG_TILE><<<ntiles_cap, RS_THREADS, sh_h, m->stream>>>(m->d_sk[which], d_n, shift, bins, hist, gtot + p * bins);
+            rs_hist_kernel<RS_BIG_TILE><<<ntiles_cap, RS_THREADS, sh_h, m->stream>>>(*keys, d_n, shift, bins, hist, gtot + p * bins);
             rs_colscan_kernel<RS_BIG_TILE><<<gcs, 256, 0, m->stream>>>(d_n, bins, hist, gtot + p * bins);
             rs_scatter_kernel<RS_BIG_TILE, true><<<ntiles_cap, RS_THREADS, sh_l, m->stream>>>(
-                m->d_sk[which], m->d_sv[which], m->d_sk2[which], m->d_sv2[which], d_n, shift, bins, hist, gtot + p * bins);
+                *keys, *vals, *keys2, *vals2, d_n, shift, bins, hist, gtot + p * bins);
         } else {
-            rs_hist_kernel<kSortTile><<<ntiles_cap, RS_THREADS, sh_h, m->stream>>>(m->d_sk[which], d_n, shift, bins, hist, gtot + p * bins);
+            rs_hist_kernel<kSortTile><<<ntiles_cap, RS_THREADS, sh_h, m->stream>>>(*keys, d_n, shift, bins, hist, gtot + p * bins);
             rs_colscan_kernel<kSortTile><<<gcs, 256, 0, m->stream>>>(d_n, bins, hist, gtot + p * bins);
             rs_scatter_kernel<kSortTile, false><<<ntiles_cap, RS_THREADS, sh_s, m->stream>>>(
-                m->d_sk[which], m->d_sv[which], m->d_sk2[which], m->d_sv2[which], d_n, shift, bins, hist, gtot + p * bins);
+                *keys, *vals, *keys2, *vals2, d_n, shift, bins, hist, gtot + p * bins);
         }
         m->launches += 3;
-        std::swap(m->d_sk[which], m->d_sk2[which]);
-        std::swap(m->d_sv[which], m->d_sv2[which]);
+        std::swap(*keys, *keys2);
+        std::swap(*vals, *vals2);
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;

@@ -235,9 +235,9 @@ __global__ void sort_keys_kernel(const int32_t* __restrict__ d_nnz, const uint32
 // APPLY (single-GPU step, row-local optimizer): the optimizer update of a directly summed row follows its sum in the same thread —
 // the summed gradient never reaches memory; the hot rows are updated by chunk_combine_kernel<1>.
 // tab_stage (null without host tables): per table 0 = record in place, else the table is staged — the record of unique row `it`
-// is at tab_data[t] (the staging buffer) + it * tab_stage[t].
+// is at tab_data[t] (the staging buffer) + uslot[it] * tab_stage[t], or + it * tab_stage[t] when uslot is null (no HBM cache).
 struct RowApply { const uint32_t* urow; float* const* tab_data; const int32_t* tab_stride; const int64_t* tab_row_base; OptParams o;
-                  const int32_t* tab_stage; };
+                  const int32_t* tab_stage; const int32_t* uslot; };
 template <bool APPLY>
 __global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ d_nchunks,
                                                            const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff,
@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __rest
                 if (q * 4 < dim) {
                     const int stride = ra.tab_stride[t];
                     const int sst = ra.tab_stage ? ra.tab_stage[t] : 0;
-                    float* rec = ra.tab_data[t] + (sst ? it * sst : ((int64_t)ra.urow[it] - ra.tab_row_base[t]) * stride);
+                    float* rec = ra.tab_data[t] + (sst ? (ra.uslot ? (int64_t)ra.uslot[it] : it) * sst : ((int64_t)ra.urow[it] - ra.tab_row_base[t]) * stride);
                     const int nslots = stride / dim - 1;
                     float4 w = *reinterpret_cast<float4*>(rec + q * 4);
                     float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + q * 4) : make_float4(0, 0, 0, 0);
@@ -330,6 +330,7 @@ struct HotApply {
     float4* wide;                                                                                                                          // KIND 2
     OptParams o;
     const int32_t* tab_stage;     // KIND 1, as RowApply::tab_stage (tables in row order): staged record of unique row uu at tab_data + uu * tab_stage
+    const int32_t* uslot;         // KIND 1, as RowApply::uslot: with an HBM cache the record is at tab_data + uslot[uu] * tab_stage
 };
 template <int KIND>
 __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ choff,
@@ -383,7 +384,7 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
                         const int dim = ha.tab_dim[lo], stride = ha.tab_stride[lo];
                         if (lq * 4 < dim) {
                             const int sst = ha.tab_stage ? ha.tab_stage[lo] : 0;
-                            float* rec = ha.tab_data[lo] + (sst ? uu * sst : (row - ha.tab_row_base[lo]) * stride);
+                            float* rec = ha.tab_data[lo] + (sst ? (ha.uslot ? (int64_t)ha.uslot[uu] : uu) * sst : (row - ha.tab_row_base[lo]) * stride);
                             const int nslots = stride / dim - 1;
                             float4 w = *reinterpret_cast<float4*>(rec + lq * 4);
                             float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + lq * 4) : make_float4(0, 0, 0, 0);
@@ -507,7 +508,7 @@ static int group_rows(WdModel* m, int which, const int32_t* d_n, const uint32_t*
     int g = grid_for(m->max_nnz, 256);
     sort_keys_kernel<<<g, 256, 0, m->stream>>>(d_n, e_row, invalid, m->d_sk[which], m->d_sv[which], val_src);
     m->launches++;
-    int rc = radix_sort_pairs(m, which, m->sort_bits[which] + 1, d_n);
+    int rc = radix_sort_pairs(m, &m->d_sk[which], &m->d_sv[which], &m->d_sk2[which], &m->d_sv2[which], m->sort_bits[which] + 1, d_n);
     if (rc) return rc;
     return group_tail(m, which, d_n);
 }
@@ -632,9 +633,9 @@ int sparse_reduce_emb(WdModel* m) {
         // the hot rows' update lives in the lane-group branch of chunk_combine_kernel: widths 4, 8, ..., 128
         const bool fused = fuse_row_apply(m, m->dnn_opt) && width >= 4 && (G4 & (G4 - 1)) == 0 && G4 <= 32;
         // (host tables: the fused updates go to the staged records, host_tables_write_back copies them home after the list's apply)
-        const RowApply ra{m->d_urow[0], m->d_gtab_data, m->d_tab_stride, m->d_tab_row_base, make_opt(m->dnn_opt), m->d_tab_stage};
+        const RowApply ra{m->d_urow[0], m->d_gtab_data, m->d_tab_stride, m->d_tab_row_base, make_opt(m->dnn_opt), m->d_tab_stage, m->d_uslot};
         const HotApply ha{m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_gdata, m->d_rtab_dim, m->d_rtab_stride, nullptr, make_opt(m->dnn_opt),
-                          m->d_rtab_stage};
+                          m->d_rtab_stage, m->d_uslot};
         if (fused) {
             emb_grad_sum_kernel<true><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], m->d_sv[0],
                 m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->d_tab_dim, m->d_tab_x0, m->d_dX0, m->d0_phys, m->d_ugrad[0], m->d_cpart[0], width, ra);
@@ -841,6 +842,10 @@ int sparse_apply_which(WdModel* m, int which) {
     // the fused updates of host-table rows went to their staged copies: copy those home (the unfused kernels below update host
     // records in place, through the mapped pointers of d_rtab_data)
     if (done) return (which == 0 && m->n_host_tab > 0) ? host_tables_write_back(m) : WD_OK;
+    if (which == 0 && m->cache_slots > 0) {       // the unfused updates below would write host records behind the cache's back
+        set_error("embedding rows of a model with a host-table cache are only updated by the fused single-GPU step");
+        return WD_EUNSUPPORTED;
+    }
     if (which == 0 && m->use_deep && !m->tables.empty()) {
         const bool adam = m->dnn_opt.kind == WD_OPT_ADAM;
         if (adam && (rc = adam_dense_pass(m, 0, false))) return rc;
@@ -866,7 +871,7 @@ int sparse_apply_which(WdModel* m, int which) {
 int list_sort_by_key(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_key) {
     sort_keys_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(d_n, e_key, 1u << m->sort_bits[which], m->d_sk[which], m->d_sv[which], nullptr);
     m->launches++;
-    return radix_sort_pairs(m, which, m->sort_bits[which] + 1, d_n);
+    return radix_sort_pairs(m, &m->d_sk[which], &m->d_sv[which], &m->d_sk2[which], &m->d_sv2[which], m->sort_bits[which] + 1, d_n);
 }
 int list_group(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row) {
     int rc = group_rows(m, which, d_n, e_row);

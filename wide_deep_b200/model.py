@@ -75,6 +75,8 @@ class WideDeepModel(object):
         self._h = h
         self.device = int(device)
         self.global_step = 0
+        if getattr(plan, "host_cache_bytes", 0) > 0:
+            check(self._lib.wd_host_cache_enable(self._h, int(plan.host_cache_bytes)))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -104,6 +106,13 @@ class WideDeepModel(object):
         dev, host = ctypes.c_int64(), ctypes.c_int64()
         check(self._lib.wd_memory_usage(self._h, ctypes.byref(dev), ctypes.byref(host)))
         return dev.value, host.value
+
+    def host_cache_stats(self, reset=False):
+        """Cumulative counters of the HBM cache of host-table records: dict(capacity (slots), hits, loads (misses loaded into a
+        slot), overflow (rows staged without a slot), evictions (dirty records written home)).  All 0 without a cache."""
+        out = (ctypes.c_int64 * 5)()
+        check(self._lib.wd_host_cache_stats(self._h, out, 5, 1 if reset else 0))
+        return dict(zip(("capacity", "hits", "loads", "overflow", "evictions"), (int(v) for v in out)))
 
     def n_slots(self, name):
         o = self.plan.lin_opt if name.startswith("linear/") else self.plan.dnn_opt
@@ -242,10 +251,10 @@ class WideDeepModel(object):
     def last_timings(self):
         """OrderedDict phase -> ms of the last synchronised step ('total' first); needs set_profile(True)."""
         from collections import OrderedDict
-        out = np.zeros(64, dtype=np.float32)
-        n = self._lib.wd_last_timings(self._h, out.ctypes.data, 64)
+        out = np.zeros(160, dtype=np.float32)                # PhaseTimer::kMax marks
+        n = self._lib.wd_last_timings(self._h, out.ctypes.data, out.size)
         res = OrderedDict()
-        for i in range(max(n, 0)):
+        for i in range(max(min(n, out.size), 0)):
             name = self._lib.wd_timing_name(self._h, i).decode()
             res[name] = res.get(name, 0.0) + float(out[i])
         return res

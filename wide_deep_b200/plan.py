@@ -148,7 +148,8 @@ class Plan(object):
 
     def __init__(self, feature_conf, cross_conf, model_conf, model_type="wide_deep", max_batch=8192,
                  embedding_dim_override=None, tf_compat_pad=False, gemm_engine="auto", max_nnz=0, max_keys=0,
-                 dense_exchange_max_rows=0, shard_world=1, shard_rank=0, shard_capacity=0, shard_slack=2.0, host_tables=None):
+                 dense_exchange_max_rows=0, shard_world=1, shard_rank=0, shard_capacity=0, shard_slack=2.0, host_tables=None,
+                 host_cache_bytes=0):
         if model_type not in ("wide", "deep", "wide_deep"):
             raise ValueError("Invalid model type: {}, must be one of `wide`, `deep`, `wide_deep`".format(model_type))
         self.model_type, self.max_batch, self.tf_compat_pad = model_type, int(max_batch), bool(tf_compat_pad)
@@ -330,6 +331,11 @@ class Plan(object):
                 raise ValueError("host_tables: no embedding table named {} (tables: {})".format(unknown, names))
         for t in self.tables:
             t["placement"] = PLACE_AUTO if want is None else (PLACE_HOST if t["name"] in want else PLACE_HBM)
+        # HBM budget (bytes) of the write-back cache of host-table records (wd_host_cache_enable); 0 = no cache.  The model has
+        # a cache only when some table ended up on the host.
+        if isinstance(host_cache_bytes, bool) or not isinstance(host_cache_bytes, (int, np.integer)) or host_cache_bytes < 0:
+            raise ValueError("host_cache_bytes must be an int >= 0, got {!r}".format(host_cache_bytes))
+        self.host_cache_bytes = int(host_cache_bytes)
 
         # ---- MLP
         hu = model_conf.get("dnn_hidden_units") or []
