@@ -282,7 +282,9 @@ uint64_t wd_fingerprint_cat64(uint64_t a, uint64_t b);
 int wd_debug_column_ids(WdModel *m, int32_t *offsets_out, int64_t offsets_cap, int64_t *ids_out, int64_t ids_cap, int64_t *nnz_out);
 /* Deep input matrix of the last forward: [batch, d0_phys]. */
 int wd_debug_deep_input(WdModel *m, float *out, int64_t cap);
-/* Output of hidden layer `layer` of tower `tower` after the last forward: [batch, N_phys]; returns N_phys. */
+/* Output of hidden layer `layer` of tower `tower` after the last forward: [batch, N_phys]; returns N_phys.  On the bf16x3 engine a
+ * layer that only other hidden layers read has no fp32 copy: it comes back as hi + lo of its bf16 copies, the value those layers'
+ * GEMMs read. */
 int wd_debug_hidden(WdModel *m, int tower, int layer, float *out, int64_t cap);
 /* Kernel launch counter (launches of this library's kernels since creation). */
 int64_t wd_launch_count(WdModel *m);

@@ -1550,11 +1550,15 @@ extern "C" int wd_debug_hidden(WdModel* m, int tower, int layer, float* out, int
     Layer& L = m->towers[tower].layers[layer];
     int64_t n = (int64_t)m->dbatch.B * L.N_phys;
     if (cap < n) { set_error("buffer too small"); return WD_EINVAL; }
-    if (m->gemm_engine == WD_GEMM_BF16X3 && !L.h_fp32) {
-        set_error("hidden layer %d is not materialised in fp32 by the bf16x3 engine (use gemm_engine ffma / tc3x to inspect it)", layer);
-        return WD_EUNSUPPORTED;
-    }
     WD_CUDA(cudaStreamSynchronize(m->stream));
+    if (m->gemm_engine == WD_GEMM_BF16X3 && !L.h_fp32) {
+        // no fp32 copy of this layer: hi + lo of its bf16 copies, the value the next layer's GEMM reads
+        std::vector<__nv_bfloat16> hi(n), lo(n);
+        WD_CUDA(cudaMemcpy(hi.data(), L.Hs[0], n * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
+        WD_CUDA(cudaMemcpy(lo.data(), L.Hs[1], n * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
+        for (int64_t i = 0; i < n; ++i) out[i] = __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
+        return L.N_phys;
+    }
     WD_CUDA(cudaMemcpy(out, L.H, n * 4, cudaMemcpyDeviceToHost));
     return L.N_phys;
 }

@@ -232,7 +232,9 @@ class WideDeepModel(object):
         return out
 
     def hidden_output(self, tower, layer, batch_size):
-        out = np.empty(batch_size * 4096, dtype=np.float32)
+        """[batch_size, N_phys] output of a hidden layer after the last forward (bf16x3 layers without an fp32 copy: hi + lo)."""
+        n_phys = (self.plan.out_width(self.plan.towers[tower]["hidden"][layer]) + 31) // 32 * 32
+        out = np.empty(batch_size * n_phys, dtype=np.float32)
         n = self._lib.wd_debug_hidden(self._h, tower, layer, out.ctypes.data, out.size)
         if n < 0:
             check(n)
