@@ -25,10 +25,13 @@
 // the layer output as bf16 hi/lo copies (what the next layer and the weight gradient read) and, only for layers the logits layer
 // reads, the fp32 layer output.  A quad of lanes owns 8 consecutive columns of a row, so every fp32 store instruction writes
 // whole 32-byte sectors.
+// The forward epilogue's per-column constants (bias, gamma' and beta of the tile's 128 columns) are fetched before the main loop
+// and handed to the epilogue through 3 KB of shared memory, so no global-load latency sits between its stores.
 #include <cuda.h>
 #include <stdlib.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "gemm.cuh"
@@ -73,6 +76,7 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
     auto b_lo = [&](int s) { return base + s * STAGE_BYTES + 2 * A_BYTES + B_BYTES; };
     uint64_t* bars = reinterpret_cast<uint64_t*>(base + QNST * STAGE_BYTES);
     uint64_t* full = bars; uint64_t* empty = bars + QNST;
+    float* epi_vec = reinterpret_cast<float*>(base + QNST * STAGE_BYTES + 64);   // FWD: 2 x [bias | gamma' | beta] of a tile's 128 columns
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int tiles_n = (N + QBN - 1) / QBN, tiles_m = (M + QBM - 1) / QBM;
@@ -159,6 +163,21 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
 #pragma unroll
                 for (int i = 0; i < QBN / 2; ++i) d[i] = 0.f;
             }
+            // FWD: the 384 per-column epilogue constants of this tile (bias, gamma * 1/sqrt(1 + eps), beta; each consumer thread
+            // fetches v = ct and ct + 256) are loaded now, so their latency hides under the main loop, and handed over through
+            // shared memory after it
+            const int ct = threadIdx.x - 128;
+            float pre[2] = {0.f, 0.f};
+            if (MODE == EPI_FWD) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int v = ct + 256 * i, c = n0 + (v & 127);
+                    const bool in = c < ep.n_logical;
+                    if (v < 128) pre[i] = in ? __ldg(ep.bias + c) : 0.f;
+                    else if (v < 256) pre[i] = (in && ep.bn) ? __ldg(ep.gamma + c) * 0.99950037468777f : 1.f;
+                    else if (v < 384) pre[i] = (in && ep.bn) ? __ldg(ep.beta + c) : 0.f;
+                }
+            }
             int prev = -1;
             for (int kb = 0; kb < nkb; ++kb, ++g) {
                 const int s = g % QNST, it = g / QNST;
@@ -187,50 +206,63 @@ __global__ void __launch_bounds__(Q_THREADS, 1) tc_gemm_bf16_kernel(const __grid
             wgmma_wait<0>();                                      // the accumulator is final
             if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
             if (cwarp == 0) PROBE(use == 0 ? 2 : 3);
+            // two buffers by tile parity: a thread writes tile t + 2's constants only after the barrier of tile t + 1, which every
+            // consumer thread reaches after its epilogue of tile t
+            const float* ev = epi_vec + (use & 1) * 384;
+            if (MODE == EPI_FWD) {
+                epi_vec[(use & 1) * 384 + ct] = pre[0];
+                if (ct < 128) epi_vec[(use & 1) * 384 + ct + 256] = pre[1];
+                bar_sync(1, 256);                                 // the two consumer warp groups
+            }
 
             // ---- epilogue from the accumulator fragment: rows r0 and r0 + 8, columns n0 + 8 j + 2 (lane % 4) + {0, 1}
             const int r0 = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
             const int cq = 2 * (lane & 3);
+            // The activation is dispatched once per tile, not per element: the relu body is then straight-line code the compiler
+            // can schedule across column groups (loads of the next group's bias / gamma / beta under the current group's stores).
+            auto epilogue = [&](auto relu) {
+                constexpr bool RELU = decltype(relu)::value;
 #pragma unroll
-            for (int j = 0; j < QBN / 8; ++j) {
-                const int c = n0 + 8 * j + cq;
-                if (n0 + 8 * j < N) {
-                    if (MODE == EPI_FWD) {
-                        const bool in0 = c < ep.n_logical, in1 = c + 1 < ep.n_logical;
-                        const float b0 = in0 ? __ldg(ep.bias + c) : 0.f, b1 = in1 ? __ldg(ep.bias + c + 1) : 0.f;
-                        const float g0 = (in0 && ep.bn) ? __ldg(ep.gamma + c) * 0.99950037468777f : 1.f;
-                        const float g1 = (in1 && ep.bn) ? __ldg(ep.gamma + c + 1) * 0.99950037468777f : 1.f;
-                        const float e0 = (in0 && ep.bn) ? __ldg(ep.beta + c) : 0.f, e1 = (in1 && ep.bn) ? __ldg(ep.beta + c + 1) : 0.f;
+                for (int j = 0; j < QBN / 8; ++j) {
+                    const int c = n0 + 8 * j + cq;
+                    if (n0 + 8 * j < N) {
+                        if (MODE == EPI_FWD) {
+                            const bool in0 = c < ep.n_logical, in1 = c + 1 < ep.n_logical;
+                            const int cl = 8 * j + cq;                   // column inside the tile
+                            const float b0 = ev[cl], b1 = ev[cl + 1], g0 = ev[128 + cl], g1 = ev[129 + cl], e0 = ev[256 + cl], e1 = ev[257 + cl];
 #pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            const int r = r0 + 8 * hh;
-                            if (r >= M) continue;
-                            const bool rv = r < ep.m_valid;          // rows past the batch: zeros
-                            float a0 = 0.f, a1 = 0.f, h0 = 0.f, h1 = 0.f;
-                            if (rv && in0) { a0 = ep.act == WD_ACT_RELU ? fmaxf(d[4 * j + 2 * hh] + b0, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh] + b0); h0 = fmaf(a0, g0, e0); }
-                            if (rv && in1) { a1 = ep.act == WD_ACT_RELU ? fmaxf(d[4 * j + 2 * hh + 1] + b1, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh + 1] + b1); h1 = fmaf(a1, g1, e1); }
-                            const int64_t o = (int64_t)r * ep.ldh + c;
-                            if (ep.A_out != ep.H_out) *reinterpret_cast<float2*>(ep.A_out + o) = make_float2(a0, a1);
-                            if (ep.H_out) *reinterpret_cast<float2*>(ep.H_out + o) = make_float2(h0, h1);   // fp32 copy only where something reads it
-                            uint32_t ph, pl;
-                            split_pair(h0, h1, ph, pl);
-                            *reinterpret_cast<uint32_t*>(ep.Hs_hi + o) = ph;
-                            *reinterpret_cast<uint32_t*>(ep.Hs_lo + o) = pl;
-                        }
-                    } else {
-                        float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0);
+                            for (int hh = 0; hh < 2; ++hh) {
+                                const int r = r0 + 8 * hh;
+                                if (r >= M) continue;
+                                const bool rv = r < ep.m_valid;          // rows past the batch: zeros
+                                float a0 = 0.f, a1 = 0.f, h0 = 0.f, h1 = 0.f;
+                                if (rv && in0) { a0 = RELU ? fmaxf(d[4 * j + 2 * hh] + b0, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh] + b0); h0 = fmaf(a0, g0, e0); }
+                                if (rv && in1) { a1 = RELU ? fmaxf(d[4 * j + 2 * hh + 1] + b1, 0.f) : act_fwd(ep.act, d[4 * j + 2 * hh + 1] + b1); h1 = fmaf(a1, g1, e1); }
+                                const int64_t o = (int64_t)r * ep.ldh + c;
+                                if (ep.A_out != ep.H_out) *reinterpret_cast<float2*>(ep.A_out + o) = make_float2(a0, a1);
+                                if (ep.H_out) *reinterpret_cast<float2*>(ep.H_out + o) = make_float2(h0, h1);   // fp32 copy only where something reads it
+                                uint32_t ph, pl;
+                                split_pair(h0, h1, ph, pl);
+                                *reinterpret_cast<uint32_t*>(ep.Hs_hi + o) = ph;
+                                *reinterpret_cast<uint32_t*>(ep.Hs_lo + o) = pl;
+                            }
+                        } else {
+                            float* Cb = ep.C + (MODE == EPI_WGRAD ? (int64_t)z * ep.split_stride : 0);
 #pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            const int r = r0 + 8 * hh;
-                            if (r >= M) continue;
-                            float2* pc = reinterpret_cast<float2*>(Cb + (int64_t)r * ep.ldc + c);
-                            float2 o = make_float2(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1]);
-                            if (MODE == EPI_STORE && ep.accumulate) { const float2 p = *pc; o.x += p.x; o.y += p.y; }
-                            *pc = o;
+                            for (int hh = 0; hh < 2; ++hh) {
+                                const int r = r0 + 8 * hh;
+                                if (r >= M) continue;
+                                float2* pc = reinterpret_cast<float2*>(Cb + (int64_t)r * ep.ldc + c);
+                                float2 o = make_float2(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1]);
+                                if (MODE == EPI_STORE && ep.accumulate) { const float2 p = *pc; o.x += p.x; o.y += p.y; }
+                                *pc = o;
+                            }
                         }
                     }
                 }
-            }
+            };
+            if (MODE == EPI_FWD && ep.act == WD_ACT_RELU) epilogue(std::true_type{});
+            else epilogue(std::false_type{});
             if (cwarp == 0) PROBE(use == 0 ? 4 : 5);
             ++use;
         }
@@ -241,7 +273,7 @@ int g_probe_slot = 0;
 
 template <int MODE>
 int launch_q(WdModel* m, const QMaps& maps, const QSegs& segs, int M, int N, int ktot, int splits, int ksplit_len, const Epi& ep) {
-    constexpr int smem = QNST * 2 * (QBM * 128 + QBN * 128) + 1024 + 128;
+    constexpr int smem = QNST * 2 * (QBM * 128 + QBN * 128) + 1024 + 64 + 2 * 384 * 4;
     static bool configured = false;
     static int num_sms = 0;
     if (!configured) {

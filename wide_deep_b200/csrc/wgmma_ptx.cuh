@@ -31,6 +31,9 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
                  ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
+// named barrier `id` (1-15; 0 is __syncthreads) over `n` threads, a multiple of 32
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
 // register budget of a warp group: the TMA / splitter groups hand registers to the groups that hold the accumulators
 template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
