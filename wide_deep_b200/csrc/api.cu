@@ -26,7 +26,7 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 int init_sparse_tables(WdModel* m, uint64_t seed, int random_w);
-int dense_refresh_transposes(WdModel* m);
+int refresh_weight_copies(WdModel* m);
 int wide_bias_grad(WdModel* m);
 int metrics_setup();
 int merge_sparse(WdModel* m, int which, const void* rows, const void* grads, int64_t n);
@@ -181,6 +181,8 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     m->ldt = m->max_batch_pad;
     m->row_tiles = m->max_batch_pad / 128;
     m->gemm_engine = d->gemm_engine == WD_GEMM_AUTO ? WD_GEMM_TC3X : d->gemm_engine;
+    m->operands = m->gemm_engine == WD_GEMM_BF16X3 ? kBf16Operands : kFp32Operands;
+    const bool fp32_ops = m->operands == kFp32Operands;
     m->dense_exchange_max_rows = d->dense_exchange_max_rows > 0 ? d->dense_exchange_max_rows : 0;
     m->small_base[1] = (m->dense_exchange_max_rows > 0 && d->wide_small_base >= 0 && d->wide_small_base <= d->wide_rows) ? d->wide_small_base : d->wide_rows;
     m->max_nnz = d->max_nnz > 0 ? d->max_nnz : (int64_t)d->max_batch * std::max(C, 1) * 2;
@@ -386,9 +388,9 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         }
         const int64_t actn = (int64_t)m->max_batch_pad * d->d0_phys;
         if ((rc = dev_alloc(m, &m->d_X0, actn))) return rc;
-        if ((rc = dev_alloc(m, &m->d_X0T, actn))) return rc;
+        if (fp32_ops && (rc = dev_alloc(m, &m->d_X0T, actn))) return rc;
         if (G == 1 && (rc = dev_alloc(m, &m->d_dX0, actn))) return rc;      // (sharded runs: inside the exchange segment, peers read it)
-        if (m->gemm_engine == WD_GEMM_BF16X3)
+        if (!fp32_ops)
             for (int part = 0; part < 2; ++part) {
                 if ((rc = dev_alloc(m, &m->d_X0s[part], actn))) return rc;
             }
@@ -425,8 +427,8 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
                 L.N_phys = hidden ? pad_to(hu[l], 32) : 1;
                 L.N_param = hidden ? units[l] : 1;
                 L.t_gamma = L.t_beta = -1;
-                L.h_fp32 = false;
-                for (int src : srcs[tw.n_hidden]) if (src == l) L.h_fp32 = true;      // read by the logits layer
+                bool logits_reads = false;
+                for (int src : srcs[tw.n_hidden]) if (src == l) logits_reads = true;
                 std::vector<int> idx(4, -1);
                 if (hidden) {
                     // split-K factor of the weight gradient: enough (tile x split) work items to fill one wave of SMs,
@@ -447,14 +449,16 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
                         L.t_beta = add_dense(1, L.N_phys, m->row_tiles, 1, L.N_phys, false);
                     }
                     const int64_t n = (int64_t)m->max_batch_pad * L.N_phys;
-                    if ((rc = dev_alloc(m, &L.H, n))) return rc;
+                    // the bf16 family keeps the layer output in fp32 only where the logits layer (not a GEMM) reads it
+                    if ((fp32_ops || logits_reads) && (rc = dev_alloc(m, &L.H, n))) return rc;
                     // post-activation values are kept apart from the layer output whenever something sits between them (BN affine, dropout)
-                    if (m->batch_norm || m->dropout_rate > 0.f) { if ((rc = dev_alloc(m, &L.A, n))) return rc; } else L.A = L.H;
-                    if ((rc = dev_alloc(m, &L.HT, n))) return rc;
+                    if (m->batch_norm || m->dropout_rate > 0.f || !L.H) { if ((rc = dev_alloc(m, &L.A, n))) return rc; } else L.A = L.H;
+                    if (fp32_ops && (rc = dev_alloc(m, &L.HT, n))) return rc;
                     if ((rc = dev_alloc(m, &L.dH, n))) return rc;
-                    if ((rc = dev_alloc(m, &L.dZ, n))) return rc;
-                    if ((rc = dev_alloc(m, &L.dZT, n))) return rc;
-                    if (m->gemm_engine == WD_GEMM_BF16X3)
+                    if (fp32_ops) {
+                        if ((rc = dev_alloc(m, &L.dZ, n))) return rc;
+                        if ((rc = dev_alloc(m, &L.dZT, n))) return rc;
+                    } else
                         for (int part = 0; part < 2; ++part) {
                             if ((rc = dev_alloc(m, &L.Hs[part], n))) return rc;
                             if ((rc = dev_alloc(m, &L.dZs[part], n))) return rc;
@@ -488,8 +492,15 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         if ((rc = dev_alloc(m, &m->d_S2, m->dense_count))) return rc;
         if (G == 1 && (rc = dev_alloc(m, &m->d_G, m->dense_count + m->gs_count))) return rc;
         if ((rc = dev_alloc(m, &m->d_gpart, m->gpart_count))) return rc;
-        if ((rc = dev_alloc(m, &m->d_Wt, std::max<int64_t>(m->wt_count, 1)))) return rc;
-        if ((rc = dev_alloc(m, &m->d_Wsplit, std::max<int64_t>(4 * m->wt_count, 1)))) return rc;
+        if (fp32_ops) {
+            if ((rc = dev_alloc(m, &m->d_Wt, m->wt_count))) return rc;
+            float* split;                                            // the four tf32 splits share one allocation
+            if ((rc = dev_alloc(m, &split, 4 * m->wt_count))) return rc;
+            m->d_W_hi = split; m->d_W_lo = split + m->wt_count; m->d_Wt_hi = split + 2 * m->wt_count; m->d_Wt_lo = split + 3 * m->wt_count;
+        } else {
+            if ((rc = dev_alloc(m, &m->d_Wq_hi, m->wt_count))) return rc;
+            if ((rc = dev_alloc(m, &m->d_Wq_lo, m->wt_count))) return rc;
+        }
         const DenseTensor* dp;
         if ((rc = upload_vec(m, m->dense.data(), (int64_t)m->dense.size(), &dp))) return rc;
         m->d_dense_desc = (DenseTensor*)dp;
@@ -632,7 +643,7 @@ static int init_dense(WdModel* m, WdModelExtra* x, uint64_t seed) {
     WD_CUDA(cudaMemcpyAsync(m->d_S1, S1.data(), S1.size() * 4, cudaMemcpyHostToDevice, m->stream));
     WD_CUDA(cudaMemcpyAsync(m->d_S2, S2.data(), S2.size() * 4, cudaMemcpyHostToDevice, m->stream));
     WD_CUDA(cudaStreamSynchronize(m->stream));
-    return dense_refresh_transposes(m);
+    return refresh_weight_copies(m);
 }
 
 extern "C" int wd_model_init(WdModel* m, uint64_t seed) {
@@ -768,7 +779,7 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         // kernel on this (non-blocking) stream starts
         WD_CUDA(cudaMemcpyAsync(arena + t.off, phys.data(), t.count * 4, cudaMemcpyHostToDevice, m->stream));
         WD_CUDA(cudaStreamSynchronize(m->stream));
-        if (slot == 0 && t.wt_off >= 0) return dense_refresh_transposes(m);
+        if (slot == 0 && t.wt_off >= 0) return refresh_weight_copies(m);
     }
     return WD_OK;
 }
@@ -1019,7 +1030,7 @@ static int backward_core(WdModel* m) {
     // single-GPU fused step with the wide list on its side stream: the dense optimizer of everything but the first layer's kernel
     // runs there (after the wide rows' updates), under that kernel's weight-gradient GEMM
     m->dense_split_tensor = -1;
-    m->record_wgrad_rest = m->fuse_dense && m->side_active[1] && m->gemm_engine == WD_GEMM_BF16X3 && !m->timer.enabled && !m->crelu;
+    m->record_wgrad_rest = m->fuse_dense && m->side_active[1] && m->operands == kBf16Operands && !m->timer.enabled && !m->crelu;
     if ((rc = mlp_backward(m))) return rc;
     m->record_dx0 = false;
     m->record_wgrad_rest = false;
@@ -1551,7 +1562,7 @@ extern "C" int wd_debug_hidden(WdModel* m, int tower, int layer, float* out, int
     int64_t n = (int64_t)m->dbatch.B * L.N_phys;
     if (cap < n) { set_error("buffer too small"); return WD_EINVAL; }
     WD_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->gemm_engine == WD_GEMM_BF16X3 && !L.h_fp32) {
+    if (!L.H) {
         // no fp32 copy of this layer: hi + lo of its bf16 copies, the value the next layer's GEMM reads
         std::vector<__nv_bfloat16> hi(n), lo(n);
         WD_CUDA(cudaMemcpy(hi.data(), L.Hs[0], n * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));

@@ -104,9 +104,13 @@ struct DenseTensor {         // one trainable dense tensor inside the dense aren
     int gparts;
     int g_rowtiles;          // 1: partials are per 128-row batch tile (only the tiles of the current batch are live)
     int64_t gstride;
-    int64_t wt_off;          // offset of the transposed copy in the wt buffer, -1 if none
+    int64_t wt_off;          // offset in each GEMM weight copy (WdModel::d_Wt ... d_Wq_lo), -1 if none
     int mirror_u;            // crelu layers (kernel, bias): column n + mirror_u holds minus column n, n < mirror_u (0: plain tensor)
 };
+
+// Stored operand forms the MLP GEMMs read (table at the top of mlp.cu): fp32 and transposed fp32 copies for the ffma, tc1x and
+// tc3x engines, bf16 hi / lo copies for bf16x3.  A model allocates and writes only its family's copies.
+enum OperandFamily { kFp32Operands = 0, kBf16Operands = 1 };
 
 struct Seg {                 // one source of a layer input
     int src;                 // -1: deep input x, >=0: hidden layer index of the same tower
@@ -123,16 +127,15 @@ struct Layer {
     int N_param;             // logical columns of kernel / bias: N, or N / 2 for a crelu layer (the other half mirrors them)
     int t_kernel, t_bias, t_gamma, t_beta;   // indices into Model::dense (-1 if absent)
     int wgrad_splits;        // split-K factor of this layer's weight gradient (= gparts of its kernel tensor)
-    // activations (hidden layers only), all [max_batch_pad, N_phys] unless noted
-    float* A;                // post-activation (pre-BN); == H when no batch norm
-    float* H;                // layer output
-    float* HT;               // transposed output [N_phys, ldt]
+    // activations (hidden layers only), all [max_batch_pad, N_phys] unless noted; null where the model's operand family has no
+    // such copy (table at the top of mlp.cu)
+    float* A;                // post-activation (pre-BN); the same buffer as H when neither batch norm nor dropout sits between them
+    float* H;                // layer output (bf16 family: only for layers the logits layer reads)
+    float* HT;               // fp32 family: transposed output [N_phys, ldt]
     float* dH;               // gradient w.r.t. H (accumulated over consumers)
-    float* dZ;               // gradient w.r.t. pre-activation
-    float* dZT;              // transposed [N_phys, ldt]
-    // 3xBF16 engine: bf16 hi / lo copies of H and dZ (what the tensor-core GEMMs read; no transposed copies)
-    __nv_bfloat16 *Hs[2], *dZs[2];
-    bool h_fp32;             // 3xBF16 engine: H is also stored in fp32 (only layers the logits layer reads)
+    float* dZ;               // fp32 family: gradient w.r.t. pre-activation
+    float* dZT;              // fp32 family: transposed [N_phys, ldt]
+    __nv_bfloat16 *Hs[2], *dZs[2];   // bf16 family: hi / lo copies of H and dZ
     float* colpart;          // [3][row_tiles][N_phys] partial column sums: dbias, dgamma, dbeta
 };
 
@@ -257,6 +260,7 @@ struct WdModel {
     int max_batch = 0, max_batch_pad = 0;   // pad: multiple of 128 (leading dim of transposed buffers)
     int64_t max_nnz = 0;
     int gemm_engine = 0;
+    wd::OperandFamily operands = wd::kFp32Operands;   // of gemm_engine, decided in wd_model_create
 
     cudaStream_t stream = nullptr;
     // side streams, one per sparse gradient list (0 = embedding rows, 1 = wide rows): the id-only grouping, the gradient sums,
@@ -361,16 +365,22 @@ struct WdModel {
     float** d_tab_data = nullptr;
     int32_t *d_tab_dim = nullptr, *d_tab_stride = nullptr, *d_tab_x0 = nullptr, *d_tab_col = nullptr;
     int64_t* d_tab_row_base = nullptr;
-    float *d_X0 = nullptr, *d_X0T = nullptr, *d_dX0 = nullptr;
-    __nv_bfloat16* d_X0s[2] = {nullptr, nullptr};   // bf16 hi / lo copy of X0 (3xBF16 engine)
+    float *d_X0 = nullptr, *d_dX0 = nullptr;
+    float* d_X0T = nullptr;                  // fp32 family: transposed X0 [d0_phys, ldt]
+    __nv_bfloat16* d_X0s[2] = {nullptr, nullptr};   // bf16 family: hi / lo copies of X0
     int ldt = 0;                             // leading dim of transposed activations (= max_batch_pad)
     std::vector<wd::Tower> towers;
 
     // ---- dense parameter arena
     std::vector<wd::DenseTensor> dense;
     int64_t dense_count = 0, gpart_count = 0, wt_count = 0;
-    float *d_P = nullptr, *d_S1 = nullptr, *d_S2 = nullptr, *d_G = nullptr, *d_gpart = nullptr, *d_Wt = nullptr;
-    float* d_Wsplit = nullptr;               // [W_hi | W_lo | Wt_hi | Wt_lo], each wt_count floats (3xTF32 pre-split weights)
+    float *d_P = nullptr, *d_S1 = nullptr, *d_S2 = nullptr, *d_G = nullptr, *d_gpart = nullptr;
+    // GEMM operand copies of the hidden layers' kernels W [K, N], wt_count elements each (DenseTensor::wt_off), rewritten after
+    // every optimizer step; only the operand family's exist
+    float* d_Wt = nullptr;                                      // fp32 family: Wt [N, K]
+    float *d_W_hi = nullptr, *d_W_lo = nullptr;                 // fp32 family: tf32 hi / lo splits of W (3xTF32)
+    float *d_Wt_hi = nullptr, *d_Wt_lo = nullptr;               // fp32 family: tf32 hi / lo splits of Wt (3xTF32)
+    __nv_bfloat16 *d_Wq_hi = nullptr, *d_Wq_lo = nullptr;       // bf16 family: bf16 hi / lo splits of W
     wd::DenseTensor* d_dense_desc = nullptr;
     int row_tiles = 0;                       // max_batch_pad / 128
     int wgrad_splits = 4;

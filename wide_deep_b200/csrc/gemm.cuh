@@ -1,6 +1,8 @@
 // Shared GEMM interface of the MLP engines (FFMA in mlp.cu, wgmma in gemm_tc.cu and gemm_bf16.cu): operand descriptions,
-// epilogue description and the activation functions (reference python/lib/utils/model_util.py:28-59).
+// epilogue description and the activation functions (reference python/lib/utils/model_util.py:28-59).  Which stored copy each
+// operand is read from is tabled at the top of mlp.cu.
 #pragma once
+#include <cuda.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -47,6 +49,11 @@ struct GemmA {                         // A operand: up to kMaxSegs K-contiguous
     const __nv_bfloat16* hi[kMaxSegs]; // 3xBF16 engine: the same segments pre-split into bf16 hi / lo copies (same ld)
     const __nv_bfloat16* lo[kMaxSegs];
 };
+struct GemmB {                         // B operand: one segment (host side only; the FFMA kernel takes ptr / ld)
+    const float* ptr; int ld;
+    const float *tf32_hi, *tf32_lo;    // 3xTF32 forward / data gradient: ptr pre-split into tf32 hi / lo copies (same ld)
+    const __nv_bfloat16 *hi, *lo;      // 3xBF16 engine: bf16 hi / lo copies (same ld)
+};
 enum { EPI_FWD = 0, EPI_STORE = 1, EPI_WGRAD = 2 };
 struct Epi {
     float* C; int ldc;                 // STORE / WGRAD target
@@ -64,6 +71,13 @@ struct Epi {
     // Criteo shape: 8.47 M against 8.84 M examples/s for the whole step).
     uint64_t reserved[5];
 };
+
+// wgmma engines; tc_gemm returns WD_EUNSUPPORTED when the shape is not covered
+int tc_gemm(WdModel* m, int mode, const GemmA& A, const GemmB& B, int M, int N, const Epi& ep, int splits, int ksplit_len);
+int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const GemmB& B, int M, int N, const Epi& ep, int splits, int ksplit_len);
+// 2-D TMA tensor map of a row-major fp32 or bf16 matrix [rows, cols] with leading dimension ld (elements): box = one 128-byte
+// row of columns x box_rows, 128-byte swizzle.  Encoded maps are cached (gemm_tc.cu).
+int make_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, const void* ptr, int rows, int cols, int ld, int box_rows);
 
 // ---- dropout (tf.layers.dropout after a hidden layer's activation, TRAIN only; reference dnn.py:111-112).  TensorFlow's random
 // stream cannot be reproduced, so the keep mask is DEFINED by a counter-based generator shared bit for bit with the oracle

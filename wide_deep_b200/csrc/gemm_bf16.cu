@@ -40,8 +40,6 @@
 
 namespace wd {
 
-int tc_make_map_bf16(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int box_rows);   // gemm_tc.cu
-
 namespace {
 
 constexpr int QBM = 128;         // tile rows: two warp groups x wgmma M = 64
@@ -322,9 +320,9 @@ extern "C" int wd_debug_gemm_probe(unsigned long long* out) {
     return e == cudaSuccess ? 0 : -1;
 }
 
-int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, int M, int N,
-                 const Epi& ep, int splits, int ksplit_len) {
-    if (N % 32 != 0 || A.n > kMaxSegs || !B_hi || !B_lo) { set_error("bf16 GEMM engine: unsupported operands"); return WD_EUNSUPPORTED; }
+int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const GemmB& B, int M, int N, const Epi& ep, int splits, int ksplit_len) {
+    constexpr CUtensorMapDataType BF16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    if (N % 32 != 0 || A.n > kMaxSegs || !B.hi || !B.lo) { set_error("bf16 GEMM engine: unsupported operands"); return WD_EUNSUPPORTED; }
     QMaps maps;
     QSegs segs{};
     segs.n = A.n;
@@ -334,22 +332,22 @@ int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi
         if (!A.hi[s] || !A.lo[s]) { set_error("bf16 GEMM engine: operand without hi/lo copies"); return WD_EINVAL; }
         // K-major: [M rows][k contiguous], box 64 k x 128 rows.  MN-major: [k rows][M contiguous], box 64 columns x 64 k-rows
         if (!a_mn) {
-            if ((rc = tc_make_map_bf16(&maps.a_hi[s], A.hi[s], M, A.k[s], A.ld[s], QBM))) return rc;
-            if ((rc = tc_make_map_bf16(&maps.a_lo[s], A.lo[s], M, A.k[s], A.ld[s], QBM))) return rc;
+            if ((rc = make_tensor_map(&maps.a_hi[s], BF16, A.hi[s], M, A.k[s], A.ld[s], QBM))) return rc;
+            if ((rc = make_tensor_map(&maps.a_lo[s], BF16, A.lo[s], M, A.k[s], A.ld[s], QBM))) return rc;
         } else {
-            if ((rc = tc_make_map_bf16(&maps.a_hi[s], A.hi[s], A.k[s], M, A.ld[s], 64))) return rc;
-            if ((rc = tc_make_map_bf16(&maps.a_lo[s], A.lo[s], A.k[s], M, A.ld[s], 64))) return rc;
+            if ((rc = make_tensor_map(&maps.a_hi[s], BF16, A.hi[s], A.k[s], M, A.ld[s], 64))) return rc;
+            if ((rc = make_tensor_map(&maps.a_lo[s], BF16, A.lo[s], A.k[s], M, A.ld[s], 64))) return rc;
         }
         segs.k[s] = A.k[s]; segs.koff[s] = ktot;
         ktot += A.k[s];
     }
     for (int s = A.n; s < kMaxSegs; ++s) { maps.a_hi[s] = maps.a_hi[0]; maps.a_lo[s] = maps.a_lo[0]; }
     if (!b_mn) {
-        if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, N, ktot, ldb, QBN))) return rc;
-        if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, N, ktot, ldb, QBN))) return rc;
+        if ((rc = make_tensor_map(&maps.b_hi, BF16, B.hi, N, ktot, B.ld, QBN))) return rc;
+        if ((rc = make_tensor_map(&maps.b_lo, BF16, B.lo, N, ktot, B.ld, QBN))) return rc;
     } else {
-        if ((rc = tc_make_map_bf16(&maps.b_hi, B_hi, ktot, N, ldb, 64))) return rc;
-        if ((rc = tc_make_map_bf16(&maps.b_lo, B_lo, ktot, N, ldb, 64))) return rc;
+        if ((rc = make_tensor_map(&maps.b_hi, BF16, B.hi, ktot, N, B.ld, 64))) return rc;
+        if ((rc = make_tensor_map(&maps.b_lo, BF16, B.lo, ktot, N, B.ld, 64))) return rc;
     }
     if (mode == EPI_WGRAD) ksplit_len = (ksplit_len + QBK - 1) / QBK * QBK;
     if (mode == EPI_FWD && (!ep.Hs_hi || !ep.Hs_lo)) { set_error("bf16 GEMM engine: epilogue without hi/lo outputs"); return WD_EINVAL; }

@@ -283,36 +283,22 @@ void tc_map_cache_clear() {
     g_map_cache.clear();
 }
 
-// row-major fp32 matrix [rows, cols] with leading dimension ld (floats); box = 32 floats x box_rows, 128B swizzle
-static int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows) {
-    const MapKey key{ptr, rows, cols, ld, box_rows, 4};
-    if (map_cache_get(key, map)) return WD_OK;
-    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-    cuuint32_t box[2] = {(cuuint32_t)TBK, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%d", (int)r, rows, cols, ld); return WD_ECUDA; }
-    map_cache_put(key, *map);
-    return WD_OK;
-}
-
-// row-major bf16 matrix [rows, cols], leading dimension ld (elements); box = 64 elements (128 B) x box_rows, 128B swizzle
-int tc_make_map_bf16(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int box_rows) {
+int make_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, const void* ptr, int rows, int cols, int ld, int box_rows) {
     int rc = get_encode();
     if (rc) return rc;
-    const MapKey key{ptr, rows, cols, ld, box_rows, 2};
+    const int esize = dtype == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2;       // fp32 or bf16
+    const MapKey key{ptr, rows, cols, ld, box_rows, esize};
     if (map_cache_get(key, map)) return WD_OK;
     cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-    cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * esize};
+    cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(bf16) failed (%d) rows=%d cols=%d ld=%d", (int)r, rows, cols, ld); return WD_ECUDA; }
+    CUresult r = g_encode(map, dtype, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled failed (%d) rows=%d cols=%d ld=%d element=%d bytes", (int)r, rows, cols, ld, esize);
+        return WD_ECUDA;
+    }
     map_cache_put(key, *map);
     return WD_OK;
 }
@@ -338,26 +324,25 @@ static int launch_tc(WdModel* m, const TcMaps& maps, int nseg, const int* segk, 
     return WD_OK;
 }
 
-int tc_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M, int N, const Epi& ep, int splits, int ksplit_len,
-            const float* B_hi, const float* B_lo) {
-    int rc = get_encode();
-    if (rc) return rc;
+int tc_gemm(WdModel* m, int mode, const GemmA& A, const GemmB& B, int M, int N, const Epi& ep, int splits, int ksplit_len) {
+    constexpr CUtensorMapDataType F32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    int rc;
     if (N % 32 != 0 || A.n > kMaxSegs) return WD_EUNSUPPORTED;
     TcMaps maps;
     int segk[kMaxSegs] = {0};
     int ktot = 0;
     for (int s = 0; s < A.n; ++s) {
         if (A.k[s] % TBK != 0 && A.n > 1) return WD_EUNSUPPORTED;     // interior segment boundaries must sit on k-block edges
-        if ((rc = make_map(&maps.a[s], A.ptr[s], M, A.k[s], A.ld[s], TBM))) return rc;
+        if ((rc = make_tensor_map(&maps.a[s], F32, A.ptr[s], M, A.k[s], A.ld[s], TBM))) return rc;
         segk[s] = A.k[s];
         ktot += A.k[s];
     }
     for (int s = A.n; s < kMaxSegs; ++s) maps.a[s] = maps.a[0];
     const bool split3 = m->gemm_engine == WD_GEMM_TC3X;
     const bool bpre = split3 && mode != EPI_WGRAD;                     // (tc_gemm_kernel's BPRE)
-    if (bpre && (!B_hi || !B_lo)) { set_error("3xTF32 GEMM engine: weights without hi/lo copies"); return WD_EINVAL; }
-    if ((rc = make_map(&maps.b, bpre ? B_hi : B, N, ktot, ldb, TBN))) return rc;
-    if (bpre) { if ((rc = make_map(&maps.b_lo, B_lo, N, ktot, ldb, TBN))) return rc; }
+    if (bpre && (!B.tf32_hi || !B.tf32_lo)) { set_error("3xTF32 GEMM engine: weights without hi/lo copies"); return WD_EINVAL; }
+    if ((rc = make_tensor_map(&maps.b, F32, bpre ? B.tf32_hi : B.ptr, N, ktot, B.ld, TBN))) return rc;
+    if (bpre) { if ((rc = make_tensor_map(&maps.b_lo, F32, B.tf32_lo, N, ktot, B.ld, TBN))) return rc; }
     else maps.b_lo = maps.b;
     if (mode == EPI_WGRAD) ksplit_len = (ksplit_len + TBK - 1) / TBK * TBK;
 #define WD_TC_LAUNCH(MODE_)                                                                                      \

@@ -6,13 +6,28 @@
 //   backward         MatMul grads, activation / affine grads                  (reference joint.py:234-239 minimize())
 //   dense optimizer  ApplyAdagrad / ApplyFtrl / SGD with constant LR (Q1)     (reference model_util.py:62-105)
 //
-// Every matrix product is a "TN" GEMM  C[M,N] = sum_k A[M,k] * B[N,k]  (both operands K-contiguous):
-//   forward   A = layer input segments [batch, K],  B = Wt [N, K]
-//   dgrad     A = dZ [batch, N],                    B = W  [K, N] rows of one input segment
-//   wgrad     A = inputT [K, batch],                B = dZT [N, batch]     (split over the batch)
-// which is why activations and gradients are also kept transposed.  This file holds the fp32 CUDA-core
-// (FFMA) engine — exact fp32 products, used as the parity engine and as the reference the wgmma engine
-// (gemm_tc.cu) is validated against.
+// Every matrix product is a GEMM  C[M,N] = sum_k A[M,k] * B[k,N]  over a GemmA (up to kMaxSegs input segments) and a GemmB.
+// Each engine reads its operands from stored copies of one operand family (WdModel::operands, decided in wd_model_create), and a
+// model allocates and writes only its family's copies:
+//
+//                fp32 family: ffma, tc1x, tc3x                        bf16 family: bf16x3
+//                fp32, both operands K-contiguous ("TN")              bf16 hi / lo copies (GemmA::hi / lo, GemmB::hi / lo)
+//   forward  A   X0 / H [B, K] input segments                         X0s / Hs [B, K]                        K-major
+//            B   Wt [N, K]           (tc3x: tf32 splits Wt_hi / Wt_lo)   Wq [K, N]                           MN-major
+//   dgrad    A   dZ [B, N]                                            dZs [B, N]                             K-major
+//            B   W [K, N] rows of one input segment (tc3x: W_hi / W_lo)  Wq rows of the segment             K-major
+//   wgrad    A   X0T / HT [K, ldt], reduction over the batch padded   X0s / Hs [B, K], reduction over B      MN-major
+//            B   dZT [N, ldt]        to 16 (split over the batch)     dZs [B, N]                             MN-major
+//   written by   the forward epilogue (H, HT), transpose_kernel        the forward epilogue (Hs), x0_split_kernel (X0s),
+//                (X0T), act_bn_bwd_kernel (dZ, dZT),                   act_bn_bwd_q_kernel / logits_act_bwd_q_kernel (dZs),
+//                dense_apply_kernel (Wt and the tf32 splits)           dense_vec_kernel (Wq)
+// Both families keep the post-activation values A and the gradients dH in fp32.  The bf16 family keeps the layer output H in
+// fp32 only for layers the logits layer reads (logits_head_kernel and the logits backward are not GEMMs).  fwd_operands,
+// dgrad_operands and wgrad_operands fill GemmA / GemmB from this table; the drivers mlp_forward / mlp_backward only choose
+// between the family's named kernels.
+//
+// This file also holds the fp32 CUDA-core (FFMA) engine: exact fp32 products, the parity engine and the reference the tensor-core
+// engines (tf32: gemm_tc.cu, bf16: gemm_bf16.cu) are validated against.
 #include "common.cuh"
 #include "gemm.cuh"
 
@@ -148,42 +163,34 @@ __global__ void __launch_bounds__(GT) gemm_tn_ffma(GemmA A, const float* __restr
     }
 }
 
-static void launch_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M, int N, const Epi& ep, int splits, int ksplit_len) {
+static void launch_gemm(WdModel* m, int mode, const GemmA& A, const GemmB& B, int M, int N, const Epi& ep, int splits, int ksplit_len) {
     dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM, mode == EPI_WGRAD ? splits : 1);
-    if (mode == EPI_FWD) gemm_tn_ffma<EPI_FWD><<<grid, GT, 0, m->stream>>>(A, B, ldb, M, N, 0, ep);
-    else if (mode == EPI_STORE) gemm_tn_ffma<EPI_STORE><<<grid, GT, 0, m->stream>>>(A, B, ldb, M, N, 0, ep);
-    else gemm_tn_ffma<EPI_WGRAD><<<grid, GT, 0, m->stream>>>(A, B, ldb, M, N, ksplit_len, ep);
+    if (mode == EPI_FWD) gemm_tn_ffma<EPI_FWD><<<grid, GT, 0, m->stream>>>(A, B.ptr, B.ld, M, N, 0, ep);
+    else if (mode == EPI_STORE) gemm_tn_ffma<EPI_STORE><<<grid, GT, 0, m->stream>>>(A, B.ptr, B.ld, M, N, 0, ep);
+    else gemm_tn_ffma<EPI_WGRAD><<<grid, GT, 0, m->stream>>>(A, B.ptr, B.ld, M, N, ksplit_len, ep);
     m->launches++;
 }
 
-// wgmma tf32 engine (gemm_tc.cu); returns WD_EUNSUPPORTED when the shape is not covered
-int tc_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M, int N, const Epi& ep, int splits, int ksplit_len,
-            const float* B_hi, const float* B_lo);
-// 3xBF16 wgmma engine (gemm_bf16.cu): operands are the bf16 hi / lo copies (GemmA::hi/lo, Bq_hi/Bq_lo)
-int tc_gemm_bf16(WdModel* m, int mode, const GemmA& A, const __nv_bfloat16* B_hi, const __nv_bfloat16* B_lo, int ldb, int M, int N,
-                 const Epi& ep, int splits, int ksplit_len);
-
-static int run_gemm(WdModel* m, int mode, const GemmA& A, const float* B, int ldb, int M, int N, const Epi& ep, int splits = 1, int ksplit_len = 0,
-                    const float* B_hi = nullptr, const float* B_lo = nullptr, const __nv_bfloat16* Bq_hi = nullptr, const __nv_bfloat16* Bq_lo = nullptr) {
+static int run_gemm(WdModel* m, int mode, const GemmA& A, const GemmB& B, int M, int N, const Epi& ep, int splits = 1, int ksplit_len = 0) {
     static const char* kNamesL[3][4] = {{"gemm_fwd_l0", "gemm_fwd_l1", "gemm_fwd_l2", "gemm_fwd_l3+"},
                                         {"gemm_dgrad_l0", "gemm_dgrad_l1", "gemm_dgrad_l2", "gemm_dgrad_l3+"},
                                         {"gemm_wgrad_l0", "gemm_wgrad_l1", "gemm_wgrad_l2", "gemm_wgrad_l3+"}};
     const char* kNames[3] = {kNamesL[0][m->cur_layer < 3 ? m->cur_layer : 3], kNamesL[1][m->cur_layer < 3 ? m->cur_layer : 3],
                              kNamesL[2][m->cur_layer < 3 ? m->cur_layer : 3]};
     mark(m, "mlp_other");
-    if (m->gemm_engine == WD_GEMM_BF16X3) {
-        int rc = tc_gemm_bf16(m, mode, A, Bq_hi, Bq_lo, ldb, M, N, ep, splits, ksplit_len);
+    if (m->operands == kBf16Operands) {
+        int rc = tc_gemm_bf16(m, mode, A, B, M, N, ep, splits, ksplit_len);
         mark(m, kNames[mode]);
         return rc;
     }
     if (m->gemm_engine == WD_GEMM_TC3X || m->gemm_engine == WD_GEMM_TC1X) {
-        int rc = tc_gemm(m, mode, A, B, ldb, M, N, ep, splits, ksplit_len, B_hi, B_lo);
+        int rc = tc_gemm(m, mode, A, B, M, N, ep, splits, ksplit_len);
         if (rc != WD_EUNSUPPORTED) { mark(m, kNames[mode]); return rc; }
         m->gemm_fallbacks++;                              // loud: counted, reported by wd_gemm_fallback_count, asserted 0 in the tests
         static bool warned = false;
         if (!warned) { fprintf(stderr, "libwd_b200: wgmma engine does not cover a GEMM (M=%d N=%d segs=%d): running it on the FFMA kernel\n", M, N, A.n); warned = true; }
     }
-    launch_gemm(m, mode, A, B, ldb, M, N, ep, splits, ksplit_len);
+    launch_gemm(m, mode, A, B, M, N, ep, splits, ksplit_len);
     mark(m, kNames[mode]);
     return WD_OK;
 }
@@ -612,27 +619,22 @@ __device__ __forceinline__ void opt_update_d(const OptParamsD& o, float g, float
         w -= o.lr * g;
     }
 }
-// hi/lo split of a weight for the 3xTF32 engine (same split the GEMM applies to activations in shared memory)
-__device__ __forceinline__ void store_split(float* __restrict__ Wsplit, int64_t wt_count, int64_t wt_off, int64_t e, int64_t et, float w) {
+// tf32 hi/lo split of a weight for the 3xTF32 engine (same split the GEMM applies to activations in shared memory), stored at
+// e in W [K, N] and at et in Wt [N, K]
+__device__ __forceinline__ void store_split(float* __restrict__ W_hi, float* __restrict__ W_lo, float* __restrict__ Wt_hi,
+                                            float* __restrict__ Wt_lo, int64_t e, int64_t et, float w) {
     float hi = __uint_as_float(__float_as_uint(w) & 0xFFFFE000u), lo = w - hi;
-    Wsplit[wt_off + e] = hi;                       // W  [K, N] hi
-    Wsplit[wt_count + wt_off + e] = lo;            // W  [K, N] lo
-    Wsplit[2 * wt_count + wt_off + et] = hi;       // Wt [N, K] hi
-    Wsplit[3 * wt_count + wt_off + et] = lo;       // Wt [N, K] lo
+    W_hi[e] = hi;
+    W_lo[e] = lo;
+    Wt_hi[et] = hi;
+    Wt_lo[et] = lo;
 }
-// 3xBF16 engine: W [K, N] as bf16 hi / lo (the first two quarter-size arrays of the buffer); no transposed copy is needed
-__device__ __forceinline__ void store_split_bf16(float* __restrict__ Wsplit, int64_t wt_count, int64_t wt_off, int64_t e, float w) {
-    __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(Wsplit);
-    __nv_bfloat16 hi, lo;
-    split_bf16(w, hi, lo);
-    q[wt_off + e] = hi;
-    q[wt_count + wt_off + e] = lo;
-}
-// applies the optimizer over the dense arena (every engine but 3xBF16); kernels also refresh their transposed copy Wt[n][k] and
-// its hi / lo split
+// applies the optimizer over the dense arena (fp32 operand family); kernels also refresh their transposed copy Wt[n][k] and the
+// tf32 hi / lo splits
 __global__ void dense_apply_kernel(const DenseTensor* __restrict__ T, int nt, int64_t total, const float* __restrict__ G,
                                    float* __restrict__ P, float* __restrict__ S1, float* __restrict__ S2, float* __restrict__ Wt,
-                                   float* __restrict__ Wsplit, int64_t wt_count, OptParamsD dnn, OptParamsD lin, int lin_tensor) {
+                                   float* __restrict__ W_hi, float* __restrict__ W_lo, float* __restrict__ Wt_hi, float* __restrict__ Wt_lo,
+                                   OptParamsD dnn, OptParamsD lin, int lin_tensor) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         int lo = 0, hi = nt - 1;
         while (lo < hi) {
@@ -648,11 +650,11 @@ __global__ void dense_apply_kernel(const DenseTensor* __restrict__ T, int nt, in
             int64_t e = i - t.off;
             int k = (int)(e / t.cols), n = (int)(e % t.cols);
             Wt[t.wt_off + (int64_t)n * t.rows + k] = w;
-            store_split(Wsplit, wt_count, t.wt_off, e, (int64_t)n * t.rows + k, w);
+            store_split(W_hi, W_lo, Wt_hi, Wt_lo, t.wt_off + e, t.wt_off + (int64_t)n * t.rows + k, w);
         }
     }
 }
-// Vectorised dense-gradient reduction / optimizer for the 3xBF16 engine (no transposed weight copies to scatter): one thread per
+// Vectorised dense-gradient reduction / optimizer for the bf16 operand family (no transposed weight copies to scatter): one thread per
 // four consecutive arena floats (tensor offsets, partial strides and kernel widths are multiples of 4), one tensor lookup per
 // thread instead of per element.
 //   MODE 0: G = sum of the live partials                      (data-parallel runs: G is exchanged before the optimizer)
@@ -661,7 +663,7 @@ __global__ void dense_apply_kernel(const DenseTensor* __restrict__ T, int nt, in
 template <int MODE>
 __global__ void __launch_bounds__(256) dense_vec_kernel(const DenseTensor* __restrict__ T, int nt, int64_t total4, const float* __restrict__ gpart,
                                                         float* __restrict__ G, float* __restrict__ P, float* __restrict__ S1, float* __restrict__ S2,
-                                                        float* __restrict__ Wsplit, int64_t wt_count, OptParamsD dnn, OptParamsD lin, int lin_tensor,
+                                                        __nv_bfloat16* __restrict__ Wq_hi, __nv_bfloat16* __restrict__ Wq_lo, OptParamsD dnn, OptParamsD lin, int lin_tensor,
                                                         int live_row_tiles, int64_t begin4, int64_t hole_lo4, int64_t hole_hi4) {
     // arena range [begin4, total4) minus the hole [hole_lo4, hole_hi4): the single-GPU step updates everything but the first
     // layer's kernel on a side stream while that kernel's weight gradient is still being computed (dense_apply_split)
@@ -715,16 +717,16 @@ __global__ void __launch_bounds__(256) dense_vec_kernel(const DenseTensor* __res
         reinterpret_cast<float4*>(P)[i4] = w;
         reinterpret_cast<float4*>(S1)[i4] = s1;
         reinterpret_cast<float4*>(S2)[i4] = s2;
-        if (t.wt_off >= 0) {                                              // bf16 hi / lo copies of W [K, N] (what the GEMMs read)
-            __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(Wsplit);
-            store_split4(q + t.wt_off + e, q + wt_count + t.wt_off + e, w.x, w.y, w.z, w.w);
-        }
+        if (t.wt_off >= 0)                                                // bf16 hi / lo copies of W [K, N] (what the GEMMs read)
+            store_split4(Wq_hi + t.wt_off + e, Wq_lo + t.wt_off + e, w.x, w.y, w.z, w.w);
     }
 }
 
-// Wt refresh only (after init / tensor upload)
-__global__ void dense_transpose_kernel(const DenseTensor* __restrict__ T, int nt, int64_t total, const float* __restrict__ P, float* __restrict__ Wt,
-                                       float* __restrict__ Wsplit, int64_t wt_count, int bf16) {
+// Rewrites the GEMM operand copies of the weights from P (after init / tensor upload): Wt and the tf32 splits for the fp32
+// family, the bf16 splits (Wq_hi non-null) for the bf16 family
+__global__ void weight_copies_kernel(const DenseTensor* __restrict__ T, int nt, int64_t total, const float* __restrict__ P, float* __restrict__ Wt,
+                                     float* __restrict__ W_hi, float* __restrict__ W_lo, float* __restrict__ Wt_hi, float* __restrict__ Wt_lo,
+                                     __nv_bfloat16* __restrict__ Wq_hi, __nv_bfloat16* __restrict__ Wq_lo) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         int lo = 0, hi = nt - 1;
         while (lo < hi) {
@@ -734,40 +736,78 @@ __global__ void dense_transpose_kernel(const DenseTensor* __restrict__ T, int nt
         const DenseTensor t = T[lo];
         if (t.wt_off >= 0 && i - t.off < t.count) {
             int64_t e = i - t.off;
+            if (Wq_hi) {
+                __nv_bfloat16 qh, ql;
+                split_bf16(P[i], qh, ql);
+                Wq_hi[t.wt_off + e] = qh;
+                Wq_lo[t.wt_off + e] = ql;
+                continue;
+            }
             int k = (int)(e / t.cols), n = (int)(e % t.cols);
             Wt[t.wt_off + (int64_t)n * t.rows + k] = P[i];
-            if (bf16) store_split_bf16(Wsplit, wt_count, t.wt_off, e, P[i]);
-            else store_split(Wsplit, wt_count, t.wt_off, e, (int64_t)n * t.rows + k, P[i]);
+            store_split(W_hi, W_lo, Wt_hi, Wt_lo, t.wt_off + e, t.wt_off + (int64_t)n * t.rows + k, P[i]);
         }
     }
 }
-int dense_refresh_transposes(WdModel* m) {
+int refresh_weight_copies(WdModel* m) {
     if (m->dense_count == 0) return WD_OK;
-    dense_transpose_kernel<<<grid_for(m->dense_count, 256), 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), m->dense_count, m->d_P, m->d_Wt, m->d_Wsplit, m->wt_count, m->gemm_engine == WD_GEMM_BF16X3);
+    weight_copies_kernel<<<grid_for(m->dense_count, 256), 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), m->dense_count, m->d_P, m->d_Wt,
+                                                                               m->d_W_hi, m->d_W_lo, m->d_Wt_hi, m->d_Wt_lo, m->d_Wq_hi, m->d_Wq_lo);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 
 // ------------------------------------------------------------------------------------------ host drivers
-static const float* src_ptr(WdModel* m, Tower& tw, int src, bool transposed) {
-    if (src < 0) return transposed ? m->d_X0T : m->d_X0;
-    return transposed ? tw.layers[src].HT : tw.layers[src].H;
+// a layer input: src -1 is the deep input X0, src >= 0 hidden layer src of the same tower
+static const float* src_ptr(WdModel* m, Tower& tw, int src) { return src < 0 ? m->d_X0 : tw.layers[src].H; }
+static const __nv_bfloat16* src_split(WdModel* m, Tower& tw, int src, int part) { return src < 0 ? m->d_X0s[part] : tw.layers[src].Hs[part]; }
+static int src_ld(WdModel* m, Tower& tw, int src) { return src < 0 ? m->d0_phys : tw.layers[src].N_phys; }
+
+// ---- GEMM operands of a hidden layer (A, B zero-initialised), read off the operand-family table at the top of this file.
+// GemmB = {ptr, ld, tf32_hi, tf32_lo, hi, lo}.
+// forward: A = the layer's input segments, B = its kernel
+static void fwd_operands(WdModel* m, Tower& tw, const Layer& L, GemmA& A, GemmB& B) {
+    const int64_t wo = m->dense[L.t_kernel].wt_off;
+    A.n = L.n_in_segs;
+    for (int s = 0; s < L.n_in_segs; ++s) {
+        const int src = L.segs[s].src;
+        A.ld[s] = src_ld(m, tw, src); A.k[s] = L.segs[s].width_phys;
+        if (m->operands == kFp32Operands) A.ptr[s] = src_ptr(m, tw, src);
+        else { A.hi[s] = src_split(m, tw, src, 0); A.lo[s] = src_split(m, tw, src, 1); }
+    }
+    if (m->operands == kFp32Operands) B = GemmB{m->d_Wt + wo, L.K_phys, m->d_Wt_hi + wo, m->d_Wt_lo + wo, nullptr, nullptr};
+    else B = GemmB{nullptr, L.N_phys, nullptr, nullptr, m->d_Wq_hi + wo, m->d_Wq_lo + wo};
 }
-static const __nv_bfloat16* src_split(WdModel* m, Tower& tw, int src, int part) {
-    return src < 0 ? m->d_X0s[part] : tw.layers[src].Hs[part];
+// data gradient into input segment sg: A = the layer's dZ, B = the kernel rows that segment feeds
+static void dgrad_operands(WdModel* m, const Layer& L, const Seg& sg, GemmA& A, GemmB& B) {
+    const DenseTensor& tk = m->dense[L.t_kernel];
+    const int64_t eo = (int64_t)sg.k_off * L.N_phys, wo = tk.wt_off + eo;
+    A.n = 1; A.ld[0] = L.N_phys; A.k[0] = L.N_phys;
+    if (m->operands == kFp32Operands) {
+        A.ptr[0] = L.dZ;
+        B = GemmB{m->d_P + tk.off + eo, L.N_phys, m->d_W_hi + wo, m->d_W_lo + wo, nullptr, nullptr};
+    } else {
+        A.hi[0] = L.dZs[0]; A.lo[0] = L.dZs[1];
+        B = GemmB{nullptr, L.N_phys, nullptr, nullptr, m->d_Wq_hi + wo, m->d_Wq_lo + wo};
+    }
 }
-static int src_ld(WdModel* m, Tower& tw, int src, bool transposed) {
-    if (transposed) return m->ldt;
-    return src < 0 ? m->d0_phys : tw.layers[src].N_phys;
+// weight gradient of the kernel rows input segment sg feeds: A = that input, B = the layer's dZ, the batch being the reduction
+static void wgrad_operands(WdModel* m, Tower& tw, const Layer& L, const Seg& sg, GemmA& A, GemmB& B) {
+    A.n = 1;
+    if (m->operands == kFp32Operands) {                // transposed copies; the batch padded to 16 (rows past it are zero)
+        A.ptr[0] = sg.src < 0 ? m->d_X0T : tw.layers[sg.src].HT; A.ld[0] = m->ldt; A.k[0] = (m->dbatch.B + 15) / 16 * 16;
+        B = GemmB{L.dZT, m->ldt, nullptr, nullptr, nullptr, nullptr};
+    } else {                                           // row-major [B, width] copies (TMA zero-fills the batch tail)
+        A.hi[0] = src_split(m, tw, sg.src, 0); A.lo[0] = src_split(m, tw, sg.src, 1); A.ld[0] = src_ld(m, tw, sg.src); A.k[0] = m->dbatch.B;
+        B = GemmB{nullptr, L.N_phys, nullptr, nullptr, L.dZs[0], L.dZs[1]};
+    }
 }
 
 int mlp_forward(WdModel* m, bool train) {
     const int B = m->dbatch.B;
     if (!m->use_deep) return WD_OK;
-    const bool q = m->gemm_engine == WD_GEMM_BF16X3;
-    const __nv_bfloat16* Wq = reinterpret_cast<const __nv_bfloat16*>(m->d_Wsplit);
-    if (q) {                                           // bf16 hi / lo copies of X0
+    if (m->operands == kBf16Operands) {                // bf16 hi / lo copies of X0
         const int64_t n4 = (int64_t)B * m->d0_phys / 4;
         x0_split_kernel<<<grid_for(n4, 256), 256, 0, m->stream>>>(m->d_X0, n4, m->d_X0s[0], m->d_X0s[1]);
         m->launches++;
@@ -781,35 +821,23 @@ int mlp_forward(WdModel* m, bool train) {
         for (int l = 0; l < tw.n_hidden; ++l) {
             Layer& L = tw.layers[l];
             m->cur_layer = l;
-            GemmA A{};
-            A.n = L.n_in_segs;
-            for (int s = 0; s < L.n_in_segs; ++s) {
-                A.ptr[s] = src_ptr(m, tw, L.segs[s].src, false);
-                A.ld[s] = src_ld(m, tw, L.segs[s].src, false);
-                A.k[s] = L.segs[s].width_phys;
-                if (q) { A.hi[s] = src_split(m, tw, L.segs[s].src, 0); A.lo[s] = src_split(m, tw, L.segs[s].src, 1); }
-            }
+            GemmA A{}; GemmB W{};
+            fwd_operands(m, tw, L, A, W);
+            // the layer's outputs: whichever of H, HT (train steps) and the bf16 copies Hs the model has
             Epi ep{};
             ep.A_out = L.A; ep.H_out = L.H; ep.ldh = L.N_phys;
-            ep.HT = (train && !q) ? L.HT : nullptr; ep.ldt = m->ldt;
-            if (q) {                                   // fp32 H only where the logits layer reads it
-                ep.Hs_hi = L.Hs[0]; ep.Hs_lo = L.Hs[1];
-                if (!L.h_fp32) ep.H_out = nullptr;
-            }
+            ep.HT = train ? L.HT : nullptr; ep.ldt = m->ldt;
+            ep.Hs_hi = L.Hs[0]; ep.Hs_lo = L.Hs[1];
             ep.bias = m->d_P + m->dense[L.t_bias].off;
             ep.gamma = L.t_gamma >= 0 ? m->d_P + m->dense[L.t_gamma].off : nullptr;
             ep.beta = L.t_beta >= 0 ? m->d_P + m->dense[L.t_beta].off : nullptr;
             ep.n_logical = L.N; ep.act = m->activation; ep.bn = m->batch_norm; ep.m_valid = B;
-            const int64_t wo = m->dense[L.t_kernel].wt_off;
-            const float* Wt = m->d_Wt + wo;
-            // (3xBF16: B = W [K, N] itself, N-contiguous, leading dimension N_phys)
-            int rc = run_gemm(m, EPI_FWD, A, Wt, q ? L.N_phys : L.K_phys, B, L.N_phys, ep, 1, 0, m->d_Wsplit + 2 * m->wt_count + wo,
-                              m->d_Wsplit + 3 * m->wt_count + wo, Wq + wo, Wq + m->wt_count + wo);
+            int rc = run_gemm(m, EPI_FWD, A, W, B, L.N_phys, ep);
             if (rc) return rc;
             if (train && m->dropout_rate > 0.f) {              // tf.layers.dropout(training=True): TRAIN steps only (dnn.py:111-112)
                 const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l};
                 dropout_fwd_kernel<<<grid_for((int64_t)B * L.N_phys, 256), 256, 0, m->stream>>>(B, L.N_phys, L.N, L.A, L.N_phys, ep.gamma, ep.beta, m->batch_norm,
-                    (!q || L.h_fp32) ? L.H : nullptr, q ? L.Hs[0] : nullptr, q ? L.Hs[1] : nullptr, ep.HT, m->ldt, dr);
+                    L.H, L.Hs[0], L.Hs[1], ep.HT, m->ldt, dr);
                 m->launches++;
             }
         }
@@ -828,8 +856,8 @@ int loss_forward(WdModel* m, bool need_grad) {
         Layer& LL = tw.layers[tw.n_hidden];
         in.S[t].n = LL.n_in_segs;
         for (int s = 0; s < LL.n_in_segs; ++s) {
-            in.S[t].ptr[s] = src_ptr(m, tw, LL.segs[s].src, false);
-            in.S[t].ld[s] = src_ld(m, tw, LL.segs[s].src, false);
+            in.S[t].ptr[s] = src_ptr(m, tw, LL.segs[s].src);
+            in.S[t].ld[s] = src_ld(m, tw, LL.segs[s].src);
             in.S[t].k[s] = LL.segs[s].width_phys;
             in.S[t].koff[s] = LL.segs[s].k_off;
         }
@@ -853,8 +881,7 @@ int mlp_backward(WdModel* m) {
     const int Bk = (B + 15) / 16 * 16;                                // reduction length of wgrad
     bool dx0_written = false;
     const bool need_dx0 = !m->tables.empty();
-    const bool q = m->gemm_engine == WD_GEMM_BF16X3;
-    const __nv_bfloat16* Wq = reinterpret_cast<const __nv_bfloat16*>(m->d_Wsplit);
+    const bool bf16_ops = m->operands == kBf16Operands;
     for (auto& tw : m->towers) {
         std::vector<char> written(tw.n_hidden, 0);
         std::vector<int> readers(tw.n_hidden, 0);
@@ -872,16 +899,16 @@ int mlp_backward(WdModel* m) {
         const DenseTensor& tb = m->dense[LL.t_bias];
         for (int s = 0; s < LL.n_in_segs; ++s) {
             const Seg& sg = LL.segs[s];
-            const float* src = src_ptr(m, tw, sg.src, false);
-            int ld = src_ld(m, tw, sg.src, false);
+            const float* src = src_ptr(m, tw, sg.src);
+            int ld = src_ld(m, tw, sg.src);
             dim3 g((sg.width_phys + 63) / 64, rts);
             float* dst = nullptr; int dld = 0, acc = 0;
             if (!(sg.src < 0 && !need_dx0)) grad_dst(sg.src, &dst, &dld, &acc);
             // (the first segment of the first tower also leaves the wide bias's gradient partials: both are tile sums of dlogit)
             const bool wb = m->use_wide && s == 0 && &tw == &m->towers.front();
-            // 3xBF16 engine, a hidden layer read by the logits layer alone: its activation / batch-norm backward runs in the same
+            // bf16 family, a hidden layer read by the logits layer alone: its activation / batch-norm backward runs in the same
             // pass (logits_act_bwd_q_kernel), so its dH is never stored and act_bn_bwd_q_kernel is not launched for it
-            if (q && LL.n_in_segs == 1 && sg.src >= 0 && readers[sg.src] == 2 && m->dropout_rate <= 0.f &&
+            if (bf16_ops && LL.n_in_segs == 1 && sg.src >= 0 && readers[sg.src] == 2 && m->dropout_rate <= 0.f &&
                 sg.width_phys == tw.layers[sg.src].N_phys) {
                 Layer& S = tw.layers[sg.src];
                 logits_act_bwd_q_kernel<<<dim3((S.N_phys + 63) / 64, rts), 256, 0, m->stream>>>(B, S.N_phys, S.N, src, ld, S.A, S.N_phys, m->d_dlogit,
@@ -904,7 +931,6 @@ int mlp_backward(WdModel* m) {
         for (int l = tw.n_hidden - 1; l >= 0; --l) {
             Layer& L = tw.layers[l];
             m->cur_layer = l;
-            const DenseTensor& tkn = m->dense[L.t_kernel];
             float* pb = m->d_gpart + m->dense[L.t_bias].gpart_off;
             float* pg = L.t_gamma >= 0 ? m->d_gpart + m->dense[L.t_gamma].gpart_off : nullptr;
             float* pbe = L.t_beta >= 0 ? m->d_gpart + m->dense[L.t_beta].gpart_off : nullptr;
@@ -915,7 +941,7 @@ int mlp_backward(WdModel* m) {
             const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l};
             if (fused[l]) {
                 // dZ and the partials of this layer were written by logits_act_bwd_q_kernel
-            } else if (q)
+            } else if (bf16_ops)
                 act_bn_bwd_q_kernel<<<dim3((L.N_phys + 63) / 64, rts), 256, 0, m->stream>>>(B, L.N_phys, L.N, L.dH, L.A, L.N_phys,
                     L.t_gamma >= 0 ? m->d_P + m->dense[L.t_gamma].off : nullptr, m->activation, m->batch_norm, pb, pg, pbe,
                     m->dense[L.t_bias].gstride, L.dZs[0], L.dZs[1], dr);
@@ -931,14 +957,11 @@ int mlp_backward(WdModel* m) {
                 if (sg.src < 0 && !need_dx0) continue;
                 float* dst; int dld, acc;
                 grad_dst(sg.src, &dst, &dld, &acc);
-                GemmA A2{};
-                A2.n = 1; A2.ptr[0] = L.dZ; A2.ld[0] = L.N_phys; A2.k[0] = L.N_phys;
-                A2.hi[0] = L.dZs[0]; A2.lo[0] = L.dZs[1];
-                Epi e2{};
-                e2.C = dst; e2.ldc = dld; e2.accumulate = acc;
-                const int64_t woff = tkn.wt_off + (int64_t)sg.k_off * L.N_phys;
-                int rc = run_gemm(m, EPI_STORE, A2, m->d_P + tkn.off + (int64_t)sg.k_off * L.N_phys, L.N_phys, B, sg.width_phys, e2, 1, 0,
-                                  m->d_Wsplit + woff, m->d_Wsplit + m->wt_count + woff, Wq + woff, Wq + m->wt_count + woff);
+                GemmA A{}; GemmB W{};
+                dgrad_operands(m, L, sg, A, W);
+                Epi ep{};
+                ep.C = dst; ep.ldc = dld; ep.accumulate = acc;
+                int rc = run_gemm(m, EPI_STORE, A, W, B, sg.width_phys, ep);
                 if (rc) return rc;
             }
             if (l == 0 && &tw == &m->towers.back() && need_dx0 && m->ev_dx0 && m->record_dx0) {
@@ -960,19 +983,13 @@ int mlp_backward(WdModel* m) {
             }
             for (int s = 0; s < L.n_in_segs; ++s) {
                 const Seg& sg = L.segs[s];
-                // weight gradient of the rows fed by this segment: [width_phys, N] = srcT * dZT^T, split over the batch
-                GemmA A{};
-                A.n = 1; A.ptr[0] = src_ptr(m, tw, sg.src, true); A.ld[0] = m->ldt; A.k[0] = Bk;
-                if (q) {                               // row-major [B, width] copies; the batch is the reduction dimension
-                    A.hi[0] = src_split(m, tw, sg.src, 0); A.lo[0] = src_split(m, tw, sg.src, 1);
-                    A.ld[0] = src_ld(m, tw, sg.src, false); A.k[0] = B;
-                }
+                // weight gradient of the rows fed by this segment: [width_phys, N], split over the batch
+                GemmA A{}; GemmB W{};
+                wgrad_operands(m, tw, L, sg, A, W);
                 Epi ep{};
                 ep.C = m->d_gpart + tkn.gpart_off + (int64_t)sg.k_off * L.N_phys; ep.ldc = L.N_phys; ep.split_stride = tkn.gstride;
-                int ks = ((Bk + L.wgrad_splits - 1) / L.wgrad_splits + 31) / 32 * 32;
-                if (q) ks = (ks + 63) / 64 * 64;
-                int rc = run_gemm(m, EPI_WGRAD, A, L.dZT, q ? L.N_phys : m->ldt, sg.width_phys, L.N_phys, ep, L.wgrad_splits, ks, nullptr, nullptr,
-                                  L.dZs[0], L.dZs[1]);
+                const int ks = ((Bk + L.wgrad_splits - 1) / L.wgrad_splits + 31) / 32 * 32;     // (engines round it up to their k-block)
+                int rc = run_gemm(m, EPI_WGRAD, A, W, sg.width_phys, L.N_phys, ep, L.wgrad_splits, ks);
                 if (rc) return rc;
             }
         }
@@ -1025,18 +1042,18 @@ static int crelu_mirror(WdModel* m) {
         m->launches++;
     }
     WD_CUDA(cudaGetLastError());
-    return dense_refresh_transposes(m);
+    return refresh_weight_copies(m);
 }
 
 int dense_reduce_grads(WdModel* m) {
     if (m->dense_count == 0) return WD_OK;
     const int rts = (m->dbatch.B + 127) / 128;
     if (m->crelu) { int rc = crelu_fold(m); if (rc) return rc; }
-    if (m->gemm_engine == WD_GEMM_BF16X3) {
+    if (m->operands == kBf16Operands) {
         if (m->fuse_dense) return WD_OK;                              // single-GPU step: reduced inside dense_apply's kernel
         OptParamsD z{};
         dense_vec_kernel<0><<<grid_for(m->dense_count / 4, 256), 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), m->dense_count / 4, m->d_gpart,
-            m->d_G, nullptr, nullptr, nullptr, nullptr, 0, z, z, -1, rts, 0, 0, 0);
+            m->d_G, nullptr, nullptr, nullptr, nullptr, nullptr, z, z, -1, rts, 0, 0, 0);
         m->launches++;
         WD_CUDA(cudaGetLastError());
         return WD_OK;
@@ -1053,7 +1070,7 @@ static int dense_apply_plain(WdModel* m) {
     OptParamsD d = make_opt_d(m->dnn_opt, m->d_bpow + 2);
     OptParamsD l = make_opt_d(m->lin_opt, m->d_bpow);
     int lin_tensor = m->use_wide ? 0 : -1;                       // tensor 0 is the wide bias when the wide part exists
-    if (m->gemm_engine == WD_GEMM_BF16X3) {
+    if (m->operands == kBf16Operands) {
         const int rts = (m->dbatch.B + 127) / 128;
         const int g = grid_for(m->dense_count / 4, 256);
         if (m->fuse_dense) {
@@ -1065,16 +1082,17 @@ static int dense_apply_plain(WdModel* m) {
                 if (m->dense_part == 1) { b4 = k0; e4 = k1; } else { hlo = k0; hhi = k1; }
             }
             dense_vec_kernel<2><<<grid_for(e4 - b4, 256), 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), e4, m->d_gpart, m->d_G, m->d_P,
-                                                                                m->d_S1, m->d_S2, m->d_Wsplit, m->wt_count, d, l, lin_tensor, rts, b4, hlo, hhi);
+                                                                                m->d_S1, m->d_S2, m->d_Wq_hi, m->d_Wq_lo, d, l, lin_tensor, rts, b4, hlo, hhi);
         } else
             dense_vec_kernel<1><<<g, 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), m->dense_count / 4, m->d_gpart, m->d_G, m->d_P, m->d_S1,
-                                                          m->d_S2, m->d_Wsplit, m->wt_count, d, l, lin_tensor, rts, 0, 0, 0);
+                                                          m->d_S2, m->d_Wq_hi, m->d_Wq_lo, d, l, lin_tensor, rts, 0, 0, 0);
         m->launches++;
         WD_CUDA(cudaGetLastError());
         return WD_OK;
     }
     dense_apply_kernel<<<grid_for(m->dense_count, 256), 256, 0, m->stream>>>(m->d_dense_desc, (int)m->dense.size(), m->dense_count, m->d_G,
-                                                                            m->d_P, m->d_S1, m->d_S2, m->d_Wt, m->d_Wsplit, m->wt_count, d, l, lin_tensor);
+                                                                            m->d_P, m->d_S1, m->d_S2, m->d_Wt, m->d_W_hi, m->d_W_lo, m->d_Wt_hi,
+                                                                            m->d_Wt_lo, d, l, lin_tensor);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
