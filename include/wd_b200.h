@@ -137,8 +137,11 @@ typedef struct WdPlanDesc {
      * step copies the records of the rows it touches into an HBM staging buffer, runs the same kernels on them and writes them
      * back, so results are bit-identical to the table in HBM.  WD_PLACE_AUTO: wd_model_create allocates the auto tables largest
      * first and moves to host memory only a table whose HBM allocation fails (with room kept for the buffers allocated after
-     * creation).  Host placement is refused (WD_EUNSUPPORTED) with shard_world > 1, dense_exchange_max_rows > 0 or Adam as the
-     * dnn optimizer; auto tables stay in HBM in those cases. */
+     * creation).  With shard_world > 1 only the row-sharded tables (table_sharded[t] = 1) may be placed on the host: each rank's
+     * shard lives in its own host memory and its owner stages the rows it owns (results bit-identical to the shards in HBM); the
+     * auto placement then also keeps room for the sharded exchange buffers.  Host placement is refused (WD_EUNSUPPORTED) for a
+     * replicated table of a sharded model, with dense_exchange_max_rows > 0 and shard_world <= 1, or with Adam as the dnn
+     * optimizer; auto tables stay in HBM in those cases. */
     const uint8_t *table_placement;
 } WdPlanDesc;
 
@@ -178,7 +181,7 @@ int wd_set_opt_step(WdModel *m, int64_t steps);
 int wd_tensor_io(WdModel *m, int kind, int index, int sub, int slot, void *host, int64_t count, int to_device);
 int64_t wd_tensor_size(WdModel *m, int kind, int index, int sub);
 /* Memory the model holds: device_bytes = HBM it allocated, host_bytes = page-locked host memory of its host-placed embedding
- * tables (WdPlanDesc::table_placement).  Either pointer may be NULL.  (The reference's parameters sit in host RAM on the CPU
+ * tables (WdPlanDesc::table_placement; a rank of a row-sharded model counts its own shards).  Either pointer may be NULL.  (The reference's parameters sit in host RAM on the CPU
  * or on the parameter servers, reference python/lib/build_estimator.py:211-214.) */
 int wd_memory_usage(WdModel *m, int64_t *device_bytes, int64_t *host_bytes);
 /* HBM cache of host-placed table records: an 8-way set-associative, write-back cache of whole [w | slots] records, with LRU
@@ -187,7 +190,8 @@ int wd_memory_usage(WdModel *m, int64_t *device_bytes, int64_t *host_bytes);
  * `bytes` is the HBM budget of the records: it is rounded down to 8 x 2^k slots of the widest host record; the slot metadata
  * (9 bytes per slot) comes on top.  A no-op (capacity 0) when no table is on the host.  WD_ENOMEM when the cache would leave less
  * free HBM than the model keeps in reserve for its later allocations (batch slots, step graphs).  The cache is opt-in:
- * wd_step_backward(_slot) is refused (WD_EUNSUPPORTED) on a model with a cache. */
+ * wd_step_backward(_slot) is refused (WD_EUNSUPPORTED) on a model with a cache.  The cache is single-GPU only: on a row-sharded
+ * model (shard_world > 1) with host-placed shards it returns WD_EUNSUPPORTED. */
 int wd_host_cache_enable(WdModel *m, int64_t bytes);
 /* Cumulative cache counters: out[0] capacity in slots, [1] hits, [2] misses loaded into a slot, [3] overflow rows (staged
  * without a slot: more misses in a set than it has ways), [4] dirty evictions written home.  Copies the first min(n, 5);

@@ -531,8 +531,9 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     m->sort_hist_cap = 1024 * ((m->max_nnz + kSortTile - 1) / kSortTile + 1) + 4 * 1024 + 64;
     for (int k = 0; k < 4; ++k) if ((rc = dev_alloc(m, &m->d_sort_hist_s[k], m->sort_hist_cap))) return rc;
     if (m->use_deep) {
-        // Embedding tables come last, so an auto-placed table competes only with what is allocated after wd_model_create returns.
-        if ((rc = place_tables(m, hbm_reserve_bytes(m)))) return rc;
+        // Embedding tables come last, so an auto-placed table competes only with what is allocated after wd_model_create returns
+        // (and, in a row-sharded model, with what shard_build allocates right below).
+        if ((rc = place_tables(m, hbm_reserve_bytes(m) + (G > 1 ? shard_hbm_bytes(m, d) : 0)))) return rc;
     }
     if (G > 1) {
         if ((rc = shard_build(m, d))) return rc;

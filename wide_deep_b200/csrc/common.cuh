@@ -203,6 +203,10 @@ struct ShardSpace {           // one sharded table space on this rank: 0 = embed
     int64_t* d_slot_base = nullptr;    // [n_slots] first local row of the slot's shard
     int32_t *d_slot_dim = nullptr, *d_slot_x0 = nullptr, *d_slot_stride = nullptr;
     float** d_slot_data = nullptr;     // [n_slots] shard of the table (embedding space)
+    // host-placed shards (embedding space): the owner stages the records of the step's unique owned host rows (list 2) in HBM
+    int stage_stride = 0;              // widest stride of the space's host slots; 0: every shard in HBM
+    int32_t* d_slot_stage = nullptr;   // [n_slots] 0: HBM slot; stage_stride: record of unique row u at d_stage + u * stage_stride
+    float* d_stage = nullptr;          // [max_nnz + 1][stage_stride] owner staging buffer
     float4* d_wide = nullptr;          // wide space: {w, n, z, -} per local row
     uint32_t* d_own = nullptr;         // [max_nnz] owner rank of entry j or kInvalidRow (not a sharded column)
     uint32_t* d_lrow = nullptr;        // [max_nnz] local row at the owner
@@ -461,6 +465,11 @@ int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.
 int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
 int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
 int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
+// host_tables.cu: records of the unique rows urow[0 .. *d_nuniq) of tables with stage_of[t] != 0 (tables found by row base) from their
+// host records into stage row u (in) or back (!in); S = stride of the staging rows
+int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, int ntab, const int64_t* row_base,
+                       float* const* data, const int32_t* stride, const int32_t* stage_of, float* stage, int S);
+int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d);  // shard.cu: HBM shard_build allocates (held back by auto placement)
 int64_t hbm_reserve_bytes(const WdModel* m);                     // api.cu: HBM the model keeps free for its later allocations
 int metrics_accumulate(WdModel* m);                              // metrics.cu
 int metrics_finish(WdModel* m, double* out10);

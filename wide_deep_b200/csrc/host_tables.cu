@@ -14,6 +14,9 @@
 // Every kernel downstream of the stage-in runs on bit-identical values in the same order, so the result equals the HBM-resident
 // model's bit for bit.  Updates that do not go through the fused kernels (data-parallel lists: wd_step_backward + wd_step_apply)
 // address the host records directly through their mapped pointers.
+// Row-sharded tables (shard_world > 1) keep a rank's shard here instead: its owner groups the rows it received (list 2) before
+// serving them and stages them into its own buffer through host_rows_transfer (the owner-side step is in shard.cu).  Only the
+// sharded tables may go to the host then; the replicated ones, the single-GPU staging buffer and the HBM cache stay out of it.
 #include <algorithm>
 
 #include "common.cuh"
@@ -283,6 +286,19 @@ int host_tables_write_back(WdModel* m) {
     return WD_OK;
 }
 
+// The same transfer over any table list without a cache (staging row = u): the host-placed shards of a row-sharded space (shard.cu)
+int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, int ntab, const int64_t* row_base,
+                       float* const* data, const int32_t* stride, const int32_t* stage_of, float* stage, int S) {
+    const StageMap sm{nullptr, nullptr, nullptr, 0};
+    const int g = grid_for(m->max_nnz * (S / 4) / kInFlight, 256);
+    if (in) host_rows_kernel<true><<<g, 256, 0, m->stream>>>(d_nuniq, urow, ntab, row_base, data, stride, stage_of, stage, S, sm);
+    else host_rows_kernel<false><<<g, 256, 0, m->stream>>>(d_nuniq, urow, ntab, row_base, data, stride, stage_of, stage, S, sm);
+    m->launches++;
+    mark(m, in ? "shard_stage_in" : "shard_write_back");
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+
 // Everything that reads or writes host records outside the step: flush = dirty slots home (they stay cached, now clean),
 // invalidate = empty every slot (after the host records were rewritten).  Enqueued on the model stream.
 int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
@@ -361,14 +377,19 @@ static int stage_descriptors(WdModel* m, bool alloc) {
 // Allocates every embedding table — in HBM (WD_PLACE_HBM, and WD_PLACE_AUTO tables while they fit, largest first, with
 // `hbm_reserve` bytes held back for the buffers allocated after wd_model_create) or in mapped page-locked host memory — and fills
 // in the table pointers of the descriptors build_model uploaded, plus the staging buffer and the gather / apply descriptors of the
-// host tables.
+// host tables.  A row-sharded model (shard_world > 1) may place only its sharded tables on the host: this rank's shard lives there
+// and is staged by its owner-side step (shard.cu), nothing here stages it.
 int place_tables(WdModel* m, int64_t hbm_reserve) {
     const int nt = (int)m->tables.size();
-    const bool host_ok = m->shard.world <= 1 && m->dense_exchange_max_rows <= 0 && m->dnn_opt.kind != WD_OPT_ADAM;
+    auto host_ok = [&](const EmbTable& tb) {
+        if (m->dnn_opt.kind == WD_OPT_ADAM) return false;
+        return m->shard.world > 1 ? tb.sharded : m->dense_exchange_max_rows <= 0;
+    };
     for (int t = 0; t < nt; ++t)
-        if (m->tables[t].place == WD_PLACE_HOST && !host_ok) {
-            set_error("table %d: host placement is not supported with row-sharded tables, dense_exchange_max_rows > 0 or the Adam "
-                      "dnn optimizer (its sparse update decays the whole table every step)", t);
+        if (m->tables[t].place == WD_PLACE_HOST && !host_ok(m->tables[t])) {
+            set_error("table %d: host placement is not supported for a replicated table of a row-sharded model, with "
+                      "dense_exchange_max_rows > 0 on one GPU or with the Adam dnn optimizer (its sparse update decays the whole table "
+                      "every step)", t);
             return WD_EUNSUPPORTED;
         }
     auto bytes_of = [&](int t) { return m->tables[t].arows * (int64_t)m->tables[t].stride * 4; };
@@ -377,7 +398,7 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
     for (int t = 0; t < nt; ++t) {
         EmbTable& tb = m->tables[t];
         tb.host = tb.place == WD_PLACE_HOST;
-        if (tb.place == WD_PLACE_AUTO && host_ok) autos.push_back(t);
+        if (tb.place == WD_PLACE_AUTO && host_ok(tb)) autos.push_back(t);
         else if (!tb.host && (rc = dev_alloc(m, &tb.data, tb.arows * tb.stride, true))) return rc;
     }
     if (!autos.empty()) {
@@ -405,6 +426,7 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
         void* dp = nullptr;
         WD_CUDA(cudaHostGetDevicePointer(&dp, p, 0));
         tb.data = (float*)dp;                // every element is written by init_sparse_tables before first use
+        if (tb.sharded) continue;            // staged by its owner (shard_build sizes that buffer)
         m->n_host_tab++;
         m->stage_stride = std::max(m->stage_stride, tb.stride);
     }
@@ -435,6 +457,10 @@ extern "C" int wd_host_cache_enable(WdModel* m, int64_t bytes) {
     WD_CUDA(cudaSetDevice(m->device));
     if (m->stepped) { set_error("wd_host_cache_enable after the first step or forward: the step graphs are already captured"); return WD_ESTATE; }
     if (m->cache_slots > 0) { set_error("wd_host_cache_enable: the cache is already enabled"); return WD_ESTATE; }
+    if (m->shard.world > 1 && m->host_bytes > 0) {
+        set_error("wd_host_cache_enable: the HBM cache is not supported for the host-placed shards of a row-sharded model");
+        return WD_EUNSUPPORTED;
+    }
     if (m->n_host_tab == 0) return WD_OK;                                // nothing on the host: capacity 0
     const int64_t S = m->stage_stride, slot_bytes = S * 4;
     const int64_t sets = bytes / (kWays * slot_bytes);

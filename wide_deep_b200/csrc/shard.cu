@@ -18,6 +18,17 @@
 //   dense          gradients of the MLP / wide bias / small replicated tables: two-shot all-reduce over peer memory (each rank
 //                  reduces one slice in rank order, then every rank gathers the slices) — deterministic, identical on all ranks
 //
+// A rank's shard of an embedding table may live in mapped, page-locked host memory (WdPlanDesc::table_placement).  The owner then
+// moves exactly one record per unique owned host row each way per train step (inward only for a forward):
+//   1. group        after barrier A, on the main stream: flatten + group the received rows (list 2) — the grouping the backward
+//                   needs anyway, moved in front of the serve
+//   2. stage-in     host_rows_kernel<true> (host_tables.cu): record of unique row u of a host slot -> owner staging buffer row u
+//   3. serve        a host slot's records are read from staging row u (lower_bound of the local row in urow[2])
+//   4. apply        emb_apply_kernel updates the staged record of u (per-slot stage stride; 0 = HBM slot, updated in place)
+//   5. write-back   host_rows_kernel<false>, right after the apply on the same stream, which joins the main stream before the step
+//                   ends (before the next stage-in); forward-only calls skip it
+// Every kernel reads the same values and sums them in the same order as with the shard in HBM: the results are bit-identical.
+//
 // Ranks synchronise with flag barriers in peer memory (st.release.sys / ld.acquire.sys); when all ranks live in ONE process
 // (tests on a single GPU) the caller orders the phases with events instead (wd_shard_phase + wd_shard_local_sync).
 #include <stdlib.h>
@@ -128,12 +139,17 @@ __device__ __forceinline__ bool shard_locate(int64_t f, const int32_t* __restric
     return false;
 }
 
-// embedding space: 8 lanes per received entry; the lanes of a bag's first entry pool the whole run and store the partial sum
+// embedding space: 8 lanes per received entry; the lanes of a bag's first entry pool the whole run and store the partial sum.
+// slot_stage (null: every shard in HBM): a host slot's records are read from the owner staging buffer, row u = position of the
+// local row in the step's unique owned rows urow[0 .. *d_nuniq) (list 2, sorted ascending).  (Entries beyond the max_nnz the grouping
+// keeps — flagged as truncated — find u <= max_nnz: the staging buffer has one spare row.)
 __global__ void __launch_bounds__(256) shard_serve_emb_kernel(const uint2* __restrict__ inbox, const int32_t* __restrict__ cnt, int G, int me,
                                                               int64_t pair_cap, int n_slots, const int64_t* __restrict__ slot_base,
                                                               float* const* __restrict__ slot_data, const int32_t* __restrict__ slot_dim,
                                                               const int32_t* __restrict__ slot_stride, const ShardPeer* __restrict__ peers,
-                                                              int64_t nbags_cap, int width) {
+                                                              int64_t nbags_cap, int width, const int32_t* __restrict__ slot_stage,
+                                                              const float* __restrict__ stage, const uint32_t* __restrict__ urow,
+                                                              const int32_t* __restrict__ d_nuniq) {
     const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
     int64_t total = 0;
     for (int r = 0; r < G; ++r) total += __ldcg(cnt + r);
@@ -147,17 +163,20 @@ __global__ void __launch_bounds__(256) shard_serve_emb_kernel(const uint2* __res
         if (i > 0 && __ldcg(box + i - 1).y == en.y) continue;     // not the head of its bag
         int lo = 0, hi = n_slots - 1;
         while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (slot_base[mid] <= (int64_t)en.x) lo = mid; else hi = mid - 1; }
-        const int dim = slot_dim[lo], stride = slot_stride[lo];
-        const float* data = slot_data[lo];
+        const int sst = slot_stage ? slot_stage[lo] : 0;
+        const int dim = slot_dim[lo], stride = sst ? sst : slot_stride[lo];
+        const float* data = sst ? stage : slot_data[lo];
         const int64_t base = slot_base[lo];
+        const int nu = sst ? *d_nuniq : 0;
+        auto rec = [&](uint32_t lrow) -> int64_t { return sst ? (int64_t)lower_bound_u32(urow, nu, lrow) : (int64_t)lrow - base; };
         const int n = __ldcg(cnt + r);
         float* dst = peers[r].recv + ((int64_t)me * nbags_cap + en.y) * width;
         for (int q = lig; q * 4 < dim; q += 8) {
-            float4 acc = ldg_nc_f4(data + ((int64_t)en.x - base) * stride + q * 4);
+            float4 acc = ldg_nc_f4(data + rec(en.x) * stride + q * 4);
             for (int j = i + 1; j < n; ++j) {
                 const uint2 e2 = __ldcg(box + j);
                 if (e2.y != en.y) break;
-                const float4 v = ldg_nc_f4(data + ((int64_t)e2.x - base) * stride + q * 4);
+                const float4 v = ldg_nc_f4(data + rec(e2.x) * stride + q * 4);
                 acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
             }
             *reinterpret_cast<float4*>(dst + q * 4) = acc;
@@ -379,7 +398,7 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     // ---- embedding space
     {
         ShardSpace& sp = S.sp[0];
-        std::vector<int32_t> col_slot(C, -1), dim, x0, stride;
+        std::vector<int32_t> col_slot(C, -1), dim, x0, stride, host;
         std::vector<int64_t> base;
         std::vector<float*> data;
         int64_t rows = 0;
@@ -388,6 +407,8 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
             if (!tb.sharded) continue;
             col_slot[tb.col] = sp.n_slots++;
             base.push_back(rows); dim.push_back(tb.dim); x0.push_back(tb.x0_off); stride.push_back(tb.stride); data.push_back(tb.data);
+            host.push_back(tb.host);
+            if (tb.host) sp.stage_stride = std::max(sp.stage_stride, tb.stride);
             tb.row_base = rows;
             rows += (tb.rows + G - 1) / G;            // the SAME layout on every rank (a requester computes the owner's local row): ceil(rows / G) per table
             sp.width = std::max(sp.width, tb.dim);
@@ -403,6 +424,11 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
             if ((rc = upload_arr(m, x0, &sp.d_slot_x0))) return rc;
             if ((rc = upload_arr(m, stride, &sp.d_slot_stride))) return rc;
             if ((rc = upload_arr(m, data, &sp.d_slot_data))) return rc;
+        }
+        if (sp.stage_stride > 0) {               // host-placed shards: staging rows of the step's unique owned rows (+1: see the serve)
+            for (int32_t& h : host) h = h ? sp.stage_stride : 0;
+            if ((rc = upload_arr(m, host, &sp.d_slot_stage))) return rc;
+            if ((rc = dev_alloc(m, &sp.d_stage, (m->max_nnz + 1) * (int64_t)sp.stage_stride, false))) return rc;
         }
     }
     // ---- wide space
@@ -508,6 +534,36 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     return WD_OK;
 }
 
+// HBM that shard_build allocates after the embedding tables, for their auto placement to hold back: the wide shard, the per-space
+// scratch and sort lists 2 + s / 4 + s, the exchange segment, and 1 MB for descriptors, flags and alignment.  (The owner staging
+// buffer is covered by hbm_reserve_bytes, whose single-GPU staging buffer a sharded model never allocates.)
+int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d) {
+    const int G = std::max(d->shard_world, 1);
+    const int64_t n = m->max_nnz + 8;
+    int emb_width = 0, n_slots = 0;
+    for (const EmbTable& tb : m->tables)
+        if (tb.sharded) { emb_width = std::max(emb_width, tb.dim); n_slots++; }
+    int64_t wide_rows = 0;
+    bool wide_on = false;
+    if (m->use_wide && d->col_wide_sharded)
+        for (int c = 0; c < m->n_columns; ++c)
+            if (d->col_wide_sharded[c]) { wide_on = true; wide_rows += (d->col_buckets[c] + G - 1) / G; }
+    int64_t bytes = (1 << 20) + wide_rows * 16;
+    for (int s = 0; s < 2; ++s) {
+        if (s == 0 ? n_slots == 0 : !wide_on) continue;
+        const int64_t width = s == 0 ? emb_width : 1, w = s == 0 ? std::max(emb_width, 4) : 1;
+        const int64_t nbags = (int64_t)m->max_batch * (s == 0 ? n_slots : 1);
+        bytes += 4 * (4 * n + nbags + 8)                              // own, lrow, rtag, rrow, bagmask
+                 + 4 * 8 * n                                          // keys / values (+ ping-pong) of lists 2 + s and 4 + s
+                 + 4 * (3 * n + n * w + m->cpart_cap * w)             // urow, ustart, choff, ugrad, cpart
+                 + (int64_t)G * m->max_nnz * 8                        // inbox
+                 + (int64_t)G * nbags * width * 4 + nbags * 4;        // recv, bagscale
+    }
+    const int64_t x0n = m->use_deep ? (int64_t)m->max_batch_pad * std::max(m->d0_phys, 1) : 4;
+    bytes += x0n * 4 + (int64_t)m->max_batch * 4 + 2 * align_up(m->dense_count + m->gs_count + 4, 4) * 4;
+    return bytes;
+}
+
 // peer segment bases known: fill the per-peer pointer tables
 static int shard_finish_connect(WdModel* m) {
     ShardState& S = m->shard;
@@ -576,15 +632,27 @@ static int shard_route_send(WdModel* m, int s) {
     return WD_OK;
 }
 
+static int shard_owner_group(WdModel* m, int s);
+
+// a space whose owner stages host-placed shards groups its received rows before serving them (the serve reads the staged records)
+static bool staged(const WdModel* m, int s) { return m->shard.sp[s].stage_stride > 0; }
+
 // ---- owner: pooled partial sums of the received bags -> requesters' receive buffers
 static int shard_serve(WdModel* m, int s) {
     ShardState& S = m->shard;
     ShardSpace& sp = S.sp[s];
     if (!sp.on) return WD_OK;
     const ShardPeer& me = sp.peers[S.rank];
+    int rc;
+    if (staged(m, s)) {                          // unique owned rows (list 2), then the records of the host rows among them -> HBM
+        if ((rc = shard_owner_group(m, s))) return rc;
+        if ((rc = host_rows_transfer(m, true, m->d_nuniq[2], m->d_urow[2], sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_stride,
+                                     sp.d_slot_stage, sp.d_stage, sp.stage_stride))) return rc;
+    }
     if (s == 0)
         shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
-            sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_peers, sp.nbags_cap, sp.width);
+            sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_peers, sp.nbags_cap, sp.width,
+            sp.d_slot_stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2]);
     else
         shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
             sp.d_wide, sp.d_peers, sp.nbags_cap);
@@ -636,7 +704,11 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
             m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0, m->d0_phys, m->d_cpart[L], sp.width);
         m->launches += 2;
         if ((rc = list_chunk_combine(m, L, sp.width))) return rc;
-        if ((rc = list_apply_emb(m, L, sp.width, sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, m->dnn_opt))) return rc;
+        if ((rc = list_apply_emb(m, L, sp.width, sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, m->dnn_opt,
+                                 sp.d_slot_stage, sp.d_stage))) return rc;
+        // staged records home, on this stream: it joins the main stream before the step ends, so the next stage-in comes after
+        if (staged(m, s) && (rc = host_rows_transfer(m, false, m->d_nuniq[L], m->d_urow[L], sp.n_slots, sp.d_slot_base, sp.d_slot_data,
+                                                     sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, sp.stage_stride))) return rc;
     } else {
         shard_wide_grad_sum_kernel<false><<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nuniq[L], m->d_ustart[L], m->d_choff[L],
             m->d_sv[L], sp.d_rtag, sp.d_peers, m->d_ugrad[L]);
@@ -740,12 +812,12 @@ static int shard_serve_both(WdModel* m) {
     for (int s = 0; s < 2; ++s) if ((rc = shard_serve(m, s))) return rc;
     return sparse_forward(m);
 }
-// phase 1: serve the peers, local gathers; sort what was received
+// phase 1: (group + stage-in of a staged space,) serve the peers, local gathers; sort what was received
 int shard_phase1(WdModel* m, bool train) {
     int rc;
     if ((rc = shard_serve_both(m))) return rc;
     if (train)
-        for (int s = 0; s < 2; ++s) if ((rc = shard_owner_group(m, s))) return rc;
+        for (int s = 0; s < 2; ++s) if (!staged(m, s) && (rc = shard_owner_group(m, s))) return rc;
     return WD_OK;
 }
 // phase 2: combine, towers forward / backward, dense gradient arena
@@ -790,7 +862,7 @@ int shard_step_ipc(WdModel* m, bool train) {
     if (train) {
         WD_CUDA(cudaEventRecord(S.ev_a, m->stream));
         for (int s = 0; s < 2; ++s) {
-            if (!S.sp[s].on) continue;
+            if (!S.sp[s].on || staged(m, s)) continue;             // (a staged space was grouped before its serve)
             if (m->side_pending[s]) {
                 WD_CUDA(cudaStreamWaitEvent(m->sstream[s], S.ev_a, 0));
                 if ((rc = on_side(m, s, [&] { return shard_owner_group(m, s); }))) return rc;

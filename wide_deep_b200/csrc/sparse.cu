@@ -453,12 +453,13 @@ __global__ void wide_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const 
 
 // --------------------------------------------------------------------------------------------- optimizers
 
-// embedding rows: record = [w[dim] | s1[dim] | s2[dim]]
+// embedding rows: record = [w[dim] | s1[dim] | s2[dim]]; tab_stage (null: every record in place): 0 = in place, else the record of
+// unique row u is staged at stage + u * tab_stage[t] (host-placed shards of a row-sharded space, shard.cu)
 __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow,
                                                         const float* __restrict__ ugrad, int width, int ntab,
                                                         const int64_t* __restrict__ tab_row_base, float* const* __restrict__ tab_data,
                                                         const int32_t* __restrict__ tab_dim, const int32_t* __restrict__ tab_stride,
-                                                        OptParams o) {
+                                                        OptParams o, const int32_t* __restrict__ tab_stage, float* __restrict__ stage) {
     const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
     const int nu = *d_nuniq;
     const int64_t g0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4 + grp;
@@ -471,7 +472,8 @@ __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restric
             if (tab_row_base[mid] <= row) lo = mid; else hi = mid - 1;
         }
         const int dim = tab_dim[lo], stride = tab_stride[lo];
-        float* rec = tab_data[lo] + (row - tab_row_base[lo]) * stride;
+        const int sst = tab_stage ? tab_stage[lo] : 0;
+        float* rec = sst ? stage + u * sst : tab_data[lo] + (row - tab_row_base[lo]) * stride;
         const int nslots = stride / dim - 1;
         for (int q = lig; q * 4 < dim; q += 8) {
             float4 g = *reinterpret_cast<const float4*>(ugrad + (int64_t)u * width + q * 4);
@@ -851,7 +853,7 @@ int sparse_apply_which(WdModel* m, int which) {
         if (adam && (rc = adam_dense_pass(m, 0, false))) return rc;
         emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(
             m->d_nuniq[0], m->d_urow[0], m->d_ugrad[0], m->emb_max_dim, m->n_rtab, m->d_rtab_row_base, m->d_rtab_data,
-            m->d_rtab_dim, m->d_rtab_stride, make_opt(m->dnn_opt));          // tables in row order (binary search by row)
+            m->d_rtab_dim, m->d_rtab_stride, make_opt(m->dnn_opt), nullptr, nullptr);   // tables in row order (binary search by row)
         m->launches++;
         if (adam && (rc = adam_dense_pass(m, 0, true))) return rc;
     }
@@ -887,9 +889,9 @@ int list_chunk_combine(WdModel* m, int which, int width) {
     return WD_OK;
 }
 int list_apply_emb(WdModel* m, int which, int width, int ntab, const int64_t* d_row_base, float* const* d_data, const int32_t* d_dim,
-                   const int32_t* d_stride, const WdOptimizer& o) {
+                   const int32_t* d_stride, const WdOptimizer& o, const int32_t* d_stage, float* stage) {
     emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], width, ntab,
-                                                                            d_row_base, d_data, d_dim, d_stride, make_opt(o));
+                                                                            d_row_base, d_data, d_dim, d_stride, make_opt(o), d_stage, stage);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;

@@ -81,9 +81,10 @@ int list_group(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row)
 int list_sort_by_key(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_key);
 // ugrad[u] = fixed-order sum of the chunk partials of multi-chunk rows (after the two gradient-sum passes)
 int list_chunk_combine(WdModel* m, int which, int width);
-// optimizer over the unique rows of list `which`: embedding tables given in row order / one wide record array
+// optimizer over the unique rows of list `which`: embedding tables given in row order / one wide record array.  d_stage (optional,
+// [ntab]): 0 = record in place, else the table is staged and the record of unique row u is at stage + u * d_stage[t]
 int list_apply_emb(WdModel* m, int which, int width, int ntab, const int64_t* d_row_base, float* const* d_data, const int32_t* d_dim,
-                   const int32_t* d_stride, const WdOptimizer& o);
+                   const int32_t* d_stride, const WdOptimizer& o, const int32_t* d_stage = nullptr, float* stage = nullptr);
 int list_apply_wide(WdModel* m, int which, float4* wide, const WdOptimizer& o);
 
 }  // namespace wd

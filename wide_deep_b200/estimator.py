@@ -50,8 +50,9 @@ class WideAndDeepClassifier(object):
         self._trainer = None
         # embedding tables in page-locked host memory (the reference's tables live in host RAM: it trains on the CPU or on
         # parameter servers, build_estimator.py:211-214): None = only the tables that do not fit in HBM, "all" or a list of table
-        # names = exactly those.  Checkpoints do not depend on the placement.  host_cache_bytes > 0: HBM budget of a write-back
-        # cache of the host tables' most recently used records (results do not change, PCIe traffic does).
+        # names = exactly those.  Checkpoints do not depend on the placement.  With shard_world > 1 only row-sharded tables can go
+        # there (each rank keeps its own shard).  host_cache_bytes > 0 (one GPU only): HBM budget of a write-back cache of the host
+        # tables' most recently used records (results do not change, PCIe traffic does).
         self.plan = compile_plan(self.config, model_type, mb, tf_compat_pad=tf_compat_pad, gemm_engine=gemm_engine, host_tables=host_tables,
                                  host_cache_bytes=host_cache_bytes,
                                  shard_world=self.shard_world, shard_rank=self.shard_rank, shard_slack=float(max(2, self.shard_world)),
