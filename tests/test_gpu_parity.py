@@ -40,10 +40,11 @@ def small_conf(hidden=(64, 32), mode="simple", act="relu", bn=1, dnn_opt="Adagra
     return fc, cross, model
 
 
-def build_pair(fc, cross, model, model_type="wide_deep", B=96, seed=0, tf_compat_pad=False, emb_dim=None, max_batch=None, dense_rows=0):
+def build_pair(fc, cross, model, model_type="wide_deep", B=96, seed=0, tf_compat_pad=False, emb_dim=None, max_batch=None, dense_rows=0,
+               engine="ffma"):
     om = OM.OracleModel(fc, cross, model, model_type, embedding_dim_override=emb_dim, tf_compat_pad=tf_compat_pad).init(seed)
     plan = Plan(fc, cross, model, model_type, max_batch=max_batch or B, embedding_dim_override=emb_dim,
-                tf_compat_pad=tf_compat_pad, max_nnz=(max_batch or B) * 64, max_keys=(max_batch or B) * 64, gemm_engine="ffma",
+                tf_compat_pad=tf_compat_pad, max_nnz=(max_batch or B) * 64, max_keys=(max_batch or B) * 64, gemm_engine=engine,
                 dense_exchange_max_rows=dense_rows)
     pm = WideDeepModel(plan)
     copy_params_to_product(om, pm)

@@ -110,13 +110,14 @@ extern "C" int wd_model_destroy(WdModel* m) {
     if (m->stream) cudaStreamSynchronize(m->stream);
     tc_map_cache_clear();
     for (auto& sl : m->slots) {
-        if (sl.graph) cudaGraphExecDestroy(sl.graph);
-        if (sl.graph_bwd) cudaGraphExecDestroy(sl.graph_bwd);
+        sl.train.destroy();
+        sl.bwd.destroy();
+        sl.shard.destroy();
         if (sl.ev_up) cudaEventDestroy(sl.ev_up);
         if (sl.ev_used) cudaEventDestroy(sl.ev_used);
     }
     if (m->stream_up) { cudaStreamSynchronize(m->stream_up); cudaStreamDestroy(m->stream_up); }
-    for (auto& g : m->merge_graph) if (g.exec) cudaGraphExecDestroy(g.exec);
+    for (auto& g : m->merge_graph) g.destroy();
     if (m->ev_bwd_done) cudaEventDestroy(m->ev_bwd_done);
     for (void* p : m->allocs) cudaFree(p);
     for (void* p : m->host_allocs) cudaFreeHost(p);
@@ -1118,51 +1119,60 @@ static int train_eager(WdModel* m) {
     return rc;
 }
 
-static bool same_view(const DevBatch& a, const DevBatch& b) {
-    return a.B == b.B && a.cat_offsets == b.cat_offsets && a.cat_keys == b.cat_keys && a.dense == b.dense && a.label == b.label && a.weight == b.weight;
+enum class GraphRun { eager, captured, replayed };
+
+// Issues step work through a CUDA graph.  issue(capturing) enqueues the work on `st`; under capture it joins every other stream it
+// forks back into `st`.  The work runs eagerly twice, is then captured once and replayed for as long as `key` equals the key the
+// capture baked in; a different key re-captures at once.  A replay removes the launch gaps between the work's many small kernels,
+// and the host cost becomes one cudaGraphLaunch.  With WD_NO_GRAPH=1 or profiling on, or for good once a capture has failed,
+// the work runs eagerly.  *how tells the caller which of the three happened.
+template <class Key, class F>
+static int run_graphed(WdModel* m, StepGraph<Key>& g, const Key& key, cudaStream_t st, F issue, GraphRun* how) {
+    *how = GraphRun::eager;
+    if (!m->graphs_enabled || m->timer.enabled) return issue(false);
+    if (g.exec && g.key == key) {
+        *how = GraphRun::replayed;
+    } else if (g.eager < 2) {
+        const int rc = issue(false);
+        if (rc == WD_OK) g.eager++;
+        return rc;
+    } else {
+        g.destroy();
+        const int64_t l0 = m->launches;
+        cudaGraph_t graph = nullptr;
+        cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
+        if (e == cudaSuccess) {
+            const int rc = issue(true);
+            const cudaError_t e2 = cudaStreamEndCapture(st, &graph);
+            if (rc == WD_OK && e2 == cudaSuccess && graph) e = cudaGraphInstantiate(&g.exec, graph, 0);
+            else e = e2 != cudaSuccess ? e2 : cudaErrorUnknown;
+            if (graph) cudaGraphDestroy(graph);
+        }
+        if (e != cudaSuccess || !g.exec) {                  // not capturable here: stay eager for good
+            cudaGetLastError();
+            g.exec = nullptr;
+            m->graphs_enabled = false;
+            return issue(false);
+        }
+        g.key = key;
+        g.launches = m->launches - l0;                      // counted again on every launch of the graph
+        m->launches = l0;
+        *how = GraphRun::captured;
+    }
+    WD_CUDA(cudaGraphLaunch(g.exec, st));
+    m->launches += g.launches;
+    return WD_OK;
 }
 
-// One whole train step on the current slot.  After two eager steps the step (three streams, ~55 kernels, no host sync)
-// is captured once into a CUDA graph per batch slot and replayed: launch gaps between the many small kernels
-// disappear and the host cost of a step becomes one cudaGraphLaunch.
+// One whole train step on the current slot (three streams, ~55 kernels, no host sync), graphed per slot.
 static int train_current(WdModel* m, float* loss_out) {
-    int rc;
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
-    BatchSlot& sl = m->slots[m->cur_slot];
-    const bool can_graph = m->graphs_enabled && !m->timer.enabled;
-    if (can_graph && sl.graph && same_view(sl.graph_view, m->dbatch)) {
-        WD_CUDA(cudaGraphLaunch(sl.graph, m->stream));
-        m->launches += sl.graph_launches;
+    GraphRun how;
+    int rc = run_graphed(m, m->slots[m->cur_slot].train, m->dbatch, m->stream, [&](bool) { return train_eager(m); }, &how);
+    if (rc) return rc;
+    if (how != GraphRun::eager) {                           // a graphed step ends as an eager one does: nothing left pending
+        m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
         m->grads_pending = false;
-    } else if (can_graph && sl.eager_steps >= 2) {
-        if (sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }
-        const int64_t l0 = m->launches;
-        cudaGraph_t g = nullptr;
-        cudaError_t e = cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal);
-        if (e == cudaSuccess) {
-            rc = train_eager(m);
-            cudaError_t e2 = cudaStreamEndCapture(m->stream, &g);
-            if (rc == WD_OK && e2 == cudaSuccess && g) e = cudaGraphInstantiate(&sl.graph, g, 0);
-            else e = e2 != cudaSuccess ? e2 : cudaErrorUnknown;
-            if (g) cudaGraphDestroy(g);
-        }
-        if (e != cudaSuccess || !sl.graph) {            // capture not possible here: stay eager for good
-            cudaGetLastError();
-            m->graphs_enabled = false;
-            sl.graph = nullptr;
-            m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
-            if ((rc = train_eager(m))) return rc;
-        } else {
-            sl.graph_view = m->dbatch;
-            sl.graph_launches = m->launches - l0;
-            m->launches = l0;
-            m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false; m->grads_pending = false;
-            WD_CUDA(cudaGraphLaunch(sl.graph, m->stream));
-            m->launches += sl.graph_launches;
-        }
-    } else {
-        if ((rc = train_eager(m))) return rc;
-        sl.eager_steps++;
     }
     if ((rc = mark_slot_used(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);
@@ -1226,9 +1236,8 @@ static int backward_eager(WdModel* m, bool join) {
 }
 
 // Data-parallel steps run forward + backward, then the exchange (NCCL, outside the library), then merge + apply.  The first part
-// is ~65 launches on three streams: like the full step it is captured per batch slot after two eager runs and replayed.  Inside
-// the graph the streams overlap as in the eager schedule; after it the sparse lists continue on their side streams, which wait for
-// the graph through ev_bwd_done.
+// is ~65 launches on three streams, graphed per batch slot.  Inside the graph the streams overlap as in the eager schedule; after
+// it the sparse lists continue on their side streams, which wait for the graph through ev_bwd_done.
 // The split step applies the embedding rows with the unfused kernels, which update host records through their mapped pointers:
 // with an HBM cache in front of those records the update would bypass it.
 static int refuse_split_step_with_cache(WdModel* m) {
@@ -1246,10 +1255,11 @@ extern "C" int wd_step_backward_slot(WdModel* m, int slot, float* loss_out) {
     if ((rc = refuse_split_step_with_cache(m))) return rc;
     timer_begin(m);
     BatchSlot& sl = m->slots[slot];
-    const bool can_graph = m->graphs_enabled && !m->timer.enabled;
-    auto after_graph = [&]() -> int {
-        WD_CUDA(cudaGraphLaunch(sl.graph_bwd, m->stream));
-        m->launches += sl.graph_bwd_launches;
+    GraphRun how;
+    if ((rc = run_graphed(m, sl.bwd, m->dbatch, m->stream, [&](bool capturing) { return backward_eager(m, capturing); }, &how))) return rc;
+    if (how == GraphRun::captured)
+        for (int w = 0; w < 2; ++w) sl.bwd_side_active[w] = m->side_active[w];
+    if (how != GraphRun::eager) {
         WD_CUDA(cudaEventRecord(m->ev_bwd_done, m->stream));
         for (int w = 0; w < 2; ++w) {
             m->side_pending[w] = false;
@@ -1257,38 +1267,6 @@ extern "C" int wd_step_backward_slot(WdModel* m, int slot, float* loss_out) {
             if (m->side_active[w]) WD_CUDA(cudaStreamWaitEvent(m->sstream[w], m->ev_bwd_done, 0));
         }
         m->grads_pending = true;
-        return WD_OK;
-    };
-    if (can_graph && sl.graph_bwd && same_view(sl.graph_bwd_view, m->dbatch)) {
-        if ((rc = after_graph())) return rc;
-    } else if (can_graph && sl.bwd_eager_steps >= 2) {
-        if (sl.graph_bwd) { cudaGraphExecDestroy(sl.graph_bwd); sl.graph_bwd = nullptr; }
-        const int64_t l0 = m->launches;
-        cudaGraph_t g = nullptr;
-        cudaError_t e = cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal);
-        if (e == cudaSuccess) {
-            rc = backward_eager(m, true);
-            cudaError_t e2 = cudaStreamEndCapture(m->stream, &g);
-            if (rc == WD_OK && e2 == cudaSuccess && g) e = cudaGraphInstantiate(&sl.graph_bwd, g, 0);
-            else e = e2 != cudaSuccess ? e2 : cudaErrorUnknown;
-            if (g) cudaGraphDestroy(g);
-        }
-        if (e != cudaSuccess || !sl.graph_bwd) {             // capture not possible here: stay eager for good
-            cudaGetLastError();
-            m->graphs_enabled = false;
-            sl.graph_bwd = nullptr;
-            m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
-            if ((rc = backward_eager(m, false))) return rc;
-        } else {
-            sl.graph_bwd_view = m->dbatch;
-            sl.graph_bwd_launches = m->launches - l0;
-            m->launches = l0;
-            sl.bwd_side_active[0] = m->side_active[0]; sl.bwd_side_active[1] = m->side_active[1];
-            if ((rc = after_graph())) return rc;
-        }
-    } else {
-        if ((rc = backward_eager(m, false))) return rc;
-        sl.bwd_eager_steps++;
     }
     if ((rc = mark_slot_used(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);
@@ -1344,63 +1322,30 @@ extern "C" int wd_sparse_grads(WdModel* m, int which, void** rows, void** grads,
     return WD_OK;
 }
 
-// n_lists = 0: general (unsorted) list of n rows; n_lists > 0: n_lists sorted, duplicate-free lists of n / n_lists rows each
-static int sparse_set_impl(WdModel* m, int which, const void* rows_dev, const void* grads_dev, int64_t n, int n_lists) {
+// n_lists = 0: general (unsorted) list of n rows; n_lists > 0: n_lists sorted, duplicate-free lists of list_len rows each
+static int sparse_set_impl(WdModel* m, int which, const void* rows_dev, const void* grads_dev, int64_t n, int n_lists, int64_t list_len) {
     int rc = check_ready(m);
     if (rc) return rc;
     if (which < 0 || which > 1 || !m->d_urow[which]) { set_error("no sparse gradient list %d", which); return WD_EINVAL; }
     const bool side = m->side_active[which];
     auto merge = [&]() -> int {
-        return n_lists > 0 ? merge_sparse_sorted(m, which, rows_dev, grads_dev, n_lists, n / n_lists) : merge_sparse(m, which, rows_dev, grads_dev, n);
+        return n_lists > 0 ? merge_sparse_sorted(m, which, rows_dev, grads_dev, n_lists, list_len) : merge_sparse(m, which, rows_dev, grads_dev, n);
     };
-    auto run = [&]() -> int {
-        if (side) return on_side(m, which, merge);
-        return merge();
-    };
-    // ~25 small launches on one stream; with a fixed-size exchange the arguments never change, so after two eager runs the merge
-    // is captured and replayed (the data-parallel tail is otherwise bound by the launching thread, not by the GPU)
-    WdModel::MergeGraph& g = m->merge_graph[which];
-    cudaStream_t st = side ? m->sstream[which] : m->stream;
-    const bool same = g.rows == rows_dev && g.grads == grads_dev && g.n == n && g.on_side == side && g.n_lists == n_lists;
-    if (!m->graphs_enabled || m->timer.enabled) return run();
-    if (g.exec && same) {
-        WD_CUDA(cudaGraphLaunch(g.exec, st));
-        m->launches += g.launches;
-        return WD_OK;
-    }
-    if (!same) {
-        if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-        g.rows = rows_dev; g.grads = grads_dev; g.n = n; g.on_side = side; g.n_lists = n_lists; g.eager = 0;
-    }
-    if (g.eager < 2) { g.eager++; return run(); }
-    const int64_t l0 = m->launches;
-    cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-    if (e == cudaSuccess) {
-        rc = run();
-        cudaError_t e2 = cudaStreamEndCapture(st, &graph);
-        if (rc == WD_OK && e2 == cudaSuccess && graph) e = cudaGraphInstantiate(&g.exec, graph, 0);
-        else e = e2 != cudaSuccess ? e2 : cudaErrorUnknown;
-        if (graph) cudaGraphDestroy(graph);
-    }
-    if (e != cudaSuccess || !g.exec) {                        // not capturable here: stay eager
-        cudaGetLastError();
-        g.exec = nullptr; g.eager = -1000000;
-        return run();
-    }
-    g.launches = m->launches - l0;
-    m->launches = l0;
-    WD_CUDA(cudaGraphLaunch(g.exec, st));
-    m->launches += g.launches;
-    return WD_OK;
+    auto run = [&](bool) -> int { return side ? on_side(m, which, merge) : merge(); };
+    // The count-based exchange changes n, the number of exchanged rows, every step: its merge runs eagerly.  The fixed-size
+    // exchange passes the same buffers and shape every step, so its merge (~25 small launches on one stream) is graphed: the
+    // data-parallel tail is otherwise bound by the launching thread, not by the GPU.
+    if (n_lists == 0) return run(false);
+    GraphRun how;
+    return run_graphed(m, m->merge_graph[which], MergeKey{rows_dev, grads_dev, n_lists, list_len, side}, side ? m->sstream[which] : m->stream, run, &how);
 }
 
 extern "C" int wd_sparse_set(WdModel* m, int which, const void* rows_dev, const void* grads_dev, int64_t n) {
-    return sparse_set_impl(m, which, rows_dev, grads_dev, n, 0);
+    return sparse_set_impl(m, which, rows_dev, grads_dev, n, 0, 0);
 }
 extern "C" int wd_sparse_set_sorted(WdModel* m, int which, const void* rows_dev, const void* grads_dev, int32_t n_lists, int64_t list_len) {
     if (n_lists < 1 || list_len < 1) { set_error("wd_sparse_set_sorted: bad list shape"); return WD_EINVAL; }
-    return sparse_set_impl(m, which, rows_dev, grads_dev, (int64_t)n_lists * list_len, n_lists);
+    return sparse_set_impl(m, which, rows_dev, grads_dev, 0, n_lists, list_len);
 }
 
 // ------------------------------------------------------------------------------------- row-sharded tables
@@ -1446,47 +1391,18 @@ extern "C" int wd_shard_finish(WdModel* m, float* loss_out, float* logits_out) {
 
 // The whole step of one rank of a multi-process job: ids, routing, serve, combine, towers, owners' updates, dense all-reduce and
 // optimizers, with flag barriers in peer memory between the phases.  Every rank must call it once per step (it is a collective).
-// After two eager steps per batch slot the step is captured into one CUDA graph (barrier kernels included) and replayed.
+// Graphed per batch slot, barrier kernels included.
 extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
     int rc = shard_ready(m, slot);
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_train_step_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase)"); return WD_ESTATE; }
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
-    if (slot >= 64) { set_error("slot out of range"); return WD_EINVAL; }
-    ShardState& S = m->shard;
-    const bool can_graph = m->graphs_enabled && !m->timer.enabled;
-    if (can_graph && S.graph[slot] && same_view(S.graph_view[slot], m->dbatch)) {
-        WD_CUDA(cudaGraphLaunch(S.graph[slot], m->stream));
-        m->launches += S.graph_launches[slot];
-        S.step++;
-    } else if (can_graph && S.eager_steps[slot] >= 2) {
-        if (S.graph[slot]) { cudaGraphExecDestroy(S.graph[slot]); S.graph[slot] = nullptr; }
-        const int64_t l0 = m->launches;
-        cudaGraph_t g = nullptr;
-        cudaError_t e = cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal);
-        if (e == cudaSuccess) {
-            rc = shard_step_ipc(m, true);
-            cudaError_t e2 = cudaStreamEndCapture(m->stream, &g);
-            if (rc == WD_OK && e2 == cudaSuccess && g) e = cudaGraphInstantiate(&S.graph[slot], g, 0);
-            else e = e2 != cudaSuccess ? e2 : cudaErrorUnknown;
-            if (g) cudaGraphDestroy(g);
-        }
-        m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false; m->grads_pending = false;
-        if (e != cudaSuccess || !S.graph[slot]) {              // not capturable here: stay eager for good
-            cudaGetLastError();
-            m->graphs_enabled = false;
-            S.graph[slot] = nullptr;
-            if ((rc = shard_step_ipc(m, true))) return rc;
-        } else {
-            S.graph_view[slot] = m->dbatch;
-            S.graph_launches[slot] = m->launches - l0;
-            m->launches = l0;
-            WD_CUDA(cudaGraphLaunch(S.graph[slot], m->stream));
-            m->launches += S.graph_launches[slot];
-        }
-    } else {
-        if ((rc = shard_step_ipc(m, true))) return rc;
-        S.eager_steps[slot]++;
+    GraphRun how;
+    if ((rc = run_graphed(m, m->slots[slot].shard, m->dbatch, m->stream, [&](bool) { return shard_step_ipc(m, true); }, &how))) return rc;
+    if (how == GraphRun::replayed) m->shard.step++;          // (a capture ran shard_step_ipc, which advanced it)
+    if (how == GraphRun::captured) {
+        m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
+        m->grads_pending = false;
     }
     if ((rc = mark_slot_used(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);

@@ -155,6 +155,33 @@ struct PhaseTimer {          // named CUDA-event marks on the model stream (wd_s
     bool enabled = false;
 };
 
+// A CUDA graph of step work (api.cu run_graphed), replayed only while the key it was captured with stays equal.
+template <class Key>
+struct StepGraph {
+    cudaGraphExec_t exec = nullptr;
+    Key key{};
+    int64_t launches = 0;    // kernel launches the capture recorded (added to WdModel::launches on every replay)
+    int eager = 0;           // eager runs so far
+    void destroy() {
+        if (exec) cudaGraphExecDestroy(exec);
+        exec = nullptr;
+    }
+};
+// key of a slot's step graphs: the batch view (a slot re-uploaded with the same B, labels and weights keeps its graphs)
+inline bool operator==(const DevBatch& a, const DevBatch& b) {
+    return a.B == b.B && a.cat_offsets == b.cat_offsets && a.cat_keys == b.cat_keys && a.dense == b.dense && a.label == b.label && a.weight == b.weight;
+}
+struct MergeKey {            // key of a list's merge graph (wd_sparse_set_sorted)
+    const void* rows;
+    const void* grads;
+    int n_lists;
+    int64_t list_len;
+    bool on_side;
+    bool operator==(const MergeKey& o) const {
+        return rows == o.rows && grads == o.grads && n_lists == o.n_lists && list_len == o.list_len && on_side == o.on_side;
+    }
+};
+
 struct BatchSlot {           // one device-resident batch (ring used by benchmarks / prefetch)
     int32_t* off = nullptr;
     uint64_t* keys = nullptr;
@@ -165,17 +192,11 @@ struct BatchSlot {           // one device-resident batch (ring used by benchmar
     cudaEvent_t ev_up = nullptr;             // recorded on the upload stream after the slot's copies
     cudaEvent_t ev_used = nullptr;           // recorded on the model stream after the last step that read the slot
     bool up_pending = false, used_recorded = false;
-    // CUDA graph of one whole train step on this slot (captured after a few eager steps; keyed by the batch view)
-    cudaGraphExec_t graph = nullptr;
-    DevBatch graph_view{};
-    int64_t graph_launches = 0;
-    int eager_steps = 0;
-    // CUDA graph of forward + backward only (data-parallel steps: wd_step_backward_slot), side streams joined at its end
-    cudaGraphExec_t graph_bwd = nullptr;
-    DevBatch graph_bwd_view{};
-    int64_t graph_bwd_launches = 0;
-    int bwd_eager_steps = 0;
-    bool bwd_side_active[2] = {false, false};
+    // step graphs on this slot, one per entry point
+    StepGraph<DevBatch> train;               // whole train step (wd_train_step_slot)
+    StepGraph<DevBatch> bwd;                 // forward + backward of the split step (wd_step_backward_slot), side streams joined at its end
+    StepGraph<DevBatch> shard;               // whole rank-step of a row-sharded model (wd_shard_train_step_slot)
+    bool bwd_side_active[2] = {false, false};   // side_active as the captured backward left it
 };
 
 
@@ -239,10 +260,6 @@ struct ShardState {
     cudaEvent_t ev_a = nullptr;         // after barrier A on the main stream (owner-side grouping may start)
     cudaStream_t aux = nullptr;         // the wide space's routing / serving and the local gathers, beside the embedding space's chain
     cudaEvent_t ev_ids2 = nullptr, ev_routed1 = nullptr, ev_a2 = nullptr, ev_aux_done = nullptr;
-    cudaGraphExec_t graph[64] = {};     // whole sharded step per batch slot
-    DevBatch graph_view[64];
-    int64_t graph_launches[64] = {};
-    int eager_steps[64] = {};
 };
 constexpr int kBarriers = 8;
 
@@ -281,9 +298,7 @@ struct WdModel {
     bool side_pending[2] = {false, false};   // the list's grouping of this step was issued on its side stream
     bool side_active[2] = {false, false};    // the list's sums live on its side stream (merge / apply follow there)
     bool record_dx0 = false, dx0_recorded = false;
-    // CUDA graph of the data-parallel merge of list w (wd_sparse_set with the same buffers every step: fixed-size exchange)
-    struct MergeGraph { cudaGraphExec_t exec = nullptr; const void* rows = nullptr; const void* grads = nullptr; int64_t n = 0; int n_lists = 0;
-                        bool on_side = false; int eager = 0; int64_t launches = 0; } merge_graph[2];
+    wd::StepGraph<wd::MergeKey> merge_graph[2];   // data-parallel merge of list w (fixed-size exchange: wd_sparse_set_sorted)
     // ---- dense exchange of small tables (WdPlanDesc::dense_exchange_max_rows)
     int64_t dense_exchange_max_rows = 0;
     int64_t small_base[2] = {0, 0};          // first global row of the small embedding tables / small wide columns
