@@ -274,6 +274,8 @@ int wd_shard_forward_slot(WdModel *m, int slot, float *logits_out, float *loss_o
 int wd_eval_reset(WdModel *m);
 int wd_eval_accumulate(WdModel *m, const WdBatch *batch);
 int wd_eval_finish(WdModel *m, double *out10);
+/* wd_eval_accumulate on the batch a slot already holds (wd_batch_prefetch_slot, wd_tsv_parse_slot). */
+int wd_eval_accumulate_slot(WdModel *m, int slot);
 
 /* Stand-alone integer kernels (device), exposed so parity tests can check them bit-exactly:
  * Fingerprint64 over byte strings; hash-bucket; SparseCross chain. */
@@ -284,6 +286,11 @@ uint64_t wd_fingerprint_cat64(uint64_t a, uint64_t b);
 
 /* Column ids of the last uploaded/stepped batch, for parity tests: CSR over (row, column). */
 int wd_debug_column_ids(WdModel *m, int32_t *offsets_out, int64_t offsets_cap, int64_t *ids_out, int64_t ids_cap, int64_t *nnz_out);
+/* The batch slot `slot` holds, read back after its pending refill: *batch_out rows, *nnz_out keys, *parts_out bit 0 / 1 / 2 =
+ * offsets / label / weight present.  Non-NULL arrays receive offsets[B * n_cat_fields + 1], keys[nnz], dense[B * n_dense_fields],
+ * label[B], weight[B] (call with NULL arrays first for the sizes). */
+int wd_debug_slot(WdModel *m, int slot, int32_t *batch_out, int64_t *nnz_out, int32_t *parts_out, int32_t *offsets_out,
+                  uint64_t *keys_out, float *dense_out, float *label_out, float *weight_out);
 /* Deep input matrix of the last forward: [batch, d0_phys]. */
 int wd_debug_deep_input(WdModel *m, float *out, int64_t cap);
 /* Output of hidden layer `layer` of tower `tower` after the last forward: [batch, N_phys]; returns N_phys.  On the bf16x3 engine a
@@ -342,6 +349,22 @@ int64_t wd_tsv_index_lines(const char *text, int64_t text_len, int64_t *starts_o
 int64_t wd_tsv_parse_lines(const WdTsvSpec *spec, const char *text, const int64_t *starts, const int32_t *lens, const int64_t *idx,
                            int32_t n_lines, int32_t *offsets_out, uint64_t *keys_out, int64_t keys_cap,
                            float *dense_out, float *label_out, float *weight_out, int32_t n_threads);
+
+/* The lines idx[0 .. n) of a file image (starts / lens from wd_tsv_index_lines; idx NULL: lines 0 .. n) copied into `out`, each
+ * followed by '\n', on the loader's worker threads; out_starts[i] = offset of line i, out_starts[n] = total bytes.  Returns the
+ * total; when it exceeds out_cap (or out is NULL) only out_starts is written.  Needs no GPU. */
+int64_t wd_tsv_gather_lines(const char *text, const int64_t *starts, const int32_t *lens, const int64_t *idx, int32_t n,
+                            char *out, int64_t out_cap, int64_t *out_starts, int32_t n_threads);
+/* Device TSV parser: the n_lines lines of `text` (line i = text[starts[i], starts[i + 1] - 1), a trailing '\r' excluded; the
+ * layout wd_tsv_gather_lines writes) are copied to the GPU and parsed there straight into batch slot `slot`, on the upload stream
+ * behind the last step that read the slot (as wd_batch_prefetch_slot).  The slot then holds exactly what wd_tsv_parse_lines +
+ * wd_batch_prefetch_slot would put there (label only with spec->has_label, weight only with use_weight and has_label).  Returns
+ * when this parse has finished; `text` and `starts` may then be reused.  Records outside the exact int / float fast paths, a
+ * wrong field count or more keys than the slot holds are parsed on the host instead, so errors carry the host parser's messages. */
+int wd_tsv_parse_slot(WdModel *m, int slot, const WdTsvSpec *spec, const char *text, int64_t text_len, const int64_t *starts,
+                      int32_t n_lines);
+/* out[0] batches wd_tsv_parse_slot parsed on the device, out[1] batches it handed to the host parser (first min(n, 2)). */
+int wd_tsv_parse_stats(WdModel *m, int64_t *out, int32_t n, int32_t reset);
 
 /* Page-locked host buffers for the input pipeline (the `dataset.prefetch` buffers of the reference's input_fn, python/lib/
  * dataset.py:181-184): parse into these, hand them to wd_batch_prefetch_slot.  WD_ENODEVICE without a CUDA device. */

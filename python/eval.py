@@ -34,7 +34,8 @@ def main():
         raise ValueError("No model checkpoint found, please check the model dir.")
     print("INFO: " + "=" * 30 + " START TESTING" + "=" * 30)
     s_time = time.time()
-    results = model.evaluate(input_fn=lambda: input_fn(FLAGS.test_data, None, "eval", FLAGS.batch_size, config=CONF, plan=model.plan),
+    results = model.evaluate(input_fn=lambda: input_fn(FLAGS.test_data, None, "eval", FLAGS.batch_size, config=CONF, plan=model.plan,
+                                                       device_parse=True),
                              checkpoint_path=FLAGS.checkpoint_path)
     print("INFO: " + "=" * 30 + "FINISH TESTING, TAKE {} mins".format(round((time.time() - s_time) / 60, 2)) + "=" * 30)
     print("-" * 80)

@@ -44,7 +44,7 @@ def elapse_time(t0):
 
 
 def _fn(model, path, mode):
-    return lambda: input_fn(path, None, mode, FLAGS.batch_size, config=CONF, plan=model.plan, pinned=(mode == "train"))
+    return lambda: input_fn(path, None, mode, FLAGS.batch_size, config=CONF, plan=model.plan, device_parse=True)
 
 
 def _show(results):
@@ -165,7 +165,7 @@ def main_distributed(rank, world, local):
         for f in list_files(FLAGS.train_data):
             t0 = time.time()
             log("INFO: <EPOCH {}>: Start training {}".format(n + 1, f))
-            model.train(input_fn=lambda f=f: input_fn(f, None, "train", FLAGS.batch_size, config=CONF, plan=model.plan, rank=rank, world=world, pinned=True))
+            model.train(input_fn=lambda f=f: input_fn(f, None, "train", FLAGS.batch_size, config=CONF, plan=model.plan, rank=rank, world=world, device_parse=True))
             log("INFO: <EPOCH {}>: Finish training {}, take {} mins".format(n + 1, f, elapse_time(t0)))
     dist.barrier()
     dist.destroy_process_group()

@@ -73,10 +73,13 @@ SYMBOLS = {
     "wd_eval_reset": (ctypes.c_int, [_vp]),
     "wd_eval_accumulate": (ctypes.c_int, [_vp, _vp]),
     "wd_eval_finish": (ctypes.c_int, [_vp, _vp]),
+    "wd_eval_accumulate_slot": (ctypes.c_int, [_vp, ctypes.c_int]),
     "wd_fingerprint64_device": (ctypes.c_int, [_vp, _vp, _i64, _vp]),
     "wd_fingerprint64": (_u64, [ctypes.c_char_p, ctypes.c_size_t]),
     "wd_fingerprint_cat64": (_u64, [_u64, _u64]),
     "wd_debug_column_ids": (ctypes.c_int, [_vp, _vp, _i64, _vp, _i64, ctypes.POINTER(_i64)]),
+    "wd_debug_slot": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.POINTER(_i32), ctypes.POINTER(_i64), ctypes.POINTER(_i32), _vp, _vp, _vp,
+                                     _vp, _vp]),
     "wd_debug_deep_input": (ctypes.c_int, [_vp, _vp, _i64]),
     "wd_debug_hidden": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, _vp, _i64]),
     "wd_launch_count": (_i64, [_vp]),
@@ -97,6 +100,9 @@ SYMBOLS = {
     "wd_tsv_parse": (_i64, [_vp, ctypes.c_char_p, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _i32]),
     "wd_tsv_index_lines": (_i64, [_vp, _i64, _vp, _vp, _i64]),
     "wd_tsv_parse_lines": (_i64, [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _i32]),
+    "wd_tsv_gather_lines": (_i64, [_vp, _vp, _vp, _vp, _i32, _vp, _i64, _vp, _i32]),
+    "wd_tsv_parse_slot": (ctypes.c_int, [_vp, ctypes.c_int, _vp, _vp, _i64, _vp, _i32]),
+    "wd_tsv_parse_stats": (ctypes.c_int, [_vp, ctypes.POINTER(_i64), _i32, _i32]),
 }
 
 

@@ -117,6 +117,7 @@ extern "C" int wd_model_destroy(WdModel* m) {
         if (sl.ev_used) cudaEventDestroy(sl.ev_used);
     }
     if (m->stream_up) { cudaStreamSynchronize(m->stream_up); cudaStreamDestroy(m->stream_up); }
+    tsv_dev_destroy(m);
     for (auto& g : m->merge_graph) g.destroy();
     if (m->ev_bwd_done) cudaEventDestroy(m->ev_bwd_done);
     for (void* p : m->allocs) cudaFree(p);
@@ -892,6 +893,51 @@ extern "C" int wd_batch_prefetch_slot(WdModel* m, int slot, const WdBatch* b) {
     return WD_OK;
 }
 
+// TSV text -> batch slot on the device (tsv.cu), ordered like wd_batch_prefetch_slot: behind the last step that read the slot, on
+// the upload stream.  Waits for this parse only; a batch the device parser declines is parsed on the host and uploaded instead.
+extern "C" int wd_tsv_parse_slot(WdModel* m, int slot, const WdTsvSpec* sp, const char* text, int64_t text_len, const int64_t* starts,
+                                 int32_t n_lines) {
+    int rc = check_ready(m);
+    if (rc) return rc;
+    if (!sp || !text || !starts || n_lines < 0 || text_len < 0) { set_error("wd_tsv_parse_slot: bad arguments"); return WD_EINVAL; }
+    if ((rc = ensure_slot(m, slot))) return rc;
+    BatchSlot& sl = m->slots[slot];
+    if (!sl.ev_up) WD_CUDA(cudaEventCreateWithFlags(&sl.ev_up, cudaEventDisableTiming));
+    if (sl.used_recorded) WD_CUDA(cudaStreamWaitEvent(m->stream_up, sl.ev_used, 0));
+    int status = 0;
+    if ((rc = tsv_parse_device(m, sp, text, text_len, starts, n_lines, sl.off, sl.keys, sl.dense, sl.label, sl.weight, m->stream_up, &status))) return rc;
+    DevBatch view{};
+    bool has_label = false;
+    if (status == 0) {
+        view.B = n_lines;
+        view.cat_offsets = m->n_cat_fields > 0 ? sl.off : nullptr;
+        view.cat_keys = sl.keys;
+        view.dense = sl.dense;
+        view.label = sp->has_label ? sl.label : nullptr;
+        view.weight = (sp->use_weight && sp->has_label) ? sl.weight : nullptr;
+        has_label = sp->has_label != 0;
+        m->tsv_device_batches++;
+    } else {
+        WdBatch hb{};
+        if ((rc = tsv_parse_host(sp, text, starts, n_lines, &hb))) return rc;
+        if ((rc = upload_into(m, sl, &hb, m->stream_up, &view, &has_label))) return rc;
+        m->tsv_host_batches++;
+    }
+    WD_CUDA(cudaEventRecord(sl.ev_up, m->stream_up));
+    if (status != 0) WD_CUDA(cudaEventSynchronize(sl.ev_up));      // the host batch lives in per-thread buffers
+    sl.view = view; sl.has_label = has_label; sl.filled = true; sl.up_pending = true;
+    if (slot == m->cur_slot) { m->dbatch = view; m->batch_has_label = has_label; }
+    return WD_OK;
+}
+
+extern "C" int wd_tsv_parse_stats(WdModel* m, int64_t* out, int32_t n, int32_t reset) {
+    if (!m) { set_error("null model"); return WD_EINVAL; }
+    const int64_t v[2] = {m->tsv_device_batches, m->tsv_host_batches};
+    for (int i = 0; i < n && i < 2; ++i) out[i] = v[i];
+    if (reset) m->tsv_device_batches = m->tsv_host_batches = 0;
+    return WD_OK;
+}
+
 extern "C" int wd_batch_upload_slot(WdModel* m, int slot, const WdBatch* b) {
     int rc = check_ready(m);
     if (rc) return rc;
@@ -1434,6 +1480,17 @@ extern "C" int wd_eval_accumulate(WdModel* m, const WdBatch* b) {
     if ((rc = metrics_accumulate(m))) return rc;
     return finish_step(m, nullptr, nullptr);
 }
+extern "C" int wd_eval_accumulate_slot(WdModel* m, int slot) {
+    int rc = check_ready(m);
+    if (rc) return rc;
+    if ((rc = select_slot(m, slot))) return rc;
+    if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
+    if (!m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
+    if ((rc = forward_core(m, false))) return rc;
+    if ((rc = metrics_accumulate(m))) return rc;
+    if ((rc = mark_slot_used(m))) return rc;
+    return finish_step(m, nullptr, nullptr);
+}
 extern "C" int wd_eval_finish(WdModel* m, double* out10) {
     int rc = check_ready(m);
     if (rc) return rc;
@@ -1459,6 +1516,31 @@ extern "C" int wd_debug_column_ids(WdModel* m, int32_t* offsets_out, int64_t off
         WD_CUDA(cudaMemcpy(tmp.data(), m->d_e_id, (int64_t)nnz * 4, cudaMemcpyDeviceToHost));
         for (int i = 0; i < nnz; ++i) ids_out[i] = tmp[i];
     }
+    return WD_OK;
+}
+// The batch a slot holds, read back (after its pending upload or parse): *batch_out rows, *nnz_out keys, *parts_out bit 0 offsets,
+// bit 1 label, bit 2 weight present.  Arrays that are not NULL receive offsets [B * F + 1], keys [nnz], dense [B * Nd], label [B],
+// weight [B]; pass NULLs first to learn the sizes.
+extern "C" int wd_debug_slot(WdModel* m, int slot, int32_t* batch_out, int64_t* nnz_out, int32_t* parts_out, int32_t* offsets_out,
+                             uint64_t* keys_out, float* dense_out, float* label_out, float* weight_out) {
+    int rc = check_ready(m);
+    if (rc) return rc;
+    if (slot < 0 || slot >= (int)m->slots.size() || !m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
+    WD_CUDA(cudaStreamSynchronize(m->stream_up));
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    const BatchSlot& sl = m->slots[slot];
+    const DevBatch& v = sl.view;
+    const int64_t B = v.B, F = m->n_cat_fields, Nd = m->n_dense_fields;
+    int32_t nnz32 = (int32_t)(B * F);
+    if (v.cat_offsets) WD_CUDA(cudaMemcpy(&nnz32, v.cat_offsets + B * F, 4, cudaMemcpyDeviceToHost));
+    if (batch_out) *batch_out = (int32_t)B;
+    if (nnz_out) *nnz_out = nnz32;
+    if (parts_out) *parts_out = (v.cat_offsets ? 1 : 0) | (v.label ? 2 : 0) | (v.weight ? 4 : 0);
+    if (offsets_out && v.cat_offsets) WD_CUDA(cudaMemcpy(offsets_out, v.cat_offsets, (B * F + 1) * 4, cudaMemcpyDeviceToHost));
+    if (keys_out && nnz32 > 0) WD_CUDA(cudaMemcpy(keys_out, v.cat_keys, (int64_t)nnz32 * 8, cudaMemcpyDeviceToHost));
+    if (dense_out && Nd > 0) WD_CUDA(cudaMemcpy(dense_out, v.dense, B * Nd * 4, cudaMemcpyDeviceToHost));
+    if (label_out && v.label) WD_CUDA(cudaMemcpy(label_out, v.label, B * 4, cudaMemcpyDeviceToHost));
+    if (weight_out && v.weight) WD_CUDA(cudaMemcpy(weight_out, v.weight, B * 4, cudaMemcpyDeviceToHost));
     return WD_OK;
 }
 extern "C" int wd_debug_deep_input(WdModel* m, float* out, int64_t cap) {

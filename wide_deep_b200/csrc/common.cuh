@@ -263,6 +263,8 @@ struct ShardState {
 };
 constexpr int kBarriers = 8;
 
+struct TsvDev;                                 // device TSV parser: spec copy and scratch (tsv.cu)
+
 }  // namespace wd
 
 struct WdModel {
@@ -449,6 +451,8 @@ struct WdModel {
     int cur_layer = 0;                       // layer being launched (names the profiling marks)
     wd::PhaseTimer timer;
     std::vector<wd::BatchSlot> slots;        // slot 0 aliases the d_cat_* buffers above
+    wd::TsvDev* tsv = nullptr;               // device TSV parser (wd_tsv_parse_slot), created on first use
+    int64_t tsv_device_batches = 0, tsv_host_batches = 0;   // batches wd_tsv_parse_slot parsed on the device / on the host
     bool initialized = false;
     bool grads_pending = false;
 };
@@ -486,6 +490,12 @@ int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32
                        float* const* data, const int32_t* stride, const int32_t* stage_of, float* stage, int S);
 int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d);  // shard.cu: HBM shard_build allocates (held back by auto placement)
 int64_t hbm_reserve_bytes(const WdModel* m);                     // api.cu: HBM the model keeps free for its later allocations
+// tsv.cu: device parse of n lines into the batch buffers on stream st, waiting for it; *status != 0: the buffers do not hold the
+// batch (parse it on the host)
+int tsv_parse_device(WdModel* m, const WdTsvSpec* sp, const char* text, int64_t text_len, const int64_t* starts, int n, int32_t* off,
+                     uint64_t* keys, float* dense, float* label, float* weight, cudaStream_t st, int* status);
+int tsv_parse_host(const WdTsvSpec* sp, const char* text, const int64_t* starts, int n, WdBatch* out);   // tsv.cu
+void tsv_dev_destroy(WdModel* m);                                // tsv.cu
 int metrics_accumulate(WdModel* m);                              // metrics.cu
 int metrics_finish(WdModel* m, double* out10);
 

@@ -34,6 +34,17 @@ def list_files(path):
     return [path]
 
 
+def _host_buffer(lib, pinned, nbytes, raw):
+    """uint8 array of at least ``nbytes``: page-locked (its pointer appended to ``raw``, for wd_host_free) or, without a CUDA
+    device, ordinary memory."""
+    if not pinned:
+        return np.zeros(max(nbytes, 8), dtype=np.uint8)
+    p = ctypes.c_void_p()
+    _native.check(lib.wd_host_alloc(max(nbytes, 8), ctypes.byref(p)))
+    raw.append(p)
+    return np.ctypeslib.as_array((ctypes.c_uint8 * max(nbytes, 8)).from_address(p.value))
+
+
 class PinnedRing(object):
     """A ring of page-locked host buffer sets (one set = the arrays of one batch), allocated ONCE through the library
     (cudaHostAlloc).  The parser writes straight into a set and ``wd_batch_prefetch_slot`` copies from it asynchronously — the
@@ -49,12 +60,7 @@ class PinnedRing(object):
         self.sets = [self._make_set() for _ in range(depth)]
 
     def _buf(self, nbytes):
-        if not self.pinned:
-            return np.zeros(max(nbytes, 8), dtype=np.uint8)
-        p = ctypes.c_void_p()
-        _native.check(self._lib.wd_host_alloc(max(nbytes, 8), ctypes.byref(p)))
-        self._raw.append(p)
-        return np.ctypeslib.as_array((ctypes.c_uint8 * max(nbytes, 8)).from_address(p.value))
+        return _host_buffer(self._lib, self.pinned, nbytes, self._raw)
 
     def _make_set(self):
         n, F, Nd = self.n_rows, self.F, self.Nd
@@ -71,6 +77,56 @@ class PinnedRing(object):
     def next(self):
         s = self.sets[self._i % self.depth]
         self._i += 1
+        return s
+
+    def close(self):
+        for p in self._raw:
+            self._lib.wd_host_free(p)
+        self._raw, self.sets = [], []
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TsvTextBatch(object):
+    """The text of one batch for the device parser (``WideDeepModel.parse_slot``): ``n`` lines in ``text`` (uint8, page-locked when a
+    CUDA device is present), line i = ``text[starts[i]:starts[i + 1] - 1]``, and the parse spec of the reader that picked them.
+    ``text`` and ``starts`` alias a ring set and stay valid for the next ``depth - 1`` batches of that ring."""
+
+    def __init__(self, reader, text, starts, n):
+        self.reader, self.text, self.starts, self.n = reader, text, starts, int(n)
+
+    @property
+    def batch_size(self):
+        return self.n
+
+    @property
+    def has_label(self):
+        return not self.reader.is_pred
+
+
+class TextRing(object):
+    """A ring of ``depth`` page-locked text buffers (plus line starts) for ``TsvTextBatch``: gathered lines land here so the device
+    parser's host->device copy reads pinned memory.  A buffer that is too small for a batch is replaced by a larger one (the old
+    one stays allocated until ``close``: a batch still in flight may alias it).  Without a CUDA device: numpy arrays."""
+
+    def __init__(self, n_rows, text_cap, depth=6):
+        self._lib = _native.lib()
+        self.depth, self._i, self._raw = depth, 0, []
+        self.pinned = self._lib.wd_device_count() > 0
+        self.sets = [dict(text=self._buf(text_cap), starts=self._buf((n_rows + 1) * 8).view(np.int64)) for _ in range(depth)]
+
+    def _buf(self, nbytes):
+        return _host_buffer(self._lib, self.pinned, nbytes, self._raw)
+
+    def next(self, text_bytes):
+        s = self.sets[self._i % self.depth]
+        self._i += 1
+        if s["text"].size < text_bytes:
+            s["text"] = self._buf(text_bytes + text_bytes // 4)
         return s
 
     def close(self):
@@ -183,7 +239,8 @@ def _parse_into_ring(self, text, n, ring, index=None):
     if nnz < 0:
         raise ValueError(self._lib.wd_last_error().decode())
     b = Batch.__new__(Batch)                                         # views of the pinned set: no copies (Batch() would copy)
-    b.batch_size = n
+    b._ring = ring                                                   # the ring outlives every batch it holds (a prefetch queue may
+    b.batch_size = n                                                 # still hold batches when the generator that owns it is done)
     b.keys, b.offsets = s["keys"][:nnz], s["offsets"][:n * F + 1]
     b.dense = s["dense"][:n * Nd].reshape(n, Nd) if Nd else None
     b.label = None if self.is_pred else s["label"][:n]
@@ -218,7 +275,24 @@ def _parse_indexed(self, text, starts, lens, idx, ring=None):
                  weight if (self.use_weight and not self.is_pred) else None)
 
 
+def _gather_text(self, text, starts, lens, idx, ring):
+    """TsvTextBatch of the lines ``idx`` of the file image ``text``: one copy of the lines into the ring's next buffer."""
+    n = len(idx)
+    idx = np.ascontiguousarray(idx, dtype=np.int64)
+    nbytes = int(lens[idx].sum()) + n
+    s = ring.next(nbytes)
+    out_starts = s["starts"][:n + 1]
+    got = self._lib.wd_tsv_gather_lines(text, starts.ctypes.data, lens.ctypes.data, idx.ctypes.data, n, s["text"].ctypes.data,
+                                        s["text"].size, out_starts.ctypes.data, self.n_threads)
+    if got < 0 or got != nbytes:
+        raise ValueError(self._lib.wd_last_error().decode() if got < 0 else "wd_tsv_gather_lines: %d bytes, %d expected" % (got, nbytes))
+    tb = TsvTextBatch(self, s["text"], out_starts, n)
+    tb._ring = ring                                                  # (as in _parse_into_ring: the buffers live while the batch does)
+    return tb
+
+
 TsvReader._parse_into_ring = _parse_into_ring
+TsvReader.gather_text = _gather_text
 TsvReader.parse_indexed = _parse_indexed
 
 
@@ -256,12 +330,15 @@ class Prefetcher(object):
         return item
 
 
-def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=None, rank=0, world=1, seed=123, pinned=False):
+def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=None, rank=0, world=1, seed=123, pinned=False,
+             device_parse=False):
     """Iterator of ``Batch`` for one pass over the data (one epoch), mirroring the reference's
     ``input_fn(csv_data_file, img_data_file, mode, batch_size)`` (dataset.py:293-310).  ``img_data_file`` is
     accepted for signature compatibility and must be None (the CNN branch is out of scope).
     The files are read and the pinned ring is allocated HERE (on the caller's thread, whose CUDA device is the model's); only
-    the per-batch parsing is lazy, so the returned iterator may be drained from a prefetch thread."""
+    the per-batch parsing is lazy, so the returned iterator may be drained from a prefetch thread.
+    ``device_parse=True``: the same lines, in the same batches, are yielded as ``TsvTextBatch`` (the batch's text gathered into a
+    ring of page-locked buffers) for ``WideDeepModel.parse_slot``, which parses them on the GPU; ``pinned`` is then irrelevant."""
     assert mode in ("train", "eval", "pred"), "mode must in `train`, `eval`, or `pred`, found {}".format(mode)
     if img_data_file:
         raise ValueError("image inputs are not supported by this library (cnn_use_flag: 0)")
@@ -290,6 +367,15 @@ def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=N
         perm = np.random.Generator(np.random.Philox(seed)).permutation(len(order))
         order = order[perm]
     order = np.ascontiguousarray(order)
+    if device_parse:
+        mean_len = float(lens[:n_all].mean()) if n_all else 0.0
+        tring = TextRing(batch_size, int(batch_size * (mean_len + 1) * 1.25) + 4096)
+
+        def texts():
+            for i in range(0, len(order), batch_size):
+                yield reader.gather_text(text, starts, lens, order[i:i + batch_size], tring)
+
+        return texts()
     # pinned=True (estimator.train, which consumes batch by batch): parse into a ring of page-locked buffers so the host->device
     # refill of a batch slot is truly asynchronous; a yielded Batch stays valid for the next `depth - 1` batches
     ring = None

@@ -152,13 +152,14 @@ class WideAndDeepClassifier(object):
             ck_secs = 600
         last_save = time.time()
         # one batch of look-ahead, as the reference's input_fn prefetches (python/lib/dataset.py:181-184): while step i runs on the
-        # GPU, batch i+1 is parsed and its host->device copy issued (wd_batch_prefetch_slot, two alternating slots)
+        # GPU, batch i+1 is parsed and its host->device copy issued (wd_batch_prefetch_slot, two alternating slots); a TsvTextBatch
+        # (input_fn(device_parse=True)) is parsed on the GPU into the slot instead (wd_tsv_parse_slot, beside step i)
         from .dataset import Prefetcher
         it = Prefetcher(input_fn(), depth=2)             # batches are parsed on a background thread, two ahead of the step
         cur = next(it, None)
         slot = 0
         if cur is not None:
-            m.prefetch_slot(slot, cur)
+            m.feed_slot(slot, cur)
         while cur is not None:
             if self._trainer is not None:
                 self._trainer.step_slot(slot, want_loss=False)   # collective: every rank steps on its shard of the batch
@@ -166,7 +167,7 @@ class WideAndDeepClassifier(object):
                 m.train_step_slot(slot, want_loss=False)     # enqueue step i ...
             nxt = next(it, None)                             # ... parse batch i+1 on the host while it runs ...
             if nxt is not None:
-                m.prefetch_slot(1 - slot, nxt)               # ... start its copy on the upload stream ...
+                m.feed_slot(1 - slot, nxt)                   # ... start its copy (or parse) on the upload stream ...
             loss = m.last_loss()                             # ... and only then wait for step i's loss
             n += 1
             if n % log_every == 0:
@@ -201,11 +202,17 @@ class WideAndDeepClassifier(object):
         m = self._ensure_model(checkpoint_path, need_trained=True)
         m.eval_reset()
         n = 0
+        from .dataset import TsvTextBatch
         for batch in input_fn():
-            if batch.label is None:
+            text = isinstance(batch, TsvTextBatch)          # parsed on the GPU into slot 0, where eval_accumulate uploads
+            if not (batch.has_label if text else batch.label is not None):
                 raise ValueError("evaluate needs labelled data (the reference's `pred`-mode test call, train.py:96-101, "
                                  "fails the same way inside TensorFlow)")
-            m.eval_accumulate(batch)
+            if text:
+                m.parse_slot(0, batch)
+                m.eval_accumulate_slot(0)
+            else:
+                m.eval_accumulate(batch)
             n += 1
             if steps and n >= steps:
                 break

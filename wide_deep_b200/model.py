@@ -210,6 +210,10 @@ class WideDeepModel(object):
         c = batch.to_c()
         check(self._lib.wd_eval_accumulate(self._h, ctypes.byref(c)))
 
+    def eval_accumulate_slot(self, slot):
+        """Metrics of the batch a slot already holds (``prefetch_slot`` / ``parse_slot``)."""
+        check(self._lib.wd_eval_accumulate_slot(self._h, int(slot)))
+
     def eval_finish(self):
         out = np.zeros(10, dtype=np.float64)
         check(self._lib.wd_eval_finish(self._h, out.ctypes.data))
@@ -275,6 +279,43 @@ class WideDeepModel(object):
             self._prefetched = {}
         self._prefetched[int(slot)] = (batch, c)
         self._rows_hint = batch.batch_size
+
+    def parse_slot(self, slot, tb):
+        """Parse a ``TsvTextBatch`` on the GPU straight into a batch slot (wd_tsv_parse_slot): the slot then holds what
+        ``prefetch_slot`` of the host-parsed batch would.  Returns when the parse is done; ``tb``'s buffers may then be reused."""
+        r = tb.reader
+        check(self._lib.wd_tsv_parse_slot(self._h, int(slot), ctypes.byref(r._spec), tb.text.ctypes.data, int(tb.starts[tb.n]),
+                                          tb.starts.ctypes.data, tb.n))
+        self._rows_hint = tb.n
+
+    def feed_slot(self, slot, item):
+        """Fill a batch slot from an input_fn item: ``parse_slot`` for a ``TsvTextBatch``, ``prefetch_slot`` for a ``Batch``."""
+        from .dataset import TsvTextBatch
+        if isinstance(item, TsvTextBatch):
+            self.parse_slot(slot, item)
+        else:
+            self.prefetch_slot(slot, item)
+
+    def tsv_parse_stats(self, reset=False):
+        """dict(device = batches parse_slot parsed on the GPU, host = batches it handed to the host parser)."""
+        out = (ctypes.c_int64 * 2)()
+        check(self._lib.wd_tsv_parse_stats(self._h, out, 2, 1 if reset else 0))
+        return dict(device=int(out[0]), host=int(out[1]))
+
+    def slot_batch(self, slot):
+        """The batch a slot holds, read back from the device (wd_debug_slot), as a ``Batch``."""
+        B, nnz, parts = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int32()
+        check(self._lib.wd_debug_slot(self._h, int(slot), ctypes.byref(B), ctypes.byref(nnz), ctypes.byref(parts), None, None, None, None, None))
+        n, F, Nd = B.value, len(self.plan.cat_fields), len(self.plan.dense_fields)
+        offs = np.zeros(n * F + 1, dtype=np.int32)
+        keys = np.zeros(max(nnz.value, 1), dtype=np.uint64)
+        dense = np.zeros(max(n * Nd, 1), dtype=np.float32)
+        label, weight = np.zeros(n, dtype=np.float32), np.zeros(n, dtype=np.float32)
+        check(self._lib.wd_debug_slot(self._h, int(slot), ctypes.byref(B), ctypes.byref(nnz), ctypes.byref(parts), offs.ctypes.data,
+                                      keys.ctypes.data, dense.ctypes.data, label.ctypes.data, weight.ctypes.data))
+        p = parts.value
+        return Batch(n, keys[:nnz.value], offs if p & 1 else None, dense[:n * Nd].reshape(n, Nd) if Nd else None,
+                     label if p & 2 else None, weight if p & 4 else None)
 
     def last_loss(self):
         loss = ctypes.c_float()
