@@ -18,10 +18,18 @@ LISTS = (0, 1)          # embedding rows, wide rows (a wide_deep model has both)
 
 
 def _split_steps(plan, om, batches, exchange):
-    import torch
-    from wide_deep_b200.parallel import wrap_device
     pm = WideDeepModel(plan)
     copy_params_to_product(om, pm)
+    losses = split_train(pm, batches, exchange)
+    out = losses, {name: pm.get_tensor(name) for name in pm.tensor_names()}, pm.launch_count()
+    pm.close()
+    return out
+
+
+def split_train(pm, batches, exchange):
+    """The split step over two alternating slots with a world-1 exchange ("sorted" or "counted"); returns the losses."""
+    import torch
+    from wide_deep_b200.parallel import wrap_device
     dev = torch.device("cuda", pm.device)
     # the exchange's destination buffers are allocated once, so the sorted merge sees the same key every step; the merge cannot
     # read the library's own list in place (it writes the summed gradients there)
@@ -48,9 +56,7 @@ def _split_steps(plan, om, batches, exchange):
         pm.step_apply()
         losses.append(pm.last_loss())
     pm.sync()
-    out = losses, {name: pm.get_tensor(name) for name in pm.tensor_names()}, pm.launch_count()
-    pm.close()
-    return out
+    return losses
 
 
 @pytest.mark.parametrize("engine", ["ffma", "bf16x3"])

@@ -990,16 +990,6 @@ static int finish_step(WdModel* m, float* loss_out, float* logits_out) {
 
 static bool list_present(const WdModel* m, int which) { return which == 0 ? (m->use_deep && !m->tables.empty()) : m->use_wide; }
 
-// run `fn` on the side stream of sparse list `which` with that stream's scratch set
-template <typename F>
-static int on_side(WdModel* m, int which, F fn) {
-    cudaStream_t main_stream = m->stream;
-    m->stream = m->sstream[which]; m->scratch_sel = 1 + which;
-    int rc = fn();
-    m->stream = main_stream; m->scratch_sel = 0;
-    return rc;
-}
-
 // launch the id-only grouping of both sparse lists on their side streams (overlaps forward + backward of the towers)
 // WD_STEP_TRACE=1: stamp i of the step timeline on whatever stream is current (captured into the step's graph like any kernel)
 __global__ void step_stamp_kernel(unsigned long long* t) { unsigned long long v; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(v)); *t = v; }

@@ -324,14 +324,13 @@ struct WdModel {
     float* d_stage = nullptr;                // [max_nnz][stage_stride] records of the step's unique host rows, row u at u * stage_stride
     int stage_stride = 0;                    // largest stride of the host tables
     uint32_t* d_g_emb = nullptr;             // [max_nnz] ids the gather reads: e_emb, host-table entries replaced by their unique index u
-    // what the gather kernels and the fused row updates address: the tables' own arrays, or for host tables the staging buffer
-    // (data = d_stage, row base 0, stride stage_stride); all alias the arrays above when no table is on the host
-    float** d_gtab_data = nullptr;           // [n_tables] data (gather, RowApply)
+    // what the gather kernels address: the tables' own arrays, or for host tables the staging buffer (data = d_stage, row base 0,
+    // stride stage_stride); all alias the arrays above when no table is on the host
+    float** d_gtab_data = nullptr;           // [n_tables] data (gather)
     int32_t* d_gtab_stride = nullptr;        // [n_tables] stride (gather)
     int64_t* d_gtab_row_base = nullptr;      // [n_tables] row base (gather)
-    int32_t* d_tab_stage = nullptr;          // [n_tables] 0: record in place; stage_stride: staged (RowApply); null without host tables
-    float** d_rtab_gdata = nullptr;          // [n_rtab] data in row order, d_stage for host tables (HotApply)
-    int32_t* d_rtab_stage = nullptr;         // [n_rtab] 0 / stage_stride in row order (HotApply, stage-in / write-back); null without host tables
+    int32_t* d_tab_stage = nullptr;          // [n_tables] 0: record in place; stage_stride: staged (fused row updates); null without host tables
+    int32_t* d_rtab_stage = nullptr;         // [n_rtab] 0 / stage_stride in row order (fused hot-row updates, stage-in / write-back); null without host tables
     // HBM cache of host records (wd_host_cache_enable): d_stage is then [cache_slots slots | max_nnz overflow rows]
     int64_t cache_slots = 0;                 // C = 8 x 2^cache_set_bits; 0: no cache (every staged row is an overflow row)
     int cache_set_bits = 0;
@@ -535,6 +534,22 @@ inline void mark(WdModel* m, const char* name) {
     cudaEventRecord(t.ev[t.n], m->stream);
     t.n++;
 }
+
+// run `fn` with the model's launches going to `stream` and its scan / sort scratch set `scratch_sel` (d_scan_tmp_s)
+template <typename F>
+int on_stream(WdModel* m, cudaStream_t stream, int scratch_sel, F fn) {
+    cudaStream_t main_stream = m->stream;
+    m->stream = stream; m->scratch_sel = scratch_sel;
+    int rc = fn();
+    m->stream = main_stream; m->scratch_sel = 0;
+    return rc;
+}
+// on the side stream of sparse list `which`
+template <typename F>
+int on_side(WdModel* m, int which, F fn) { return on_stream(m, m->sstream[which], 1 + which, fn); }
+// on the auxiliary stream of a row-sharded step (ShardState::aux)
+template <typename F>
+int on_aux(WdModel* m, F fn) { return on_stream(m, m->shard.aux, 3, fn); }
 
 inline int grid_for(int64_t n, int block, int cap = kNumSms * 16) {
     int64_t g = (n + block - 1) / block;

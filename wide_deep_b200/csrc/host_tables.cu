@@ -7,7 +7,7 @@
 //   stage-in    host_rows_kernel<true>: record of unique row u (host tables only) -> HBM staging buffer row u
 //   remap       host_remap_kernel: the gather reads ids in which a host-table entry carries u instead of its global row; the
 //               gather kernels see the host tables as (data = staging buffer, row base 0, stride = staging stride)
-//   apply       the fused updates (RowApply / HotApply in sparse.cu) address the staged record of u
+//   apply       the fused updates address the staged record of u (RowRecords::stage in sparse_dev.cuh)
 //   write-back  host_rows_kernel<false>: staging buffer row u -> host record, after the list's apply, on its stream
 // With the opt-in HBM cache (wd_host_cache_enable, below) row u is staged in a cache slot that outlives the step, and only the
 // rows that miss are moved.
@@ -23,16 +23,6 @@
 #include "sparse_dev.cuh"
 
 namespace wd {
-
-// table (index in row order) of a global embedding row: tables are few, binary search over their row bases
-__device__ __forceinline__ int rtab_of(const int64_t* __restrict__ rtab_row_base, int ntab, int64_t row) {
-    int lo = 0, hi = ntab - 1;
-    while (lo < hi) {
-        int mid = (lo + hi + 1) >> 1;
-        if (rtab_row_base[mid] <= row) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
 
 // ---------------------------------------------------------------------------------------------------------- HBM cache
 // wd_host_cache_enable turns the front of the staging buffer into an 8-way set-associative, write-back cache of host records:
@@ -61,7 +51,7 @@ __global__ void __launch_bounds__(256) cache_keys_kernel(const int32_t* __restri
     const int nu = *d_nuniq;
     for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) {
         const uint32_t row = urow[u];
-        keys[u] = rtab_stage[rtab_of(rtab_row_base, ntab, row)] != 0 ? cache_set_of(row, set_bits) : (1u << set_bits);
+        keys[u] = rtab_stage[table_of(rtab_row_base, ntab, row)] != 0 ? cache_set_of(row, set_bits) : (1u << set_bits);
         vals[u] = (uint32_t)u;
     }
 }
@@ -172,7 +162,7 @@ __global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restric
             const int64_t u = i / q4;
             const int q = (int)(i - u * q4);
             const int64_t row = urow[u];
-            const int lo = rtab_of(rtab_row_base, ntab, row);
+            const int lo = table_of(rtab_row_base, ntab, row);
             if (rtab_stage[lo] == 0) continue;                           // HBM table
             int64_t srow = u;
             if (sm.uslot) {
@@ -182,7 +172,7 @@ __global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restric
                     if (!(f & kLoad)) continue;                              // hit: the slot holds the record
                     if (f & kVictimDirty) {
                         const int64_t vr = sm.uvict[u];
-                        const int vlo = rtab_of(rtab_row_base, ntab, vr);
+                        const int vlo = table_of(rtab_row_base, ntab, vr);
                         const int vstride = rtab_stride[vlo];
                         if (q * 4 < vstride) {
                             vv[k] = *reinterpret_cast<const float4*>(stage + srow * S + q * 4);
@@ -216,7 +206,7 @@ __global__ void __launch_bounds__(256) host_remap_kernel(const int32_t* __restri
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t r = e_emb[i];
         uint32_t g = r;
-        if (r != kInvalidRow && rtab_stage[rtab_of(rtab_row_base, ntab, r)] != 0) {
+        if (r != kInvalidRow && rtab_stage[table_of(rtab_row_base, ntab, r)] != 0) {
             const int u = lower_bound_u32(urow, nu, r);
             g = uslot ? (uint32_t)uslot[u] : (uint32_t)u;
         }
@@ -235,7 +225,7 @@ __global__ void __launch_bounds__(256) cache_flush_kernel(int64_t C, int S, cons
         const int q = (int)(i - slot * q4);
         if (!dirty[slot] || tag[slot] == kInvalidRow) continue;
         const int64_t row = tag[slot];
-        const int lo = rtab_of(rtab_row_base, ntab, row);
+        const int lo = table_of(rtab_row_base, ntab, row);
         const int stride = rtab_stride[lo];
         if (q * 4 >= stride) continue;
         *reinterpret_cast<float4*>(rtab_data[lo] + (row - rtab_row_base[lo]) * stride + q * 4) =
@@ -328,13 +318,13 @@ static int overwrite(WdModel* m, T* dst, const std::vector<T>& h) {
     return WD_OK;
 }
 
-// What the gather kernels and the fused updates address: host tables through the staging buffer (data = d_stage, row base 0,
-// stride stage_stride), every other table in place.  alloc: upload the descriptor arrays (place_tables); else overwrite the ones
-// that carry the staging buffer's address (wd_host_cache_enable replaces the buffer).
+// What the gather kernels address: host tables through the staging buffer (data = d_stage, row base 0, stride stage_stride), every
+// other table in place; and which tables the fused updates find staged (d_tab_stage / d_rtab_stage).  alloc: upload the descriptor
+// arrays (place_tables); else overwrite the ones that carry the staging buffer's address (wd_host_cache_enable replaces the buffer).
 static int stage_descriptors(WdModel* m, bool alloc) {
     const int nt = (int)m->tables.size();
     int rc;
-    std::vector<float*> gdata(nt), rgdata;
+    std::vector<float*> gdata(nt);
     std::vector<int32_t> gstride(nt), stage(nt, 0), rstage;
     std::vector<int64_t> grb(nt);
     for (int t = 0; t < nt; ++t) {
@@ -344,23 +334,15 @@ static int stage_descriptors(WdModel* m, bool alloc) {
         grb[t] = tb.host ? 0 : tb.row_base;
         stage[t] = tb.host ? m->stage_stride : 0;
     }
-    for (int t : m->rtab_order) {
-        const EmbTable& tb = m->tables[t];
-        rgdata.push_back(tb.host ? m->d_stage : tb.data);
-        rstage.push_back(tb.host ? m->stage_stride : 0);
-    }
+    for (int t : m->rtab_order) rstage.push_back(m->tables[t].host ? m->stage_stride : 0);
     if (m->n_host_tab > 0) {
         if (alloc) {
             if ((rc = upload(m, &m->d_gtab_data, gdata))) return rc;
             if ((rc = upload(m, &m->d_gtab_stride, gstride))) return rc;
             if ((rc = upload(m, &m->d_gtab_row_base, grb))) return rc;
             if ((rc = upload(m, &m->d_tab_stage, stage))) return rc;
-            if ((rc = upload(m, &m->d_rtab_gdata, rgdata))) return rc;
             if ((rc = upload(m, &m->d_rtab_stage, rstage))) return rc;
-        } else {
-            if ((rc = overwrite(m, m->d_gtab_data, gdata))) return rc;
-            if (!rgdata.empty() && (rc = overwrite(m, m->d_rtab_gdata, rgdata))) return rc;
-        }
+        } else if ((rc = overwrite(m, m->d_gtab_data, gdata))) return rc;
     }
     for (int i = 0; i < m->n_dims; ++i) {    // per-width descriptors of the short-bag gather (table ids ascending, as build_model)
         std::vector<TabDesc> descs;
@@ -443,7 +425,6 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
     } else {                                 // nothing on the host: the step addresses the tables' own arrays
         m->d_g_emb = m->d_e_emb;
         m->d_gtab_data = m->d_tab_data; m->d_gtab_stride = m->d_tab_stride; m->d_gtab_row_base = m->d_tab_row_base;
-        m->d_rtab_gdata = m->d_rtab_data;
     }
     if ((rc = stage_descriptors(m, true))) return rc;
     WD_CUDA(cudaStreamSynchronize(m->stream));

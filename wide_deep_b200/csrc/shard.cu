@@ -13,8 +13,9 @@
 //   combine        (requester) sums the <= G partials of a bag in rank order, applies the mean, writes the deep-input slice /
 //                  adds the wide partial logits
 //   backward       (owner)     sorts the received rows, then PULLS each occurrence's gradient (the requester's dX0 slice or
-//                  dlogit, P2P loads) while summing per row in a fixed order, and applies Adagrad / FTRL to its shard: the
-//                  all-to-all of gradients is fused into the segmented reduction, the optimizer runs once per touched row
+//                  dlogit, P2P loads) while summing per row in a fixed order — the gradient-sum kernels of the local lists
+//                  (sparse_dev.cuh) over a peer occurrence source —, and applies Adagrad / FTRL to its shard: the all-to-all of
+//                  gradients is fused into the segmented reduction, the optimizer runs once per touched row
 //   dense          gradients of the MLP / wide bias / small replicated tables: two-shot all-reduce over peer memory (each rank
 //                  reduces one slice in rank order, then every rank gathers the slices) — deterministic, identical on all ranks
 //
@@ -24,7 +25,8 @@
 //                   needs anyway, moved in front of the serve
 //   2. stage-in     host_rows_kernel<true> (host_tables.cu): record of unique row u of a host slot -> owner staging buffer row u
 //   3. serve        a host slot's records are read from staging row u (lower_bound of the local row in urow[2])
-//   4. apply        emb_apply_kernel updates the staged record of u (per-slot stage stride; 0 = HBM slot, updated in place)
+//   4. apply        emb_apply_kernel updates the staged record of u (RowRecords with a per-slot stage stride; 0 = HBM slot,
+//                   updated in place)
 //   5. write-back   host_rows_kernel<false>, right after the apply on the same stream, which joins the main stream before the step
 //                   ends (before the next stage-in); forward-only calls skip it
 // Every kernel reads the same values and sums them in the same order as with the shard in HBM: the results are bit-identical.
@@ -161,8 +163,7 @@ __global__ void __launch_bounds__(256) shard_serve_emb_kernel(const uint2* __res
         const uint2* box = inbox + (int64_t)r * pair_cap;
         const uint2 en = __ldcg(box + i);
         if (i > 0 && __ldcg(box + i - 1).y == en.y) continue;     // not the head of its bag
-        int lo = 0, hi = n_slots - 1;
-        while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (slot_base[mid] <= (int64_t)en.x) lo = mid; else hi = mid - 1; }
+        const int lo = table_of(slot_base, n_slots, en.x);
         const int sst = slot_stage ? slot_stage[lo] : 0;
         const int dim = slot_dim[lo], stride = sst ? sst : slot_stride[lo];
         const float* data = sst ? stage : slot_data[lo];
@@ -266,86 +267,45 @@ __global__ void __launch_bounds__(256) shard_combine_wide_kernel(int B, const in
 }
 
 // -------------------------------------------------------------------------------------- owner: gradient sums (P2P pull)
-// Per unique owned row: ordered sum over its occurrences of (requester's dX0 slice of the bag) / (ids in the bag), read from the
-// requester's memory.  Same decomposition as emb_grad_sum_kernel (8 lanes per item, 4 rows in flight, hot rows in chunks).
-template <bool CHUNKED>
-__global__ void __launch_bounds__(256) shard_emb_grad_sum_kernel(const int32_t* __restrict__ d_nitems, const int32_t* __restrict__ d_nuniq,
-                                                                 const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff,
-                                                                 const uint32_t* __restrict__ svals, const uint32_t* __restrict__ rtag,
-                                                                 const ShardPeer* __restrict__ peers, int n_slots, const int32_t* __restrict__ slot_dim,
-                                                                 const int32_t* __restrict__ slot_x0, int ld, float* __restrict__ out, int width) {
-    const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
-    const int nitems = *d_nitems, nu = *d_nuniq;
-    const int64_t g0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4 + grp;
-    const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
-    for (int64_t it = g0; it < nitems; it += gstep) {
-        int s, e;
-        if (!CHUNKED) {
-            s = ustart[it]; e = ustart[it + 1];
-            if (e - s > kChunk) continue;
-        } else {
-            int u = chunk_owner(choff, nu, (int)it);
-            s = ustart[u] + ((int)it - choff[u]) * kChunk;
-            e = min(ustart[u + 1], s + kChunk);
-        }
-        const int slot = (int)((rtag[svals[s]] & kTagBagMask) % (uint32_t)n_slots);
-        const int dim = slot_dim[slot], x0 = slot_x0[slot];
-        for (int q = lig; q * 4 < width; q += 8) {
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (q * 4 < dim) {
-                int j = s;
-                for (; j + 4 <= e; j += 4) {
-                    uint32_t tg[4]; float4 v[4]; float inv[4];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) tg[r] = rtag[svals[j + r]];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) {
-                        const ShardPeer& pr = peers[tg[r] >> kTagBagBits];
-                        const uint32_t bag = tg[r] & kTagBagMask;
-                        v[r] = __ldcg(reinterpret_cast<const float4*>(pr.gradbase + (int64_t)(bag / (uint32_t)n_slots) * ld + x0 + q * 4));
-                        inv[r] = __ldcg(pr.bagscale + bag);
-                    }
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) { acc.x += v[r].x * inv[r]; acc.y += v[r].y * inv[r]; acc.z += v[r].z * inv[r]; acc.w += v[r].w * inv[r]; }
-                }
-                for (; j < e; ++j) {
-                    const uint32_t tg = rtag[svals[j]];
-                    const ShardPeer& pr = peers[tg >> kTagBagBits];
-                    const uint32_t bag = tg & kTagBagMask;
-                    const float4 v = __ldcg(reinterpret_cast<const float4*>(pr.gradbase + (int64_t)(bag / (uint32_t)n_slots) * ld + x0 + q * 4));
-                    const float inv = __ldcg(pr.bagscale + bag);
-                    acc.x += v.x * inv; acc.y += v.y * inv; acc.z += v.z * inv; acc.w += v.w * inv;
-                }
-            }
-            *reinterpret_cast<float4*>(out + (int64_t)it * width + q * 4) = acc;
-        }
-    }
+// Occurrence sources of the owner's per-row gradient sums (emb_grad_sum_kernel / wide_grad_sum_kernel, sparse_dev.cuh): occurrence
+// j of the sorted received rows is the received entry svals[j], whose tag (source rank << kTagBagBits | bag) says where its
+// gradient is — read from the requester's memory.
+// embedding space: (requester's dX0 slice of the bag) / (ids in the bag); a bag is example * n_slots + slot
+// (the tags, lists and peer table are read-only during the sums: loaded through the read-only path; the peers' gradients with
+// ld.global.cg, they live in another device's memory)
+__device__ __forceinline__ const ShardPeer& peer_of(const ShardPeer* peers, uint32_t tg) { return peers[tg >> kTagBagBits]; }
+__device__ __forceinline__ const float* ldg_ptr(const float* const* p) {
+    return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(p)));
 }
-
-template <bool CHUNKED>
-__global__ void shard_wide_grad_sum_kernel(const int32_t* __restrict__ d_nitems, const int32_t* __restrict__ d_nuniq,
-                                           const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff,
-                                           const uint32_t* __restrict__ svals, const uint32_t* __restrict__ rtag,
-                                           const ShardPeer* __restrict__ peers, float* __restrict__ out) {
-    const int nitems = *d_nitems, nu = *d_nuniq;
-    for (int it = blockIdx.x * blockDim.x + threadIdx.x; it < nitems; it += gridDim.x * blockDim.x) {
-        int s, e;
-        if (!CHUNKED) {
-            s = ustart[it]; e = ustart[it + 1];
-            if (e - s > kChunk) continue;
-        } else {
-            int u = chunk_owner(choff, nu, it);
-            s = ustart[u] + (it - choff[u]) * kChunk;
-            e = min(ustart[u + 1], s + kChunk);
-        }
-        float acc = 0.f;
-        for (int j = s; j < e; ++j) {
-            const uint32_t tg = rtag[svals[j]];
-            acc += __ldcg(peers[tg >> kTagBagBits].gradbase + (tg & kTagBagMask));       // the example's dlogit on its own rank
-        }
-        out[it] = acc;
+struct PeerEmb {
+    const uint32_t* svals;
+    const uint32_t* rtag;
+    const ShardPeer* peers;
+    int n_slots;
+    const int32_t* slot_dim;
+    const int32_t* slot_x0;
+    int ld;
+    __device__ __forceinline__ uint32_t key(int j) const { return __ldg(rtag + __ldg(svals + j)); }
+    __device__ __forceinline__ void layout(uint32_t tg, int& t, int& dim, int& x0) const {
+        t = (int)((tg & kTagBagMask) % (uint32_t)n_slots);
+        dim = __ldg(slot_dim + t); x0 = __ldg(slot_x0 + t);
     }
-}
+    __device__ __forceinline__ float4 row(uint32_t tg, int x0, int q, float& inv) const {
+        const ShardPeer& pr = peer_of(peers, tg);
+        const uint32_t bag = tg & kTagBagMask;
+        const float4 v = __ldcg(reinterpret_cast<const float4*>(ldg_ptr(&pr.gradbase) + (int64_t)(bag / (uint32_t)n_slots) * ld + x0 + q * 4));
+        inv = __ldcg(ldg_ptr(&pr.bagscale) + bag);
+        return v;
+    }
+};
+// wide space: the example's dlogit on its own rank
+struct PeerWide {
+    const uint32_t* svals;
+    const uint32_t* rtag;
+    const ShardPeer* peers;
+    __device__ __forceinline__ uint32_t key(int j) const { return __ldg(rtag + __ldg(svals + j)); }
+    __device__ __forceinline__ float row(uint32_t tg) const { return __ldcg(ldg_ptr(&peer_of(peers, tg).gradbase) + (tg & kTagBagMask)); }
+};
 
 // ----------------------------------------------------------------------------------------- dense gradients: all-reduce
 // two-shot over peer memory: rank `me` sums slice `me` of every rank's arena in rank order, then every rank copies all slices
@@ -698,23 +658,21 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
     const int L = 2 + s;
     int rc;
     if (s == 0) {
-        shard_emb_grad_sum_kernel<false><<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nuniq[L], m->d_ustart[L], m->d_choff[L],
-            m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0, m->d0_phys, m->d_ugrad[L], sp.width);
-        shard_emb_grad_sum_kernel<true><<<grid_for(m->cpart_cap * 8, 256), 256, 0, m->stream>>>(m->d_nchunks[L], m->d_nuniq[L], m->d_ustart[L], m->d_choff[L],
-            m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0, m->d0_phys, m->d_cpart[L], sp.width);
-        m->launches += 2;
+        const PeerEmb src{m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0, m->d0_phys};
+        emb_grad_sum_kernel<PeerEmb, false><<<grid_for((m->max_nnz + m->cpart_cap) * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],
+            m->d_ustart[L], m->d_choff[L], src, m->d_ugrad[L], m->d_cpart[L], sp.width, RowApply{});
+        m->launches++;
         if ((rc = list_chunk_combine(m, L, sp.width))) return rc;
-        if ((rc = list_apply_emb(m, L, sp.width, sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, m->dnn_opt,
-                                 sp.d_slot_stage, sp.d_stage))) return rc;
+        const RowRecords rec{sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, nullptr};
+        if ((rc = list_apply_emb(m, L, sp.width, rec, m->dnn_opt))) return rc;
         // staged records home, on this stream: it joins the main stream before the step ends, so the next stage-in comes after
         if (staged(m, s) && (rc = host_rows_transfer(m, false, m->d_nuniq[L], m->d_urow[L], sp.n_slots, sp.d_slot_base, sp.d_slot_data,
                                                      sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, sp.stage_stride))) return rc;
     } else {
-        shard_wide_grad_sum_kernel<false><<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nuniq[L], m->d_ustart[L], m->d_choff[L],
-            m->d_sv[L], sp.d_rtag, sp.d_peers, m->d_ugrad[L]);
-        shard_wide_grad_sum_kernel<true><<<grid_for(m->cpart_cap, 256), 256, 0, m->stream>>>(m->d_nchunks[L], m->d_nuniq[L], m->d_ustart[L], m->d_choff[L],
-            m->d_sv[L], sp.d_rtag, sp.d_peers, m->d_cpart[L]);
-        m->launches += 2;
+        const PeerWide src{m->d_sv[L], sp.d_rtag, sp.d_peers};
+        wide_grad_sum_kernel<PeerWide, false><<<grid_for(m->max_nnz + m->cpart_cap, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],
+            m->d_ustart[L], m->d_choff[L], src, m->d_ugrad[L], m->d_cpart[L], RowApply{});
+        m->launches++;
         if ((rc = list_chunk_combine(m, L, 1))) return rc;
         if ((rc = list_apply_wide(m, L, sp.d_wide, m->lin_opt))) return rc;
     }
@@ -749,26 +707,6 @@ int ids_prepare(WdModel* m);
 int shard_backward_local(WdModel* m, bool overlap);     // api.cu: towers' backward + replicated lists + dense gradient arena
 int shard_apply_local(WdModel* m);                     // api.cu: dense optimizer + small-table block + joins
 int shard_group_async(WdModel* m);                     // api.cu: replicated lists' grouping on the side streams
-
-// run `fn` on the side stream of sparse list `w` (its scratch set), as api.cu does for the replicated lists
-template <typename F>
-static int on_side(WdModel* m, int w, F fn) {
-    cudaStream_t main_stream = m->stream;
-    m->stream = m->sstream[w]; m->scratch_sel = 1 + w;
-    int rc = fn();
-    m->stream = main_stream; m->scratch_sel = 0;
-    return rc;
-}
-
-// run `fn` on the auxiliary stream (scratch set 3)
-template <typename F>
-static int on_aux(WdModel* m, F fn) {
-    cudaStream_t main_stream = m->stream;
-    m->stream = m->shard.aux; m->scratch_sel = 3;
-    int rc = fn();
-    m->stream = main_stream; m->scratch_sel = 0;
-    return rc;
-}
 
 // The critical chain in front of the towers is   ids -> route + send (embedding space) -> [A] -> serve (embedding space) -> [B].
 // Everything else that must exist before the towers — the wide space's routing, its serve, and this rank's local gathers

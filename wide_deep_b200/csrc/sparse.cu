@@ -223,99 +223,39 @@ __global__ void sort_keys_kernel(const int32_t* __restrict__ d_nnz, const uint32
 }
 
 
-// ---- per unique row: g = ordered sum of its occurrences' gradients.
-// Rows touched at most kChunk times are summed by one lane group directly.  Hotter rows (small tables,
-// skewed ids) are split into chunks of kChunk occurrences that are summed in parallel and then combined in
-// chunk order, so the result stays deterministic and no single group walks thousands of occurrences.
-
-// embedding rows: contribution of occurrence j = dX0[b, x0_off : x0_off + dim] / bag_size(b, column)
-// 8 lanes per work item, each lane covers float4 chunks lig, lig+8, ... of the row.  One launch covers both kinds of work item:
-// items [0, nu) are the unique rows (summed directly into ugrad unless they are hot), items [nu, nu + nchunks) are the chunks of
-// the hot rows (summed into cpart, combined afterwards by chunk_combine_kernel).
-// APPLY (single-GPU step, row-local optimizer): the optimizer update of a directly summed row follows its sum in the same thread —
-// the summed gradient never reaches memory; the hot rows are updated by chunk_combine_kernel<1>.
-// tab_stage (null without host tables): per table 0 = record in place, else the table is staged — the record of unique row `it`
-// is at tab_data[t] (the staging buffer) + uslot[it] * tab_stage[t], or + it * tab_stage[t] when uslot is null (no HBM cache).
-struct RowApply { const uint32_t* urow; float* const* tab_data; const int32_t* tab_stride; const int64_t* tab_row_base; OptParams o;
-                  const int32_t* tab_stage; const int32_t* uslot; };
-template <bool APPLY>
-__global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ d_nchunks,
-                                                           const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff,
-                                                           const uint32_t* __restrict__ sbc /* sorted cell indices bc = b * C + c */,
-                                                           const int32_t* __restrict__ offs,
-                                                           int C, const int32_t* __restrict__ col_table,
-                                                           const int32_t* __restrict__ tab_dim, const int32_t* __restrict__ tab_x0,
-                                                           const float* __restrict__ dX0, int ld, float* __restrict__ ugrad,
-                                                           float* __restrict__ cpart, int width, RowApply ra) {
-    const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
-    const int nu = *d_nuniq;
-    const int64_t nitems = (int64_t)nu + *d_nchunks;
-    const int64_t g0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4 + grp;
-    const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
-    for (int64_t it = g0; it < nitems; it += gstep) {
-        int s, e;
-        float* out;
-        const bool direct = it < nu;
-        if (direct) {
-            s = ustart[it]; e = ustart[it + 1];
-            if (e - s > kChunk) continue;                     // hot row: summed chunk by chunk below
-            out = ugrad + it * width;
-        } else {
-            const int c = (int)(it - nu);
-            const int u = chunk_owner(choff, nu, c);
-            s = ustart[u] + (c - choff[u]) * kChunk;
-            e = min(ustart[u + 1], s + kChunk);
-            out = cpart + (int64_t)c * width;
-        }
-        int bc0 = (int)sbc[s];
-        int t = col_table[bc0 % C];
-        int dim = tab_dim[t], x0 = tab_x0[t];
-        for (int q = lig; q * 4 < width; q += 8) {
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (q * 4 < dim) {
-                int j = s;
-                for (; j + 4 <= e; j += 4) {                  // 4 gradient rows in flight
-                    int bcs[4]; float4 v[4]; float inv[4];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) bcs[r] = (int)sbc[j + r];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) {
-                        v[r] = *reinterpret_cast<const float4*>(dX0 + (int64_t)(bcs[r] / C) * ld + x0 + q * 4);
-                        inv[r] = 1.f / (float)(offs[bcs[r] + 1] - offs[bcs[r]]);
-                    }
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) { acc.x += v[r].x * inv[r]; acc.y += v[r].y * inv[r]; acc.z += v[r].z * inv[r]; acc.w += v[r].w * inv[r]; }
-                }
-                for (; j < e; ++j) {
-                    int bc = (int)sbc[j];
-                    float4 v = *reinterpret_cast<const float4*>(dX0 + (int64_t)(bc / C) * ld + x0 + q * 4);
-                    float inv = 1.f / (float)(offs[bc + 1] - offs[bc]);
-                    acc.x += v.x * inv; acc.y += v.y * inv; acc.z += v.z * inv; acc.w += v.w * inv;
-                }
-            }
-            if (APPLY && direct) {
-                if (q * 4 < dim) {
-                    const int stride = ra.tab_stride[t];
-                    const int sst = ra.tab_stage ? ra.tab_stage[t] : 0;
-                    float* rec = ra.tab_data[t] + (sst ? (ra.uslot ? (int64_t)ra.uslot[it] : it) * sst : ((int64_t)ra.urow[it] - ra.tab_row_base[t]) * stride);
-                    const int nslots = stride / dim - 1;
-                    float4 w = *reinterpret_cast<float4*>(rec + q * 4);
-                    float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + q * 4) : make_float4(0, 0, 0, 0);
-                    float4 s2 = nslots >= 2 ? *reinterpret_cast<float4*>(rec + 2 * dim + q * 4) : make_float4(0, 0, 0, 0);
-                    opt_update(ra.o, acc.x, w.x, s1.x, s2.x);
-                    opt_update(ra.o, acc.y, w.y, s1.y, s2.y);
-                    opt_update(ra.o, acc.z, w.z, s1.z, s2.z);
-                    opt_update(ra.o, acc.w, w.w, s1.w, s2.w);
-                    *reinterpret_cast<float4*>(rec + q * 4) = w;
-                    if (nslots >= 1) *reinterpret_cast<float4*>(rec + dim + q * 4) = s1;
-                    if (nslots >= 2) *reinterpret_cast<float4*>(rec + 2 * dim + q * 4) = s2;
-                }
-            } else {
-                *reinterpret_cast<float4*>(out + q * 4) = acc;
-            }
-        }
+// ---- per-row gradient sums of the batch's own lists (emb_grad_sum_kernel / wide_grad_sum_kernel, sparse_dev.cuh).  The sorted
+// values are the occurrences' cell indices bc = b * C + c: that is all a sum needs to find an occurrence's gradient.
+// embedding rows: occurrence bc contributes dX0[b, x0 : x0 + dim] / bag_size(b, c), x0 and dim of column c's table
+// (the sources' arrays are read-only during the sums: loaded through the read-only path, as restrict kernel arguments would be)
+struct LocalEmb {
+    const uint32_t* sbc;
+    const int32_t* offs;
+    int C;
+    const int32_t* col_table;
+    const int32_t* tab_dim;
+    const int32_t* tab_x0;
+    const float* dX0;
+    int ld;
+    __device__ __forceinline__ uint32_t key(int j) const { return __ldg(sbc + j); }
+    __device__ __forceinline__ void layout(uint32_t k, int& t, int& dim, int& x0) const {
+        t = __ldg(col_table + (int)k % C);
+        dim = __ldg(tab_dim + t); x0 = __ldg(tab_x0 + t);
     }
-}
+    __device__ __forceinline__ float4 row(uint32_t k, int x0, int q, float& inv) const {
+        const int bc = (int)k;
+        const float4 v = __ldg(reinterpret_cast<const float4*>(dX0 + (int64_t)(bc / C) * ld + x0 + q * 4));
+        inv = 1.f / (float)(__ldg(offs + bc + 1) - __ldg(offs + bc));
+        return v;
+    }
+};
+// wide rows: occurrence bc contributes dlogit[b]
+struct LocalWide {
+    const uint32_t* sbc;
+    int C;
+    const float* dlogit;
+    __device__ __forceinline__ uint32_t key(int j) const { return __ldg(sbc + j); }
+    __device__ __forceinline__ float row(uint32_t k) const { return __ldg(dlogit + k / (uint32_t)C); }
+};
 
 // ugrad[u] = sum of the row's chunk partials (multi-chunk rows only).  Each lane checks one unique row; the (rare)
 // multi-chunk rows of a warp are combined by the whole warp: lane groups add chunks g, g+NG, ... and a fixed-order shuffle
@@ -323,18 +263,11 @@ __global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __rest
 // rows of the small tables), so a warp takes every NW-th group of rows (lane l of warp w checks row (it * 32 + l) * NW + w):
 // neighbouring hot rows land in different warps and their long chunk lists are walked concurrently, not one after the other.
 // KIND 0: the sum goes to ugrad.  KIND 1 / 2 (single-GPU step, row-local optimizer): the hot row's optimizer update follows its
-// sum here (1: embedding record, width a power of two in [4, 128]; 2: wide record, width 1) — together with the APPLY variants of
-// the gradient-sum kernels this leaves no separate optimizer launch for the list.
-struct HotApply {
-    const uint32_t* urow; int ntab; const int64_t* tab_row_base; float* const* tab_data; const int32_t* tab_dim; const int32_t* tab_stride;   // KIND 1 (tables in row order)
-    float4* wide;                                                                                                                          // KIND 2
-    OptParams o;
-    const int32_t* tab_stage;     // KIND 1, as RowApply::tab_stage (tables in row order): staged record of unique row uu at tab_data + uu * tab_stage
-    const int32_t* uslot;         // KIND 1, as RowApply::uslot: with an HBM cache the record is at tab_data + uslot[uu] * tab_stage
-};
+// sum here (1: embedding record, tables of ra.rec in row order, width a power of two in [4, 128]; 2: wide record, width 1) —
+// together with the APPLY variants of the gradient-sum kernels this leaves no separate optimizer launch for the list.
 template <int KIND>
 __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ choff,
-                                                            const float* __restrict__ cpart, float* __restrict__ ugrad, int width, HotApply ha) {
+                                                            const float* __restrict__ cpart, float* __restrict__ ugrad, int width, RowApply ra) {
     const int nu = *d_nuniq;
     const int lane = threadIdx.x & 31;
     const int64_t w0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -375,28 +308,10 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
                 }
                 if (KIND == 1) {
                     if (cg == 0) {
-                        const int64_t row = ha.urow[uu];
-                        int lo = 0, hi = ha.ntab - 1;               // table of this global row (tables are few: binary search)
-                        while (lo < hi) {
-                            int mid = (lo + hi + 1) >> 1;
-                            if (ha.tab_row_base[mid] <= row) lo = mid; else hi = mid - 1;
-                        }
-                        const int dim = ha.tab_dim[lo], stride = ha.tab_stride[lo];
-                        if (lq * 4 < dim) {
-                            const int sst = ha.tab_stage ? ha.tab_stage[lo] : 0;
-                            float* rec = ha.tab_data[lo] + (sst ? (ha.uslot ? (int64_t)ha.uslot[uu] : uu) * sst : (row - ha.tab_row_base[lo]) * stride);
-                            const int nslots = stride / dim - 1;
-                            float4 w = *reinterpret_cast<float4*>(rec + lq * 4);
-                            float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + lq * 4) : make_float4(0, 0, 0, 0);
-                            float4 s2 = nslots >= 2 ? *reinterpret_cast<float4*>(rec + 2 * dim + lq * 4) : make_float4(0, 0, 0, 0);
-                            opt_update(ha.o, acc.x, w.x, s1.x, s2.x);
-                            opt_update(ha.o, acc.y, w.y, s1.y, s2.y);
-                            opt_update(ha.o, acc.z, w.z, s1.z, s2.z);
-                            opt_update(ha.o, acc.w, w.w, s1.w, s2.w);
-                            *reinterpret_cast<float4*>(rec + lq * 4) = w;
-                            if (nslots >= 1) *reinterpret_cast<float4*>(rec + dim + lq * 4) = s1;
-                            if (nslots >= 2) *reinterpret_cast<float4*>(rec + 2 * dim + lq * 4) = s2;
-                        }
+                        const int64_t row = ra.urow[uu];
+                        const int t = table_of(ra.rec.row_base, ra.rec.ntab, row);
+                        const int dim = ra.rec.dim[t];
+                        if (lq * 4 < dim) update_record4(ra.o, record(ra.rec, t, ra.urow, uu) + lq * 4, dim, ra.rec.stride[t] / dim - 1, acc);
                     }
                 } else if (cg == 0) *reinterpret_cast<float4*>(ugrad + uu * width + lq * 4) = acc;
             } else {
@@ -406,11 +321,8 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
 #pragma unroll
                     for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
                     if (lane == 0) {
-                        if (KIND == 2) {                            // width == 1
-                            float4 r = ha.wide[ha.urow[uu]];
-                            opt_update(ha.o, acc, r.x, r.y, r.z);
-                            ha.wide[ha.urow[uu]] = r;
-                        } else ugrad[uu * width + q] = acc;
+                        if (KIND == 2) update_wide(ra.o, ra.wide + ra.urow[uu], acc);     // width == 1
+                        else ugrad[uu * width + q] = acc;
                     }
                 }
             }
@@ -418,76 +330,22 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
     }
 }
 
-// wide rows: contribution of occurrence j = dlogit[b]; one thread per work item.  Items [0, nu) = unique rows (hot ones skipped),
-// items [nu, nu + nchunks) = chunks of the hot rows, as in emb_grad_sum_kernel; APPLY: record {w, s1, s2, -} updated in place.
-template <bool APPLY>
-__global__ void wide_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ d_nchunks,
-                                     const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff,
-                                     const uint32_t* __restrict__ sbc /* sorted cell indices bc = b * C + c */, int C,
-                                     const float* __restrict__ dlogit, float* __restrict__ ugrad, float* __restrict__ cpart,
-                                     const uint32_t* __restrict__ urow, float4* __restrict__ wide, OptParams o) {
-    const int nu = *d_nuniq;
-    const int64_t nitems = (int64_t)nu + *d_nchunks;
-    for (int64_t it = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; it < nitems; it += (int64_t)gridDim.x * blockDim.x) {
-        int s, e;
-        const bool direct = it < nu;
-        if (direct) {
-            s = ustart[it]; e = ustart[it + 1];
-            if (e - s > kChunk) continue;
-        } else {
-            const int c = (int)(it - nu);
-            const int u = chunk_owner(choff, nu, c);
-            s = ustart[u] + (c - choff[u]) * kChunk;
-            e = min(ustart[u + 1], s + kChunk);
-        }
-        float acc = 0.f;
-        for (int j = s; j < e; ++j) acc += dlogit[sbc[j] / (uint32_t)C];
-        if (!direct) cpart[it - nu] = acc;
-        else if (APPLY) {
-            float4 r = wide[urow[it]];
-            opt_update(o, acc, r.x, r.y, r.z);
-            wide[urow[it]] = r;
-        } else ugrad[it] = acc;
-    }
-}
-
 // --------------------------------------------------------------------------------------------- optimizers
 
-// embedding rows: record = [w[dim] | s1[dim] | s2[dim]]; tab_stage (null: every record in place): 0 = in place, else the record of
-// unique row u is staged at stage + u * tab_stage[t] (host-placed shards of a row-sharded space, shard.cu)
+// embedding rows: record = [w[dim] | s1[dim] | s2[dim]], tables of rr in row order
 __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow,
-                                                        const float* __restrict__ ugrad, int width, int ntab,
-                                                        const int64_t* __restrict__ tab_row_base, float* const* __restrict__ tab_data,
-                                                        const int32_t* __restrict__ tab_dim, const int32_t* __restrict__ tab_stride,
-                                                        OptParams o, const int32_t* __restrict__ tab_stage, float* __restrict__ stage) {
+                                                        const float* __restrict__ ugrad, int width, RowRecords rr, OptParams o) {
     const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
     const int nu = *d_nuniq;
     const int64_t g0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4 + grp;
     const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
     for (int64_t u = g0; u < nu; u += gstep) {
-        int64_t row = urow[u];
-        int lo = 0, hi = ntab - 1;                  // table of this global row (tables are few: binary search)
-        while (lo < hi) {
-            int mid = (lo + hi + 1) >> 1;
-            if (tab_row_base[mid] <= row) lo = mid; else hi = mid - 1;
-        }
-        const int dim = tab_dim[lo], stride = tab_stride[lo];
-        const int sst = tab_stage ? tab_stage[lo] : 0;
-        float* rec = sst ? stage + u * sst : tab_data[lo] + (row - tab_row_base[lo]) * stride;
-        const int nslots = stride / dim - 1;
-        for (int q = lig; q * 4 < dim; q += 8) {
-            float4 g = *reinterpret_cast<const float4*>(ugrad + (int64_t)u * width + q * 4);
-            float4 w = *reinterpret_cast<float4*>(rec + q * 4);
-            float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim + q * 4) : make_float4(0, 0, 0, 0);
-            float4 s2 = nslots >= 2 ? *reinterpret_cast<float4*>(rec + 2 * dim + q * 4) : make_float4(0, 0, 0, 0);
-            opt_update(o, g.x, w.x, s1.x, s2.x);
-            opt_update(o, g.y, w.y, s1.y, s2.y);
-            opt_update(o, g.z, w.z, s1.z, s2.z);
-            opt_update(o, g.w, w.w, s1.w, s2.w);
-            *reinterpret_cast<float4*>(rec + q * 4) = w;
-            if (nslots >= 1) *reinterpret_cast<float4*>(rec + dim + q * 4) = s1;
-            if (nslots >= 2) *reinterpret_cast<float4*>(rec + 2 * dim + q * 4) = s2;
-        }
+        const int64_t row = urow[u];
+        const int t = table_of(rr.row_base, rr.ntab, row);
+        const int dim = rr.dim[t], nslots = rr.stride[t] / dim - 1;
+        float* rec = record(rr, t, urow, u);
+        for (int q = lig; q * 4 < dim; q += 8)
+            update_record4(o, rec + q * 4, dim, nslots, *reinterpret_cast<const float4*>(ugrad + (int64_t)u * width + q * 4));
     }
 }
 
@@ -495,11 +353,7 @@ __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restric
 __global__ void wide_apply_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow,
                                   const float* __restrict__ ugrad, float4* __restrict__ wide, OptParams o) {
     const int nu = *d_nuniq;
-    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) {
-        float4 r = wide[urow[u]];
-        opt_update(o, ugrad[u], r.x, r.y, r.z);
-        wide[urow[u]] = r;
-    }
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) update_wide(o, wide + urow[u], ugrad[u]);
 }
 
 
@@ -634,17 +488,21 @@ int sparse_reduce_emb(WdModel* m) {
         const int ge = grid_for((m->max_nnz + m->cpart_cap) * 8, 256);
         // the hot rows' update lives in the lane-group branch of chunk_combine_kernel: widths 4, 8, ..., 128
         const bool fused = fuse_row_apply(m, m->dnn_opt) && width >= 4 && (G4 & (G4 - 1)) == 0 && G4 <= 32;
-        // (host tables: the fused updates go to the staged records, host_tables_write_back copies them home after the list's apply)
-        const RowApply ra{m->d_urow[0], m->d_gtab_data, m->d_tab_stride, m->d_tab_row_base, make_opt(m->dnn_opt), m->d_tab_stage, m->d_uslot};
-        const HotApply ha{m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_gdata, m->d_rtab_dim, m->d_rtab_stride, nullptr, make_opt(m->dnn_opt),
-                          m->d_rtab_stage, m->d_uslot};
+        // the direct rows' records by table in plan order (a sum knows its table from the column), the hot rows' by table in row
+        // order; host tables: the fused updates go to the staged records, host_tables_write_back copies them home after the list's apply
+        const OptParams o = make_opt(m->dnn_opt);
+        const RowApply ra{m->d_urow[0], RowRecords{(int)m->tables.size(), m->d_tab_row_base, m->d_tab_data, m->d_tab_dim, m->d_tab_stride,
+                                                   m->d_tab_stage, m->d_stage, m->d_uslot}, nullptr, o};
+        const RowApply ha{m->d_urow[0], RowRecords{m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride,
+                                                   m->d_rtab_stage, m->d_stage, m->d_uslot}, nullptr, o};
+        const LocalEmb src{m->d_sv[0], m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->d_tab_dim, m->d_tab_x0, m->d_dX0, m->d0_phys};
         if (fused) {
-            emb_grad_sum_kernel<true><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], m->d_sv[0],
-                m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->d_tab_dim, m->d_tab_x0, m->d_dX0, m->d0_phys, m->d_ugrad[0], m->d_cpart[0], width, ra);
+            emb_grad_sum_kernel<LocalEmb, true><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], src,
+                                                                          m->d_ugrad[0], m->d_cpart[0], width, ra);
             chunk_combine_kernel<1><<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_choff[0], m->d_cpart[0], m->d_ugrad[0], width, ha);
         } else {
-            emb_grad_sum_kernel<false><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], m->d_sv[0],
-                m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->d_tab_dim, m->d_tab_x0, m->d_dX0, m->d0_phys, m->d_ugrad[0], m->d_cpart[0], width, ra);
+            emb_grad_sum_kernel<LocalEmb, false><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], src,
+                                                                           m->d_ugrad[0], m->d_cpart[0], width, ra);
             chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_choff[0], m->d_cpart[0], m->d_ugrad[0], width, ha);
         }
         m->list_apply_fused[0] = fused;
@@ -660,16 +518,17 @@ int sparse_reduce_wide(WdModel* m) {
     const int g = grid_for(m->max_nnz, 256);
     if (m->use_wide) {
         const bool fused = fuse_row_apply(m, m->lin_opt);
-        const HotApply ha{m->d_urow[1], 0, nullptr, nullptr, nullptr, nullptr, m->d_wide, make_opt(m->lin_opt)};
+        const RowApply ra{m->d_urow[1], RowRecords{}, m->d_wide, make_opt(m->lin_opt)};
+        const LocalWide src{m->d_sv[1], m->n_columns, m->d_dlogit};
         const int gw = grid_for(m->max_nnz + m->cpart_cap, 256);
         if (fused) {
-            wide_grad_sum_kernel<true><<<gw, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_nchunks[1], m->d_ustart[1], m->d_choff[1], m->d_sv[1],
-                                                                 m->n_columns, m->d_dlogit, m->d_ugrad[1], m->d_cpart[1], m->d_urow[1], m->d_wide, ha.o);
-            chunk_combine_kernel<2><<<g, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_choff[1], m->d_cpart[1], m->d_ugrad[1], 1, ha);
+            wide_grad_sum_kernel<LocalWide, true><<<gw, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_nchunks[1], m->d_ustart[1], m->d_choff[1], src,
+                                                                            m->d_ugrad[1], m->d_cpart[1], ra);
+            chunk_combine_kernel<2><<<g, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_choff[1], m->d_cpart[1], m->d_ugrad[1], 1, ra);
         } else {
-            wide_grad_sum_kernel<false><<<gw, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_nchunks[1], m->d_ustart[1], m->d_choff[1], m->d_sv[1],
-                                                                  m->n_columns, m->d_dlogit, m->d_ugrad[1], m->d_cpart[1], m->d_urow[1], m->d_wide, ha.o);
-            chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_choff[1], m->d_cpart[1], m->d_ugrad[1], 1, ha);
+            wide_grad_sum_kernel<LocalWide, false><<<gw, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_nchunks[1], m->d_ustart[1], m->d_choff[1], src,
+                                                                             m->d_ugrad[1], m->d_cpart[1], ra);
+            chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_choff[1], m->d_cpart[1], m->d_ugrad[1], 1, ra);
         }
         m->list_apply_fused[1] = fused;
         m->launches += 2;
@@ -697,10 +556,9 @@ __global__ void __launch_bounds__(256) small_scatter_emb_kernel(const int32_t* _
     const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
     for (int64_t u = lb + g0; u < nu; u += gstep) {
         const int64_t row = urow[u];
-        int lo = 0, hi = ntab - 1;
-        while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (rtab_row_base[mid] <= row) lo = mid; else hi = mid - 1; }
-        const int dim = rtab_dim[lo];
-        float* dst = Gs + rtab_gs_off[lo] + (row - rtab_row_base[lo]) * dim;
+        const int t = table_of(rtab_row_base, ntab, row);
+        const int dim = rtab_dim[t];
+        float* dst = Gs + rtab_gs_off[t] + (row - rtab_row_base[t]) * dim;
         for (int q = lig; q * 4 < dim; q += 8)
             *reinterpret_cast<float4*>(dst + q * 4) = *reinterpret_cast<const float4*>(ugrad + u * width + q * 4);
         __syncwarp();
@@ -752,34 +610,20 @@ __global__ void __launch_bounds__(256) small_apply_emb_kernel(const float* __res
                                                               const int64_t* __restrict__ rtab_gs_off, float* const* __restrict__ rtab_data,
                                                               const int32_t* __restrict__ rtab_dim, const int32_t* __restrict__ rtab_stride, OptParams o) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-        int lo = first_small, hi = ntab - 1;                       // small tables are the last entries, offsets ascending
-        while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (rtab_gs_off[mid] <= i * 4) lo = mid; else hi = mid - 1; }
-        const int dim = rtab_dim[lo], stride = rtab_stride[lo];
-        const int64_t local = i * 4 - rtab_gs_off[lo];
-        if (touched[rtab_row_base[lo] - small_base + local / dim] == 0.f) continue;
+        // small tables are the last entries, offsets ascending
+        const int t = first_small + table_of(rtab_gs_off + first_small, ntab - first_small, i * 4);
+        const int dim = rtab_dim[t], stride = rtab_stride[t];
+        const int64_t local = i * 4 - rtab_gs_off[t];
+        if (touched[rtab_row_base[t] - small_base + local / dim] == 0.f) continue;
         const float4 g = *reinterpret_cast<const float4*>(Gs + i * 4);
-        float* rec = rtab_data[lo] + (local / dim) * stride + (local % dim);
-        const int nslots = stride / dim - 1;
-        float4 w = *reinterpret_cast<float4*>(rec);
-        float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(rec + dim) : make_float4(0, 0, 0, 0);
-        float4 s2 = nslots >= 2 ? *reinterpret_cast<float4*>(rec + 2 * dim) : make_float4(0, 0, 0, 0);
-        opt_update(o, g.x, w.x, s1.x, s2.x);
-        opt_update(o, g.y, w.y, s1.y, s2.y);
-        opt_update(o, g.z, w.z, s1.z, s2.z);
-        opt_update(o, g.w, w.w, s1.w, s2.w);
-        *reinterpret_cast<float4*>(rec) = w;
-        if (nslots >= 1) *reinterpret_cast<float4*>(rec + dim) = s1;
-        if (nslots >= 2) *reinterpret_cast<float4*>(rec + 2 * dim) = s2;
+        update_record4(o, rtab_data[t] + (local / dim) * stride + (local % dim), dim, stride / dim - 1, g);
     }
 }
 __global__ void __launch_bounds__(256) small_apply_wide_kernel(const float* __restrict__ Gs, const float* __restrict__ touched, int64_t n,
                                                                float4* __restrict__ wide, OptParams o) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         if (touched[i] == 0.f) continue;
-        const float g = Gs[i];
-        float4 r = wide[i];
-        opt_update(o, g, r.x, r.y, r.z);
-        wide[i] = r;
+        update_wide(o, wide + i, Gs[i]);
     }
 }
 int small_apply(WdModel* m) {
@@ -851,18 +695,14 @@ int sparse_apply_which(WdModel* m, int which) {
     if (which == 0 && m->use_deep && !m->tables.empty()) {
         const bool adam = m->dnn_opt.kind == WD_OPT_ADAM;
         if (adam && (rc = adam_dense_pass(m, 0, false))) return rc;
-        emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(
-            m->d_nuniq[0], m->d_urow[0], m->d_ugrad[0], m->emb_max_dim, m->n_rtab, m->d_rtab_row_base, m->d_rtab_data,
-            m->d_rtab_dim, m->d_rtab_stride, make_opt(m->dnn_opt), nullptr, nullptr);   // tables in row order (binary search by row)
-        m->launches++;
+        const RowRecords rec{m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride, nullptr, nullptr, nullptr};
+        if ((rc = list_apply_emb(m, 0, m->emb_max_dim, rec, m->dnn_opt))) return rc;
         if (adam && (rc = adam_dense_pass(m, 0, true))) return rc;
     }
     if (which == 1 && m->use_wide) {
         const bool adam = m->lin_opt.kind == WD_OPT_ADAM;
         if (adam && (rc = adam_dense_pass(m, 1, false))) return rc;
-        wide_apply_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[1], m->d_urow[1], m->d_ugrad[1], m->d_wide,
-                                                                          make_opt(m->lin_opt));
-        m->launches++;
+        if ((rc = list_apply_wide(m, 1, m->d_wide, m->lin_opt))) return rc;
         if (adam && (rc = adam_dense_pass(m, 1, true))) return rc;
     }
     WD_CUDA(cudaGetLastError());
@@ -883,15 +723,14 @@ int list_group(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row)
     return WD_OK;
 }
 int list_chunk_combine(WdModel* m, int which, int width) {
-    chunk_combine_kernel<0><<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_choff[which], m->d_cpart[which], m->d_ugrad[which], width, HotApply{});
+    chunk_combine_kernel<0><<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_choff[which], m->d_cpart[which], m->d_ugrad[which], width, RowApply{});
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int list_apply_emb(WdModel* m, int which, int width, int ntab, const int64_t* d_row_base, float* const* d_data, const int32_t* d_dim,
-                   const int32_t* d_stride, const WdOptimizer& o, const int32_t* d_stage, float* stage) {
-    emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], width, ntab,
-                                                                            d_row_base, d_data, d_dim, d_stride, make_opt(o), d_stage, stage);
+int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const WdOptimizer& o) {
+    emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], width, rec,
+                                                                            make_opt(o));
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;

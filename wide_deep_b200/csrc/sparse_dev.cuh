@@ -1,5 +1,7 @@
-// Device helpers shared by sparse.cu (replicated tables) and shard.cu (row-sharded tables): cache-hinted loads, binary searches,
-// the hot-row chunk layout and the per-row optimizer update (reference python/lib/utils/model_util.py:62-105; SURVEY A.9).
+// Device code shared by sparse.cu (replicated tables) and shard.cu (row-sharded tables): cache-hinted loads, binary searches, the
+// hot-row chunk layout, the per-row optimizer update (reference python/lib/utils/model_util.py:62-105; SURVEY A.9) and where it
+// finds a row's record (RowRecords), and the per-row gradient sums over an occurrence source (emb_grad_sum_kernel /
+// wide_grad_sum_kernel).
 #pragma once
 #include "common.cuh"
 
@@ -39,6 +41,15 @@ __device__ __forceinline__ int upper_bound_u32(const uint32_t* __restrict__ a, i
     while (lo < hi) { int mid = (lo + hi) >> 1; if (a[mid] <= key) lo = mid + 1; else hi = mid; }
     return lo;
 }
+// last i with base[i] <= key (base ascending, base[0] <= key): the table of a row from the tables' row bases (tables are few)
+__device__ __forceinline__ int table_of(const int64_t* __restrict__ base, int n, int64_t key) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        int mid = (lo + hi + 1) >> 1;
+        if (base[mid] <= key) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
 
 struct OptParams { int kind; float lr, l1, l2, init_acc, beta1, beta2, epsilon, rho, momentum; };
 inline OptParams make_opt(const WdOptimizer& o) { return OptParams{o.kind, o.lr, o.l1, o.l2, o.init_acc, o.beta1, o.beta2, o.epsilon, o.rho, o.momentum}; }
@@ -75,16 +86,162 @@ __device__ __forceinline__ void opt_update(const OptParams& o, float g, float& w
     }
 }
 
+// One update of four consecutive elements of an embedding record [w | s1 | s2]: w points at them, slot k at w + k * gap.
+__device__ __forceinline__ void update_record4(const OptParams& o, float* w, int gap, int nslots, float4 g) {
+    float4 x = *reinterpret_cast<float4*>(w);
+    float4 s1 = nslots >= 1 ? *reinterpret_cast<float4*>(w + gap) : make_float4(0, 0, 0, 0);
+    float4 s2 = nslots >= 2 ? *reinterpret_cast<float4*>(w + 2 * gap) : make_float4(0, 0, 0, 0);
+    opt_update(o, g.x, x.x, s1.x, s2.x);
+    opt_update(o, g.y, x.y, s1.y, s2.y);
+    opt_update(o, g.z, x.z, s1.z, s2.z);
+    opt_update(o, g.w, x.w, s1.w, s2.w);
+    *reinterpret_cast<float4*>(w) = x;
+    if (nslots >= 1) *reinterpret_cast<float4*>(w + gap) = s1;
+    if (nslots >= 2) *reinterpret_cast<float4*>(w + 2 * gap) = s2;
+}
+// One update of a wide record {w, s1, s2, -}.
+__device__ __forceinline__ void update_wide(const OptParams& o, float4* rec, float g) {
+    float4 r = *rec;
+    opt_update(o, g, r.x, r.y, r.z);
+    *rec = r;
+}
+
+// Where the [w | s1 | s2] records of a list's embedding rows are.  Tables t < ntab with first row row_base[t] (ascending), records
+// of stride[t] floats at data[t].  A staged table (stage[t] != 0; stage null: none is) keeps the records of the step's rows in
+// stage_base instead, unique row u at staging row uslot[u] (u without a cache) with stride stage[t].
+struct RowRecords {
+    int ntab;
+    const int64_t* row_base;
+    float* const* data;
+    const int32_t* dim;
+    const int32_t* stride;
+    const int32_t* stage;
+    float* stage_base;
+    const int32_t* uslot;
+};
+// record of unique row u of the list (global row urow[u], read only for a record in place) in table t.  (Both cases are offsets
+// from the table pointer data[t], a pointer loaded from global memory: the compiler then keeps the record's loads and stores global
+// ones, where a choice between two pointers would make them generic.)
+__device__ __forceinline__ float* record(const RowRecords& r, int t, const uint32_t* urow, int64_t u) {
+    float* data = r.data[t];
+    const int sst = r.stage ? r.stage[t] : 0;
+    return data + (sst ? (r.stage_base - data) + (r.uslot ? (int64_t)r.uslot[u] : u) * sst : ((int64_t)urow[u] - r.row_base[t]) * r.stride[t]);
+}
+
+// The optimizer the single-GPU step fuses into its gradient sums: unique row u of the list is global row urow[u]; embedding records
+// as `rec` says, wide records at wide[row].
+struct RowApply {
+    const uint32_t* urow;
+    RowRecords rec;
+    float4* wide;
+    OptParams o;
+};
+
+// ---- per unique row: g = ordered sum of its occurrences' gradients.
+// Rows touched at most kChunk times are summed by one lane group directly.  Hotter rows (small tables, skewed ids) are split into
+// chunks of kChunk occurrences that are summed in parallel and then combined in chunk order (chunk_combine_kernel in sparse.cu),
+// so the result stays deterministic and no single group walks thousands of occurrences.  One launch covers both kinds of work
+// item: items [0, nu) are the unique rows (summed directly into ugrad unless they are hot), items [nu, nu + nchunks) are the
+// chunks of the hot rows (summed into cpart).
+
+// Where an occurrence's gradient comes from is the source's business (Src: LocalEmb / LocalWide in sparse.cu for the batch's own
+// lists, PeerEmb / PeerWide in shard.cu for the rows a rank owns).  key(j) is occurrence j of the sorted list; the rows of an item
+// all belong to one table, layout(key of its first occurrence) gives (t, dim, x0); row(key, x0, q) is float4 q of the
+// occurrence's gradient row and its bag scale inv (embedding), row(key) its dlogit (wide).  Keys are loaded four at a time, then
+// their rows, so that four gradient rows are in flight.
+// Embedding rows: 8 lanes per work item, each lane covers float4 chunks lig, lig + 8, ... of the row.  APPLY (single-GPU step,
+// row-local optimizer): a directly summed row is updated right after its sum — the summed gradient never reaches memory; the hot
+// rows are updated by chunk_combine_kernel<1>.
+template <class Src, bool APPLY>
+__global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ d_nchunks,
+                                                           const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff, Src src,
+                                                           float* __restrict__ ugrad, float* __restrict__ cpart, int width, RowApply ra) {
+    const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
+    const int nu = *d_nuniq;
+    const int64_t nitems = (int64_t)nu + *d_nchunks;
+    const int64_t g0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4 + grp;
+    const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
+    for (int64_t it = g0; it < nitems; it += gstep) {
+        int s, e;
+        float* out;
+        const bool direct = it < nu;
+        if (direct) {
+            s = ustart[it]; e = ustart[it + 1];
+            if (e - s > kChunk) continue;                     // hot row: summed chunk by chunk
+            out = ugrad + it * width;
+        } else {
+            const int c = (int)(it - nu);
+            const int u = chunk_owner(choff, nu, c);
+            s = ustart[u] + (c - choff[u]) * kChunk;
+            e = min(ustart[u + 1], s + kChunk);
+            out = cpart + (int64_t)c * width;
+        }
+        int t, dim, x0;
+        src.layout(src.key(s), t, dim, x0);
+        for (int q = lig; q * 4 < width; q += 8) {
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (q * 4 < dim) {
+                int j = s;
+                for (; j + 4 <= e; j += 4) {                  // 4 gradient rows in flight
+                    uint32_t k[4]; float4 v[4]; float inv[4];
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) k[r] = src.key(j + r);
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) v[r] = src.row(k[r], x0, q, inv[r]);
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) { acc.x += v[r].x * inv[r]; acc.y += v[r].y * inv[r]; acc.z += v[r].z * inv[r]; acc.w += v[r].w * inv[r]; }
+                }
+                for (; j < e; ++j) {
+                    float inv;
+                    const float4 v = src.row(src.key(j), x0, q, inv);
+                    acc.x += v.x * inv; acc.y += v.y * inv; acc.z += v.z * inv; acc.w += v.w * inv;
+                }
+            }
+            if (APPLY && direct) {
+                if (q * 4 < dim)
+                    update_record4(ra.o, record(ra.rec, t, ra.urow, it) + q * 4, dim, ra.rec.stride[t] / dim - 1, acc);
+            } else {
+                *reinterpret_cast<float4*>(out + q * 4) = acc;
+            }
+        }
+    }
+}
+
+// Wide rows: one thread per work item, items as in emb_grad_sum_kernel; APPLY: record {w, s1, s2, -} updated in place.
+template <class Src, bool APPLY>
+__global__ void wide_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ d_nchunks,
+                                     const int32_t* __restrict__ ustart, const int32_t* __restrict__ choff, Src src,
+                                     float* __restrict__ ugrad, float* __restrict__ cpart, RowApply ra) {
+    const int nu = *d_nuniq;
+    const int64_t nitems = (int64_t)nu + *d_nchunks;
+    for (int64_t it = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; it < nitems; it += (int64_t)gridDim.x * blockDim.x) {
+        int s, e;
+        const bool direct = it < nu;
+        if (direct) {
+            s = ustart[it]; e = ustart[it + 1];
+            if (e - s > kChunk) continue;
+        } else {
+            const int c = (int)(it - nu);
+            const int u = chunk_owner(choff, nu, c);
+            s = ustart[u] + (c - choff[u]) * kChunk;
+            e = min(ustart[u + 1], s + kChunk);
+        }
+        float acc = 0.f;
+        for (int j = s; j < e; ++j) acc += src.row(src.key(j));
+        if (!direct) cpart[it - nu] = acc;
+        else if (APPLY) update_wide(ra.o, ra.wide + ra.urow[it], acc);
+        else ugrad[it] = acc;
+    }
+}
+
 // ---- list machinery implemented in sparse.cu, used by shard.cu for the rows a rank owns
 // sort (row, occurrence) pairs of e_row[0 .. *d_n) by row, unique rows, segment starts, hot-row chunk layout -> list `which`
 int list_group(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row);
 int list_sort_by_key(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_key);
 // ugrad[u] = fixed-order sum of the chunk partials of multi-chunk rows (after the two gradient-sum passes)
 int list_chunk_combine(WdModel* m, int which, int width);
-// optimizer over the unique rows of list `which`: embedding tables given in row order / one wide record array.  d_stage (optional,
-// [ntab]): 0 = record in place, else the table is staged and the record of unique row u is at stage + u * d_stage[t]
-int list_apply_emb(WdModel* m, int which, int width, int ntab, const int64_t* d_row_base, float* const* d_data, const int32_t* d_dim,
-                   const int32_t* d_stride, const WdOptimizer& o, const int32_t* d_stage = nullptr, float* stage = nullptr);
+// optimizer over the unique rows of list `which`: embedding records as `rec` says (tables in row order) / one wide record array
+int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const WdOptimizer& o);
 int list_apply_wide(WdModel* m, int which, float4* wide, const WdOptimizer& o);
 
 }  // namespace wd
