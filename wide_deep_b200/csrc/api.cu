@@ -286,6 +286,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     if (m->use_wide) {
         add_dense(1, 1, m->row_tiles, 1, 4, false);            // [0] wide bias
         if ((rc = dev_alloc(m, &m->d_wide, m->wide_rows))) return rc;
+        if (m->lin_opt.kind == WD_OPT_ADAM && (rc = dev_alloc(m, &m->d_adam_touched[1], (m->wide_rows + 31) / 32))) return rc;
         if ((rc = dev_alloc(m, &m->d_wide_logit, Bm))) return rc;
     }
 
@@ -329,12 +330,12 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         }
         for (int t = 0; t < d->n_tables; ++t) h_row_base.push_back(m->tables[t].row_base);
         {
-            std::vector<int64_t> rb, go; std::vector<float*> dt; std::vector<int32_t> dm, st;
+            std::vector<int64_t> rb, go, nr; std::vector<float*> dt; std::vector<int32_t> dm, st;
             int64_t off = 0;
             for (int t : row_order) {
                 const EmbTable& tb = m->tables[t];
                 const bool small = m->dense_exchange_max_rows > 0 && tb.rows <= m->dense_exchange_max_rows;
-                rb.push_back(tb.row_base); dt.push_back(tb.data); dm.push_back(tb.dim); st.push_back(tb.stride);
+                rb.push_back(tb.row_base); nr.push_back(tb.rows); dt.push_back(tb.data); dm.push_back(tb.dim); st.push_back(tb.stride);
                 go.push_back(small ? off : -1);
                 if (small) off += tb.rows * tb.dim;
             }
@@ -343,12 +344,14 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             m->rtab_order = row_order;
             { const int64_t* t_; if ((rc = upload_vec(m, rb.data(), m->n_rtab, &t_))) return rc; m->d_rtab_row_base = (int64_t*)t_; }
             { const int64_t* t_; if ((rc = upload_vec(m, go.data(), m->n_rtab, &t_))) return rc; m->d_rtab_gs_off = (int64_t*)t_; }
+            { const int64_t* t_; if ((rc = upload_vec(m, nr.data(), m->n_rtab, &t_))) return rc; m->d_rtab_rows = (int64_t*)t_; }
             { float* const* t_; if ((rc = upload_vec<float*>(m, dt.data(), m->n_rtab, (float* const**)&t_))) return rc; m->d_rtab_data = (float**)t_; }
             { const int32_t* t_;
               if ((rc = upload_vec(m, dm.data(), m->n_rtab, &t_))) return rc; m->d_rtab_dim = (int32_t*)t_;
               if ((rc = upload_vec(m, st.data(), m->n_rtab, &t_))) return rc; m->d_rtab_stride = (int32_t*)t_; }
         }
         m->emb_total_rows = row_base;
+        if (m->dnn_opt.kind == WD_OPT_ADAM && (rc = dev_alloc(m, &m->d_adam_touched[0], (row_base + 31) / 32))) return rc;
         if (row_base >= (1ll << 31)) { set_error("more than 2^31 embedding rows on one device"); return WD_EUNSUPPORTED; }
         for (int i = 0; i < d->n_numeric; ++i) x->x0_real[d->num_x0_off[i]] = 1;
         for (int c = 0; c < C; ++c)
@@ -1131,10 +1134,16 @@ static int apply_core(WdModel* m) {
     stamp(m, ST_MAIN_END);
     if (m->dropout_rate > 0.f && (rc = step_tick(m))) return rc;          // the dropout counter advances once per train step
     if (m->lin_opt.kind == WD_OPT_ADAM || m->dnn_opt.kind == WD_OPT_ADAM) {
-        // AdamOptimizer._finish: beta powers advance once per step, after every variable of the optimizer has been updated (the
-        // sparse lists may still be running on their side streams and read the powers: join them first)
+        // Sparse Adam moves every row of a table each step, and each row exactly once (sparse_dev.cuh).  Per record set: first
+        // every touched-row update of the step, then the set's untouched pass, on the stream that ran the last of those updates.
+        // A replicated set is updated by its list (possibly on its side stream, after the data-parallel merge) and by the dense
+        // block (small_apply, here): join the lists, then its pass runs here.  A row-sharded set is updated only by its owner,
+        // whose pass follows on the owner's stream (shard.cu), which has joined this one by now.  AdamOptimizer._finish: the beta
+        // powers advance once per step, after all of that.
         for (int w = 0; w < 2; ++w)
             if (m->side_active[w]) WD_CUDA(cudaStreamWaitEvent(m->stream, m->ev_done[w], 0));
+        if ((rc = adam_untouched_replicated(m))) return rc;
+        mark(m, "adam_untouched");
         if ((rc = adam_tick(m))) return rc;
     }
     for (int w = 0; w < 2; ++w)

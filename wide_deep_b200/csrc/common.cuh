@@ -224,6 +224,8 @@ struct ShardSpace {           // one sharded table space on this rank: 0 = embed
     int64_t* d_slot_base = nullptr;    // [n_slots] first local row of the slot's shard
     int32_t *d_slot_dim = nullptr, *d_slot_x0 = nullptr, *d_slot_stride = nullptr;
     float** d_slot_data = nullptr;     // [n_slots] shard of the table (embedding space)
+    int64_t* d_slot_rows = nullptr;    // [n_slots] rows of the slot's shard on this rank (embedding space)
+    uint32_t* d_adam_touched = nullptr;   // Adam: [ceil(local_rows / 32)] bit r: local row r was updated this step (sparse_dev.cuh)
     // host-placed shards (embedding space): the owner stages the records of the step's unique owned host rows (list 2) in HBM
     int stage_stride = 0;              // widest stride of the space's host slots; 0: every shard in HBM
     int32_t* d_slot_stage = nullptr;   // [n_slots] 0: HBM slot; stage_stride: record of unique row u at d_stage + u * stage_stride
@@ -311,6 +313,10 @@ struct WdModel {
     float** d_rtab_data = nullptr;
     int32_t *d_rtab_dim = nullptr, *d_rtab_stride = nullptr;
     int64_t* d_rtab_gs_off = nullptr;        // [n_rtab] float offset inside the block (-1: large table)
+    int64_t* d_rtab_rows = nullptr;          // [n_rtab] rows
+    // Adam: bitmaps of the replicated record sets (0: embedding rows, emb_total_rows bits; 1: wide rows, wide_rows bits), bit r set
+    // when row r was updated this step, cleared by the set's untouched pass (sparse_dev.cuh); null unless that optimizer is Adam
+    uint32_t* d_adam_touched[2] = {nullptr, nullptr};
     int32_t* d_nubig[2] = {nullptr, nullptr};   // unique rows below small_base (what stays in the list)
     wd::ShardState shard;                    // row-sharded tables (world == 1: unused)
     wd::DevPlan dplan{};
@@ -465,12 +471,13 @@ int sparse_forward_emb(WdModel* m);                              //   the deep h
 int sparse_group(WdModel* m);                                    // sparse.cu: sort (row, occurrence) pairs, unique rows, chunks
 int sparse_reduce_emb(WdModel* m);                               // sparse.cu: per-row gradient sums (needs dX0)
 int sparse_reduce_wide(WdModel* m);                              // sparse.cu: per-row gradient sums (needs dlogit only)
-int sparse_apply(WdModel* m);                                    // sparse.cu: Adagrad / FTRL / SGD on touched rows (both lists)
+int sparse_apply(WdModel* m);                                    // sparse.cu: optimizer on the touched rows (both lists)
 int sparse_apply_which(WdModel* m, int which);                   // sparse.cu: one list (0 = embedding rows, 1 = wide rows)
 int sparse_group_which(WdModel* m, int which);                   // sparse.cu: grouping of one list
 int merge_sparse_sorted(WdModel* m, int which, const void* rows, const void* grads, int n_lists, int64_t list_len);   // sparse.cu
 int small_scatter(WdModel* m, int which);                        // sparse.cu: small-table rows of list `which` -> dense block
 int small_apply(WdModel* m);                                     // sparse.cu: optimizer over the dense block (after its all-reduce)
+int adam_untouched_replicated(WdModel* m);                       // sparse.cu: Adam rows of the replicated tables no update touched this step
 int mlp_forward(WdModel* m, bool want_transposes);               // mlp.cu: towers -> logits, loss
 int mlp_backward(WdModel* m);                                    // mlp.cu: grads of dense params, dX0
 int dense_reduce_grads(WdModel* m);                              // mlp.cu

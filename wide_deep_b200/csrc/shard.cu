@@ -359,14 +359,14 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     {
         ShardSpace& sp = S.sp[0];
         std::vector<int32_t> col_slot(C, -1), dim, x0, stride, host;
-        std::vector<int64_t> base;
+        std::vector<int64_t> base, srows;
         std::vector<float*> data;
         int64_t rows = 0;
         for (size_t t = 0; t < m->tables.size(); ++t) {
             EmbTable& tb = m->tables[t];
             if (!tb.sharded) continue;
             col_slot[tb.col] = sp.n_slots++;
-            base.push_back(rows); dim.push_back(tb.dim); x0.push_back(tb.x0_off); stride.push_back(tb.stride); data.push_back(tb.data);
+            base.push_back(rows); srows.push_back(tb.arows); dim.push_back(tb.dim); x0.push_back(tb.x0_off); stride.push_back(tb.stride); data.push_back(tb.data);
             host.push_back(tb.host);
             if (tb.host) sp.stage_stride = std::max(sp.stage_stride, tb.stride);
             tb.row_base = rows;
@@ -384,6 +384,7 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
             if ((rc = upload_arr(m, x0, &sp.d_slot_x0))) return rc;
             if ((rc = upload_arr(m, stride, &sp.d_slot_stride))) return rc;
             if ((rc = upload_arr(m, data, &sp.d_slot_data))) return rc;
+            if ((rc = upload_arr(m, srows, &sp.d_slot_rows))) return rc;
         }
         if (sp.stage_stride > 0) {               // host-placed shards: staging rows of the step's unique owned rows (+1: see the serve)
             for (int32_t& h : host) h = h ? sp.stage_stride : 0;
@@ -415,6 +416,9 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
             if ((rc = dev_alloc(m, &sp.d_wide, rows))) return rc;
         }
     }
+    for (int s = 0; s < 2; ++s)
+        if (S.sp[s].on && (s == 0 ? m->dnn_opt : m->lin_opt).kind == WD_OPT_ADAM &&
+            (rc = dev_alloc(m, &S.sp[s].d_adam_touched, (S.sp[s].local_rows + 31) / 32))) return rc;
     for (int s = 0; s < 2; ++s)
         if (S.sp[s].local_rows >= (1ll << 30)) { set_error("more than 2^30 sharded rows per rank in one table space"); return WD_EUNSUPPORTED; }
     // ---- per-space scratch (requester + owner) and the sort lists 2 + s (owned rows) / 4 + s (routing)
@@ -664,7 +668,10 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
         m->launches++;
         if ((rc = list_chunk_combine(m, L, sp.width))) return rc;
         const RowRecords rec{sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, nullptr};
-        if ((rc = list_apply_emb(m, L, sp.width, rec, m->dnn_opt))) return rc;
+        const OptParams o = space_opt(m, 0, sp.d_adam_touched);
+        if ((rc = list_apply_emb(m, L, sp.width, rec, o))) return rc;
+        // Adam: the shard's rows no rank touched, after its touched ones (no host-placed shards with Adam: no staged records)
+        if ((rc = adam_untouched_emb(m, rec, sp.d_slot_rows, sp.local_rows, o))) return rc;
         // staged records home, on this stream: it joins the main stream before the step ends, so the next stage-in comes after
         if (staged(m, s) && (rc = host_rows_transfer(m, false, m->d_nuniq[L], m->d_urow[L], sp.n_slots, sp.d_slot_base, sp.d_slot_data,
                                                      sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, sp.stage_stride))) return rc;
@@ -674,7 +681,9 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
             m->d_ustart[L], m->d_choff[L], src, m->d_ugrad[L], m->d_cpart[L], RowApply{});
         m->launches++;
         if ((rc = list_chunk_combine(m, L, 1))) return rc;
-        if ((rc = list_apply_wide(m, L, sp.d_wide, m->lin_opt))) return rc;
+        const OptParams o = space_opt(m, 1, sp.d_adam_touched);
+        if ((rc = list_apply_wide(m, L, sp.d_wide, o))) return rc;
+        if ((rc = adam_untouched_wide(m, sp.d_wide, sp.local_rows, o))) return rc;
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;

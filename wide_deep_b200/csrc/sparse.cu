@@ -334,7 +334,8 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
 
 // embedding rows: record = [w[dim] | s1[dim] | s2[dim]], tables of rr in row order
 __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow,
-                                                        const float* __restrict__ ugrad, int width, RowRecords rr, OptParams o) {
+                                                        const float* __restrict__ ugrad, int width, RowRecords rr, OptParams op) {
+    const OptParams o = with_lr_t(op);
     const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
     const int nu = *d_nuniq;
     const int64_t g0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4 + grp;
@@ -346,14 +347,59 @@ __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restric
         float* rec = record(rr, t, urow, u);
         for (int q = lig; q * 4 < dim; q += 8)
             update_record4(o, rec + q * 4, dim, nslots, *reinterpret_cast<const float4*>(ugrad + (int64_t)u * width + q * 4));
+        if (lig == 0) mark_touched(o, row);
     }
 }
 
 // wide rows: record {w, s1, s2, -}; also the bias record (dense gradient = sum of dlogit)
 __global__ void wide_apply_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow,
-                                  const float* __restrict__ ugrad, float4* __restrict__ wide, OptParams o) {
+                                  const float* __restrict__ ugrad, float4* __restrict__ wide, OptParams op) {
+    const OptParams o = with_lr_t(op);
     const int nu = *d_nuniq;
-    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) update_wide(o, wide + urow[u], ugrad[u]);
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) {
+        update_wide(o, wide + urow[u], ugrad[u]);
+        mark_touched(o, urow[u]);
+    }
+}
+
+// Adam, untouched pass over the embedding records of one set (adam_untouched_emb): one warp per 32-bit word of the bitmap, i.e. per
+// 32 rows; lane groups of 8 take rows grp, grp + 4, ..., each lane float4 chunks lig, lig + 8, ... of the row.  The warp clears the
+// word once every row of it has read its bit.
+__global__ void __launch_bounds__(256) adam_untouched_emb_kernel(RowRecords rr, const int64_t* __restrict__ rows, int64_t nbits, OptParams op) {
+    const OptParams o = with_lr_t(op);
+    const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
+    const int64_t nwords = (nbits + 31) >> 5;
+    for (int64_t wd = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; wd < nwords; wd += ((int64_t)gridDim.x * blockDim.x) >> 5) {
+        const uint32_t bits = o.touched[wd];
+        for (int k = grp; k < 32; k += 4) {
+            const int64_t row = wd * 32 + k;
+            if (row >= nbits || ((bits >> k) & 1u)) continue;
+            const int t = table_of(rr.row_base, rr.ntab, row);
+            const int64_t local = row - rr.row_base[t];
+            if (local >= rows[t]) continue;                        // (a row-sharded space: past this rank's share of table t)
+            const int dim = rr.dim[t];
+            float* rec = rr.data[t] + local * rr.stride[t];
+            for (int q = lig; q * 4 < dim; q += 8) adam_untouched4(o, rec + q * 4, dim);
+        }
+        __syncwarp();
+        if (lane == 0 && bits) o.touched[wd] = 0u;
+    }
+}
+// ... over the wide records {w, m, v, -}: one thread per row, a warp per word
+__global__ void __launch_bounds__(256) adam_untouched_wide_kernel(float4* __restrict__ wide, int64_t nbits, OptParams op) {
+    const OptParams o = with_lr_t(op);
+    const int64_t npad = (nbits + 31) & ~(int64_t)31;              // warp-uniform trip count
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < npad; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t bits = o.touched[i >> 5];
+        if (i < nbits && !((bits >> (i & 31)) & 1u)) {
+            float4 r = wide[i];
+            adam_decay(o, r.y, r.z);
+            adam_step(o, r.x, r.y, r.z);
+            wide[i] = r;
+        }
+        __syncwarp();
+        if ((i & 31) == 0 && bits) o.touched[i >> 5] = 0u;
+    }
 }
 
 
@@ -608,7 +654,8 @@ int small_scatter(WdModel* m, int which) {
 __global__ void __launch_bounds__(256) small_apply_emb_kernel(const float* __restrict__ Gs, const float* __restrict__ touched, int64_t n4, int ntab,
                                                               int first_small, int64_t small_base, const int64_t* __restrict__ rtab_row_base,
                                                               const int64_t* __restrict__ rtab_gs_off, float* const* __restrict__ rtab_data,
-                                                              const int32_t* __restrict__ rtab_dim, const int32_t* __restrict__ rtab_stride, OptParams o) {
+                                                              const int32_t* __restrict__ rtab_dim, const int32_t* __restrict__ rtab_stride, OptParams op) {
+    const OptParams o = with_lr_t(op);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
         // small tables are the last entries, offsets ascending
         const int t = first_small + table_of(rtab_gs_off + first_small, ntab - first_small, i * 4);
@@ -617,13 +664,17 @@ __global__ void __launch_bounds__(256) small_apply_emb_kernel(const float* __res
         if (touched[rtab_row_base[t] - small_base + local / dim] == 0.f) continue;
         const float4 g = *reinterpret_cast<const float4*>(Gs + i * 4);
         update_record4(o, rtab_data[t] + (local / dim) * stride + (local % dim), dim, stride / dim - 1, g);
+        if (local % dim == 0) mark_touched(o, rtab_row_base[t] + local / dim);
     }
 }
+// (wide: the small wide rows from global row row0)
 __global__ void __launch_bounds__(256) small_apply_wide_kernel(const float* __restrict__ Gs, const float* __restrict__ touched, int64_t n,
-                                                               float4* __restrict__ wide, OptParams o) {
+                                                               float4* __restrict__ wide, int64_t row0, OptParams op) {
+    const OptParams o = with_lr_t(op);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         if (touched[i] == 0.f) continue;
-        update_wide(o, wide + i, Gs[i]);
+        update_wide(o, wide + row0 + i, Gs[i]);
+        mark_touched(o, row0 + i);
     }
 }
 int small_apply(WdModel* m) {
@@ -632,52 +683,27 @@ int small_apply(WdModel* m) {
     if (m->gs_emb_floats > 0) {
         small_apply_emb_kernel<<<grid_for(m->gs_emb_floats / 4, 256), 256, 0, m->stream>>>(block, block + m->gs_touch_off[0], m->gs_emb_floats / 4, m->n_rtab,
             m->n_rtab - m->n_small_tab, m->small_base[0], m->d_rtab_row_base, m->d_rtab_gs_off, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride,
-            make_opt(m->dnn_opt));
+            space_opt(m, 0, m->d_adam_touched[0]));
         m->launches++;
     }
     const int64_t nw = m->use_wide ? m->wide_rows - m->small_base[1] : 0;
     if (nw > 0) {
         small_apply_wide_kernel<<<grid_for(nw, 256), 256, 0, m->stream>>>(block + m->gs_emb_floats, block + m->gs_touch_off[1], nw,
-            reinterpret_cast<float4*>(m->d_wide) + m->small_base[1], make_opt(m->lin_opt));
+            m->d_wide, m->small_base[1], space_opt(m, 1, m->d_adam_touched[1]));
         m->launches++;
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 
-// ---- sparse Adam (tf.train.AdamOptimizer on IndexedSlices, AdamOptimizer._apply_sparse_shared): m *= beta1, v *= beta2 over the
-// WHOLE variable, scatter-add of the summed gradients (opt_update's Adam branch, touched rows), then every row moves by
-// lr_t * m / (sqrt(v) + eps) with lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t).  Record layout [w | m | v]; bpow = {beta1^t, beta2^t}.
-__global__ void __launch_bounds__(256) adam_decay_kernel(float* __restrict__ data, int64_t rows, int dim, int stride, float b1, float b2) {
-    const int64_t total = rows * dim;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        float* rec = data + (i / dim) * stride + (i % dim);
-        rec[dim] *= b1;
-        rec[2 * dim] *= b2;
-    }
+OptParams space_opt(const WdModel* m, int space, uint32_t* touched) {
+    const WdOptimizer& o = space == 0 ? m->dnn_opt : m->lin_opt;
+    const bool adam = o.kind == WD_OPT_ADAM;
+    return make_opt(o, adam ? m->d_bpow + (space == 0 ? 2 : 0) : nullptr, adam ? touched : nullptr);
 }
-__global__ void __launch_bounds__(256) adam_step_kernel(float* __restrict__ data, int64_t rows, int dim, int stride, float lr, float eps,
-                                                       const float* __restrict__ bpow) {
-    const int64_t total = rows * dim;
-    const float lr_t = lr * sqrtf(1.f - bpow[1]) / (1.f - bpow[0]);
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        float* rec = data + (i / dim) * stride + (i % dim);
-        rec[0] -= lr_t * rec[dim] / (sqrtf(rec[2 * dim]) + eps);
-    }
-}
-static int adam_dense_pass(WdModel* m, int which, bool step) {
-    const WdOptimizer& o = which == 0 ? m->dnn_opt : m->lin_opt;
-    const float* bpow = m->d_bpow + (which == 0 ? 2 : 0);
-    auto run = [&](float* data, int64_t rows, int dim, int stride) {
-        if (rows <= 0) return;
-        if (!step) adam_decay_kernel<<<grid_for(rows * dim, 256), 256, 0, m->stream>>>(data, rows, dim, stride, o.beta1, o.beta2);
-        else adam_step_kernel<<<grid_for(rows * dim, 256), 256, 0, m->stream>>>(data, rows, dim, stride, o.lr, o.epsilon, bpow);
-        m->launches++;
-    };
-    if (which == 0) { for (auto& tb : m->tables) run(tb.data, tb.arows, tb.dim, tb.stride); }
-    else run(reinterpret_cast<float*>(m->d_wide), m->wide_rows, 1, 4);          // wide record {w, m, v, -}
-    WD_CUDA(cudaGetLastError());
-    return WD_OK;
+// the replicated tables' records in row order, in place (the unfused updates write host records through their mapped pointers)
+static RowRecords replicated_records(const WdModel* m) {
+    return RowRecords{m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride, nullptr, nullptr, nullptr};
 }
 
 int sparse_apply_which(WdModel* m, int which) {
@@ -692,19 +718,9 @@ int sparse_apply_which(WdModel* m, int which) {
         set_error("embedding rows of a model with a host-table cache are only updated by the fused single-GPU step");
         return WD_EUNSUPPORTED;
     }
-    if (which == 0 && m->use_deep && !m->tables.empty()) {
-        const bool adam = m->dnn_opt.kind == WD_OPT_ADAM;
-        if (adam && (rc = adam_dense_pass(m, 0, false))) return rc;
-        const RowRecords rec{m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride, nullptr, nullptr, nullptr};
-        if ((rc = list_apply_emb(m, 0, m->emb_max_dim, rec, m->dnn_opt))) return rc;
-        if (adam && (rc = adam_dense_pass(m, 0, true))) return rc;
-    }
-    if (which == 1 && m->use_wide) {
-        const bool adam = m->lin_opt.kind == WD_OPT_ADAM;
-        if (adam && (rc = adam_dense_pass(m, 1, false))) return rc;
-        if ((rc = list_apply_wide(m, 1, m->d_wide, m->lin_opt))) return rc;
-        if (adam && (rc = adam_dense_pass(m, 1, true))) return rc;
-    }
+    if (which == 0 && m->use_deep && !m->tables.empty() && (rc = list_apply_emb(m, 0, m->emb_max_dim, replicated_records(m), space_opt(m, 0, m->d_adam_touched[0]))))
+        return rc;
+    if (which == 1 && m->use_wide && (rc = list_apply_wide(m, 1, m->d_wide, space_opt(m, 1, m->d_adam_touched[1])))) return rc;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
@@ -728,18 +744,38 @@ int list_chunk_combine(WdModel* m, int which, int width) {
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const WdOptimizer& o) {
-    emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], width, rec,
-                                                                            make_opt(o));
+int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const OptParams& o) {
+    emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], width, rec, o);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int list_apply_wide(WdModel* m, int which, float4* wide, const WdOptimizer& o) {
-    wide_apply_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], wide, make_opt(o));
+int list_apply_wide(WdModel* m, int which, float4* wide, const OptParams& o) {
+    wide_apply_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], wide, o);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
+}
+int adam_untouched_emb(WdModel* m, const RowRecords& rec, const int64_t* rows, int64_t nbits, const OptParams& o) {
+    if (o.kind != WD_OPT_ADAM || rec.ntab == 0 || nbits <= 0) return WD_OK;
+    adam_untouched_emb_kernel<<<grid_for(nbits, 256), 256, 0, m->stream>>>(rec, rows, nbits, o);    // (a warp per 32 rows)
+    m->launches++;
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+int adam_untouched_wide(WdModel* m, float4* wide, int64_t nbits, const OptParams& o) {
+    if (o.kind != WD_OPT_ADAM || nbits <= 0) return WD_OK;
+    adam_untouched_wide_kernel<<<grid_for(nbits, 256), 256, 0, m->stream>>>(wide, nbits, o);
+    m->launches++;
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+// Adam, the untouched passes of the replicated record sets: after both their lists and the dense block's small-table rows
+int adam_untouched_replicated(WdModel* m) {
+    int rc;
+    if (m->use_deep && (rc = adam_untouched_emb(m, replicated_records(m), m->d_rtab_rows, m->emb_total_rows, space_opt(m, 0, m->d_adam_touched[0]))))
+        return rc;
+    return m->use_wide ? adam_untouched_wide(m, m->d_wide, m->wide_rows, space_opt(m, 1, m->d_adam_touched[1])) : WD_OK;
 }
 
 int sparse_apply(WdModel* m) {

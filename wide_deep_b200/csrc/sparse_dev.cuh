@@ -51,8 +51,23 @@ __device__ __forceinline__ int table_of(const int64_t* __restrict__ base, int n,
     return lo;
 }
 
-struct OptParams { int kind; float lr, l1, l2, init_acc, beta1, beta2, epsilon, rho, momentum; };
-inline OptParams make_opt(const WdOptimizer& o) { return OptParams{o.kind, o.lr, o.l1, o.l2, o.init_acc, o.beta1, o.beta2, o.epsilon, o.rho, o.momentum}; }
+// Adam also carries its device beta powers bpow = {beta1^t, beta2^t} (step size lr_t: with_lr_t) and `touched`, the bitmap of the
+// record set being updated (bit r: row r of the set was updated this step; adam_untouched_* moves the others and clears it).
+struct OptParams {
+    int kind; float lr, l1, l2, init_acc, beta1, beta2, epsilon, rho, momentum;
+    const float* bpow; uint32_t* touched; float lr_t;
+};
+inline OptParams make_opt(const WdOptimizer& o, const float* bpow = nullptr, uint32_t* touched = nullptr) {
+    return OptParams{o.kind, o.lr, o.l1, o.l2, o.init_acc, o.beta1, o.beta2, o.epsilon, o.rho, o.momentum, bpow, touched, 0.f};
+}
+// Adam: lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t) of this step, read once per thread
+__device__ __forceinline__ OptParams with_lr_t(OptParams o) {
+    if (o.kind == WD_OPT_ADAM) o.lr_t = o.lr * sqrtf(1.f - o.bpow[1]) / (1.f - o.bpow[0]);
+    return o;
+}
+__device__ __forceinline__ void mark_touched(const OptParams& o, int64_t row) {
+    if (o.touched) atomicOr(o.touched + (row >> 5), 1u << (row & 31));
+}
 // initial value of optimizer slot 1 (Adagrad accumulator / FTRL n / Adam m / RMSProp rms); slot 2 always starts at 0
 inline float slot1_init(const WdOptimizer& o) {
     if (o.kind == WD_OPT_ADAGRAD || o.kind == WD_OPT_FTRL) return o.init_acc;
@@ -60,10 +75,18 @@ inline float slot1_init(const WdOptimizer& o) {
 }
 inline int opt_nslots(const WdOptimizer& o) { return o.kind == WD_OPT_SGD ? 0 : (o.kind == WD_OPT_ADAGRAD ? 1 : 2); }
 
+// Sparse Adam (tf.train.AdamOptimizer on IndexedSlices, AdamOptimizer._apply_sparse_shared) decays m and v over the WHOLE variable,
+// scatter-adds the summed gradients of the touched rows, then moves EVERY row by lr_t * m / (sqrt(v) + eps).  A touched row does all
+// three in opt_update, a row nobody touched the decay and the step in adam_untouched4: one read and one write of each record.  The
+// decay is rounded on its own (__fmul_rn: never contracted into the scatter-add's multiply-add), so either way the row gets exactly
+// the values of three separate passes.
+__device__ __forceinline__ void adam_decay(const OptParams& o, float& m, float& v) {
+    m = __fmul_rn(m, o.beta1);
+    v = __fmul_rn(v, o.beta2);
+}
+__device__ __forceinline__ void adam_step(const OptParams& o, float& w, float m, float v) { w -= o.lr_t * m / (sqrtf(v) + o.epsilon); }
+
 // One update of a TOUCHED row element from its summed gradient g (duplicates already summed: "sum duplicates, apply once").
-// Adam is the exception: TensorFlow's sparse Adam decays m and v over the whole variable and moves every row each step
-// (AdamOptimizer._apply_sparse_shared), so here the touched rows only receive the scatter-add of (1 - beta) * g terms; the decay
-// before it and the step after it are dense passes over the table (adam_decay_kernel / adam_step_kernel in sparse.cu).
 __device__ __forceinline__ void opt_update(const OptParams& o, float g, float& w, float& s1, float& s2) {
     if (o.kind == WD_OPT_ADAGRAD) {                 // tf.train.AdagradOptimizer: acc += g^2; w -= lr*g/sqrt(acc)
         s1 += g * g;
@@ -78,9 +101,11 @@ __device__ __forceinline__ void opt_update(const OptParams& o, float g, float& w
         s1 += (g * g - s1) * (1.f - o.rho);
         s2 = s2 * o.momentum + (g * o.lr) / sqrtf(s1 + o.epsilon);
         w -= s2;
-    } else if (o.kind == WD_OPT_ADAM) {             // scatter-add stage of sparse Adam
+    } else if (o.kind == WD_OPT_ADAM) {             // sparse Adam: decay, scatter-add, step (o.lr_t: with_lr_t)
+        adam_decay(o, s1, s2);
         s1 += g * (1.f - o.beta1);
         s2 += g * g * (1.f - o.beta2);
+        adam_step(o, w, s1, s2);
     } else {
         w -= o.lr * g;
     }
@@ -98,6 +123,19 @@ __device__ __forceinline__ void update_record4(const OptParams& o, float* w, int
     *reinterpret_cast<float4*>(w) = x;
     if (nslots >= 1) *reinterpret_cast<float4*>(w + gap) = s1;
     if (nslots >= 2) *reinterpret_cast<float4*>(w + 2 * gap) = s2;
+}
+// Adam on four consecutive elements of an embedding record [w | m | v] that no gradient touched this step.
+__device__ __forceinline__ void adam_untouched4(const OptParams& o, float* w, int gap) {
+    float4 x = *reinterpret_cast<float4*>(w);
+    float4 m = *reinterpret_cast<float4*>(w + gap);
+    float4 v = *reinterpret_cast<float4*>(w + 2 * gap);
+    adam_decay(o, m.x, v.x); adam_step(o, x.x, m.x, v.x);
+    adam_decay(o, m.y, v.y); adam_step(o, x.y, m.y, v.y);
+    adam_decay(o, m.z, v.z); adam_step(o, x.z, m.z, v.z);
+    adam_decay(o, m.w, v.w); adam_step(o, x.w, m.w, v.w);
+    *reinterpret_cast<float4*>(w) = x;
+    *reinterpret_cast<float4*>(w + gap) = m;
+    *reinterpret_cast<float4*>(w + 2 * gap) = v;
 }
 // One update of a wide record {w, s1, s2, -}.
 __device__ __forceinline__ void update_wide(const OptParams& o, float4* rec, float g) {
@@ -241,7 +279,15 @@ int list_sort_by_key(WdModel* m, int which, const int32_t* d_n, const uint32_t* 
 // ugrad[u] = fixed-order sum of the chunk partials of multi-chunk rows (after the two gradient-sum passes)
 int list_chunk_combine(WdModel* m, int which, int width);
 // optimizer over the unique rows of list `which`: embedding records as `rec` says (tables in row order) / one wide record array
-int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const WdOptimizer& o);
-int list_apply_wide(WdModel* m, int which, float4* wide, const WdOptimizer& o);
+int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const OptParams& o);
+int list_apply_wide(WdModel* m, int which, float4* wide, const OptParams& o);
+// the optimizer of table space `space` (0 embedding rows: dnn_optimizer, 1 wide rows: linear_optimizer); Adam: with its beta powers
+// and the bitmap `touched` of the record set it updates
+OptParams space_opt(const WdModel* m, int space, uint32_t* touched);
+// Adam, the untouched pass of one record set (after every touched-row update of the step, on the stream that ran the last of
+// them): decay + step of every row whose bit in o.touched is clear, all bits cleared.  Embedding records as `rec` says (no staged
+// tables), table t holding rows[t] rows from row_base[t], bits 0 .. nbits; wide records wide[0 .. nbits).  Nothing unless o is Adam.
+int adam_untouched_emb(WdModel* m, const RowRecords& rec, const int64_t* rows, int64_t nbits, const OptParams& o);
+int adam_untouched_wide(WdModel* m, float4* wide, int64_t nbits, const OptParams& o);
 
 }  // namespace wd

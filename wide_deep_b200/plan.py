@@ -362,9 +362,6 @@ class Plan(object):
         self.dnn_opt = parse_optimizer(model_conf.get("dnn_optimizer") or "Adagrad",
                                        model_conf.get("dnn_initial_learning_rate") or 0.001)
 
-        if self.dense_exchange_max_rows > 0 and (self.dnn_opt["kind"] in ("adam", "rmsprop") or self.lin_opt["kind"] in ("adam", "rmsprop")):
-            raise ValueError("Adam / RMSProp are single-GPU only here (the multi-GPU paths implement Adagrad, Ftrl and SGD: sparse Adam "
-                             "decays its moments over whole tables every step)")
         # ---- tensor names (TensorFlow variable names of the reference's checkpoint)
         T = self.tensor_names = OrderedDict()
         for c in self.wide_columns:
