@@ -45,16 +45,6 @@ static int bits_for(int64_t n) {
     return b;
 }
 
-template <typename T>
-static int upload_vec(WdModel* m, const T* src, int64_t n, const T** dst) {
-    T* p = nullptr;
-    int rc = dev_alloc(m, &p, n, true);
-    if (rc) return rc;
-    if (n > 0) WD_CUDA(cudaMemcpyAsync(p, src, n * sizeof(T), cudaMemcpyHostToDevice, m->stream));
-    *dst = p;
-    return WD_OK;
-}
-
 // sources of each layer input, in concat order (reference dnn.py:92-193); -1 = deep input x
 static std::vector<std::vector<int>> layer_sources(int mode, int L) {
     std::vector<std::vector<int>> out;
@@ -206,31 +196,27 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     // ---- plan tables on the device
     DevPlan& p = m->dplan;
     p.n_cat_fields = d->n_cat_fields; p.n_dense_fields = d->n_dense_fields; p.n_columns = C; p.d0_phys = d->d0_phys;
-    if ((rc = upload_vec(m, d->cat_field_is_string, d->n_cat_fields, &p.field_is_string))) return rc;
-    if ((rc = upload_vec(m, d->col_kind, C, &p.col_kind))) return rc;
-    if ((rc = upload_vec(m, d->col_field, C, &p.col_field))) return rc;
-    if ((rc = upload_vec(m, d->col_buckets, C, &p.col_buckets))) return rc;
-    if ((rc = upload_vec(m, d->col_aux_off, C, &p.col_aux_off))) return rc;
-    if ((rc = upload_vec(m, d->col_aux_n, C, &p.col_aux_n))) return rc;
-    if ((rc = upload_vec(m, d->col_norm_kind, C, &p.col_norm_kind))) return rc;
-    if ((rc = upload_vec(m, d->col_norm_a, C, &p.col_norm_a))) return rc;
-    if ((rc = upload_vec(m, d->col_norm_b, C, &p.col_norm_b))) return rc;
-    if ((rc = upload_vec(m, d->col_wide_base, C, &p.col_wide_base))) return rc;
-    if ((rc = upload_vec(m, d->col_emb_table, C, &p.col_emb_table))) return rc;
-    if ((rc = upload_vec(m, d->col_ind_off, C, &p.col_ind_off))) return rc;
-    if ((rc = upload_vec(m, d->vocab_fp, d->n_vocab_fp, &p.vocab_fp))) return rc;
-    if ((rc = upload_vec(m, d->boundaries, d->n_boundaries, &p.boundaries))) return rc;
-    if ((rc = upload_vec(m, d->cross_key_type, d->n_cross_keys, &p.cross_key_type))) return rc;
-    if ((rc = upload_vec(m, d->cross_key_idx, d->n_cross_keys, &p.cross_key_idx))) return rc;
-    {
-        const int32_t* t;
-        const float* f;
-        if ((rc = upload_vec(m, d->num_field, d->n_numeric, &t))) return rc; m->d_num_field = (int32_t*)t;
-        if ((rc = upload_vec(m, d->num_norm_kind, d->n_numeric, &t))) return rc; m->d_num_norm_kind = (int32_t*)t;
-        if ((rc = upload_vec(m, d->num_x0_off, d->n_numeric, &t))) return rc; m->d_num_x0_off = (int32_t*)t;
-        if ((rc = upload_vec(m, d->num_norm_a, d->n_numeric, &f))) return rc; m->d_num_a = (float*)f;
-        if ((rc = upload_vec(m, d->num_norm_b, d->n_numeric, &f))) return rc; m->d_num_b = (float*)f;
-    }
+    if ((rc = upload(m, &p.field_is_string, d->cat_field_is_string, d->n_cat_fields))) return rc;
+    if ((rc = upload(m, &p.col_kind, d->col_kind, C))) return rc;
+    if ((rc = upload(m, &p.col_field, d->col_field, C))) return rc;
+    if ((rc = upload(m, &p.col_buckets, d->col_buckets, C))) return rc;
+    if ((rc = upload(m, &p.col_aux_off, d->col_aux_off, C))) return rc;
+    if ((rc = upload(m, &p.col_aux_n, d->col_aux_n, C))) return rc;
+    if ((rc = upload(m, &p.col_norm_kind, d->col_norm_kind, C))) return rc;
+    if ((rc = upload(m, &p.col_norm_a, d->col_norm_a, C))) return rc;
+    if ((rc = upload(m, &p.col_norm_b, d->col_norm_b, C))) return rc;
+    if ((rc = upload(m, &p.col_wide_base, d->col_wide_base, C))) return rc;
+    if ((rc = upload(m, &p.col_emb_table, d->col_emb_table, C))) return rc;
+    if ((rc = upload(m, &p.col_ind_off, d->col_ind_off, C))) return rc;
+    if ((rc = upload(m, &p.vocab_fp, d->vocab_fp, d->n_vocab_fp))) return rc;
+    if ((rc = upload(m, &p.boundaries, d->boundaries, d->n_boundaries))) return rc;
+    if ((rc = upload(m, &p.cross_key_type, d->cross_key_type, d->n_cross_keys))) return rc;
+    if ((rc = upload(m, &p.cross_key_idx, d->cross_key_idx, d->n_cross_keys))) return rc;
+    if ((rc = upload(m, &m->d_num_field, d->num_field, d->n_numeric))) return rc;
+    if ((rc = upload(m, &m->d_num_norm_kind, d->num_norm_kind, d->n_numeric))) return rc;
+    if ((rc = upload(m, &m->d_num_x0_off, d->num_x0_off, d->n_numeric))) return rc;
+    if ((rc = upload(m, &m->d_num_a, d->num_norm_a, d->n_numeric))) return rc;
+    if ((rc = upload(m, &m->d_num_b, d->num_norm_b, d->n_numeric))) return rc;
 
     // ---- batch buffers
     const int64_t Bm = m->max_batch;
@@ -294,14 +280,13 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     x->x0_real.assign(std::max(d->d0_phys, 1), 0);
     if (m->use_deep) {
         int64_t row_base = 0;
-        std::vector<int64_t> h_row_base;
         const int nslots = opt_nslots(m->dnn_opt);
         for (int t = 0; t < d->n_tables; ++t) {
             EmbTable tb{};
             tb.rows = d->table_rows[t]; tb.dim = d->table_dim[t]; tb.x0_off = d->table_x0_off[t];
             tb.dim_logical = d->table_dim_logical[t];
             if (tb.dim_logical < 1 || tb.dim_logical > tb.dim) { set_error("table %d: bad logical width", t); return WD_EINVAL; }
-            tb.row_base = 0; tb.stride = tb.dim * (1 + nslots); tb.col = -1;
+            tb.row_base = 0; tb.gs_off = -1; tb.stride = tb.dim * (1 + nslots); tb.col = -1;
             tb.sharded = G > 1 && d->table_sharded && d->table_sharded[t];
             tb.arows = tb.sharded ? (tb.rows - m->shard.rank + G - 1) / G : tb.rows;
             if (tb.dim % 4 || tb.x0_off % 4) { set_error("table %d: dim and deep-input offset must be multiples of 4", t); return WD_EINVAL; }
@@ -314,41 +299,24 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             m->emb_max_dim = std::max(m->emb_max_dim, tb.dim);
             m->tables.push_back(tb);
         }
-        // global row space: large tables first, then the small (dense-exchanged) ones, each group in table order
-        std::vector<int> row_order;
+        // global row space: large tables first, then the small (dense-exchanged) ones, each group in table order; the small ones'
+        // gradients in the same order in the small-table block
         for (int pass = 0; pass < 2; ++pass) {
             if (pass == 1) m->small_base[0] = row_base;
             for (int t = 0; t < d->n_tables; ++t) {
-                if (m->tables[t].sharded) continue;                  // rows live in the sharded space (shard.cu), not here
-                const bool small = m->dense_exchange_max_rows > 0 && m->tables[t].rows <= m->dense_exchange_max_rows;
-                if (small != (pass == 1)) continue;
-                if (small) m->n_small_tab++;
-                m->tables[t].row_base = row_base;
-                row_base += m->tables[t].rows;
-                row_order.push_back(t);
-            }
-        }
-        for (int t = 0; t < d->n_tables; ++t) h_row_base.push_back(m->tables[t].row_base);
-        {
-            std::vector<int64_t> rb, go, nr; std::vector<float*> dt; std::vector<int32_t> dm, st;
-            int64_t off = 0;
-            for (int t : row_order) {
-                const EmbTable& tb = m->tables[t];
+                EmbTable& tb = m->tables[t];
+                if (tb.sharded) continue;                            // rows live in the sharded space (shard.cu), not here
                 const bool small = m->dense_exchange_max_rows > 0 && tb.rows <= m->dense_exchange_max_rows;
-                rb.push_back(tb.row_base); nr.push_back(tb.rows); dt.push_back(tb.data); dm.push_back(tb.dim); st.push_back(tb.stride);
-                go.push_back(small ? off : -1);
-                if (small) off += tb.rows * tb.dim;
+                if (small != (pass == 1)) continue;
+                if (small) {
+                    m->n_small_tab++;
+                    tb.gs_off = m->gs_emb_floats;
+                    m->gs_emb_floats += tb.rows * tb.dim;
+                }
+                tb.row_base = row_base;
+                row_base += tb.rows;
+                m->rtab_order.push_back(t);
             }
-            m->gs_emb_floats = off;
-            m->n_rtab = (int)row_order.size();
-            m->rtab_order = row_order;
-            { const int64_t* t_; if ((rc = upload_vec(m, rb.data(), m->n_rtab, &t_))) return rc; m->d_rtab_row_base = (int64_t*)t_; }
-            { const int64_t* t_; if ((rc = upload_vec(m, go.data(), m->n_rtab, &t_))) return rc; m->d_rtab_gs_off = (int64_t*)t_; }
-            { const int64_t* t_; if ((rc = upload_vec(m, nr.data(), m->n_rtab, &t_))) return rc; m->d_rtab_rows = (int64_t*)t_; }
-            { float* const* t_; if ((rc = upload_vec<float*>(m, dt.data(), m->n_rtab, (float* const**)&t_))) return rc; m->d_rtab_data = (float**)t_; }
-            { const int32_t* t_;
-              if ((rc = upload_vec(m, dm.data(), m->n_rtab, &t_))) return rc; m->d_rtab_dim = (int32_t*)t_;
-              if ((rc = upload_vec(m, st.data(), m->n_rtab, &t_))) return rc; m->d_rtab_stride = (int32_t*)t_; }
         }
         m->emb_total_rows = row_base;
         if (m->dnn_opt.kind == WD_OPT_ADAM && (rc = dev_alloc(m, &m->d_adam_touched[0], (row_base + 31) / 32))) return rc;
@@ -357,18 +325,8 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         for (int c = 0; c < C; ++c)
             if (d->col_ind_off[c] >= 0) for (int64_t i = 0; i < d->col_buckets[c]; ++i) x->x0_real[d->col_ind_off[c] + i] = 1;
         for (auto v : x->x0_real) x->d0_logical += v;
-        // device table descriptors
         const int nt = (int)m->tables.size();
-        std::vector<float*> h_data; std::vector<int32_t> h_dim, h_stride, h_x0, h_col;
-        for (auto& tb : m->tables) { h_data.push_back(tb.data); h_dim.push_back(tb.dim); h_stride.push_back(tb.stride); h_x0.push_back(tb.x0_off); h_col.push_back(tb.col); }
-        { float* const* t; if ((rc = upload_vec<float*>(m, h_data.data(), nt, (float* const**)&t))) return rc; m->d_tab_data = (float**)t; }
-        { const int32_t* t;
-          if ((rc = upload_vec(m, h_dim.data(), nt, &t))) return rc; m->d_tab_dim = (int32_t*)t;
-          if ((rc = upload_vec(m, h_stride.data(), nt, &t))) return rc; m->d_tab_stride = (int32_t*)t;
-          if ((rc = upload_vec(m, h_x0.data(), nt, &t))) return rc; m->d_tab_x0 = (int32_t*)t;
-          if ((rc = upload_vec(m, h_col.data(), nt, &t))) return rc; m->d_tab_col = (int32_t*)t; }
-        { const int64_t* t; if ((rc = upload_vec(m, h_row_base.data(), nt, &t))) return rc; m->d_tab_row_base = (int64_t*)t; p.table_row_base = t; }
-        // group tables by width
+        // group the replicated tables by width (the gather view, build_record_sets)
         for (int t = 0; t < nt; ++t) {
             if (m->tables[t].sharded) continue;                      // gathered by their owners, not by the local gather kernels
             int di = -1;
@@ -378,18 +336,6 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
                 di = m->n_dims++; m->dims[di] = m->tables[t].dim; m->dim_ntables[di] = 0;
             }
             m->dim_ntables[di]++;
-        }
-        for (int i = 0; i < m->n_dims; ++i) {
-            std::vector<int32_t> ids;
-            for (int t = 0; t < nt; ++t) if (m->tables[t].dim == m->dims[i] && !m->tables[t].sharded) ids.push_back(t);
-            const int32_t* dp;
-            if ((rc = upload_vec(m, ids.data(), (int64_t)ids.size(), &dp))) return rc;
-            m->d_dim_tables[i] = (int32_t*)dp;
-            std::vector<TabDesc> descs;
-            for (int t : ids) descs.push_back(TabDesc{m->tables[t].data, m->tables[t].row_base, m->tables[t].stride, m->tables[t].x0_off, m->tables[t].col, m->tables[t].dim});
-            const TabDesc* dd;
-            if ((rc = upload_vec(m, descs.data(), (int64_t)descs.size(), &dd))) return rc;
-            m->d_dim_desc[i] = (TabDesc*)dd;
         }
         const int64_t actn = (int64_t)m->max_batch_pad * d->d0_phys;
         if ((rc = dev_alloc(m, &m->d_X0, actn))) return rc;
@@ -506,9 +452,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             if ((rc = dev_alloc(m, &m->d_Wq_hi, m->wt_count))) return rc;
             if ((rc = dev_alloc(m, &m->d_Wq_lo, m->wt_count))) return rc;
         }
-        const DenseTensor* dp;
-        if ((rc = upload_vec(m, m->dense.data(), (int64_t)m->dense.size(), &dp))) return rc;
-        m->d_dense_desc = (DenseTensor*)dp;
+        if ((rc = upload(m, &m->d_dense_desc, m->dense))) return rc;
     }
 
     // ---- sparse backward scratch
@@ -540,15 +484,16 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         // (and, in a row-sharded model, with what shard_build allocates right below).
         if ((rc = place_tables(m, hbm_reserve_bytes(m) + (G > 1 ? shard_hbm_bytes(m, d) : 0)))) return rc;
     }
+    if (G > 1 && (rc = shard_build(m, d))) return rc;
+    if ((rc = build_record_sets(m))) return rc;               // every table, staging buffer and shard row base is final now
     if (G > 1) {
-        if ((rc = shard_build(m, d))) return rc;
         DevPlan& dp = m->dplan;
         dp.sh_world = G;
         for (int sx = 0; sx < 2; ++sx) {
             ShardSpace& sp = m->shard.sp[sx];
             if (!sp.on) continue;
-            if (sx == 0) { dp.sh_col_emb = sp.d_col_slot; dp.sh_base_emb = sp.d_slot_base; dp.sh_own_emb = sp.d_own; dp.sh_lrow_emb = sp.d_lrow; }
-            else { dp.sh_col_wide = sp.d_col_slot; dp.sh_base_wide = sp.d_slot_base; dp.sh_own_wide = sp.d_own; dp.sh_lrow_wide = sp.d_lrow; }
+            if (sx == 0) { dp.sh_col_emb = sp.d_col_slot; dp.sh_base_emb = sp.set.rec.row_base; dp.sh_own_emb = sp.d_own; dp.sh_lrow_emb = sp.d_lrow; }
+            else { dp.sh_col_wide = sp.d_col_slot; dp.sh_base_wide = sp.set.rec.row_base; dp.sh_own_wide = sp.d_own; dp.sh_lrow_wide = sp.d_lrow; }
         }
     }
     if ((rc = metrics_setup())) return rc;
@@ -599,7 +544,8 @@ namespace wd {
 // HBM kept free for what is allocated after the embedding tables (see ensure_slot, place_tables and the step graphs): the auto
 // tables are placed with it held back, and wd_host_cache_enable refuses a cache that would eat into it.
 //   kReserveSlots batch slots beyond slot 0 (cat offsets, keys, dense, label, weight each; bench.py and the estimator use at most 10),
-//   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table) and their descriptors,
+//   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table) and the record sets
+//   (build_record_sets: a few hundred bytes per table, inside the kGraphReserve margin),
 //   kGraphReserve for the instantiated step graphs (one train and one backward graph per slot) and the runtime's growth.
 int64_t hbm_reserve_bytes(const WdModel* m) {
     constexpr int kReserveSlots = 16;

@@ -81,7 +81,8 @@ struct EmbTable {
     int x0_off;
     int col;                 // producing column
     int64_t row_base;        // global row id base
-    float* data;             // arows * stride floats; record = [w[dim] | slot1[dim] | slot2[dim]]
+    int64_t gs_off;          // small (dense-exchanged) table: float offset of its gradients in the small-table block; else -1
+    float* data;            // arows * stride floats; record = [w[dim] | slot1[dim] | slot2[dim]]
     int stride;              // dim * (1 + nslots)
     bool sharded;            // row-sharded over the ranks: this rank holds rows r with r mod G == rank at local index r / G
     int64_t arows;           // rows allocated on this rank (= rows unless sharded); row_base then counts in the shard's row space
@@ -93,6 +94,28 @@ struct TabDesc {            // per-table descriptor grouped by width (one 32-byt
     float* data;
     int64_t row_base;
     int stride, x0, col, dim;
+};
+
+// Where the [w | s1 | s2] records of a set of embedding tables are.  Tables t < ntab with first row row_base[t] (ascending in a
+// row-ordered set), records of stride[t] floats at data[t].  A staged table (stage[t] != 0; stage null: none is) keeps the records
+// of the step's rows in stage_base instead, unique row u at staging row uslot[u] (u without a cache) with stride stage[t].
+struct RowRecords {
+    int ntab;
+    const int64_t* row_base;
+    float* const* data;
+    const int32_t* dim;
+    const int32_t* stride;
+    const int32_t* stage;
+    float* stage_base;
+    const int32_t* uslot;
+};
+// One record set's device descriptors (the sets and who reads them: table at the top of host_tables.cu); per-table arrays a set
+// does not need are null.
+struct RecordSet {
+    RowRecords rec{};
+    const int32_t* x0 = nullptr;      // [ntab] offset of the table's slice in the deep input
+    const int64_t* rows = nullptr;    // [ntab] rows of the table this set holds on this rank
+    const int64_t* gs_off = nullptr;  // [ntab] float offset inside the small-table gradient block (-1: large table)
 };
 
 struct DenseTensor {         // one trainable dense tensor inside the dense arena
@@ -221,14 +244,13 @@ struct ShardSpace {           // one sharded table space on this rank: 0 = embed
     std::vector<int32_t> h_col_slot;   // host copies (tensor IO)
     std::vector<int64_t> h_slot_base;
     int32_t* d_col_slot = nullptr;     // [n_columns] slot fed by column c, -1
-    int64_t* d_slot_base = nullptr;    // [n_slots] first local row of the slot's shard
-    int32_t *d_slot_dim = nullptr, *d_slot_x0 = nullptr, *d_slot_stride = nullptr;
-    float** d_slot_data = nullptr;     // [n_slots] shard of the table (embedding space)
-    int64_t* d_slot_rows = nullptr;    // [n_slots] rows of the slot's shard on this rank (embedding space)
+    // the slots' records in slot order, row bases in the shard's row space (the shard set, host_tables.cu); the wide space fills
+    // only rec.row_base: the first local row of each column's shard
+    RecordSet set;
     uint32_t* d_adam_touched = nullptr;   // Adam: [ceil(local_rows / 32)] bit r: local row r was updated this step (sparse_dev.cuh)
-    // host-placed shards (embedding space): the owner stages the records of the step's unique owned host rows (list 2) in HBM
+    // host-placed shards (embedding space): the owner stages the records of the step's unique owned host rows (list 2) in HBM,
+    // record of unique row u at d_stage + u * stage_stride (set.rec.stage: 0 for an HBM slot)
     int stage_stride = 0;              // widest stride of the space's host slots; 0: every shard in HBM
-    int32_t* d_slot_stage = nullptr;   // [n_slots] 0: HBM slot; stage_stride: record of unique row u at d_stage + u * stage_stride
     float* d_stage = nullptr;          // [max_nnz + 1][stage_stride] owner staging buffer
     float4* d_wide = nullptr;          // wide space: {w, n, z, -} per local row
     uint32_t* d_own = nullptr;         // [max_nnz] owner rank of entry j or kInvalidRow (not a sharded column)
@@ -308,12 +330,7 @@ struct WdModel {
     int64_t small_base[2] = {0, 0};          // first global row of the small embedding tables / small wide columns
     int64_t gs_count = 0, gs_emb_floats = 0; // floats of the small-table gradient block behind d_G[dense_count]; its embedding part
     int64_t gs_touch_off[2] = {0, 0};        // offsets (floats, inside the block) of the per-row "touched" counts: small embedding rows / small wide rows
-    int n_rtab = 0, n_small_tab = 0;         // tables in row order (large first, then small); how many of them are small
-    int64_t* d_rtab_row_base = nullptr;      // [n_rtab] row base, ascending
-    float** d_rtab_data = nullptr;
-    int32_t *d_rtab_dim = nullptr, *d_rtab_stride = nullptr;
-    int64_t* d_rtab_gs_off = nullptr;        // [n_rtab] float offset inside the block (-1: large table)
-    int64_t* d_rtab_rows = nullptr;          // [n_rtab] rows
+    int n_small_tab = 0;                     // replicated tables that are small (the last ones of rtabs)
     // Adam: bitmaps of the replicated record sets (0: embedding rows, emb_total_rows bits; 1: wide rows, wide_rows bits), bit r set
     // when row r was updated this step, cleared by the set's untouched pass (sparse_dev.cuh); null unless that optimizer is Adam
     uint32_t* d_adam_touched[2] = {nullptr, nullptr};
@@ -326,17 +343,10 @@ struct WdModel {
     std::vector<void*> host_allocs;          // cudaHostAlloc'ed table records (freed in destroy)
     int64_t host_bytes = 0;
     int n_host_tab = 0;
-    std::vector<int> rtab_order;             // table ids in global row order (the d_rtab_* arrays)
+    std::vector<int> rtab_order;             // replicated table ids in global row order (the tables of rtabs)
     float* d_stage = nullptr;                // [max_nnz][stage_stride] records of the step's unique host rows, row u at u * stage_stride
     int stage_stride = 0;                    // largest stride of the host tables
     uint32_t* d_g_emb = nullptr;             // [max_nnz] ids the gather reads: e_emb, host-table entries replaced by their unique index u
-    // what the gather kernels address: the tables' own arrays, or for host tables the staging buffer (data = d_stage, row base 0,
-    // stride stage_stride); all alias the arrays above when no table is on the host
-    float** d_gtab_data = nullptr;           // [n_tables] data (gather)
-    int32_t* d_gtab_stride = nullptr;        // [n_tables] stride (gather)
-    int64_t* d_gtab_row_base = nullptr;      // [n_tables] row base (gather)
-    int32_t* d_tab_stage = nullptr;          // [n_tables] 0: record in place; stage_stride: staged (fused row updates); null without host tables
-    int32_t* d_rtab_stage = nullptr;         // [n_rtab] 0 / stage_stride in row order (fused hot-row updates, stage-in / write-back); null without host tables
     // HBM cache of host records (wd_host_cache_enable): d_stage is then [cache_slots slots | max_nnz overflow rows]
     int64_t cache_slots = 0;                 // C = 8 x 2^cache_set_bits; 0: no cache (every staged row is an overflow row)
     int cache_set_bits = 0;
@@ -384,13 +394,11 @@ struct WdModel {
     int emb_max_dim = 0;
     int n_dims = 0;
     int dims[wd::kMaxDims];                  // distinct widths
-    int32_t* d_dim_tables[wd::kMaxDims];     // table ids per width (device)
-    wd::TabDesc* d_dim_desc[wd::kMaxDims];    // descriptors of the same tables
     int dim_ntables[wd::kMaxDims];
-    // device table descriptors
-    float** d_tab_data = nullptr;
-    int32_t *d_tab_dim = nullptr, *d_tab_stride = nullptr, *d_tab_x0 = nullptr, *d_tab_col = nullptr;
-    int64_t* d_tab_row_base = nullptr;
+    // the record sets of the embedding tables and the gather view (table at the top of host_tables.cu)
+    wd::RecordSet tabs;                      // every table in plan order
+    wd::RecordSet rtabs;                     // the replicated tables in global row order (rtab_order)
+    wd::TabDesc* d_dim_desc[wd::kMaxDims] = {};   // [dim_ntables] gather view of the replicated tables of width dims[i]
     float *d_X0 = nullptr, *d_dX0 = nullptr;
     float* d_X0T = nullptr;                  // fp32 family: transposed X0 [d0_phys, ldt]
     __nv_bfloat16* d_X0s[2] = {nullptr, nullptr};   // bf16 family: hi / lo copies of X0
@@ -486,14 +494,14 @@ int loss_forward(WdModel* m, bool need_grad);                    // mlp.cu: logi
 int model_init_params(WdModel* m, uint64_t seed);                // init.cu
 int step_tick(WdModel* m);                                       // misc.cu: train-step counter on the device (dropout)
 int adam_tick(WdModel* m);                                       // misc.cu: beta powers advance (after every optimizer of the step)
-int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host), descriptors
+int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host) and staging buffer
+int build_record_sets(WdModel* m);                               // host_tables.cu: upload the record sets and the gather view
 int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
 int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
 int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
-// host_tables.cu: records of the unique rows urow[0 .. *d_nuniq) of tables with stage_of[t] != 0 (tables found by row base) from their
-// host records into stage row u (in) or back (!in); S = stride of the staging rows
-int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, int ntab, const int64_t* row_base,
-                       float* const* data, const int32_t* stride, const int32_t* stage_of, float* stage, int S);
+// host_tables.cu: records of the unique rows urow[0 .. *d_nuniq) of the staged tables of `rec` (tables found by row base) from
+// their host records into staging row u of rec.stage_base (in) or back (!in); S = stride of the staging rows
+int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, const RowRecords& rec, int S);
 int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d);  // shard.cu: HBM shard_build allocates (held back by auto placement)
 int64_t hbm_reserve_bytes(const WdModel* m);                     // api.cu: HBM the model keeps free for its later allocations
 // tsv.cu: device parse of n lines into the batch buffers on stream st, waiting for it; *status != 0: the buffers do not hold the
@@ -532,6 +540,20 @@ int dev_alloc(WdModel* m, T** p, int64_t count, bool zero = true) {
     *p = (T*)q;
     return WD_OK;
 }
+// copies src[0 .. n) to the device array *dst, allocated here while *dst is null; an existing array is overwritten in place (a
+// second upload of the same descriptor allocates nothing)
+template <typename T> struct same_type { using type = T; };   // (keeps `src` out of the deduction of T)
+template <typename T>
+int upload(WdModel* m, T** dst, const typename same_type<T>::type* src, int64_t n) {
+    if (!*dst) {
+        int rc = dev_alloc(m, dst, n, true);
+        if (rc) return rc;
+    }
+    if (n > 0) WD_CUDA(cudaMemcpyAsync((void*)*dst, src, n * sizeof(T), cudaMemcpyHostToDevice, m->stream));
+    return WD_OK;
+}
+template <typename T, typename A>
+int upload(WdModel* m, T** dst, const std::vector<A>& h) { return upload(m, dst, h.data(), (int64_t)h.size()); }
 
 // record a named mark on the model stream (no-op unless profiling is on)
 inline void mark(WdModel* m, const char* name) {

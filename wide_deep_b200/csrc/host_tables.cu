@@ -1,3 +1,21 @@
+// Placement of the embedding tables and the device descriptors every kernel finds their records through.
+//
+// Record sets (build_record_sets: RecordSet / RowRecords in common.cuh, record() in sparse_dev.cuh).  One builder uploads all of
+// them once every table and staging buffer exists and the shard layout is final:
+//   set                   order                 row space                 read by
+//   by table              plan order            global rows (shard rows   LocalEmb (dim, x0), the fused direct-row update
+//     WdModel::tabs                             for a sharded table)      (RowApply ra), the id stage (DevPlan::table_row_base)
+//   replicated, by row    global row order:     global rows               the fused hot-row update (ha), emb_apply_kernel, the
+//     WdModel::rtabs      large, then small                               small-table block (gs_off), stage-in / write-back /
+//                                                                         remap / flush of host tables and the cache, Adam's
+//                                                                         untouched pass (rows)
+//   shard                 slot order            this rank's shard rows    serve, combine, PeerEmb, the owner apply,
+//     ShardSpace::set                                                     host_rows_transfer, the shard's untouched pass
+//   gather view           per width,            global rows; a host       emb_pool_fwd_rows_kernel, emb_pool_fwd_kernel<G>
+//     WdModel::d_dim_desc table order           table at its staging row
+// A host table is staged in the by-table and replicated sets (stage[t] = stage_stride, records in d_stage) and read by the gather
+// from the staging buffer; a host shard is staged in the shard set (records in the owner's ShardSpace::d_stage).
+//
 // Embedding tables in page-locked host memory (WdPlanDesc::table_placement).  The reference keeps its tables in host RAM: it
 // trains on the CPU or spreads them over parameter servers (reference python/lib/build_estimator.py:211-214, joint.py:141-143).
 //
@@ -18,6 +36,7 @@
 // serving them and stages them into its own buffer through host_rows_transfer (the owner-side step is in shard.cu).  Only the
 // sharded tables may go to the host then; the replicated ones, the single-GPU staging buffer and the HBM cache stay out of it.
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "sparse_dev.cuh"
@@ -43,15 +62,14 @@ __device__ __forceinline__ uint32_t cache_set_of(uint32_t row, int set_bits) {
 }
 
 // key = set of unique row u (host rows) or nsets (HBM rows: sorted last, never assigned), value = u; bumps the call's stamp
-__global__ void __launch_bounds__(256) cache_keys_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, int ntab,
-                                                         const int64_t* __restrict__ rtab_row_base, const int32_t* __restrict__ rtab_stage,
+__global__ void __launch_bounds__(256) cache_keys_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, RowRecords rr,
                                                          int set_bits, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
                                                          uint32_t* __restrict__ now) {
     if (blockIdx.x == 0 && threadIdx.x == 0) ++*now;
     const int nu = *d_nuniq;
     for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nu; u += gridDim.x * blockDim.x) {
         const uint32_t row = urow[u];
-        keys[u] = rtab_stage[table_of(rtab_row_base, ntab, row)] != 0 ? cache_set_of(row, set_bits) : (1u << set_bits);
+        keys[u] = rr.stage[table_of(rr.row_base, rr.ntab, row)] != 0 ? cache_set_of(row, set_bits) : (1u << set_bits);
         vals[u] = (uint32_t)u;
     }
 }
@@ -135,19 +153,18 @@ __global__ void __launch_bounds__(256) cache_assign_kernel(const int32_t* __rest
     }
 }
 
-// Transfer between the host records of the step's unique host rows and their staging rows (uslot[u], or u without a cache).
-// IN: the record of every row to load -> its staging row; a dirty victim's record goes home first (uvict[u], the row the slot
-// held).  !IN: overflow staging rows (>= C) -> host records.  One thread per float4 of a staged record, consecutive threads on
-// consecutive float4 of a record (the PCIe transfers are whole records); each thread keeps kInFlight float4 in flight.  The thread
-// that writes float4 q of a slot has read the victim's float4 q before, so the eviction needs no barrier; a victim is never a row
-// of the current call (that row would have been a hit).
+// Transfer between the host records of the step's unique host rows (the staged tables of rr) and their staging rows in
+// rr.stage_base (rr.uslot[u], or u without a cache).  IN: the record of every row to load -> its staging row; a dirty victim's
+// record goes home first (uvict[u], the row the slot held).  !IN: overflow staging rows (>= C) -> host records.  One thread per
+// float4 of a staged record, consecutive threads on consecutive float4 of a record (the PCIe transfers are whole records); each
+// thread keeps kInFlight float4 in flight.  The thread that writes float4 q of a slot has read the victim's float4 q before, so the
+// eviction needs no barrier; a victim is never a row of the current call (that row would have been a hit).
 constexpr int kInFlight = 4;
-struct StageMap { const int32_t* uslot; const uint32_t* uvict; const uint8_t* uflag; int64_t C; };
+struct StageMap { const uint32_t* uvict; const uint8_t* uflag; int64_t C; };
 template <bool IN>
-__global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, int ntab,
-                                                        const int64_t* __restrict__ rtab_row_base, float* const* __restrict__ rtab_data,
-                                                        const int32_t* __restrict__ rtab_stride, const int32_t* __restrict__ rtab_stage,
-                                                        float* __restrict__ stage, int S, StageMap sm) {
+__global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, RowRecords rr,
+                                                        int S, StageMap sm) {
+    float* const stage = rr.stage_base;
     const int q4 = S >> 2;
     const int64_t total = (int64_t)*d_nuniq * q4;
     const int64_t T = (int64_t)gridDim.x * blockDim.x;
@@ -162,28 +179,28 @@ __global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restric
             const int64_t u = i / q4;
             const int q = (int)(i - u * q4);
             const int64_t row = urow[u];
-            const int lo = table_of(rtab_row_base, ntab, row);
-            if (rtab_stage[lo] == 0) continue;                           // HBM table
+            const int lo = table_of(rr.row_base, rr.ntab, row);
+            if (rr.stage[lo] == 0) continue;                                 // HBM table
             int64_t srow = u;
-            if (sm.uslot) {
-                srow = sm.uslot[u];
+            if (rr.uslot) {
+                srow = rr.uslot[u];
                 if (IN) {
                     const uint8_t f = sm.uflag[u];
                     if (!(f & kLoad)) continue;                              // hit: the slot holds the record
                     if (f & kVictimDirty) {
                         const int64_t vr = sm.uvict[u];
-                        const int vlo = table_of(rtab_row_base, ntab, vr);
-                        const int vstride = rtab_stride[vlo];
+                        const int vlo = table_of(rr.row_base, rr.ntab, vr);
+                        const int vstride = rr.stride[vlo];
                         if (q * 4 < vstride) {
                             vv[k] = *reinterpret_cast<const float4*>(stage + srow * S + q * 4);
-                            vdst[k] = rtab_data[vlo] + (vr - rtab_row_base[vlo]) * vstride + q * 4;
+                            vdst[k] = rr.data[vlo] + (vr - rr.row_base[vlo]) * vstride + q * 4;
                         }
                     }
                 } else if (srow < sm.C) continue;                            // cached: stays in its slot
             }
-            const int stride = rtab_stride[lo];
+            const int stride = rr.stride[lo];
             if (q * 4 >= stride) continue;                                   // beyond this table's record
-            float* rec = rtab_data[lo] + (row - rtab_row_base[lo]) * stride + q * 4;
+            float* rec = rr.data[lo] + (row - rr.row_base[lo]) * stride + q * 4;
             float* st = stage + srow * S + q * 4;
             if (IN) { v[k] = *reinterpret_cast<const float4*>(rec); dst[k] = st; }
             else { v[k] = *reinterpret_cast<const float4*>(st); dst[k] = rec; }
@@ -199,25 +216,23 @@ __global__ void __launch_bounds__(256) host_rows_kernel(const int32_t* __restric
 // gather ids: e_emb, with the entries of host tables replaced by the staging row of their unique row u (uslot[u], or u without a
 // cache; urow[0..nu) is sorted ascending)
 __global__ void __launch_bounds__(256) host_remap_kernel(const int32_t* __restrict__ d_nnz, const uint32_t* __restrict__ e_emb,
-                                                         const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, int ntab,
-                                                         const int64_t* __restrict__ rtab_row_base, const int32_t* __restrict__ rtab_stage,
-                                                         const int32_t* __restrict__ uslot, uint32_t* __restrict__ g_emb) {
+                                                         const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow, RowRecords rr,
+                                                         uint32_t* __restrict__ g_emb) {
     const int n = *d_nnz, nu = *d_nuniq;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t r = e_emb[i];
         uint32_t g = r;
-        if (r != kInvalidRow && rtab_stage[table_of(rtab_row_base, ntab, r)] != 0) {
+        if (r != kInvalidRow && rr.stage[table_of(rr.row_base, rr.ntab, r)] != 0) {
             const int u = lower_bound_u32(urow, nu, r);
-            g = uslot ? (uint32_t)uslot[u] : (uint32_t)u;
+            g = rr.uslot ? (uint32_t)rr.uslot[u] : (uint32_t)u;
         }
         g_emb[i] = g;
     }
 }
 
-// dirty slots -> host records (one thread per float4 of a slot)
+// dirty slots of rr.stage_base -> host records (one thread per float4 of a slot)
 __global__ void __launch_bounds__(256) cache_flush_kernel(int64_t C, int S, const uint32_t* __restrict__ tag, const uint8_t* __restrict__ dirty,
-                                                          int ntab, const int64_t* __restrict__ rtab_row_base, float* const* __restrict__ rtab_data,
-                                                          const int32_t* __restrict__ rtab_stride, const float* __restrict__ stage) {
+                                                          RowRecords rr) {
     const int q4 = S >> 2;
     const int64_t total = C * q4;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -225,11 +240,11 @@ __global__ void __launch_bounds__(256) cache_flush_kernel(int64_t C, int S, cons
         const int q = (int)(i - slot * q4);
         if (!dirty[slot] || tag[slot] == kInvalidRow) continue;
         const int64_t row = tag[slot];
-        const int lo = table_of(rtab_row_base, ntab, row);
-        const int stride = rtab_stride[lo];
+        const int lo = table_of(rr.row_base, rr.ntab, row);
+        const int stride = rr.stride[lo];
         if (q * 4 >= stride) continue;
-        *reinterpret_cast<float4*>(rtab_data[lo] + (row - rtab_row_base[lo]) * stride + q * 4) =
-            *reinterpret_cast<const float4*>(stage + slot * S + q * 4);
+        *reinterpret_cast<float4*>(rr.data[lo] + (row - rr.row_base[lo]) * stride + q * 4) =
+            *reinterpret_cast<const float4*>(rr.stage_base + slot * S + q * 4);
     }
 }
 __global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32_t* __restrict__ stamp, uint8_t* __restrict__ dirty, int invalidate) {
@@ -242,9 +257,9 @@ __global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32
 int host_tables_stage_in(WdModel* m, bool train) {
     const int64_t C = m->cache_slots;
     const int g = grid_for(m->max_nnz, 256);
+    const RowRecords& rr = m->rtabs.rec;
     if (C > 0) {
-        cache_keys_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_stage, m->cache_set_bits,
-                                                   m->d_ck[0], m->d_cv[0], m->d_cnow);
+        cache_keys_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], rr, m->cache_set_bits, m->d_ck[0], m->d_cv[0], m->d_cnow);
         m->launches++;
         int rc = radix_sort_pairs(m, &m->d_ck[0], &m->d_cv[0], &m->d_ck[1], &m->d_cv[1], m->cache_set_bits + 1, m->d_nuniq[0]);
         if (rc) return rc;
@@ -255,11 +270,10 @@ int host_tables_stage_in(WdModel* m, bool train) {
         m->launches++;
         mark(m, "cache_assign");
     }
-    const StageMap sm{m->d_uslot, m->d_uvict, m->d_uflag, C};
+    const StageMap sm{m->d_uvict, m->d_uflag, C};
     host_rows_kernel<true><<<grid_for(m->max_nnz * (m->stage_stride / 4) / kInFlight, 256), 256, 0, m->stream>>>(
-        m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_rtab_stage, m->d_stage, m->stage_stride, sm);
-    host_remap_kernel<<<g, 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], m->n_rtab,
-                                                m->d_rtab_row_base, m->d_rtab_stage, m->d_uslot, m->d_g_emb);
+        m->d_nuniq[0], m->d_urow[0], rr, m->stage_stride, sm);
+    host_remap_kernel<<<g, 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], rr, m->d_g_emb);
     m->launches += 2;
     mark(m, "stage_in");
     WD_CUDA(cudaGetLastError());
@@ -267,22 +281,21 @@ int host_tables_stage_in(WdModel* m, bool train) {
 }
 
 int host_tables_write_back(WdModel* m) {
-    const StageMap sm{m->d_uslot, m->d_uvict, m->d_uflag, m->cache_slots};
+    const StageMap sm{m->d_uvict, m->d_uflag, m->cache_slots};
     host_rows_kernel<false><<<grid_for(m->max_nnz * (m->stage_stride / 4) / kInFlight, 256), 256, 0, m->stream>>>(
-        m->d_nuniq[0], m->d_urow[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_rtab_stage, m->d_stage, m->stage_stride, sm);
+        m->d_nuniq[0], m->d_urow[0], m->rtabs.rec, m->stage_stride, sm);
     m->launches++;
     mark(m, "write_back");
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 
-// The same transfer over any table list without a cache (staging row = u): the host-placed shards of a row-sharded space (shard.cu)
-int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, int ntab, const int64_t* row_base,
-                       float* const* data, const int32_t* stride, const int32_t* stage_of, float* stage, int S) {
-    const StageMap sm{nullptr, nullptr, nullptr, 0};
+// The same transfer over another record set without a cache (staging row = u): the host-placed shards of a row-sharded space (shard.cu)
+int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, const RowRecords& rec, int S) {
+    const StageMap sm{nullptr, nullptr, 0};
     const int g = grid_for(m->max_nnz * (S / 4) / kInFlight, 256);
-    if (in) host_rows_kernel<true><<<g, 256, 0, m->stream>>>(d_nuniq, urow, ntab, row_base, data, stride, stage_of, stage, S, sm);
-    else host_rows_kernel<false><<<g, 256, 0, m->stream>>>(d_nuniq, urow, ntab, row_base, data, stride, stage_of, stage, S, sm);
+    if (in) host_rows_kernel<true><<<g, 256, 0, m->stream>>>(d_nuniq, urow, rec, S, sm);
+    else host_rows_kernel<false><<<g, 256, 0, m->stream>>>(d_nuniq, urow, rec, S, sm);
     m->launches++;
     mark(m, in ? "shard_stage_in" : "shard_write_back");
     WD_CUDA(cudaGetLastError());
@@ -295,8 +308,7 @@ int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
     const int64_t C = m->cache_slots;
     if (C == 0) return WD_OK;
     if (flush) {
-        cache_flush_kernel<<<grid_for(C * (m->stage_stride / 4), 256), 256, 0, m->stream>>>(C, m->stage_stride, m->d_ctag, m->d_cdirty, m->n_rtab,
-                                                                                          m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_stride, m->d_stage);
+        cache_flush_kernel<<<grid_for(C * (m->stage_stride / 4), 256), 256, 0, m->stream>>>(C, m->stage_stride, m->d_ctag, m->d_cdirty, m->rtabs.rec);
         m->launches++;
     }
     cache_clear_kernel<<<grid_for(C, 256), 256, 0, m->stream>>>(C, m->d_ctag, m->d_cstamp, m->d_cdirty, invalidate ? 1 : 0);
@@ -305,61 +317,9 @@ int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
     return WD_OK;
 }
 
-template <typename T>
-static int upload(WdModel* m, T** dst, const std::vector<T>& h) {
-    int rc = dev_alloc(m, dst, (int64_t)h.size(), false);
-    if (rc) return rc;
-    WD_CUDA(cudaMemcpyAsync(*dst, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, m->stream));
-    return WD_OK;
-}
-template <typename T>
-static int overwrite(WdModel* m, T* dst, const std::vector<T>& h) {
-    WD_CUDA(cudaMemcpyAsync(dst, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, m->stream));
-    return WD_OK;
-}
-
-// What the gather kernels address: host tables through the staging buffer (data = d_stage, row base 0, stride stage_stride), every
-// other table in place; and which tables the fused updates find staged (d_tab_stage / d_rtab_stage).  alloc: upload the descriptor
-// arrays (place_tables); else overwrite the ones that carry the staging buffer's address (wd_host_cache_enable replaces the buffer).
-static int stage_descriptors(WdModel* m, bool alloc) {
-    const int nt = (int)m->tables.size();
-    int rc;
-    std::vector<float*> gdata(nt);
-    std::vector<int32_t> gstride(nt), stage(nt, 0), rstage;
-    std::vector<int64_t> grb(nt);
-    for (int t = 0; t < nt; ++t) {
-        const EmbTable& tb = m->tables[t];
-        gdata[t] = tb.host ? m->d_stage : tb.data;
-        gstride[t] = tb.host ? m->stage_stride : tb.stride;
-        grb[t] = tb.host ? 0 : tb.row_base;
-        stage[t] = tb.host ? m->stage_stride : 0;
-    }
-    for (int t : m->rtab_order) rstage.push_back(m->tables[t].host ? m->stage_stride : 0);
-    if (m->n_host_tab > 0) {
-        if (alloc) {
-            if ((rc = upload(m, &m->d_gtab_data, gdata))) return rc;
-            if ((rc = upload(m, &m->d_gtab_stride, gstride))) return rc;
-            if ((rc = upload(m, &m->d_gtab_row_base, grb))) return rc;
-            if ((rc = upload(m, &m->d_tab_stage, stage))) return rc;
-            if ((rc = upload(m, &m->d_rtab_stage, rstage))) return rc;
-        } else if ((rc = overwrite(m, m->d_gtab_data, gdata))) return rc;
-    }
-    for (int i = 0; i < m->n_dims; ++i) {    // per-width descriptors of the short-bag gather (table ids ascending, as build_model)
-        std::vector<TabDesc> descs;
-        for (int t = 0; t < nt; ++t) {
-            const EmbTable& tb = m->tables[t];
-            if (tb.dim != m->dims[i] || tb.sharded) continue;
-            descs.push_back(TabDesc{gdata[t], grb[t], gstride[t], tb.x0_off, tb.col, tb.dim});
-        }
-        if ((rc = overwrite(m, m->d_dim_desc[i], descs))) return rc;
-    }
-    return WD_OK;
-}
-
 // Allocates every embedding table — in HBM (WD_PLACE_HBM, and WD_PLACE_AUTO tables while they fit, largest first, with
-// `hbm_reserve` bytes held back for the buffers allocated after wd_model_create) or in mapped page-locked host memory — and fills
-// in the table pointers of the descriptors build_model uploaded, plus the staging buffer and the gather / apply descriptors of the
-// host tables.  A row-sharded model (shard_world > 1) may place only its sharded tables on the host: this rank's shard lives there
+// `hbm_reserve` bytes held back for the buffers allocated after wd_model_create) or in mapped page-locked host memory — and the
+// staging buffer of the host tables.  The descriptors that point at them come later (build_record_sets).  A row-sharded model (shard_world > 1) may place only its sharded tables on the host: this rank's shard lives there
 // and is staged by its owner-side step (shard.cu), nothing here stages it.
 int place_tables(WdModel* m, int64_t hbm_reserve) {
     const int nt = (int)m->tables.size();
@@ -413,21 +373,81 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
         m->stage_stride = std::max(m->stage_stride, tb.stride);
     }
 
-    // table pointers of the descriptors build_model uploaded before the tables existed
-    std::vector<float*> data(nt), rdata;
-    for (int t = 0; t < nt; ++t) data[t] = m->tables[t].data;
-    for (int t : m->rtab_order) rdata.push_back(m->tables[t].data);
-    if ((rc = overwrite(m, m->d_tab_data, data))) return rc;
-    if (!rdata.empty() && (rc = overwrite(m, m->d_rtab_data, rdata))) return rc;
     if (m->n_host_tab > 0) {
         if ((rc = dev_alloc(m, &m->d_stage, m->max_nnz * (int64_t)m->stage_stride, true))) return rc;
         if ((rc = dev_alloc(m, &m->d_g_emb, m->max_nnz, true))) return rc;
-    } else {                                 // nothing on the host: the step addresses the tables' own arrays
-        m->d_g_emb = m->d_e_emb;
-        m->d_gtab_data = m->d_tab_data; m->d_gtab_stride = m->d_tab_stride; m->d_gtab_row_base = m->d_tab_row_base;
+    } else {
+        m->d_g_emb = m->d_e_emb;             // nothing on the host: the gather reads the step's own ids
     }
-    if ((rc = stage_descriptors(m, true))) return rc;
-    WD_CUDA(cudaStreamSynchronize(m->stream));
+    return WD_OK;
+}
+
+// dst = per-table values f(table) of the tables `ids`, in that order
+template <typename T, typename F>
+static int upload_per_table(WdModel* m, T** dst, const std::vector<int>& ids, F f) {
+    std::vector<std::remove_const_t<T>> h;
+    for (int t : ids) h.push_back(f(m->tables[t]));
+    return upload(m, dst, h);
+}
+// the records of the tables `ids`, in that order; a host table is staged (stage stride S, records in stage_base) when S > 0
+static int upload_records(WdModel* m, RowRecords& r, const std::vector<int>& ids, int S, float* stage_base, const int32_t* uslot) {
+    int rc;
+    r.ntab = (int)ids.size();
+    r.stage_base = stage_base;
+    r.uslot = uslot;
+    if ((rc = upload_per_table(m, &r.row_base, ids, [](const EmbTable& tb) { return tb.row_base; }))) return rc;
+    if ((rc = upload_per_table(m, &r.data, ids, [](const EmbTable& tb) { return tb.data; }))) return rc;
+    if ((rc = upload_per_table(m, &r.dim, ids, [](const EmbTable& tb) { return (int32_t)tb.dim; }))) return rc;
+    if ((rc = upload_per_table(m, &r.stride, ids, [](const EmbTable& tb) { return (int32_t)tb.stride; }))) return rc;
+    if (S > 0 && (rc = upload_per_table(m, &r.stage, ids, [&](const EmbTable& tb) { return tb.host ? S : 0; }))) return rc;
+    return WD_OK;
+}
+
+// Uploads the record sets and the gather view (table at the top of this file) from the tables as they stand.  build_model runs it
+// once every table and staging buffer exists and the shard layout is final (shard_build moves the sharded tables' row bases into
+// the shard's row space); wd_host_cache_enable runs it again after replacing the staging buffer: every array exists by then and is
+// overwritten in place.
+int build_record_sets(WdModel* m) {
+    int rc;
+    std::vector<int> all(m->tables.size()), slots;
+    for (size_t t = 0; t < m->tables.size(); ++t) {
+        all[t] = (int)t;
+        if (m->tables[t].sharded) slots.push_back((int)t);          // slot order = table order (shard_build)
+    }
+    auto x0_of = [](const EmbTable& tb) { return (int32_t)tb.x0_off; };
+    auto rows_of = [](const EmbTable& tb) { return tb.arows; };
+    if (!m->tables.empty()) {
+        // by table
+        if ((rc = upload_records(m, m->tabs.rec, all, m->stage_stride, m->d_stage, m->d_uslot))) return rc;
+        if ((rc = upload_per_table(m, &m->tabs.x0, all, x0_of))) return rc;
+        m->dplan.table_row_base = m->tabs.rec.row_base;
+        // replicated, by row
+        if ((rc = upload_records(m, m->rtabs.rec, m->rtab_order, m->stage_stride, m->d_stage, m->d_uslot))) return rc;
+        if ((rc = upload_per_table(m, &m->rtabs.rows, m->rtab_order, rows_of))) return rc;
+        if ((rc = upload_per_table(m, &m->rtabs.gs_off, m->rtab_order, [](const EmbTable& tb) { return tb.gs_off; }))) return rc;
+    }
+    // shard: the embedding space's records; the wide space has only its columns' row bases
+    ShardSpace& se = m->shard.sp[0];
+    if (se.on) {
+        if ((rc = upload_records(m, se.set.rec, slots, se.stage_stride, se.d_stage, nullptr))) return rc;
+        if ((rc = upload_per_table(m, &se.set.x0, slots, x0_of))) return rc;
+        if ((rc = upload_per_table(m, &se.set.rows, slots, rows_of))) return rc;
+    }
+    ShardSpace& sw = m->shard.sp[1];
+    if (sw.on) {
+        sw.set.rec.ntab = sw.n_slots;
+        if ((rc = upload(m, &sw.set.rec.row_base, sw.h_slot_base))) return rc;
+    }
+    // gather view: per width, the replicated tables in table order; a host table read from the staging buffer (row base 0)
+    for (int i = 0; i < m->n_dims; ++i) {
+        std::vector<TabDesc> descs;
+        for (const EmbTable& tb : m->tables) {
+            if (tb.dim != m->dims[i] || tb.sharded) continue;
+            descs.push_back(tb.host ? TabDesc{m->d_stage, 0, m->stage_stride, tb.x0_off, tb.col, tb.dim}
+                                    : TabDesc{tb.data, tb.row_base, tb.stride, tb.x0_off, tb.col, tb.dim});
+        }
+        if ((rc = upload(m, &m->d_dim_desc[i], descs))) return rc;
+    }
     return WD_OK;
 }
 
@@ -489,7 +509,7 @@ extern "C" int wd_host_cache_enable(WdModel* m, int64_t bytes) {
     }
     m->cache_slots = C;
     m->cache_set_bits = bits;
-    if ((rc = stage_descriptors(m, false))) return rc;
+    if ((rc = build_record_sets(m))) return rc;
     WD_CUDA(cudaStreamSynchronize(m->stream));
     return WD_OK;
 }

@@ -336,18 +336,9 @@ __global__ void __launch_bounds__(256) shard_ar_gather_kernel(float* const* __re
 static int bits_for64(int64_t n) { int b = 1; while ((1ll << b) < n) ++b; return b; }
 static int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
-template <typename T>
-static int upload_arr(WdModel* m, const std::vector<T>& h, T** out) {
-    T* p = nullptr;
-    int rc = dev_alloc(m, &p, (int64_t)std::max<size_t>(h.size(), 1), true);
-    if (rc) return rc;
-    if (!h.empty()) WD_CUDA(cudaMemcpyAsync(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, m->stream));
-    *out = p;
-    return WD_OK;
-}
-
 // Lays out the sharded spaces and the exchange segment.  Called at the end of build_model (world > 1): by then the dense arena
-// size is known; d_dX0 / d_dlogit / d_G live INSIDE the segment so that peers can read them.
+// size is known; d_dX0 / d_dlogit / d_G live INSIDE the segment so that peers can read them.  The sharded tables' row bases move
+// into the shard's row space here; the shard set that describes them is uploaded after (build_record_sets).
 int shard_build(WdModel* m, const WdPlanDesc* d) {
     ShardState& S = m->shard;
     S.world = d->shard_world; S.rank = d->shard_rank;
@@ -358,16 +349,13 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     // ---- embedding space
     {
         ShardSpace& sp = S.sp[0];
-        std::vector<int32_t> col_slot(C, -1), dim, x0, stride, host;
-        std::vector<int64_t> base, srows;
-        std::vector<float*> data;
+        std::vector<int32_t> col_slot(C, -1);
+        std::vector<int64_t> base;
         int64_t rows = 0;
-        for (size_t t = 0; t < m->tables.size(); ++t) {
-            EmbTable& tb = m->tables[t];
+        for (EmbTable& tb : m->tables) {
             if (!tb.sharded) continue;
             col_slot[tb.col] = sp.n_slots++;
-            base.push_back(rows); srows.push_back(tb.arows); dim.push_back(tb.dim); x0.push_back(tb.x0_off); stride.push_back(tb.stride); data.push_back(tb.data);
-            host.push_back(tb.host);
+            base.push_back(rows);
             if (tb.host) sp.stage_stride = std::max(sp.stage_stride, tb.stride);
             tb.row_base = rows;
             rows += (tb.rows + G - 1) / G;            // the SAME layout on every rank (a requester computes the owner's local row): ceil(rows / G) per table
@@ -377,20 +365,9 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
         sp.local_rows = rows;
         sp.bags_per_row = sp.n_slots;
         sp.h_col_slot = col_slot; sp.h_slot_base = base;
-        if (sp.on) {
-            if ((rc = upload_arr(m, col_slot, &sp.d_col_slot))) return rc;
-            if ((rc = upload_arr(m, base, &sp.d_slot_base))) return rc;
-            if ((rc = upload_arr(m, dim, &sp.d_slot_dim))) return rc;
-            if ((rc = upload_arr(m, x0, &sp.d_slot_x0))) return rc;
-            if ((rc = upload_arr(m, stride, &sp.d_slot_stride))) return rc;
-            if ((rc = upload_arr(m, data, &sp.d_slot_data))) return rc;
-            if ((rc = upload_arr(m, srows, &sp.d_slot_rows))) return rc;
-        }
-        if (sp.stage_stride > 0) {               // host-placed shards: staging rows of the step's unique owned rows (+1: see the serve)
-            for (int32_t& h : host) h = h ? sp.stage_stride : 0;
-            if ((rc = upload_arr(m, host, &sp.d_slot_stage))) return rc;
-            if ((rc = dev_alloc(m, &sp.d_stage, (m->max_nnz + 1) * (int64_t)sp.stage_stride, false))) return rc;
-        }
+        if (sp.on && (rc = upload(m, &sp.d_col_slot, col_slot))) return rc;
+        // host-placed shards: staging rows of the step's unique owned rows (+1: see the serve)
+        if (sp.stage_stride > 0 && (rc = dev_alloc(m, &sp.d_stage, (m->max_nnz + 1) * (int64_t)sp.stage_stride, false))) return rc;
     }
     // ---- wide space
     {
@@ -411,8 +388,7 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
         sp.width = 1;
         sp.bags_per_row = 1;
         if (sp.on) {
-            if ((rc = upload_arr(m, col_slot, &sp.d_col_slot))) return rc;
-            if ((rc = upload_arr(m, base, &sp.d_slot_base))) return rc;
+            if ((rc = upload(m, &sp.d_col_slot, col_slot))) return rc;
             if ((rc = dev_alloc(m, &sp.d_wide, rows))) return rc;
         }
     }
@@ -610,13 +586,12 @@ static int shard_serve(WdModel* m, int s) {
     int rc;
     if (staged(m, s)) {                          // unique owned rows (list 2), then the records of the host rows among them -> HBM
         if ((rc = shard_owner_group(m, s))) return rc;
-        if ((rc = host_rows_transfer(m, true, m->d_nuniq[2], m->d_urow[2], sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_stride,
-                                     sp.d_slot_stage, sp.d_stage, sp.stage_stride))) return rc;
+        if ((rc = host_rows_transfer(m, true, m->d_nuniq[2], m->d_urow[2], sp.set.rec, sp.stage_stride))) return rc;
     }
     if (s == 0)
         shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
-            sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_peers, sp.nbags_cap, sp.width,
-            sp.d_slot_stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2]);
+            sp.n_slots, sp.set.rec.row_base, sp.set.rec.data, sp.set.rec.dim, sp.set.rec.stride, sp.d_peers, sp.nbags_cap, sp.width,
+            sp.set.rec.stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2]);
     else
         shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
             sp.d_wide, sp.d_peers, sp.nbags_cap);
@@ -645,7 +620,7 @@ static int shard_combine(WdModel* m, int s) {
     const int B = m->dbatch.B;
     const ShardPeer& me = sp.peers[S.rank];
     if (s == 0)
-        shard_combine_emb_kernel<<<grid_for((int64_t)B * sp.n_slots * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(B, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0,
+        shard_combine_emb_kernel<<<grid_for((int64_t)B * sp.n_slots * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(B, sp.n_slots, sp.set.rec.dim, sp.set.x0,
             sp.d_bagmask, me.bagscale, me.recv, S.world, sp.nbags_cap, sp.width, m->d_X0, m->d0_phys);
     else
         shard_combine_wide_kernel<<<grid_for(B, 256), 256, 0, m->stream>>>(B, sp.d_bagmask, me.recv, S.world, sp.nbags_cap, m->d_wide_logit);
@@ -662,19 +637,17 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
     const int L = 2 + s;
     int rc;
     if (s == 0) {
-        const PeerEmb src{m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.d_slot_dim, sp.d_slot_x0, m->d0_phys};
+        const PeerEmb src{m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.set.rec.dim, sp.set.x0, m->d0_phys};
         emb_grad_sum_kernel<PeerEmb, false><<<grid_for((m->max_nnz + m->cpart_cap) * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],
             m->d_ustart[L], m->d_choff[L], src, m->d_ugrad[L], m->d_cpart[L], sp.width, RowApply{});
         m->launches++;
         if ((rc = list_chunk_combine(m, L, sp.width))) return rc;
-        const RowRecords rec{sp.n_slots, sp.d_slot_base, sp.d_slot_data, sp.d_slot_dim, sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, nullptr};
         const OptParams o = space_opt(m, 0, sp.d_adam_touched);
-        if ((rc = list_apply_emb(m, L, sp.width, rec, o))) return rc;
+        if ((rc = list_apply_emb(m, L, sp.width, sp.set.rec, o))) return rc;
         // Adam: the shard's rows no rank touched, after its touched ones (no host-placed shards with Adam: no staged records)
-        if ((rc = adam_untouched_emb(m, rec, sp.d_slot_rows, sp.local_rows, o))) return rc;
+        if ((rc = adam_untouched_emb(m, sp.set, sp.local_rows, o))) return rc;
         // staged records home, on this stream: it joins the main stream before the step ends, so the next stage-in comes after
-        if (staged(m, s) && (rc = host_rows_transfer(m, false, m->d_nuniq[L], m->d_urow[L], sp.n_slots, sp.d_slot_base, sp.d_slot_data,
-                                                     sp.d_slot_stride, sp.d_slot_stage, sp.d_stage, sp.stage_stride))) return rc;
+        if (staged(m, s) && (rc = host_rows_transfer(m, false, m->d_nuniq[L], m->d_urow[L], sp.set.rec, sp.stage_stride))) return rc;
     } else {
         const PeerWide src{m->d_sv[L], sp.d_rtag, sp.d_peers};
         wide_grad_sum_kernel<PeerWide, false><<<grid_for(m->max_nnz + m->cpart_cap, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],

@@ -37,14 +37,11 @@ __global__ void __launch_bounds__(256) wide_fwd_kernel(int B, int C, const int32
 }
 
 // --------------------------------------------------------------------------------------- embedding forward
-// All tables of one width D (G = D/4 lanes per bag, float4 per lane).  Bag = (example b, table k).  Long multihot bags: a full
-// warp per bag, the 32/G lane groups take interleaved ids, then a shuffle tree combines them.
+// All tables of one width D (G = D/4 lanes per bag, float4 per lane), desc[k] = table k of the width (gather view).  Bag =
+// (example b, table k).  Long multihot bags: a full warp per bag, the 32/G lane groups take interleaved ids, then a shuffle tree
+// combines them.
 template <int G>
-__global__ void __launch_bounds__(256) emb_pool_fwd_kernel(int B, int C, int ntab, const int32_t* __restrict__ tab_ids,
-                                                           float* const* __restrict__ tab_data,
-                                                           const int32_t* __restrict__ tab_stride,
-                                                           const int32_t* __restrict__ tab_x0, const int32_t* __restrict__ tab_col,
-                                                           const int64_t* __restrict__ tab_row_base,
+__global__ void __launch_bounds__(256) emb_pool_fwd_kernel(int B, int C, int ntab, const TabDesc* __restrict__ desc,
                                                            const int32_t* __restrict__ offs, const uint32_t* __restrict__ e_emb,
                                                            float* __restrict__ X0, int ld) {
     constexpr int GROUPS = 32 / G;
@@ -53,12 +50,12 @@ __global__ void __launch_bounds__(256) emb_pool_fwd_kernel(int B, int C, int nta
     const int64_t gwarp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarp = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t bag = gwarp; bag < nbags; bag += nwarp) {
-        int b = (int)(bag / ntab), t = tab_ids[bag % ntab];
-        int c = tab_col[t];
-        int s = offs[(int64_t)b * C + c], e = offs[(int64_t)b * C + c + 1];
-        const float* base = tab_data[t] + lig * 4;
-        const int stride = tab_stride[t];
-        const int64_t rb = tab_row_base[t];
+        const int b = (int)(bag / ntab);
+        const TabDesc d = desc[bag % ntab];
+        int s = offs[(int64_t)b * C + d.col], e = offs[(int64_t)b * C + d.col + 1];
+        const float* base = d.data + lig * 4;
+        const int stride = d.stride;
+        const int64_t rb = d.row_base;
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         // 32 ids of the bag per round trip (one per lane), then the rows of the chunk that belong to this lane group eight at a
         // time back to back: the chain offsets -> ids -> rows is 2 + ceil(rows / (8 GROUPS)) dependent round trips per 32 ids
@@ -97,7 +94,7 @@ __global__ void __launch_bounds__(256) emb_pool_fwd_kernel(int B, int C, int nta
             float inv = 1.f / (float)n;
             acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
         }
-        if (grp == 0) *reinterpret_cast<float4*>(X0 + (int64_t)b * ld + tab_x0[t] + lig * 4) = acc;
+        if (grp == 0) *reinterpret_cast<float4*>(X0 + (int64_t)b * ld + d.x0 + lig * 4) = acc;
     }
 }
 
@@ -163,8 +160,8 @@ static void launch_emb_fwd(WdModel* m, int di, bool widebag) {
     } else {
         const int64_t nbags = (int64_t)m->dbatch.B * ntab;            // one warp per bag
         int grid = grid_for(nbags * 32, 256, kNumSms * 8);
-        emb_pool_fwd_kernel<G><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_tables[di],
-            m->d_gtab_data, m->d_gtab_stride, m->d_tab_x0, m->d_tab_col, m->d_gtab_row_base, m->d_col_offs, m->d_g_emb, m->d_X0, m->d0_phys);
+        emb_pool_fwd_kernel<G><<<grid, 256, 0, m->stream>>>(m->dbatch.B, m->n_columns, ntab, m->d_dim_desc[di], m->d_col_offs,
+                                                             m->d_g_emb, m->d_X0, m->d0_phys);
     }
     m->launches++;
 }
@@ -537,11 +534,9 @@ int sparse_reduce_emb(WdModel* m) {
         // the direct rows' records by table in plan order (a sum knows its table from the column), the hot rows' by table in row
         // order; host tables: the fused updates go to the staged records, host_tables_write_back copies them home after the list's apply
         const OptParams o = make_opt(m->dnn_opt);
-        const RowApply ra{m->d_urow[0], RowRecords{(int)m->tables.size(), m->d_tab_row_base, m->d_tab_data, m->d_tab_dim, m->d_tab_stride,
-                                                   m->d_tab_stage, m->d_stage, m->d_uslot}, nullptr, o};
-        const RowApply ha{m->d_urow[0], RowRecords{m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride,
-                                                   m->d_rtab_stage, m->d_stage, m->d_uslot}, nullptr, o};
-        const LocalEmb src{m->d_sv[0], m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->d_tab_dim, m->d_tab_x0, m->d_dX0, m->d0_phys};
+        const RowApply ra{m->d_urow[0], m->tabs.rec, nullptr, o};
+        const RowApply ha{m->d_urow[0], m->rtabs.rec, nullptr, o};
+        const LocalEmb src{m->d_sv[0], m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->tabs.rec.dim, m->tabs.x0, m->d_dX0, m->d0_phys};
         if (fused) {
             emb_grad_sum_kernel<LocalEmb, true><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], src,
                                                                           m->d_ugrad[0], m->d_cpart[0], width, ra);
@@ -634,7 +629,7 @@ int small_scatter(WdModel* m, int which) {
     if (which == 0) {
         if (m->n_small_tab == 0 || !(m->use_deep && !m->tables.empty())) return WD_OK;
         small_scatter_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], m->d_ugrad[0], m->emb_max_dim,
-            (uint32_t)m->small_base[0], m->n_rtab, m->d_rtab_row_base, m->d_rtab_dim, m->d_rtab_gs_off, block,
+            (uint32_t)m->small_base[0], m->rtabs.rec.ntab, m->rtabs.rec.row_base, m->rtabs.rec.dim, m->rtabs.gs_off, block,
             block + m->gs_touch_off[0], m->d_nubig[0]);
     } else {
         if (!m->use_wide || m->small_base[1] >= m->wide_rows) return WD_OK;
@@ -681,8 +676,9 @@ int small_apply(WdModel* m) {
     if (m->gs_count == 0) return WD_OK;
     const float* block = m->d_G + m->dense_count;
     if (m->gs_emb_floats > 0) {
-        small_apply_emb_kernel<<<grid_for(m->gs_emb_floats / 4, 256), 256, 0, m->stream>>>(block, block + m->gs_touch_off[0], m->gs_emb_floats / 4, m->n_rtab,
-            m->n_rtab - m->n_small_tab, m->small_base[0], m->d_rtab_row_base, m->d_rtab_gs_off, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride,
+        const RecordSet& rs = m->rtabs;
+        small_apply_emb_kernel<<<grid_for(m->gs_emb_floats / 4, 256), 256, 0, m->stream>>>(block, block + m->gs_touch_off[0], m->gs_emb_floats / 4, rs.rec.ntab,
+            rs.rec.ntab - m->n_small_tab, m->small_base[0], rs.rec.row_base, rs.gs_off, rs.rec.data, rs.rec.dim, rs.rec.stride,
             space_opt(m, 0, m->d_adam_touched[0]));
         m->launches++;
     }
@@ -701,9 +697,10 @@ OptParams space_opt(const WdModel* m, int space, uint32_t* touched) {
     const bool adam = o.kind == WD_OPT_ADAM;
     return make_opt(o, adam ? m->d_bpow + (space == 0 ? 2 : 0) : nullptr, adam ? touched : nullptr);
 }
-// the replicated tables' records in row order, in place (the unfused updates write host records through their mapped pointers)
-static RowRecords replicated_records(const WdModel* m) {
-    return RowRecords{m->n_rtab, m->d_rtab_row_base, m->d_rtab_data, m->d_rtab_dim, m->d_rtab_stride, nullptr, nullptr, nullptr};
+// the records of a set in place, none staged (the unfused updates write host records through their mapped pointers)
+static RowRecords in_place(RowRecords r) {
+    r.stage = nullptr;
+    return r;
 }
 
 int sparse_apply_which(WdModel* m, int which) {
@@ -712,13 +709,13 @@ int sparse_apply_which(WdModel* m, int which) {
     const bool done = m->list_apply_fused[which] && !m->sparse_overridden[which];
     m->list_apply_fused[which] = false;
     // the fused updates of host-table rows went to their staged copies: copy those home (the unfused kernels below update host
-    // records in place, through the mapped pointers of d_rtab_data)
+    // records in place, through their mapped pointers)
     if (done) return (which == 0 && m->n_host_tab > 0) ? host_tables_write_back(m) : WD_OK;
     if (which == 0 && m->cache_slots > 0) {       // the unfused updates below would write host records behind the cache's back
         set_error("embedding rows of a model with a host-table cache are only updated by the fused single-GPU step");
         return WD_EUNSUPPORTED;
     }
-    if (which == 0 && m->use_deep && !m->tables.empty() && (rc = list_apply_emb(m, 0, m->emb_max_dim, replicated_records(m), space_opt(m, 0, m->d_adam_touched[0]))))
+    if (which == 0 && m->use_deep && !m->tables.empty() && (rc = list_apply_emb(m, 0, m->emb_max_dim, in_place(m->rtabs.rec), space_opt(m, 0, m->d_adam_touched[0]))))
         return rc;
     if (which == 1 && m->use_wide && (rc = list_apply_wide(m, 1, m->d_wide, space_opt(m, 1, m->d_adam_touched[1])))) return rc;
     WD_CUDA(cudaGetLastError());
@@ -756,9 +753,9 @@ int list_apply_wide(WdModel* m, int which, float4* wide, const OptParams& o) {
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int adam_untouched_emb(WdModel* m, const RowRecords& rec, const int64_t* rows, int64_t nbits, const OptParams& o) {
-    if (o.kind != WD_OPT_ADAM || rec.ntab == 0 || nbits <= 0) return WD_OK;
-    adam_untouched_emb_kernel<<<grid_for(nbits, 256), 256, 0, m->stream>>>(rec, rows, nbits, o);    // (a warp per 32 rows)
+int adam_untouched_emb(WdModel* m, const RecordSet& set, int64_t nbits, const OptParams& o) {
+    if (o.kind != WD_OPT_ADAM || set.rec.ntab == 0 || nbits <= 0) return WD_OK;
+    adam_untouched_emb_kernel<<<grid_for(nbits, 256), 256, 0, m->stream>>>(in_place(set.rec), set.rows, nbits, o);    // (a warp per 32 rows)
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -773,7 +770,7 @@ int adam_untouched_wide(WdModel* m, float4* wide, int64_t nbits, const OptParams
 // Adam, the untouched passes of the replicated record sets: after both their lists and the dense block's small-table rows
 int adam_untouched_replicated(WdModel* m) {
     int rc;
-    if (m->use_deep && (rc = adam_untouched_emb(m, replicated_records(m), m->d_rtab_rows, m->emb_total_rows, space_opt(m, 0, m->d_adam_touched[0]))))
+    if (m->use_deep && (rc = adam_untouched_emb(m, m->rtabs, m->emb_total_rows, space_opt(m, 0, m->d_adam_touched[0]))))
         return rc;
     return m->use_wide ? adam_untouched_wide(m, m->d_wide, m->wide_rows, space_opt(m, 1, m->d_adam_touched[1])) : WD_OK;
 }

@@ -144,19 +144,6 @@ __device__ __forceinline__ void update_wide(const OptParams& o, float4* rec, flo
     *rec = r;
 }
 
-// Where the [w | s1 | s2] records of a list's embedding rows are.  Tables t < ntab with first row row_base[t] (ascending), records
-// of stride[t] floats at data[t].  A staged table (stage[t] != 0; stage null: none is) keeps the records of the step's rows in
-// stage_base instead, unique row u at staging row uslot[u] (u without a cache) with stride stage[t].
-struct RowRecords {
-    int ntab;
-    const int64_t* row_base;
-    float* const* data;
-    const int32_t* dim;
-    const int32_t* stride;
-    const int32_t* stage;
-    float* stage_base;
-    const int32_t* uslot;
-};
 // record of unique row u of the list (global row urow[u], read only for a record in place) in table t.  (Both cases are offsets
 // from the table pointer data[t], a pointer loaded from global memory: the compiler then keeps the record's loads and stores global
 // ones, where a choice between two pointers would make them generic.)
@@ -285,9 +272,9 @@ int list_apply_wide(WdModel* m, int which, float4* wide, const OptParams& o);
 // and the bitmap `touched` of the record set it updates
 OptParams space_opt(const WdModel* m, int space, uint32_t* touched);
 // Adam, the untouched pass of one record set (after every touched-row update of the step, on the stream that ran the last of
-// them): decay + step of every row whose bit in o.touched is clear, all bits cleared.  Embedding records as `rec` says (no staged
-// tables), table t holding rows[t] rows from row_base[t], bits 0 .. nbits; wide records wide[0 .. nbits).  Nothing unless o is Adam.
-int adam_untouched_emb(WdModel* m, const RowRecords& rec, const int64_t* rows, int64_t nbits, const OptParams& o);
+// them): decay + step of every row whose bit in o.touched is clear, all bits cleared.  Embedding records of `set` in place, table t
+// holding set.rows[t] rows from its row base, bits 0 .. nbits; wide records wide[0 .. nbits).  Nothing unless o is Adam.
+int adam_untouched_emb(WdModel* m, const RecordSet& set, int64_t nbits, const OptParams& o);
 int adam_untouched_wide(WdModel* m, float4* wide, int64_t nbits, const OptParams& o);
 
 }  // namespace wd
