@@ -267,6 +267,18 @@ int wd_shard_phase(WdModel *m, int slot, int phase, int train);
 int wd_shard_finish(WdModel *m, float *loss_out /* nullable */, float *logits_out /* nullable, [batch] */);
 int wd_shard_train_step_slot(WdModel *m, int slot, float *loss_out /* NULL: enqueue only */);
 int wd_shard_forward_slot(WdModel *m, int slot, float *logits_out, float *loss_out);
+/* Evaluation of a row-sharded model.  Each rank adds the metrics of its own rows to its accumulator (wd_eval_reset first), on the
+ * device; wd_shard_eval_finish then sums the accumulators of all ranks in rank order and returns the ten values of wd_eval_finish,
+ * the same bytes on every rank.  Every rank enters every forward: a rank whose shard of the data has run out uploads any one-row
+ * batch and passes n_valid = 0 (rows are masked by n_valid, not by weights).  "loss" is the mean over steps of the step's sum over
+ * the rows of all ranks.  wd_eval_reset / wd_eval_finish still see this rank's accumulator alone.
+ *   one process per GPU : wd_shard_eval_accumulate_slot (collective, once per step) = sharded forward of the slot's batch + metrics
+ *                         of its first n_valid rows; graphed per slot and n_valid.  wd_shard_eval_finish (collective).
+ *   one process, G handles: wd_shard_phase(train = 0) for phases 0..2 as for a forward, then wd_shard_eval_accumulate_phase on every
+ *                         rank; after the last step wd_shard_local_sync, then wd_shard_eval_finish on every rank. */
+int wd_shard_eval_accumulate_slot(WdModel *m, int slot, int32_t n_valid);
+int wd_shard_eval_accumulate_phase(WdModel *m, int32_t n_valid);
+int wd_shard_eval_finish(WdModel *m, double *out10);
 
 /* Streaming eval metrics (binary head, reference joint.py:402-406): accumulate per batch, then finish.
  * out[0..9] = accuracy, accuracy_baseline, auc, auc_precision_recall, average_loss, label/mean, loss,

@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """Evaluation entry point — drop-in for the reference's python/eval.py (same flags; prints the sorted metric
-dict, reference eval.py:56-83).  Evaluates what train.py wrote under <model_dir>/<model_type>."""
+dict, reference eval.py:56-83).  Evaluates what train.py wrote under <model_dir>/<model_type>.
+Multi-GPU: `torchrun --nproc-per-node G eval.py ...` (main_distributed below) evaluates the checkpoint with its large tables
+row-sharded over the G ranks; --batch_size is then per rank."""
 import argparse
 import os
 import sys
@@ -11,6 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from wide_deep_b200.config import Config  # noqa: E402
 from wide_deep_b200.dataset import input_fn  # noqa: E402
 from wide_deep_b200.estimator import build_estimator  # noqa: E402
+from train import distributed_env  # noqa: E402
 
 CONF = Config()
 CONFIG = CONF.train
@@ -24,23 +27,47 @@ parser.add_argument("--checkpoint_path", type=str, default=CONFIG["checkpoint_pa
                     help="Path of a specific checkpoint to evaluate. If None, the latest checkpoint in model_dir is used.")
 
 
-def main():
-    print("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow")
-    print("Model type: {}".format(FLAGS.model_type))
+def evaluate(log, rank=0, world=1, **kw):
+    log("Model type: {}".format(FLAGS.model_type))
     model_dir = os.path.join(FLAGS.model_dir, FLAGS.model_type)
-    print("Model directory: {}".format(model_dir))
-    model = build_estimator(model_dir, FLAGS.model_type, config=CONF, max_batch=FLAGS.batch_size)
+    log("Model directory: {}".format(model_dir))
+    model = build_estimator(model_dir, FLAGS.model_type, config=CONF, max_batch=FLAGS.batch_size, shard_world=world, shard_rank=rank, **kw)
     if not (FLAGS.checkpoint_path or model.latest_checkpoint()):
         raise ValueError("No model checkpoint found, please check the model dir.")
-    print("INFO: " + "=" * 30 + " START TESTING" + "=" * 30)
+    log("INFO: " + "=" * 30 + " START TESTING" + "=" * 30)
     s_time = time.time()
     results = model.evaluate(input_fn=lambda: input_fn(FLAGS.test_data, None, "eval", FLAGS.batch_size, config=CONF, plan=model.plan,
-                                                       device_parse=True),
+                                                       rank=rank, world=world, keep_tail=world > 1, device_parse=True),
                              checkpoint_path=FLAGS.checkpoint_path)
-    print("INFO: " + "=" * 30 + "FINISH TESTING, TAKE {} mins".format(round((time.time() - s_time) / 60, 2)) + "=" * 30)
-    print("-" * 80)
+    log("INFO: " + "=" * 30 + "FINISH TESTING, TAKE {} mins".format(round((time.time() - s_time) / 60, 2)) + "=" * 30)
+    log("-" * 80)
     for key in sorted(results):
-        print("%s: %s" % (key, results[key]))
+        log("%s: %s" % (key, results[key]))
+
+
+def main():
+    rank, world, local = distributed_env()
+    if world > 1:
+        return main_distributed(rank, world, local)
+    print("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow")
+    evaluate(print)
+
+
+def main_distributed(rank, world, local):
+    """torchrun --nproc-per-node G eval.py ...: the checkpoint's tables larger than 16384 rows are row-sharded over the G ranks (as
+    train.py's distributed mode trains them), rank r evaluates lines r, r + G, ... of the data, and one collective sums the
+    metrics of all ranks; rank 0 alone prints.  The metrics equal a single process's with a batch of G x --batch_size lines.
+    WD_SHARD_SAME_GPU=1 puts every rank on cuda:0 (a test setup, not a multi-GPU rate)."""
+    import torch
+    import torch.distributed as dist
+    device = 0 if os.environ.get("WD_SHARD_SAME_GPU") else local
+    torch.cuda.set_device(device)
+    dist.init_process_group("gloo")                    # plumbing only (IPC handles); metrics are summed over NVLink
+    log = print if rank == 0 else (lambda *a, **k: None)
+    log("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow: rank {} of {}".format(rank, world))
+    evaluate(log, rank, world, device=device)
+    dist.barrier()
+    dist.destroy_process_group()
 
 
 if __name__ == "__main__":

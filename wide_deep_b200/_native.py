@@ -70,6 +70,9 @@ SYMBOLS = {
     "wd_shard_finish": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_float), _vp]),
     "wd_shard_train_step_slot": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.POINTER(ctypes.c_float)]),
     "wd_shard_forward_slot": (ctypes.c_int, [_vp, ctypes.c_int, _vp, ctypes.POINTER(ctypes.c_float)]),
+    "wd_shard_eval_accumulate_slot": (ctypes.c_int, [_vp, ctypes.c_int, _i32]),
+    "wd_shard_eval_accumulate_phase": (ctypes.c_int, [_vp, _i32]),
+    "wd_shard_eval_finish": (ctypes.c_int, [_vp, _vp]),
     "wd_eval_reset": (ctypes.c_int, [_vp]),
     "wd_eval_accumulate": (ctypes.c_int, [_vp, _vp]),
     "wd_eval_finish": (ctypes.c_int, [_vp, _vp]),

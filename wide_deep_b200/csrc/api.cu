@@ -103,6 +103,7 @@ extern "C" int wd_model_destroy(WdModel* m) {
         sl.train.destroy();
         sl.bwd.destroy();
         sl.shard.destroy();
+        sl.shard_eval.destroy();
         if (sl.ev_up) cudaEventDestroy(sl.ev_up);
         if (sl.ev_used) cudaEventDestroy(sl.ev_used);
     }
@@ -254,7 +255,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         WD_CUDA(cudaMemcpyAsync(m->d_bpow, bp, sizeof(bp), cudaMemcpyHostToDevice, m->stream));
         WD_CUDA(cudaStreamSynchronize(m->stream));
     }
-    if ((rc = dev_alloc(m, &m->d_metrics, 512))) return rc;
+    if (G == 1 && (rc = dev_alloc(m, &m->d_metrics, kMetricsDoubles))) return rc;   // (sharded: in the exchange segment, shard_build)
     WD_CUDA(cudaMallocHost(&m->h_loss_pinned, 64));
 
     // ---- dense tensors
@@ -1409,11 +1410,60 @@ extern "C" int wd_shard_forward_slot(WdModel* m, int slot, float* logits_out, fl
     return finish_step(m, loss_out, logits_out);
 }
 
+// ---- evaluation of a row-sharded model: every rank adds the metrics of its own rows to its accumulator (wd_eval_reset /
+// wd_eval_finish: this rank's alone), then one collective sums the accumulators of all ranks
+namespace wd { int shard_metrics_reduce(WdModel* m); }
+
+static int check_eval_rows(WdModel* m, int32_t n_valid) {
+    if (n_valid < 0 || n_valid > m->dbatch.B) { set_error("n_valid %d outside [0, batch size %d]", n_valid, m->dbatch.B); return WD_EINVAL; }
+    if (n_valid > 0 && !m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
+    return WD_OK;
+}
+
+// Collective (multi-process ranks): the sharded forward of the slot's batch, then the metrics of its first n_valid rows, all on the
+// device.  A rank without rows left enters with any one-row batch and n_valid = 0: its forward still serves its peers.  Graphed per
+// batch slot and n_valid.
+extern "C" int wd_shard_eval_accumulate_slot(WdModel* m, int slot, int32_t n_valid) {
+    int rc = shard_ready(m, slot);
+    if (rc) return rc;
+    if (!m->shard.ipc) { set_error("wd_shard_eval_accumulate_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase + wd_shard_eval_accumulate_phase)"); return WD_ESTATE; }
+    if ((rc = check_eval_rows(m, n_valid))) return rc;
+    auto issue = [&](bool) { int r = shard_step_ipc(m, false); return r ? r : metrics_accumulate(m, n_valid); };
+    GraphRun how;
+    if ((rc = run_graphed(m, m->slots[slot].shard_eval, ShardEvalKey{m->dbatch, n_valid}, m->stream, issue, &how))) return rc;
+    if (how == GraphRun::replayed) { m->shard.step++; m->eval_batches++; }   // (a capture ran the issuing code, which advanced both)
+    if ((rc = mark_slot_used(m))) return rc;
+    return finish_step(m, nullptr, nullptr);
+}
+
+// Ranks of one process: after phases 0..2 of wd_shard_phase(train = 0) on every rank, the metrics of the first n_valid rows of
+// this rank's logits.
+extern "C" int wd_shard_eval_accumulate_phase(WdModel* m, int32_t n_valid) {
+    int rc = shard_ready(m, m->cur_slot);
+    if (rc) return rc;
+    if (m->shard.ipc) { set_error("wd_shard_eval_accumulate_phase is for ranks of one process; multi-process ranks call wd_shard_eval_accumulate_slot"); return WD_ESTATE; }
+    if ((rc = check_eval_rows(m, n_valid))) return rc;
+    return metrics_accumulate(m, n_valid);
+}
+
+// Collective: the ten metrics of every rank's rows, identical bytes on every rank.  Multi-process ranks meet at flag barriers
+// inside; ranks of one process call wd_shard_local_sync after their last accumulate, then this on every rank.
+extern "C" int wd_shard_eval_finish(WdModel* m, double* out10) {
+    int rc = check_ready(m);
+    if (rc) return rc;
+    if (!out10) { set_error("wd_shard_eval_finish: null output"); return WD_EINVAL; }
+    if (m->shard.world <= 1) { set_error("model has no row-sharded tables (shard_world <= 1)"); return WD_ESTATE; }
+    if (!m->shard.connected) { set_error("row-sharded model is not connected to its peers (wd_shard_connect_ipc / wd_shard_connect_local)"); return WD_ESTATE; }
+    if ((rc = shard_metrics_reduce(m))) return rc;
+    if ((rc = finish_step(m, nullptr, nullptr))) return rc;          // (a peer that never arrived shows in the flags)
+    return metrics_finish(m, m->shard.d_msum, out10);
+}
+
 // ------------------------------------------------------------------------------------------------- eval
 extern "C" int wd_eval_reset(WdModel* m) {
     int rc = check_ready(m);
     if (rc) return rc;
-    WD_CUDA(cudaMemsetAsync(m->d_metrics, 0, 512 * sizeof(double), m->stream));
+    WD_CUDA(cudaMemsetAsync(m->d_metrics, 0, kMetricsDoubles * sizeof(double), m->stream));
     m->eval_batches = 0;
     return WD_OK;
 }
@@ -1422,7 +1472,7 @@ extern "C" int wd_eval_accumulate(WdModel* m, const WdBatch* b) {
     if (rc) return rc;
     if (!m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
     if ((rc = forward_core(m, false))) return rc;
-    if ((rc = metrics_accumulate(m))) return rc;
+    if ((rc = metrics_accumulate(m, m->dbatch.B))) return rc;
     return finish_step(m, nullptr, nullptr);
 }
 extern "C" int wd_eval_accumulate_slot(WdModel* m, int slot) {
@@ -1432,14 +1482,14 @@ extern "C" int wd_eval_accumulate_slot(WdModel* m, int slot) {
     if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
     if (!m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
     if ((rc = forward_core(m, false))) return rc;
-    if ((rc = metrics_accumulate(m))) return rc;
+    if ((rc = metrics_accumulate(m, m->dbatch.B))) return rc;
     if ((rc = mark_slot_used(m))) return rc;
     return finish_step(m, nullptr, nullptr);
 }
 extern "C" int wd_eval_finish(WdModel* m, double* out10) {
     int rc = check_ready(m);
     if (rc) return rc;
-    return metrics_finish(m, out10);
+    return metrics_finish(m, m->d_metrics, out10);
 }
 
 // ------------------------------------------------------------------------------------------ debug / misc

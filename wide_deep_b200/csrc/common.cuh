@@ -34,6 +34,7 @@ constexpr int kMaxDims = 8;      // distinct embedding widths per model
 // grouped by owner rank (routing; only the key / value ping-pong buffers exist)
 constexpr int kLists = 6;
 constexpr int kMaxRanks = 16;    // ranks of one box a row-sharded table can be split over
+constexpr int kMetricsDoubles = 512;  // doubles of an eval metric accumulator (layout: misc.cu)
 
 // ---- device image of the categorical-column plan (all pointers are device pointers)
 struct DevPlan {
@@ -205,6 +206,12 @@ struct MergeKey {            // key of a list's merge graph (wd_sparse_set_sorte
     }
 };
 
+struct ShardEvalKey {        // key of a slot's eval graph on a row-sharded model (wd_shard_eval_accumulate_slot)
+    DevBatch b;
+    int n_valid;
+    bool operator==(const ShardEvalKey& o) const { return b == o.b && n_valid == o.n_valid; }
+};
+
 struct BatchSlot {           // one device-resident batch (ring used by benchmarks / prefetch)
     int32_t* off = nullptr;
     uint64_t* keys = nullptr;
@@ -219,6 +226,7 @@ struct BatchSlot {           // one device-resident batch (ring used by benchmar
     StepGraph<DevBatch> train;               // whole train step (wd_train_step_slot)
     StepGraph<DevBatch> bwd;                 // forward + backward of the split step (wd_step_backward_slot), side streams joined at its end
     StepGraph<DevBatch> shard;               // whole rank-step of a row-sharded model (wd_shard_train_step_slot)
+    StepGraph<ShardEvalKey> shard_eval;      // sharded forward + metrics of its first n_valid rows (wd_shard_eval_accumulate_slot)
     bool bwd_side_active[2] = {false, false};   // side_active as the captured backward left it
 };
 
@@ -273,6 +281,8 @@ struct ShardState {
     ShardSpace sp[2];
     // flag barriers: flags[k][r] = last epoch rank r signalled on barrier k (written by rank r, through peer memory)
     int64_t off_flags = 0, off_gred = 0, off_G = 0;
+    int64_t off_metrics = 0;            // this rank's eval metric accumulator (WdModel::d_metrics points here)
+    double* d_msum = nullptr;           // [kMetricsDoubles] every rank's accumulator summed in rank order (wd_shard_eval_finish)
     uint32_t** d_peer_flags = nullptr;  // [G] device array of peers' flag blocks
     uint32_t* d_epoch = nullptr;        // [kBarriers] local epoch counters
     unsigned long long* d_trace = nullptr;   // WD_SHARD_TRACE=1: [kBarriers][2] enter / leave stamps of the last step's barriers
@@ -510,8 +520,8 @@ int tsv_parse_device(WdModel* m, const WdTsvSpec* sp, const char* text, int64_t 
                      uint64_t* keys, float* dense, float* label, float* weight, cudaStream_t st, int* status);
 int tsv_parse_host(const WdTsvSpec* sp, const char* text, const int64_t* starts, int n, WdBatch* out);   // tsv.cu
 void tsv_dev_destroy(WdModel* m);                                // tsv.cu
-int metrics_accumulate(WdModel* m);                              // metrics.cu
-int metrics_finish(WdModel* m, double* out10);
+int metrics_accumulate(WdModel* m, int rows);                    // misc.cu: metrics of the first `rows` logits of the batch
+int metrics_finish(WdModel* m, const double* acc, double* out10); // misc.cu: the ten metrics of an accumulator (synchronises)
 
 // sorts (*keys, *vals) of length *d_n by the low `bits` bits of the key, with (*keys2, *vals2) as ping-pong buffers; the
 // pointers are swapped so that the sorted pairs end in (*keys, *vals)

@@ -121,19 +121,19 @@ int metrics_setup() {
     return WD_OK;
 }
 
-int metrics_accumulate(WdModel* m) {
-    metrics_kernel<<<grid_for(m->dbatch.B, 256, kNumSms), 256, 0, m->stream>>>(m->dbatch.B, m->d_logits, m->d_label, m->dbatch.weight, m->d_metrics);
+int metrics_accumulate(WdModel* m, int rows) {
+    metrics_kernel<<<grid_for(rows, 256, kNumSms), 256, 0, m->stream>>>(rows, m->d_logits, m->d_label, m->dbatch.weight, m->d_metrics);
     m->launches++;
     m->eval_batches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 
-int metrics_finish(WdModel* m, double* out) {
+int metrics_finish(WdModel* m, const double* acc, double* out) {
     const int H = kNumThr + 1;
     double a[2 * H + 8];
     WD_CUDA(cudaStreamSynchronize(m->stream));
-    WD_CUDA(cudaMemcpy(a, m->d_metrics, sizeof(a), cudaMemcpyDeviceToHost));
+    WD_CUDA(cudaMemcpy(a, acc, sizeof(a), cudaMemcpyDeviceToHost));
     const double eps = 1e-7;
     double P = 0, Nn = 0;
     for (int k = 0; k < H; ++k) { P += a[k]; Nn += a[H + k]; }

@@ -332,6 +332,17 @@ __global__ void __launch_bounds__(256) shard_ar_gather_kernel(float* const* __re
     }
 }
 
+// ------------------------------------------------------------------------------------------- eval metrics: reduction
+// every rank's metric accumulator (in its exchange segment) summed in rank order: the same doubles, bit for bit, on every rank
+struct PeerMetrics { const double* acc[kMaxRanks]; };
+__global__ void __launch_bounds__(256) shard_metrics_reduce_kernel(PeerMetrics peers, int G, double* __restrict__ out) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < kMetricsDoubles; i += gridDim.x * blockDim.x) {
+        double s = __ldcg(peers.acc[0] + i);
+        for (int r = 1; r < G; ++r) s += __ldcg(peers.acc[r] + i);
+        out[i] = s;
+    }
+}
+
 // ================================================================================================== host side
 static int bits_for64(int64_t n) { int b = 1; while ((1ll << b) < n) ++b; return b; }
 static int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
@@ -448,6 +459,7 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     S.ar_count = align_up(m->dense_count + m->gs_count, 4);
     S.off_G = take(std::max<int64_t>(S.ar_count, 4) * 4);
     S.off_gred = take(std::max<int64_t>(S.ar_count, 4) * 4);
+    S.off_metrics = take(kMetricsDoubles * 8);
     S.seg_bytes = off;
     void* seg = nullptr;
     cudaError_t e = cudaMalloc(&seg, (size_t)S.seg_bytes);
@@ -460,6 +472,8 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     m->d_dlogit = reinterpret_cast<float*>(S.seg + S.sp[1].off_grad);
     m->d_G = reinterpret_cast<float*>(S.seg + S.off_G);
     S.gred = reinterpret_cast<float*>(S.seg + S.off_gred);
+    m->d_metrics = reinterpret_cast<double*>(S.seg + S.off_metrics);      // peers read it in wd_shard_eval_finish
+    if ((rc = dev_alloc(m, &S.d_msum, kMetricsDoubles))) return rc;
     if ((rc = dev_alloc(m, &S.d_peer_flags, kMaxRanks))) return rc;
     if ((rc = dev_alloc(m, &S.d_epoch, kBarriers))) return rc;
     if (getenv("WD_SHARD_TRACE") && (rc = dev_alloc(m, &S.d_trace, 2 * kBarriers))) return rc;
@@ -500,7 +514,7 @@ int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d) {
                  + (int64_t)G * nbags * width * 4 + nbags * 4;        // recv, bagscale
     }
     const int64_t x0n = m->use_deep ? (int64_t)m->max_batch_pad * std::max(m->d0_phys, 1) : 4;
-    bytes += x0n * 4 + (int64_t)m->max_batch * 4 + 2 * align_up(m->dense_count + m->gs_count + 4, 4) * 4;
+    bytes += x0n * 4 + (int64_t)m->max_batch * 4 + 2 * align_up(m->dense_count + m->gs_count + 4, 4) * 4 + 2 * kMetricsDoubles * 8;
     return bytes;
 }
 
@@ -763,6 +777,21 @@ int shard_phase4(WdModel* m) {
     if ((rc = shard_apply_local(m))) return rc;
     m->shard.step++;
     return WD_OK;
+}
+
+// Collective eval finish: every rank's metric accumulator summed in rank order into S.d_msum.  Multi-process ranks meet at a flag
+// barrier before the sum (every accumulator final) and after it (no rank resets or adds to its accumulator while a peer still
+// reads it); ranks of one process are ordered by the caller (wd_shard_local_sync after the last accumulate).
+int shard_metrics_reduce(WdModel* m) {
+    ShardState& S = m->shard;
+    int rc;
+    if ((rc = barrier(m, BAR_END))) return rc;
+    PeerMetrics peers{};
+    for (int r = 0; r < S.world; ++r) peers.acc[r] = reinterpret_cast<const double*>(S.peer_seg[r] + S.off_metrics);
+    shard_metrics_reduce_kernel<<<2, 256, 0, m->stream>>>(peers, S.world, S.d_msum);
+    m->launches++;
+    WD_CUDA(cudaGetLastError());
+    return barrier(m, BAR_END);
 }
 
 // The whole step of one rank of a multi-process job.  Main stream: ids, routing, serve, combine, towers, dense all-reduce and

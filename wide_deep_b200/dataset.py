@@ -10,7 +10,8 @@ Differences kept explicit:
   * shuffle: the reference shuffles with tf.data (buffer = num_examples, seed 123, dataset.py:180); that RNG
     stream cannot be reproduced outside TensorFlow, so 'train' mode shuffles whole files' lines with
     numpy's Philox(seed 123) instead — same intent (one seeded pass), different permutation;
-  * distributed sharding: every ``world``-th line starting at ``rank`` (dataset.shard, dataset.py:173-174).
+  * distributed sharding: every ``world``-th line starting at ``rank`` (dataset.shard, dataset.py:173-174); training drops the
+    last ``n_lines % world`` lines, evaluation and prediction keep them (``keep_tail``, ``shard_steps``).
 """
 from __future__ import annotations
 
@@ -330,15 +331,52 @@ class Prefetcher(object):
         return item
 
 
+def shard_steps(n_lines, world, batch_size):
+    """A file of ``n_lines`` lines split over ``world`` ranks with its tail kept (rank r: lines r, r + world, ...) and batched per
+    rank -> (steps, n_valid): the number of collective steps every rank runs, and n_valid[r][s], the lines rank r holds in step
+    s (0: the rank has run out and only serves its peers).  Every rank computes the same, without communicating."""
+    per = np.array([len(range(r, n_lines, world)) for r in range(world)], dtype=np.int64)
+    steps = -(-int(per[0]) // batch_size)                         # rank 0 holds the most lines
+    n_valid = np.clip(per[:, None] - np.arange(steps, dtype=np.int64)[None, :] * batch_size, 0, batch_size)
+    return steps, n_valid
+
+
+def interleave_ranks(parts):
+    """Inverse of the line split: ``parts[r]`` holds a value per line of rank r -> one array in file order (line i of the file is
+    line i // G of rank i % G)."""
+    G = len(parts)
+    out = np.empty(sum(len(p) for p in parts), dtype=np.result_type(*parts))
+    for r, p in enumerate(parts):
+        out[r::G] = p
+    return out
+
+
+class ShardPass(object):
+    """One rank's pass over its lines of a file split over ``world`` ranks with the tail kept (``input_fn(keep_tail=True)``): iterates
+    the rank's batches; ``steps`` and ``n_valid`` (this rank's lines per step) come from ``shard_steps``."""
+
+    def __init__(self, batches, n_lines, rank, world, batch_size):
+        self._batches = batches
+        self.n_lines = n_lines
+        self.steps, n_valid = shard_steps(n_lines, world, batch_size)
+        self.n_valid = [int(v) for v in n_valid[rank]]
+
+    def __iter__(self):
+        return self._batches
+
+
 def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=None, rank=0, world=1, seed=123, pinned=False,
-             device_parse=False):
+             device_parse=False, keep_tail=False):
     """Iterator of ``Batch`` for one pass over the data (one epoch), mirroring the reference's
     ``input_fn(csv_data_file, img_data_file, mode, batch_size)`` (dataset.py:293-310).  ``img_data_file`` is
     accepted for signature compatibility and must be None (the CNN branch is out of scope).
     The files are read and the pinned ring is allocated HERE (on the caller's thread, whose CUDA device is the model's); only
     the per-batch parsing is lazy, so the returned iterator may be drained from a prefetch thread.
     ``device_parse=True``: the same lines, in the same batches, are yielded as ``TsvTextBatch`` (the batch's text gathered into a
-    ring of page-locked buffers) for ``WideDeepModel.parse_slot``, which parses them on the GPU; ``pinned`` is then irrelevant."""
+    ring of page-locked buffers) for ``WideDeepModel.parse_slot``, which parses them on the GPU; ``pinned`` is then irrelevant.
+    ``keep_tail=True`` (evaluation and prediction with ``world > 1``): rank r gets every line r, r + world, ... to the end of the
+    file, and the result is a ``ShardPass``, which also tells how many steps every rank runs and how many lines rank r holds in
+    each."""
     assert mode in ("train", "eval", "pred"), "mode must in `train`, `eval`, or `pred`, found {}".format(mode)
     if img_data_file:
         raise ValueError("image inputs are not supported by this library (cnn_use_flag: 0)")
@@ -360,9 +398,11 @@ def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=N
     order = np.arange(n_all, dtype=np.int64)
     if world > 1:
         # dataset.shard(num_workers, worker_index) (reference dataset.py:173-174): every world-th line.  Synchronous training
-        # needs the same number of batches on every rank, so the few lines beyond a multiple of `world` are dropped.
-        per = n_all // world
-        order = order[rank::world][:per]
+        # needs the same number of batches on every rank, so the few lines beyond a multiple of `world` are dropped; with the
+        # tail kept, ranks that run out enter the remaining steps without rows (ShardPass.n_valid)
+        order = order[rank::world]
+        if not keep_tail:
+            order = order[:n_all // world]
     if mode == "train":
         perm = np.random.Generator(np.random.Philox(seed)).permutation(len(order))
         order = order[perm]
@@ -375,7 +415,7 @@ def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=N
             for i in range(0, len(order), batch_size):
                 yield reader.gather_text(text, starts, lens, order[i:i + batch_size], tring)
 
-        return texts()
+        return ShardPass(texts(), n_all, rank, world, batch_size) if keep_tail else texts()
     # pinned=True (estimator.train, which consumes batch by batch): parse into a ring of page-locked buffers so the host->device
     # refill of a batch slot is truly asynchronous; a yielded Batch stays valid for the next `depth - 1` batches
     ring = None
@@ -387,4 +427,4 @@ def input_fn(csv_data_file, img_data_file, mode, batch_size, config=None, plan=N
         for i in range(0, len(order), batch_size):
             yield reader.parse_indexed(text, starts, lens, order[i:i + batch_size], ring=ring)
 
-    return batches()
+    return ShardPass(batches(), n_all, rank, world, batch_size) if keep_tail else batches()

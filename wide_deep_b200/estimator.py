@@ -17,7 +17,7 @@ import time
 import numpy as np
 
 from .config import Config
-from .model import WideDeepModel
+from .model import Batch, WideDeepModel
 from .plan import compile_plan
 
 CKPT_PREFIX = "model.ckpt-"
@@ -196,10 +196,9 @@ class WideAndDeepClassifier(object):
         return due
 
     def evaluate(self, input_fn, steps=None, hooks=None, checkpoint_path=None, name=None):
-        if self.shard_world > 1:
-            raise ValueError("evaluate() on a multi-GPU (row-sharded) estimator: the reference's distributed mode trains only "
-                             "(train.py:215-216); evaluate with a single-process estimator on the saved checkpoint")
         m = self._ensure_model(checkpoint_path, need_trained=True)
+        if self.shard_world > 1:
+            return self._evaluate_sharded(m, input_fn, steps)
         m.eval_reset()
         n = 0
         from .dataset import TsvTextBatch
@@ -220,12 +219,85 @@ class WideAndDeepClassifier(object):
         out["global_step"] = m.global_step
         return out
 
+    # ------------------------------------------------------------------ multi-GPU evaluation and prediction
+    # The reference's distributed mode only trains (train.py:215-216).  Here every rank runs the collective forward of the
+    # row-sharded model on its lines of the file (input_fn(..., rank, world, keep_tail=True), a ShardPass that also says how many
+    # steps every rank runs): the tables are read where they live, in the GPUs that trained them.
+
+    def _rank_pass(self, input_fn):
+        data = input_fn()
+        if not hasattr(data, "n_valid"):
+            raise ValueError("a multi-GPU evaluate() / predict() needs this rank's lines with the file's tail kept: "
+                             "input_fn(..., rank=r, world=G, keep_tail=True)")
+        return data
+
+    def _fill_slot(self, m, slot, item, n_valid):
+        """Slot `slot` <- this step's batch of the rank, or a one-row placeholder once its lines have run out (n_valid 0: the
+        rank still serves its peers' ids in the collective forward)."""
+        from .dataset import TsvTextBatch
+        if n_valid == 0:
+            F, Nd = len(self.plan.cat_fields), len(self.plan.dense_fields)
+            item = Batch(1, np.zeros(F, dtype=np.uint64), None, np.zeros((1, Nd), dtype=np.float32) if Nd else None,
+                         np.zeros(1, dtype=np.float32))
+        if isinstance(item, TsvTextBatch):
+            m.parse_slot(slot, item)
+        else:
+            m.upload_slot(slot, item)
+        return item
+
+    def _evaluate_sharded(self, m, input_fn, steps):
+        """Every rank adds the metrics of its own rows on the device; one collective sums them in rank order.  Returns the same
+        dict on every rank.  "loss" is the mean over steps of the sum over the step's rows of all ranks: what one process computes
+        with a batch of world x batch_size lines."""
+        from .dataset import TsvTextBatch
+        data = self._rank_pass(input_fn)
+        n = min(data.steps, steps) if steps else data.steps
+        it = iter(data)
+        self._trainer.eval_reset()
+        for s in range(n):
+            nv = data.n_valid[s]
+            batch = self._fill_slot(m, 0, next(it) if nv else None, nv)
+            if nv and not (batch.has_label if isinstance(batch, TsvTextBatch) else batch.label is not None):
+                raise ValueError("evaluate needs labelled data (the reference's `pred`-mode test call, train.py:96-101, "
+                                 "fails the same way inside TensorFlow)")
+            self._trainer.eval_accumulate_slot(0, nv)
+        out = self._trainer.eval_finish()
+        out["global_step"] = m.global_step
+        return out
+
+    def _predict_sharded(self, m, input_fn):
+        """Every rank runs the collective forward on its lines; rank 0 gathers the logits through the process group and returns
+        them in file order, the other ranks None."""
+        import torch.distributed as dist
+        data = self._rank_pass(input_fn)
+        it = iter(data)
+        mine = []
+        for s in range(data.steps):
+            nv = data.n_valid[s]
+            self._fill_slot(m, 0, next(it) if nv else None, nv)
+            logits, _ = self._trainer.forward_slot(0, max(nv, 1))
+            mine.append(logits[:nv])
+        mine = np.concatenate(mine) if mine else np.zeros(0, dtype=np.float32)
+        parts = [None] * self.shard_world if self.shard_rank == 0 else None
+        dst = dist.get_global_rank(self.group, 0) if self.group is not None else 0
+        dist.gather_object(mine, parts, dst=dst, group=self.group)
+        if self.shard_rank != 0:
+            return None
+        from .dataset import interleave_ranks
+        return interleave_ranks(parts)
+
     def predict(self, input_fn, predict_keys=None, hooks=None, checkpoint_path=None):
+        """Iterator of prediction dicts in input order.  Multi-GPU: a collective, so every rank must drain it; rank 0 yields every
+        line's prediction in file order, the other ranks nothing."""
         m = self._ensure_model(checkpoint_path, need_trained=True)
-        for batch in input_fn():
-            logits, _ = m.forward(batch)
+        if self.shard_world > 1:
+            logits = self._predict_sharded(m, input_fn)
+            batches = [] if logits is None else [logits]
+        else:
+            batches = (m.forward(batch)[0] for batch in input_fn())
+        for logits in batches:
             p = 1.0 / (1.0 + np.exp(-logits.astype(np.float64)))
-            for i in range(batch.batch_size):
+            for i in range(len(logits)):
                 yield {"logits": np.array([logits[i]], dtype=np.float32), "logistic": np.array([p[i]], dtype=np.float32),
                        "probabilities": np.array([1 - p[i], p[i]], dtype=np.float32),
                        "class_ids": np.array([int(logits[i] > 0)]), "classes": np.array([str(int(logits[i] > 0)).encode()])}

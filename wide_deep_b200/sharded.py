@@ -10,6 +10,9 @@ single GPU computes on the concatenated batch.  All traffic moves through peer m
   ``ShardedTrainer``    one process per GPU (torchrun): ``step_slot`` is a collective call.
   ``LocalShardGroup``   G model handles in ONE process (any number of GPUs, also one): the phases of a step are ordered with
                         events instead of flag barriers.  This is what the single-GPU parity tests drive.
+
+Evaluation: every rank adds the metrics of its own rows to its accumulator on the device, and one collective sums the
+accumulators of all ranks in rank order (``eval_finish`` / ``evaluate``): the same ten values on every rank.
 """
 from __future__ import annotations
 
@@ -19,6 +22,7 @@ import numpy as np
 
 from . import _native
 from ._native import check
+from .model import METRIC_KEYS
 
 N_PHASES = 5
 
@@ -66,6 +70,27 @@ class LocalShardGroup(object):
             loss = ctypes.c_float()
             check(self._lib.wd_shard_finish(m._h, ctypes.byref(loss), logits.ctypes.data))
             out.append(logits)
+        return out
+
+    def evaluate(self, batches_per_rank, n_valid_per_rank, slot=0):
+        """Metrics of the first ``n_valid_per_rank[r][s]`` rows of ``batches_per_rank[r][s]`` over every rank r and step s, from
+        one collective reduction -> list of one metric dict per rank (identical).  Every rank runs every step: a rank without
+        rows left passes any one-row batch with n_valid 0."""
+        steps = len(batches_per_rank[0])
+        for m in self.models:
+            m.eval_reset()
+        for s in range(steps):
+            for m, bs in zip(self.models, batches_per_rank):
+                m.upload_slot(slot, bs[s])
+            self._run(slot, False)
+            for m, nv in zip(self.models, n_valid_per_rank):
+                check(self._lib.wd_shard_eval_accumulate_phase(m._h, int(nv[s])))
+        self._sync()
+        out = []
+        for m in self.models:
+            v = np.zeros(10, dtype=np.float64)
+            check(self._lib.wd_shard_eval_finish(m._h, v.ctypes.data))
+            out.append(dict(zip(METRIC_KEYS, (float(x) for x in v))))
         return out
 
     def get_tensor(self, name, slot=0):
@@ -118,10 +143,27 @@ class ShardedTrainer(object):
 
     def forward(self, batch, slot=0):
         self.model.upload_slot(slot, batch)
-        logits = np.empty(batch.batch_size, dtype=np.float32)
+        return self.forward_slot(slot, batch.batch_size)
+
+    def forward_slot(self, slot, batch_size):
+        """Collective forward of the batch of ``batch_size`` rows a slot holds -> (logits, loss)."""
+        logits = np.empty(batch_size, dtype=np.float32)
         loss = ctypes.c_float()
         check(self._lib.wd_shard_forward_slot(self.model._h, int(slot), logits.ctypes.data, ctypes.byref(loss)))
         return logits, loss.value
+
+    def eval_reset(self):
+        self.model.eval_reset()
+
+    def eval_accumulate_slot(self, slot, n_valid):
+        """Collective: sharded forward of the slot's batch, metrics of its first ``n_valid`` rows into this rank's accumulator."""
+        check(self._lib.wd_shard_eval_accumulate_slot(self.model._h, int(slot), int(n_valid)))
+
+    def eval_finish(self):
+        """Collective: metric dict of every rank's rows (the same on every rank)."""
+        v = np.zeros(10, dtype=np.float64)
+        check(self._lib.wd_shard_eval_finish(self.model._h, v.ctypes.data))
+        return dict(zip(METRIC_KEYS, (float(x) for x in v)))
 
     def get_tensor(self, name, slot=0):
         """Global tensor on every rank (row-sharded tensors are all-gathered through the host and interleaved)."""
