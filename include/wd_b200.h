@@ -254,8 +254,10 @@ int wd_sparse_set_sorted(WdModel *m, int which, const void *rows_dev, const void
  *   one process per GPU : every rank calls wd_shard_ipc_handle, the 64-byte handles are all-gathered by the host (any transport),
  *                         wd_shard_connect_ipc maps the peers; then wd_shard_train_step_slot / wd_shard_forward_slot are
  *                         COLLECTIVE calls (every rank, once per step); ranks meet at flag barriers in peer memory.
- *   one process, G handles (tests, also on a single GPU): wd_shard_connect_local; then for phase k = 0..4: wd_shard_phase on
- *                         every rank followed by wd_shard_local_sync (event barrier), wd_shard_finish for the loss.
+ *   one process, G handles (tests, also on a single GPU): wd_shard_connect_local; then for k = 0..4: wd_shard_phase on every
+ *                         rank, which runs segment k of the rank-step that wd_shard_train_step_slot runs whole, followed by
+ *                         wd_shard_local_sync, which stands in for the flag barriers closing the segment (events); then
+ *                         wd_shard_finish for the loss.
  * Parameters of sharded tables are addressed per rank: wd_tensor_io / wd_tensor_size see this rank's rows (global rows rank,
  * rank + G, rank + 2G, ...). */
 int wd_shard_info(WdModel *m, int32_t *world, int32_t *rank, int64_t *segment_bytes);
@@ -274,7 +276,7 @@ int wd_shard_forward_slot(WdModel *m, int slot, float *logits_out, float *loss_o
  * the rows of all ranks.  wd_eval_reset / wd_eval_finish still see this rank's accumulator alone.
  *   one process per GPU : wd_shard_eval_accumulate_slot (collective, once per step) = sharded forward of the slot's batch + metrics
  *                         of its first n_valid rows; graphed per slot and n_valid.  wd_shard_eval_finish (collective).
- *   one process, G handles: wd_shard_phase(train = 0) for phases 0..2 as for a forward, then wd_shard_eval_accumulate_phase on every
+ *   one process, G handles: wd_shard_phase(train = 0) for segments 0..2 as for a forward, then wd_shard_eval_accumulate_phase on every
  *                         rank; after the last step wd_shard_local_sync, then wd_shard_eval_finish on every rank. */
 int wd_shard_eval_accumulate_slot(WdModel *m, int slot, int32_t n_valid);
 int wd_shard_eval_accumulate_phase(WdModel *m, int32_t n_valid);

@@ -31,12 +31,7 @@ int wide_bias_grad(WdModel* m);
 int metrics_setup();
 int merge_sparse(WdModel* m, int which, const void* rows, const void* grads, int64_t n);
 int shard_build(WdModel* m, const WdPlanDesc* d);
-int shard_phase0(WdModel* m, bool train);
-int shard_phase1(WdModel* m, bool train);
-int shard_phase2(WdModel* m, bool train);
-int shard_phase3(WdModel* m);
-int shard_phase4(WdModel* m);
-int shard_step_ipc(WdModel* m, bool train);
+int shard_step(WdModel* m, bool train, int seg);
 
 static int pad_to(int n, int k) { return (n + k - 1) / k * k; }
 static int bits_for(int64_t n) {
@@ -950,7 +945,9 @@ static void stamp(WdModel* m, int i) {
     m->launches++;
 }
 
-static int group_async(WdModel* m) {
+// group_async, backward_core and apply_core are also pieces of the row-sharded rank-step (shard.cu)
+namespace wd {
+int group_async(WdModel* m) {
     if (m->timer.enabled) return WD_OK;                      // profiling: keep everything on one stream (done before the reduce)
     WD_CUDA(cudaEventRecord(m->ev_ids, m->stream));
     for (int w = 0; w < 2; ++w) {
@@ -1003,7 +1000,7 @@ static int forward_core(WdModel* m, bool train) {
 // Backward.  Main stream: towers (dgrad before wgrad per layer), dense gradient reduction.  Side streams (when the
 // grouping already lives there): wide gradient sums as soon as dlogit exists, embedding gradient sums as soon as dX0
 // exists — i.e. under the remaining weight-gradient GEMMs.
-static int backward_core(WdModel* m) {
+int backward_core(WdModel* m) {
     int rc;
     m->side_active[0] = m->side_active[1] = false;
     if (m->gs_count > 0) WD_CUDA(cudaMemsetAsync(m->d_G + m->dense_count, 0, (size_t)m->gs_count * sizeof(float), m->stream));
@@ -1052,7 +1049,7 @@ static int backward_core(WdModel* m) {
 
 // Optimizer.  A list whose sums live on its side stream is applied there (after its merge in data-parallel runs); the dense
 // optimizer runs on the main stream meanwhile and the streams join at the end of the step.
-static int apply_core(WdModel* m) {
+int apply_core(WdModel* m) {
     int rc;
     const bool split_dense = m->fuse_dense && m->dense_split_tensor >= 0 && m->side_active[1];
     for (int w = 0; w < 2; ++w) {
@@ -1098,6 +1095,7 @@ static int apply_core(WdModel* m) {
     m->grads_pending = false;
     return WD_OK;
 }
+}  // namespace wd
 
 static int train_eager(WdModel* m) {
     int rc;
@@ -1341,12 +1339,6 @@ extern "C" int wd_sparse_set_sorted(WdModel* m, int which, const void* rows_dev,
 }
 
 // ------------------------------------------------------------------------------------- row-sharded tables
-namespace wd {
-int shard_group_async(WdModel* m) { return ::group_async(m); }
-int shard_backward_local(WdModel* m, bool) { return ::backward_core(m); }
-int shard_apply_local(WdModel* m) { return ::apply_core(m); }
-}
-
 static int shard_ready(WdModel* m, int slot) {
     int rc = check_ready(m);
     if (rc) return rc;
@@ -1357,21 +1349,15 @@ static int shard_ready(WdModel* m, int slot) {
     return WD_OK;
 }
 
-// One phase of a sharded step (ranks driven by ONE process: the caller runs phase k on every rank, then wd_shard_local_sync).
+// Segment `phase` of the rank-step (ranks driven by ONE process: the caller runs segment k on every rank, then wd_shard_local_sync).
 extern "C" int wd_shard_phase(WdModel* m, int slot, int phase, int train) {
     int rc = shard_ready(m, slot);
     if (rc) return rc;
     if (m->shard.ipc) { set_error("wd_shard_phase is for ranks of one process; multi-process ranks call wd_shard_train_step_slot"); return WD_ESTATE; }
     if (train && !m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
-    switch (phase) {
-        case 0: return shard_phase0(m, train != 0);
-        case 1: return shard_phase1(m, train != 0);
-        case 2: rc = shard_phase2(m, train != 0); if (!train && rc == WD_OK) m->shard.step++; return rc;
-        case 3: return train ? shard_phase3(m) : WD_OK;
-        case 4: if (!train) return WD_OK; rc = shard_phase4(m); return rc ? rc : mark_slot_used(m);
-    }
-    set_error("wd_shard_phase: phase %d outside [0, 4]", phase);
-    return WD_EINVAL;
+    if (phase < 0 || phase > 4) { set_error("wd_shard_phase: phase %d outside [0, 4]", phase); return WD_EINVAL; }
+    if ((rc = shard_step(m, train != 0, phase))) return rc;
+    return train && phase == 4 ? mark_slot_used(m) : WD_OK;
 }
 
 // Loss (and optionally logits) of the step / forward just issued; synchronises the model stream.
@@ -1382,7 +1368,7 @@ extern "C" int wd_shard_finish(WdModel* m, float* loss_out, float* logits_out) {
 }
 
 // The whole step of one rank of a multi-process job: ids, routing, serve, combine, towers, owners' updates, dense all-reduce and
-// optimizers, with flag barriers in peer memory between the phases.  Every rank must call it once per step (it is a collective).
+// optimizers, with flag barriers in peer memory between the segments.  Every rank must call it once per step (it is a collective).
 // Graphed per batch slot, barrier kernels included.
 extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
     int rc = shard_ready(m, slot);
@@ -1390,8 +1376,7 @@ extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
     if (!m->shard.ipc) { set_error("wd_shard_train_step_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase)"); return WD_ESTATE; }
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     GraphRun how;
-    if ((rc = run_graphed(m, m->slots[slot].shard, m->dbatch, m->stream, [&](bool) { return shard_step_ipc(m, true); }, &how))) return rc;
-    if (how == GraphRun::replayed) m->shard.step++;          // (a capture ran shard_step_ipc, which advanced it)
+    if ((rc = run_graphed(m, m->slots[slot].shard, m->dbatch, m->stream, [&](bool) { return shard_step(m, true, kAllSegments); }, &how))) return rc;
     if (how == GraphRun::captured) {
         m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
         m->grads_pending = false;
@@ -1406,7 +1391,7 @@ extern "C" int wd_shard_forward_slot(WdModel* m, int slot, float* logits_out, fl
     int rc = shard_ready(m, slot);
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_forward_slot needs wd_shard_connect_ipc"); return WD_ESTATE; }
-    if ((rc = shard_step_ipc(m, false))) return rc;
+    if ((rc = shard_step(m, false, kAllSegments))) return rc;
     return finish_step(m, loss_out, logits_out);
 }
 
@@ -1428,15 +1413,15 @@ extern "C" int wd_shard_eval_accumulate_slot(WdModel* m, int slot, int32_t n_val
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_eval_accumulate_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase + wd_shard_eval_accumulate_phase)"); return WD_ESTATE; }
     if ((rc = check_eval_rows(m, n_valid))) return rc;
-    auto issue = [&](bool) { int r = shard_step_ipc(m, false); return r ? r : metrics_accumulate(m, n_valid); };
+    auto issue = [&](bool) { int r = shard_step(m, false, kAllSegments); return r ? r : metrics_accumulate(m, n_valid); };
     GraphRun how;
     if ((rc = run_graphed(m, m->slots[slot].shard_eval, ShardEvalKey{m->dbatch, n_valid}, m->stream, issue, &how))) return rc;
-    if (how == GraphRun::replayed) { m->shard.step++; m->eval_batches++; }   // (a capture ran the issuing code, which advanced both)
+    if (how == GraphRun::replayed) m->eval_batches++;        // (a capture ran the issuing code, which advanced it)
     if ((rc = mark_slot_used(m))) return rc;
     return finish_step(m, nullptr, nullptr);
 }
 
-// Ranks of one process: after phases 0..2 of wd_shard_phase(train = 0) on every rank, the metrics of the first n_valid rows of
+// Ranks of one process: after segments 0..2 of wd_shard_phase(train = 0) on every rank, the metrics of the first n_valid rows of
 // this rank's logits.
 extern "C" int wd_shard_eval_accumulate_phase(WdModel* m, int32_t n_valid) {
     int rc = shard_ready(m, m->cur_slot);

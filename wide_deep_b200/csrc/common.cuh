@@ -235,8 +235,8 @@ struct BatchSlot {           // one device-resident batch (ring used by benchmar
 // Pointers into ONE rank's exchange segment (a single cudaMalloc block that peers map through CUDA IPC, or address directly when
 // all ranks live in one process).  Every rank lays its segment out identically, so a peer pointer = peer base + own offset.
 struct ShardPeer {
-    uint2* inbox[2];          // [G][pair_cap] entries {local row, bag} written by requester ranks (double buffered by step parity)
-    int32_t* inbox_cnt[2];    // [G] entries each requester sent this step
+    uint2* inbox;             // [G][pair_cap] entries {local row, bag} written by requester ranks
+    int32_t* inbox_cnt;       // [G] entries each requester sent this step
     float* recv;              // [G][nbags][width] pooled partial sums written by owner ranks
     const float* bagscale;    // [nbags] 1 / (ids in the bag)   (embedding space: combiner = mean)
     const float* gradbase;    // dX0 (embedding space) / dlogit (wide space) of that rank: owners pull gradients from here
@@ -270,7 +270,7 @@ struct ShardSpace {           // one sharded table space on this rank: 0 = embed
     int32_t* d_nrecv = nullptr;        // device scalar
     ShardPeer* d_peers = nullptr;      // [G] device copy
     ShardPeer peers[kMaxRanks];        // host copy (pointers are device addresses)
-    int64_t off_inbox[2] = {0, 0}, off_cnt[2] = {0, 0}, off_recv = 0, off_bagscale = 0, off_grad = 0;   // offsets in the segment
+    int64_t off_inbox = 0, off_cnt = 0, off_recv = 0, off_bagscale = 0, off_grad = 0;   // offsets in the segment
 };
 struct ShardState {
     int world = 1, rank = 0;
@@ -290,12 +290,12 @@ struct ShardState {
     float** d_peer_gred = nullptr;      // [G] peers' reduced slices
     float* gred = nullptr;              // this rank's reduced slice buffer (whole-arena sized; only the own slice is written)
     int64_t ar_count = 0;               // floats all-reduced per step (dense gradients + small-table block)
-    uint64_t step = 0;                  // steps issued (inbox double buffering)
     cudaEvent_t ev_a = nullptr;         // after barrier A on the main stream (owner-side grouping may start)
     cudaStream_t aux = nullptr;         // the wide space's routing / serving and the local gathers, beside the embedding space's chain
     cudaEvent_t ev_ids2 = nullptr, ev_routed1 = nullptr, ev_a2 = nullptr, ev_aux_done = nullptr;
 };
 constexpr int kBarriers = 8;
+constexpr int kAllSegments = -1;             // shard_step (shard.cu): every segment of the rank-step
 
 struct TsvDev;                                 // device TSV parser: spec copy and scratch (tsv.cu)
 

@@ -31,8 +31,10 @@
 //                   ends (before the next stage-in); forward-only calls skip it
 // Every kernel reads the same values and sums them in the same order as with the shard in HBM: the results are bit-identical.
 //
-// Ranks synchronise with flag barriers in peer memory (st.release.sys / ld.acquire.sys); when all ranks live in ONE process
-// (tests on a single GPU) the caller orders the phases with events instead (wd_shard_phase + wd_shard_local_sync).
+// One function, shard_step, issues a rank's step; it is cut into segments at the barriers that close them.  Ranks of a
+// multi-process job run it whole and synchronise with flag barriers in peer memory (st.release.sys / ld.acquire.sys).  When all
+// ranks live in ONE process (tests on a single GPU), barriers issue nothing and the caller runs the step segment by segment on
+// every rank, with wd_shard_local_sync standing in for the barriers between segments (wd_shard_phase).
 #include <stdlib.h>
 #include <string.h>
 
@@ -112,7 +114,7 @@ __global__ void __launch_bounds__(256) shard_send_kernel(const int32_t* __restri
         const int o = threadIdx.x;
         int c = ostart[o + 1] - ostart[o];
         if ((int64_t)c > pair_cap) { c = (int)pair_cap; atomicOr(err, 2); }
-        peers[o].inbox_cnt[0][me] = c;
+        peers[o].inbox_cnt[me] = c;
     }
     for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < total; p += gridDim.x * blockDim.x) {
         const int o = (int)sk[p];
@@ -121,7 +123,7 @@ __global__ void __launch_bounds__(256) shard_send_kernel(const int32_t* __restri
         if ((int64_t)i >= pair_cap) continue;
         const int bc = e_bc[e];
         const int bag = shard_bag<EMB>(bc, C, n_slots, col_slot);
-        peers[o].inbox[0][(int64_t)me * pair_cap + i] = make_uint2(lrow[e], (uint32_t)bag);
+        peers[o].inbox[(int64_t)me * pair_cap + i] = make_uint2(lrow[e], (uint32_t)bag);
         const bool head = i == 0 || shard_bag<EMB>(e_bc[sv[p - 1]], C, n_slots, col_slot) != bag;
         if (head) {
             atomicOr(&bagmask[bag], 1 << o);
@@ -448,8 +450,8 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     for (int s = 0; s < 2; ++s) {
         ShardSpace& sp = S.sp[s];
         if (!sp.on) continue;
-        sp.off_inbox[0] = sp.off_inbox[1] = take((int64_t)G * sp.pair_cap * (int64_t)sizeof(uint2));   // (one buffer: see the hazard note below)
-        sp.off_cnt[0] = sp.off_cnt[1] = take(kMaxRanks * 4);
+        sp.off_inbox = take((int64_t)G * sp.pair_cap * (int64_t)sizeof(uint2));   // reused every step: see the hazard note at shard_step
+        sp.off_cnt = take(kMaxRanks * 4);
         sp.off_recv = take((int64_t)G * sp.nbags_cap * sp.width * 4);
         sp.off_bagscale = take(sp.nbags_cap * 4);
     }
@@ -533,10 +535,8 @@ static int shard_finish_connect(WdModel* m) {
             ShardSpace& sp = S.sp[s];
             if (!sp.on) continue;
             ShardPeer& p = sp.peers[r];
-            for (int k = 0; k < 2; ++k) {
-                p.inbox[k] = reinterpret_cast<uint2*>(b + sp.off_inbox[k]);
-                p.inbox_cnt[k] = reinterpret_cast<int32_t*>(b + sp.off_cnt[k]);
-            }
+            p.inbox = reinterpret_cast<uint2*>(b + sp.off_inbox);
+            p.inbox_cnt = reinterpret_cast<int32_t*>(b + sp.off_cnt);
             p.recv = reinterpret_cast<float*>(b + sp.off_recv);
             p.bagscale = reinterpret_cast<const float*>(b + sp.off_bagscale);
             p.gradbase = reinterpret_cast<const float*>(b + sp.off_grad);
@@ -554,7 +554,7 @@ static int shard_finish_connect(WdModel* m) {
 
 static int barrier(WdModel* m, int k) {
     ShardState& S = m->shard;
-    if (!S.ipc) return WD_OK;                                  // ranks of one process: the caller orders the phases with events
+    if (!S.ipc) return WD_OK;                                  // ranks of one process: the caller orders the segments with events
     shard_barrier_kernel<<<1, 32, 0, m->stream>>>(S.d_peer_flags, reinterpret_cast<uint32_t*>(S.seg + S.off_flags), S.d_epoch, k, S.world, S.rank,
                                                   m->d_flags, S.d_trace);
     m->launches++;
@@ -603,11 +603,11 @@ static int shard_serve(WdModel* m, int s) {
         if ((rc = host_rows_transfer(m, true, m->d_nuniq[2], m->d_urow[2], sp.set.rec, sp.stage_stride))) return rc;
     }
     if (s == 0)
-        shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
+        shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, S.rank, sp.pair_cap,
             sp.n_slots, sp.set.rec.row_base, sp.set.rec.data, sp.set.rec.dim, sp.set.rec.stride, sp.d_peers, sp.nbags_cap, sp.width,
             sp.set.rec.stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2]);
     else
-        shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, S.rank, sp.pair_cap,
+        shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, S.rank, sp.pair_cap,
             sp.d_wide, sp.d_peers, sp.nbags_cap);
     m->launches++;
     WD_CUDA(cudaGetLastError());
@@ -620,7 +620,7 @@ static int shard_owner_group(WdModel* m, int s) {
     ShardSpace& sp = S.sp[s];
     if (!sp.on) return WD_OK;
     const ShardPeer& me = sp.peers[S.rank];
-    shard_flatten_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(me.inbox[0], me.inbox_cnt[0], S.world, sp.pair_cap, sp.d_rrow, sp.d_rtag,
+    shard_flatten_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, sp.pair_cap, sp.d_rrow, sp.d_rtag,
                                                                             sp.d_nrecv, m->max_nnz, m->d_flags);
     m->launches++;
     WD_CUDA(cudaGetLastError());
@@ -700,9 +700,9 @@ int sparse_forward(WdModel* m);
 int mlp_forward(WdModel* m, bool train);
 int loss_forward(WdModel* m, bool need_grad);
 int ids_prepare(WdModel* m);
-int shard_backward_local(WdModel* m, bool overlap);     // api.cu: towers' backward + replicated lists + dense gradient arena
-int shard_apply_local(WdModel* m);                     // api.cu: dense optimizer + small-table block + joins
-int shard_group_async(WdModel* m);                     // api.cu: replicated lists' grouping on the side streams
+int group_async(WdModel* m);        // api.cu: replicated lists' grouping on the side streams
+int backward_core(WdModel* m);      // api.cu: towers' backward + replicated lists + dense gradient arena
+int apply_core(WdModel* m);         // api.cu: dense optimizer + small-table block + joins
 
 // The critical chain in front of the towers is   ids -> route + send (embedding space) -> [A] -> serve (embedding space) -> [B].
 // Everything else that must exist before the towers — the wide space's routing, its serve, and this rank's local gathers
@@ -711,24 +711,6 @@ int shard_group_async(WdModel* m);                     // api.cu: replicated lis
 // already hold the grouping of the replicated lists, ~100 us of sort launches enqueued before barrier A.)
 static bool aux_split(WdModel* m) { return m->shard.sp[0].on && m->shard.sp[1].on; }
 
-// phase 0: ids, routing
-int shard_phase0(WdModel* m, bool train) {
-    ShardState& S = m->shard;
-    int rc;
-    if ((rc = ids_prepare(m))) return rc;
-    const bool split = aux_split(m);
-    if (split) {
-        WD_CUDA(cudaEventRecord(S.ev_ids2, m->stream));
-        WD_CUDA(cudaStreamWaitEvent(S.aux, S.ev_ids2, 0));
-        if ((rc = on_aux(m, [&] { return shard_route_send(m, 1); }))) return rc;
-        WD_CUDA(cudaEventRecord(S.ev_routed1, S.aux));
-    }
-    if (train && (rc = shard_group_async(m))) return rc;
-    if ((rc = shard_route_send(m, 0))) return rc;
-    if (!split && (rc = shard_route_send(m, 1))) return rc;
-    if (split) WD_CUDA(cudaStreamWaitEvent(m->stream, S.ev_routed1, 0));
-    return WD_OK;
-}
 // after barrier A: serve both spaces and run the local part of the forward (needed only by this rank's towers, while every peer's
 // barrier B waits for the serves)
 static int shard_serve_both(WdModel* m) {
@@ -746,36 +728,82 @@ static int shard_serve_both(WdModel* m) {
     for (int s = 0; s < 2; ++s) if ((rc = shard_serve(m, s))) return rc;
     return sparse_forward(m);
 }
-// phase 1: (group + stage-in of a staged space,) serve the peers, local gathers; sort what was received
-int shard_phase1(WdModel* m, bool train) {
+
+// The whole step of one rank.  Main stream: ids, routing, serve, combine, towers, dense all-reduce and optimizers, with flag
+// barriers A (ids delivered), B (pooled sums delivered), G (gradient arenas final), R (slices reduced) and END.  Side stream of
+// each table space: the owner-side grouping of the received rows (needs only ids: runs beside the towers) and, once every rank's
+// dlogit / dX0 exists (barriers Cw / Ce, on the side streams), the owners' pulled gradient sums and optimizer — hidden behind the
+// remaining weight gradients, the dense all-reduce and the dense optimizer.
+// The step is cut into segments at the barriers that close them: segment `seg` alone, or all of them for seg = kAllSegments.
+//   0  ids, routing (+ the replicated lists' grouping)                                      closed by A
+//   1  serve both spaces, local gathers (+ owner-side grouping)                              B
+//   2  combine, towers forward (+ backward, replicated lists, dense gradient arena)          Cw / Ce / G; a forward: END
+//   3  owners' gradient sums and updates, first half of the all-reduce                      R
+//   4  second half of the all-reduce, dense optimizers, side streams joined                 END
+// A forward is segments 0-2.  Ranks of one process have no flag barriers: their driver runs segment k on every rank, then
+// wd_shard_local_sync, which stands in for every barrier that closes the segment.
+// Buffer hazards: within a step every producer / consumer pair is separated by one of the barriers; the END barrier keeps a fast
+// rank from starting the next step's sends while a slow owner still pulls this step's gradients and bag scales.
+int shard_step(WdModel* m, bool train, int seg) {
+    ShardState& S = m->shard;
+    auto runs = [&](int k) { return seg == kAllSegments || seg == k; };
     int rc;
-    if ((rc = shard_serve_both(m))) return rc;
-    if (train)
-        for (int s = 0; s < 2; ++s) if (!staged(m, s) && (rc = shard_owner_group(m, s))) return rc;
-    return WD_OK;
-}
-// phase 2: combine, towers forward / backward, dense gradient arena
-int shard_phase2(WdModel* m, bool train) {
-    int rc;
-    for (int s = 0; s < 2; ++s) if ((rc = shard_combine(m, s))) return rc;
-    if ((rc = mlp_forward(m, train))) return rc;
-    if ((rc = loss_forward(m, train))) return rc;
+    if (runs(0)) {
+        if (S.d_trace) { shard_stamp_kernel<<<1, 1, 0, m->stream>>>(S.d_trace + 2 * (kBarriers - 1)); m->launches++; }   // step start
+        if ((rc = ids_prepare(m))) return rc;
+        const bool split = aux_split(m);
+        if (split) {
+            WD_CUDA(cudaEventRecord(S.ev_ids2, m->stream));
+            WD_CUDA(cudaStreamWaitEvent(S.aux, S.ev_ids2, 0));
+            if ((rc = on_aux(m, [&] { return shard_route_send(m, 1); }))) return rc;
+            WD_CUDA(cudaEventRecord(S.ev_routed1, S.aux));
+        }
+        if (train && (rc = group_async(m))) return rc;
+        if ((rc = shard_route_send(m, 0))) return rc;
+        if (!split && (rc = shard_route_send(m, 1))) return rc;
+        if (split) WD_CUDA(cudaStreamWaitEvent(m->stream, S.ev_routed1, 0));
+        if ((rc = barrier(m, BAR_A))) return rc;
+    }
+    if (runs(1)) {
+        if ((rc = shard_serve_both(m))) return rc;
+        if (train) {
+            WD_CUDA(cudaEventRecord(S.ev_a, m->stream));
+            for (int s = 0; s < 2; ++s) {
+                if (!S.sp[s].on || staged(m, s)) continue;         // (a staged space was grouped before its serve)
+                if (m->side_pending[s]) {
+                    WD_CUDA(cudaStreamWaitEvent(m->sstream[s], S.ev_a, 0));
+                    if ((rc = on_side(m, s, [&] { return shard_owner_group(m, s); }))) return rc;
+                } else if ((rc = shard_owner_group(m, s))) return rc;
+            }
+        }
+        if ((rc = barrier(m, BAR_B))) return rc;
+    }
+    if (runs(2)) {
+        for (int s = 0; s < 2; ++s) if ((rc = shard_combine(m, s))) return rc;
+        if ((rc = mlp_forward(m, train))) return rc;
+        if ((rc = loss_forward(m, train))) return rc;
+        if (!train) return barrier(m, BAR_END);
+        if (m->side_pending[0] || m->side_pending[1]) WD_CUDA(cudaEventRecord(m->ev_head, m->stream));   // dlogit exists (as forward_core does)
+        if ((rc = backward_core(m))) return rc;
+    }
     if (!train) return WD_OK;
-    if (m->side_pending[0] || m->side_pending[1]) WD_CUDA(cudaEventRecord(m->ev_head, m->stream));   // dlogit exists (as forward_core does)
-    return shard_backward_local(m, false);
-}
-// phase 3: owners pull gradients and update their shards; first half of the all-reduce
-int shard_phase3(WdModel* m) {
-    int rc;
-    for (int s = 1; s >= 0; --s) if ((rc = shard_owner_reduce_apply(m, s))) return rc;
-    return shard_ar_reduce(m);
-}
-// phase 4: second half of the all-reduce, dense optimizers
-int shard_phase4(WdModel* m) {
-    int rc;
-    if ((rc = shard_ar_gather(m))) return rc;
-    if ((rc = shard_apply_local(m))) return rc;
-    m->shard.step++;
+    if (runs(3)) {
+        for (int s = 1; s >= 0; --s) {
+            if (!S.sp[s].on) continue;
+            auto owner = [&]() -> int { int r = barrier(m, s == 1 ? BAR_CW : BAR_CE); return r ? r : shard_owner_reduce_apply(m, s); };
+            if (m->side_active[s]) { if ((rc = on_side(m, s, owner))) return rc; }
+            else if ((rc = owner())) return rc;
+        }
+        if ((rc = barrier(m, BAR_G))) return rc;                // every rank's gradient arena (dense + small-table block) is final
+        if ((rc = shard_ar_reduce(m))) return rc;
+        if ((rc = barrier(m, BAR_R))) return rc;
+    }
+    if (runs(4)) {
+        if ((rc = shard_ar_gather(m))) return rc;
+        if ((rc = apply_core(m))) return rc;
+        if (S.d_trace) { shard_stamp_kernel<<<1, 1, 0, m->stream>>>(S.d_trace + 2 * (kBarriers - 1) + 1); m->launches++; }   // before END
+        if ((rc = barrier(m, BAR_END))) return rc;
+    }
     return WD_OK;
 }
 
@@ -791,47 +819,6 @@ int shard_metrics_reduce(WdModel* m) {
     shard_metrics_reduce_kernel<<<2, 256, 0, m->stream>>>(peers, S.world, S.d_msum);
     m->launches++;
     WD_CUDA(cudaGetLastError());
-    return barrier(m, BAR_END);
-}
-
-// The whole step of one rank of a multi-process job.  Main stream: ids, routing, serve, combine, towers, dense all-reduce and
-// optimizers, with flag barriers A (ids delivered), B (pooled sums delivered), G (gradient arenas final), R (slices reduced) and
-// END.  Side stream of each table space: the owner-side grouping of the received rows (needs only ids: runs beside the towers)
-// and, once every rank's dlogit / dX0 exists (barriers Cw / Ce, on the side streams), the owners' pulled gradient sums and
-// optimizer — hidden behind the remaining weight gradients, the dense all-reduce and the dense optimizer.
-// Buffer hazards: within a step every producer / consumer pair is separated by one of the barriers; the END barrier keeps a fast
-// rank from starting the next step's sends while a slow owner still pulls this step's gradients and bag scales.
-int shard_step_ipc(WdModel* m, bool train) {
-    ShardState& S = m->shard;
-    int rc;
-    if (S.d_trace) { shard_stamp_kernel<<<1, 1, 0, m->stream>>>(S.d_trace + 2 * (kBarriers - 1)); m->launches++; }   // step start
-    if ((rc = shard_phase0(m, train))) return rc;
-    if ((rc = barrier(m, BAR_A))) return rc;
-    if ((rc = shard_serve_both(m))) return rc;
-    if (train) {
-        WD_CUDA(cudaEventRecord(S.ev_a, m->stream));
-        for (int s = 0; s < 2; ++s) {
-            if (!S.sp[s].on || staged(m, s)) continue;             // (a staged space was grouped before its serve)
-            if (m->side_pending[s]) {
-                WD_CUDA(cudaStreamWaitEvent(m->sstream[s], S.ev_a, 0));
-                if ((rc = on_side(m, s, [&] { return shard_owner_group(m, s); }))) return rc;
-            } else if ((rc = shard_owner_group(m, s))) return rc;
-        }
-    }
-    if ((rc = barrier(m, BAR_B))) return rc;
-    if ((rc = shard_phase2(m, train))) return rc;               // combine, towers forward (+ backward, replicated lists, dense gradient arena)
-    if (!train) { S.step++; return barrier(m, BAR_END); }
-    for (int s = 1; s >= 0; --s) {
-        if (!S.sp[s].on) continue;
-        auto owner = [&]() -> int { int r = barrier(m, s == 1 ? BAR_CW : BAR_CE); return r ? r : shard_owner_reduce_apply(m, s); };
-        if (m->side_active[s]) { if ((rc = on_side(m, s, owner))) return rc; }
-        else if ((rc = owner())) return rc;
-    }
-    if ((rc = barrier(m, BAR_G))) return rc;                    // every rank's gradient arena (dense + small-table block) is final
-    if ((rc = shard_ar_reduce(m))) return rc;
-    if ((rc = barrier(m, BAR_R))) return rc;
-    if ((rc = shard_phase4(m))) return rc;                      // gather the reduced slices, dense optimizers, join the side streams
-    if (S.d_trace) { shard_stamp_kernel<<<1, 1, 0, m->stream>>>(S.d_trace + 2 * (kBarriers - 1) + 1); m->launches++; }   // before END
     return barrier(m, BAR_END);
 }
 
