@@ -8,7 +8,7 @@ import sys
 ROOT = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(ROOT, "wide_deep_b200", "csrc")
 OUT = os.path.join(ROOT, "wide_deep_b200", "libwd_b200.so")
-SOURCES = ["api.cu", "ids.cu", "sort.cu", "sparse.cu", "mlp.cu", "gemm_tc.cu", "gemm_bf16.cu", "misc.cu", "tsv.cu", "shard.cu", "host_tables.cu"]
+SOURCES = ["api.cu", "ids.cu", "sort.cu", "sparse.cu", "mlp.cu", "gemm_tc.cu", "gemm_bf16.cu", "misc.cu", "tsv.cu", "shard.cu", "host_tables.cu", "summary.cu"]
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v" if os.environ.get("WD_PTXAS_V") else "-O3"]
 

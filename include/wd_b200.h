@@ -334,6 +334,27 @@ int wd_debug_gemm_probe(unsigned long long *out);
 void *wd_stream_sparse(WdModel *m, int which);
 int wd_sync(WdModel *m);
 
+/* Layer summaries (the reference's add_layer_summary, python/lib/utils/model_util.py:15-17): statistics of the tensors a train
+ * step's towers produce, taken on the GPU in the step's forward, before its optimizer.  Segments, in this order: the deep input
+ * (its logical columns), per tower its hidden layers (the layer output, dropout and batch normalization included) and its logits,
+ * then the wide logit.  Per segment: counts over TensorFlow's 1551 default histogram limits (value v, as a double, counts in
+ * bucket i = the first i with limit[i] > v), the number of values, of zeros (-0.0 included) and of non-finite values (counted in
+ * no bucket), and min, max, sum and sum of squares of the finite values, in double. */
+#define WD_SUMMARY_BUCKETS 1551
+enum { WD_SEG_DEEP_INPUT = 0, WD_SEG_HIDDEN = 1, WD_SEG_TOWER_LOGITS = 2, WD_SEG_WIDE_LOGIT = 3 };
+/* The 1551 ascending bucket limits into out[0 .. cap); returns 1551 (out NULL: only the count).  Needs no GPU. */
+int wd_summary_limits(double *out, int32_t cap);
+/* The model's segments: kind[i] (WD_SEG_*), tower[i] and layer[i] (-1 where they do not apply) for the first `cap`; returns how
+ * many there are. */
+int wd_summary_segments(WdModel *m, int32_t *kind, int32_t *tower, int32_t *layer, int32_t cap);
+/* The next train step (wd_train_step*, wd_step_backward*, the row-sharded rank-step) takes the statistics.  It runs outside the
+ * step graphs; every other step stays as it is. */
+int wd_summary_arm(WdModel *m);
+/* Statistics of the last armed step (synchronises the model stream): counts[n][WD_SUMMARY_BUCKETS], ints[n][3] = values, zeros,
+ * non-finite values, reals[n][4] = min, max, sum, sum of squares; n_segments must be the wd_summary_segments count.  WD_ESTATE
+ * when no armed step ran since the last read. */
+int wd_summary_read(WdModel *m, int64_t *counts, int64_t *ints, double *reals, int32_t n_segments);
+
 /* TSV loader (host, multi-threaded).  Replaces _CsvDataset._parse_csv (reference python/lib/dataset.py:107-165):
  * parses `n_lines` tab-separated records into the WdBatch CSR arrays. */
 typedef struct WdTsvSpec {

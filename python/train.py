@@ -145,10 +145,13 @@ def main_distributed(rank, world, local):
     """torchrun --nproc-per-node G train.py ...: rank r trains on every G-th line of each file (dataset.shard semantics, reference
     python/lib/dataset.py:173-174) with synchronous, exact steps; tables larger than 16384 rows are row-sharded over the ranks
     (the reference partitions them over its parameter servers, python/lib/joint.py:141-143).  As in the reference, distributed
-    runs train only ("distributed can not including eval", python/train.py:215-216); rank 0 alone touches the model directory."""
+    runs train only ("distributed can not including eval", python/train.py:215-216); rank 0 alone touches the model directory and
+    writes the TensorBoard summaries (those of the global batch).  WD_SHARD_SAME_GPU=1 puts every rank on cuda:0 (a test setup, not
+    a multi-GPU rate)."""
     import torch
     import torch.distributed as dist
-    torch.cuda.set_device(local)
+    device = 0 if os.environ.get("WD_SHARD_SAME_GPU") else local
+    torch.cuda.set_device(device)
     dist.init_process_group("gloo")                    # plumbing only (IPC handles, checkpoint gather); data moves over NVLink
     log = print if rank == 0 else (lambda *a, **k: None)
     log("Using wide_deep_b200 (CUDA sm_90a) in place of TensorFlow: rank {} of {}".format(rank, world))
@@ -157,7 +160,7 @@ def main_distributed(rank, world, local):
         shutil.rmtree(model_dir, ignore_errors=True)
         log("Remove model directory: {}".format(model_dir))
     dist.barrier()
-    model = build_custom_estimator(model_dir, FLAGS.model_type, config=CONF, max_batch=FLAGS.batch_size, device=local,
+    model = build_custom_estimator(model_dir, FLAGS.model_type, config=CONF, max_batch=FLAGS.batch_size, device=device,
                                    shard_world=world, shard_rank=rank)
     log("INFO: Build estimator: {}".format(model))
     for n in range(FLAGS.train_epochs):

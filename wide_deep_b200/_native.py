@@ -106,6 +106,10 @@ SYMBOLS = {
     "wd_tsv_gather_lines": (_i64, [_vp, _vp, _vp, _vp, _i32, _vp, _i64, _vp, _i32]),
     "wd_tsv_parse_slot": (ctypes.c_int, [_vp, ctypes.c_int, _vp, _vp, _i64, _vp, _i32]),
     "wd_tsv_parse_stats": (ctypes.c_int, [_vp, ctypes.POINTER(_i64), _i32, _i32]),
+    "wd_summary_limits": (ctypes.c_int, [_vp, _i32]),
+    "wd_summary_segments": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32]),
+    "wd_summary_arm": (ctypes.c_int, [_vp]),
+    "wd_summary_read": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32]),
 }
 
 

@@ -123,6 +123,7 @@ extern "C" int wd_model_destroy(WdModel* m) {
     if (m->ev_head) cudaEventDestroy(m->ev_head);
     if (m->ev_dx0) cudaEventDestroy(m->ev_dx0);
     if (m->stream) cudaStreamDestroy(m->stream);
+    delete m->summ;
     for (size_t i = 0; i < g_extra.size(); ++i)
         if (g_extra[i].first == m) { delete g_extra[i].second; g_extra.erase(g_extra.begin() + i); break; }
     delete m;
@@ -994,6 +995,7 @@ static int forward_core(WdModel* m, bool train) {
     mark(m, "head");
     stamp(m, ST_HEAD);
     if (train && (m->side_pending[0] || m->side_pending[1])) WD_CUDA(cudaEventRecord(m->ev_head, m->stream));
+    if (train && m->summary_armed && (rc = summary_launch(m))) return rc;     // (after ev_head: the side streams do not wait for it)
     return WD_OK;
 }
 
@@ -1154,11 +1156,23 @@ static int run_graphed(WdModel* m, StepGraph<Key>& g, const Key& key, cudaStream
     return WD_OK;
 }
 
+// A train step through its slot's graph.  A step armed for layer summaries (wd_summary_arm) runs eagerly instead: it is one step
+// in save_summary_steps (1000 in conf/train.yaml), and a second graph per slot would cost a capture and its device memory to save
+// the launch gaps of that one step.  The plain step's graph stays the one every other step replays.
+template <class Key, class F>
+static int run_train_graphed(WdModel* m, StepGraph<Key>& g, const Key& key, F issue, GraphRun* how) {
+    if (m->summary_armed) {
+        *how = GraphRun::eager;
+        return issue(false);
+    }
+    return run_graphed(m, g, key, m->stream, issue, how);
+}
+
 // One whole train step on the current slot (three streams, ~55 kernels, no host sync), graphed per slot.
 static int train_current(WdModel* m, float* loss_out) {
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     GraphRun how;
-    int rc = run_graphed(m, m->slots[m->cur_slot].train, m->dbatch, m->stream, [&](bool) { return train_eager(m); }, &how);
+    int rc = run_train_graphed(m, m->slots[m->cur_slot].train, m->dbatch, [&](bool) { return train_eager(m); }, &how);
     if (rc) return rc;
     if (how != GraphRun::eager) {                           // a graphed step ends as an eager one does: nothing left pending
         m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
@@ -1246,7 +1260,7 @@ extern "C" int wd_step_backward_slot(WdModel* m, int slot, float* loss_out) {
     timer_begin(m);
     BatchSlot& sl = m->slots[slot];
     GraphRun how;
-    if ((rc = run_graphed(m, sl.bwd, m->dbatch, m->stream, [&](bool capturing) { return backward_eager(m, capturing); }, &how))) return rc;
+    if ((rc = run_train_graphed(m, sl.bwd, m->dbatch, [&](bool capturing) { return backward_eager(m, capturing); }, &how))) return rc;
     if (how == GraphRun::captured)
         for (int w = 0; w < 2; ++w) sl.bwd_side_active[w] = m->side_active[w];
     if (how != GraphRun::eager) {
@@ -1376,7 +1390,7 @@ extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
     if (!m->shard.ipc) { set_error("wd_shard_train_step_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase)"); return WD_ESTATE; }
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     GraphRun how;
-    if ((rc = run_graphed(m, m->slots[slot].shard, m->dbatch, m->stream, [&](bool) { return shard_step(m, true, kAllSegments); }, &how))) return rc;
+    if ((rc = run_train_graphed(m, m->slots[slot].shard, m->dbatch, [&](bool) { return shard_step(m, true, kAllSegments); }, &how))) return rc;
     if (how == GraphRun::captured) {
         m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
         m->grads_pending = false;
@@ -1553,6 +1567,28 @@ extern "C" int wd_debug_hidden(WdModel* m, int tower, int layer, float* out, int
     return L.N_phys;
 }
 extern "C" int64_t wd_launch_count(WdModel* m) { return m ? m->launches : 0; }
+
+// ------------------------------------------------------------------------------------------ layer summaries (summary.cu)
+extern "C" int wd_summary_segments(WdModel* m, int32_t* kind, int32_t* tower, int32_t* layer, int32_t cap) {
+    int rc = check_ready(m);
+    if (rc) return rc;
+    if ((rc = summary_prepare(m, extra_of(m)->x0_real))) return rc;
+    const SummaryState* S = m->summ;
+    const int n = (int)S->h.size();
+    for (int i = 0; i < n && i < cap; ++i) {
+        if (kind) kind[i] = S->kind[i];
+        if (tower) tower[i] = S->tower[i];
+        if (layer) layer[i] = S->layer[i];
+    }
+    return n;
+}
+extern "C" int wd_summary_arm(WdModel* m) {
+    int rc = check_ready(m);
+    if (rc) return rc;
+    if ((rc = summary_prepare(m, extra_of(m)->x0_real))) return rc;
+    m->summary_armed = true;
+    return WD_OK;
+}
 extern "C" int64_t wd_gemm_fallback_count(WdModel* m) { return m ? m->gemm_fallbacks : 0; }
 extern "C" int wd_last_timings(WdModel* m, float* ms_out, int cap) {
     if (!m) return WD_EINVAL;

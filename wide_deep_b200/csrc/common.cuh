@@ -297,6 +297,29 @@ struct ShardState {
 constexpr int kBarriers = 8;
 constexpr int kAllSegments = -1;             // shard_step (shard.cu): every segment of the rank-step
 
+// ---- layer summaries (summary.cu)
+constexpr int kSummaryThreads = 256;
+constexpr int kSummaryZeroBucket = (WD_SUMMARY_BUCKETS + 1) / 2;   // bucket of 0.0: the first limit above it (1e-12)
+struct SummarySeg {          // one segment of the statistics kernel: a [B, cols] tensor read in place
+    int kind;                // WD_SEG_*
+    const float* ptr; int ld, cols;
+    const uint8_t* mask;     // [cols] 1 = a real column (the deep input's logical columns), null: every column
+    const float *gamma, *beta; int bn;   // hidden layers: BN affine
+    float drop_rate; int layer_id;       //   and dropout (DropArgs)
+    int blk0, nblk;          // the segment's blocks in the grid
+};
+struct SummaryState {
+    std::vector<SummarySeg> h;              // segments in wd_summary_segments order
+    std::vector<int32_t> kind, tower, layer;
+    int blocks = 0;                         // grid of the statistics kernel
+    SummarySeg* d_seg = nullptr;
+    uint8_t* d_mask = nullptr;
+    double* d_limits = nullptr;             // [WD_SUMMARY_BUCKETS]
+    unsigned long long* d_counts = nullptr; // [segments][WD_SUMMARY_BUCKETS]
+    double* d_part = nullptr;               // [blocks][4] sum, sum of squares, min, max
+    long long* d_ipart = nullptr;           // [blocks][3] values, zeros, non-finite values
+};
+
 struct TsvDev;                                 // device TSV parser: spec copy and scratch (tsv.cu)
 
 }  // namespace wd
@@ -478,6 +501,9 @@ struct WdModel {
     int64_t tsv_device_batches = 0, tsv_host_batches = 0;   // batches wd_tsv_parse_slot parsed on the device / on the host
     bool initialized = false;
     bool grads_pending = false;
+    // layer summaries (summary.cu): the next train step takes the statistics (wd_summary_arm); they await wd_summary_read
+    wd::SummaryState* summ = nullptr;
+    bool summary_armed = false, summary_ready = false;
 };
 
 namespace wd {
@@ -522,6 +548,8 @@ int tsv_parse_host(const WdTsvSpec* sp, const char* text, const int64_t* starts,
 void tsv_dev_destroy(WdModel* m);                                // tsv.cu
 int metrics_accumulate(WdModel* m, int rows);                    // misc.cu: metrics of the first `rows` logits of the batch
 int metrics_finish(WdModel* m, const double* acc, double* out10); // misc.cu: the ten metrics of an accumulator (synchronises)
+int summary_prepare(WdModel* m, const std::vector<uint8_t>& x0_real);   // summary.cu: segments and buffers (first use)
+int summary_launch(WdModel* m);                                  // summary.cu: statistics of the armed train step
 
 // sorts (*keys, *vals) of length *d_n by the low `bits` bits of the key, with (*keys2, *vals2) as ping-pong buffers; the
 // pointers are swapped so that the sorted pairs end in (*keys, *vals)

@@ -100,6 +100,13 @@ __device__ __forceinline__ float drop_mult(unsigned long long key, unsigned int 
     return u >= rate ? inv_keep : 0.f;
 }
 
+// a hidden layer's output from its (dropped-out) post-activation value: the BN inference affine, gamma / sqrt(1 + 1e-3) and beta
+// (tf.layers.batch_normalization with the initial moving statistics).  The FFMA forward epilogue, dropout_fwd_kernel and the
+// layer summaries (summary.cu) all take it from here, so they agree bit for bit.
+__device__ __forceinline__ float bn_out(float a, const float* __restrict__ gamma, const float* __restrict__ beta, int n, int bn) {
+    return bn ? fmaf(a, gamma[n] * 0.99950037468777f, beta[n]) : a;
+}
+
 // hi = bf16(x) (round to nearest), lo = bf16(x - hi): x = hi + lo up to 2^-17 relative; the product a*b is rebuilt as
 // a_lo*b_hi + a_hi*b_lo + a_hi*b_hi on the bf16 tensor pipe with fp32 accumulation (dropped term ~2^-18)
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {

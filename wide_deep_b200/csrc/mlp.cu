@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(GT) gemm_tn_ffma(GemmA A, const float* __restr
                         float a = 0.f, h = 0.f;
                         if (gn < ep.n_logical && gm < ep.m_valid) {
                             a = act_fwd(ep.act, acc[ih * 4 + i][jh * 4 + j] + ep.bias[gn]);
-                            h = ep.bn ? a * (ep.gamma[gn] * 0.99950037468777f) + ep.beta[gn] : a;   // 1/sqrt(1+1e-3)
+                            h = bn_out(a, ep.gamma, ep.beta, gn, ep.bn);
                         }
                         a4[j] = a;
                         hv[i][j] = h;
@@ -233,7 +233,7 @@ __global__ void __launch_bounds__(256) dropout_fwd_kernel(int B, int N, int n_lo
         float h = 0.f;
         if (n < n_logical) {
             const float a = A[(int64_t)mrow * ld + n] * drop_mult(key, (unsigned)mrow, (unsigned)n, dr.rate, inv_keep);
-            h = bn ? a * (gamma[n] * 0.99950037468777f) + beta[n] : a;
+            h = bn_out(a, gamma, beta, n, bn);
         }
         if (H) H[(int64_t)mrow * ld + n] = h;
         if (q_hi) {

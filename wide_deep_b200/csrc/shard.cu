@@ -784,6 +784,7 @@ int shard_step(WdModel* m, bool train, int seg) {
         if ((rc = loss_forward(m, train))) return rc;
         if (!train) return barrier(m, BAR_END);
         if (m->side_pending[0] || m->side_pending[1]) WD_CUDA(cudaEventRecord(m->ev_head, m->stream));   // dlogit exists (as forward_core does)
+        if (m->summary_armed && (rc = summary_launch(m))) return rc;     // layer summaries of this rank's rows
         if ((rc = backward_core(m))) return rc;
     }
     if (!train) return WD_OK;

@@ -139,7 +139,6 @@ class WideAndDeepClassifier(object):
         """Runs ``input_fn()`` to exhaustion (one pass = one epoch, like Estimator.train on a one-shot iterator),
         restoring the latest checkpoint first and saving one at the end."""
         m = self._ensure_model()
-        n, t0, loss = 0, time.time(), float("nan")
         run = self.config.runconfig or {}
         log_every = run.get("log_step_count_steps") or 1000
         # checkpoint cadence of tf.estimator.RunConfig (reference conf/train.yaml:80-98): every `save_checkpoints_steps` global
@@ -150,17 +149,34 @@ class WideAndDeepClassifier(object):
             raise ValueError("Can not provide both save_checkpoints_steps and save_checkpoints_secs.")      # RunConfig's message
         if not ck_steps and not ck_secs:
             ck_secs = 600
+        from .summary import TrainSummaries
+        # TensorBoard event file of this call (wide_deep_b200/summary.py); in a multi-GPU job every rank takes the statistics of the
+        # same steps and rank 0 writes those of the global batch
+        summ = TrainSummaries.open(self.model_dir, run.get("save_summary_steps"), log_every, self.plan.summary_layout(),
+                                   write=self.shard_rank == 0)
+        try:
+            return self._train_loop(m, input_fn, steps, max_steps, log_every, ck_steps, ck_secs, summ)
+        finally:
+            if summ is not None:
+                summ.close()
+
+    def _train_loop(self, m, input_fn, steps, max_steps, log_every, ck_steps, ck_secs, summ):
+        from .dataset import Prefetcher
+        n, t0, loss = 0, time.time(), float("nan")
         last_save = time.time()
         # one batch of look-ahead, as the reference's input_fn prefetches (python/lib/dataset.py:181-184): while step i runs on the
         # GPU, batch i+1 is parsed and its host->device copy issued (wd_batch_prefetch_slot, two alternating slots); a TsvTextBatch
         # (input_fn(device_parse=True)) is parsed on the GPU into the slot instead (wd_tsv_parse_slot, beside step i)
-        from .dataset import Prefetcher
         it = Prefetcher(input_fn(), depth=2)             # batches are parsed on a background thread, two ahead of the step
         cur = next(it, None)
         slot = 0
         if cur is not None:
             m.feed_slot(slot, cur)
+        stats_of = self._trainer if self._trainer is not None else m
         while cur is not None:
+            armed = summ is not None and summ.cadence.arm(m.global_step + 1)
+            if armed:
+                stats_of.arm_summary()
             if self._trainer is not None:
                 self._trainer.step_slot(slot, want_loss=False)   # collective: every rank steps on its shard of the batch
             else:
@@ -170,6 +186,10 @@ class WideAndDeepClassifier(object):
                 m.feed_slot(1 - slot, nxt)                   # ... start its copy (or parse) on the upload stream ...
             loss = m.last_loss()                             # ... and only then wait for step i's loss
             n += 1
+            if armed:
+                self._write_summary(summ, m, stats_of, slot, loss)
+            if summ is not None:
+                summ.step_done(m.global_step)
             if n % log_every == 0:
                 print("INFO: global_step %d: loss = %.6g (%.1f steps/sec)" % (m.global_step, loss, n / (time.time() - t0)))
             if (steps and n >= steps) or (max_steps and m.global_step >= max_steps):
@@ -181,6 +201,15 @@ class WideAndDeepClassifier(object):
         print("INFO: Loss for final step: %s." % loss)
         self.save()
         return self
+
+    def _write_summary(self, summ, m, stats_of, slot, loss):
+        """Layer statistics, loss and average loss of the armed step just run (global batch in a multi-GPU job)."""
+        stats = stats_of.layer_statistics()
+        wsum = m.slot_weight_sum(slot)
+        if self._trainer is not None:
+            parts = self._trainer.gather((loss, wsum))
+            loss, wsum = sum(p[0] for p in parts), sum(p[1] for p in parts)
+        summ.write_step(m.global_step, stats, loss, wsum)
 
     def _checkpoint_due(self, global_step, ck_steps, ck_secs, last_save):
         if ck_steps:
@@ -217,7 +246,13 @@ class WideAndDeepClassifier(object):
                 break
         out = m.eval_finish()
         out["global_step"] = m.global_step
+        self._write_eval(out)
         return out
+
+    def _write_eval(self, out):
+        if self.shard_rank == 0:
+            from .summary import write_eval
+            write_eval(self.model_dir, out)
 
     # ------------------------------------------------------------------ multi-GPU evaluation and prediction
     # The reference's distributed mode only trains (train.py:215-216).  Here every rank runs the collective forward of the
@@ -263,6 +298,7 @@ class WideAndDeepClassifier(object):
             self._trainer.eval_accumulate_slot(0, nv)
         out = self._trainer.eval_finish()
         out["global_step"] = m.global_step
+        self._write_eval(out)
         return out
 
     def _predict_sharded(self, m, input_fn):

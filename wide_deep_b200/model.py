@@ -244,6 +244,42 @@ class WideDeepModel(object):
             check(n)
         return out[:batch_size * n].reshape(batch_size, n)
 
+    # ------------------------------------------------------------------ layer summaries
+    def summary_segments(self):
+        """Keys (kind, tower, layer) of the segments layer_statistics returns (Plan.summary_segments)."""
+        n = self._lib.wd_summary_segments(self._h, None, None, None, 0)
+        if n < 0:
+            check(n)
+        k, t, l = (np.zeros(max(n, 1), dtype=np.int32) for _ in range(3))
+        check(min(0, self._lib.wd_summary_segments(self._h, k.ctypes.data, t.ctypes.data, l.ctypes.data, n)))
+        return [(int(k[i]), int(t[i]), int(l[i])) for i in range(n)]
+
+    def arm_summary(self):
+        """The next train step also takes the layer statistics (read them with layer_statistics after it)."""
+        check(self._lib.wd_summary_arm(self._h))
+
+    def layer_statistics(self):
+        """Statistics of the last armed train step, per segment of this model's rows (summary.LayerStats)."""
+        from .summary import LayerStats
+        keys = self.summary_segments()
+        n = len(keys)
+        counts = np.zeros((n, 1551), dtype=np.int64)
+        ints = np.zeros((n, 3), dtype=np.int64)
+        reals = np.zeros((n, 4), dtype=np.float64)
+        check(self._lib.wd_summary_read(self._h, counts.ctypes.data, ints.ctypes.data, reals.ctypes.data, n))
+        return LayerStats(keys, counts, ints, reals)
+
+    def slot_weight_sum(self, slot):
+        """Sum of the example weights of the batch a slot holds (its rows when it has no weights)."""
+        B, nnz, parts = ctypes.c_int32(), ctypes.c_int64(), ctypes.c_int32()
+        check(self._lib.wd_debug_slot(self._h, int(slot), ctypes.byref(B), ctypes.byref(nnz), ctypes.byref(parts), None, None, None, None, None))
+        if not parts.value & 4:
+            return float(B.value)
+        w = np.zeros(max(B.value, 1), dtype=np.float32)
+        check(self._lib.wd_debug_slot(self._h, int(slot), ctypes.byref(B), ctypes.byref(nnz), ctypes.byref(parts), None, None, None, None,
+                                      w.ctypes.data))
+        return float(w[:B.value].astype(np.float64).sum())
+
     def launch_count(self):
         return int(self._lib.wd_launch_count(self._h))
 

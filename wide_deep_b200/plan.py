@@ -443,6 +443,42 @@ class Plan(object):
         """Features a hidden layer of `units` units hands on (tf.nn.crelu doubles them, reference model_util.py:45-50)."""
         return 2 * units if self.activation == "crelu" else units
 
+    def summary_segments(self):
+        """Segments of the layer statistics, keys (kind, tower, layer) in the library's order (wd_summary_segments): the deep
+        input, per tower its hidden layers and its logits, then the wide logit."""
+        from .summary import SEG_DEEP_INPUT, SEG_HIDDEN, SEG_TOWER_LOGITS, SEG_WIDE_LOGIT
+        out = [(SEG_DEEP_INPUT, -1, -1)] if self.use_deep else []
+        for t, tw in enumerate(self.towers):
+            out += [(SEG_HIDDEN, t, l) for l in range(len(tw["hidden"]))] + [(SEG_TOWER_LOGITS, t, -1)]
+        if self.use_wide:
+            out.append((SEG_WIDE_LOGIT, -1, -1))
+        return out
+
+    def summary_layout(self):
+        """[(tag, segments)] of the reference's add_layer_summary calls in TRAIN mode.  A hidden layer's tag summarises `net` after
+        the layer: its output followed by its connected mode's concatenation (dnn.py:92-193; resnet: quirk Q7); x is the deep
+        input."""
+        from .summary import LINEAR_TAG, SEG_DEEP_INPUT, SEG_HIDDEN, SEG_TOWER_LOGITS, SEG_WIDE_LOGIT, tower_tag
+        x = (SEG_DEEP_INPUT, -1, -1)
+        out = []
+        for t, tw in enumerate(self.towers):
+            h = lambda j: (SEG_HIDDEN, t, j)
+            for l in range(len(tw["hidden"])):
+                mode = tw["mode"]
+                if mode in ("simple", "last_dense"):
+                    segs = [h(l)]
+                elif mode == "first_dense":
+                    segs = [h(l), x]
+                elif mode == "dense":
+                    segs = [x] + [h(j) for j in range(l + 1)]
+                else:
+                    segs = [h(j) for j in range(l, -1, -1)] + [x]
+                out.append((tower_tag(t, l), segs))
+            out.append((tower_tag(t), [(SEG_TOWER_LOGITS, t, -1)]))
+        if self.use_wide:
+            out.append((LINEAR_TAG, [(SEG_WIDE_LOGIT, -1, -1)]))
+        return out
+
     def exchange_rows(self, rows_per_column):
         """Upper bounds (K_emb, K_wide) on the touched rows per step that stay in the (row, gradient) lists, given the maximum
         number of ids one column contributes per step (batch size for single-valued columns): columns whose table is exchanged

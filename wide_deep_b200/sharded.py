@@ -93,6 +93,16 @@ class LocalShardGroup(object):
             out.append(dict(zip(METRIC_KEYS, (float(x) for x in v))))
         return out
 
+    def arm_summary(self):
+        """The next step takes the layer statistics on every rank."""
+        for m in self.models:
+            m.arm_summary()
+
+    def layer_statistics(self):
+        """Layer statistics of the last armed step over the global batch (every rank's rows)."""
+        from .summary import LayerStats
+        return LayerStats.merge_ranks([m.layer_statistics() for m in self.models])
+
     def get_tensor(self, name, slot=0):
         """Global tensor: row-sharded tensors are interleaved back from the ranks' shards."""
         plan = self.models[0].plan
@@ -164,6 +174,23 @@ class ShardedTrainer(object):
         v = np.zeros(10, dtype=np.float64)
         check(self._lib.wd_shard_eval_finish(self.model._h, v.ctypes.data))
         return dict(zip(METRIC_KEYS, (float(x) for x in v)))
+
+    def arm_summary(self):
+        """The next step takes the layer statistics.  Every rank must arm the same steps (the cadence depends only on the global
+        step)."""
+        self.model.arm_summary()
+
+    def layer_statistics(self):
+        """Collective: layer statistics of the last armed step over the global batch, on every rank."""
+        from .summary import LayerStats
+        return LayerStats.merge_ranks(self.gather(self.model.layer_statistics()))
+
+    def gather(self, obj):
+        """Collective: every rank's `obj`, in rank order."""
+        import torch.distributed as dist
+        parts = [None] * self.world
+        dist.all_gather_object(parts, obj, group=self.group)
+        return parts
 
     def get_tensor(self, name, slot=0):
         """Global tensor on every rank (row-sharded tensors are all-gathered through the host and interleaved)."""
