@@ -190,12 +190,22 @@ int wd_memory_usage(WdModel *m, int64_t *device_bytes, int64_t *host_bytes);
  * `bytes` is the HBM budget of the records: it is rounded down to 8 x 2^k slots of the widest host record; the slot metadata
  * (9 bytes per slot) comes on top.  A no-op (capacity 0) when no table is on the host.  WD_ENOMEM when the cache would leave less
  * free HBM than the model keeps in reserve for its later allocations (batch slots, step graphs).  The cache is opt-in:
- * wd_step_backward(_slot) is refused (WD_EUNSUPPORTED) on a model with a cache.  The cache is single-GPU only: on a row-sharded
- * model (shard_world > 1) with host-placed shards it returns WD_EUNSUPPORTED. */
+ * wd_step_backward(_slot) is refused (WD_EUNSUPPORTED) on a model with a cache.  This cache sits in front of the host tables of a
+ * single-GPU model: on a row-sharded model (shard_world > 1) with host-placed shards it returns WD_EUNSUPPORTED (the owner's cache
+ * of its shards is wd_shard_cache_enable). */
 int wd_host_cache_enable(WdModel *m, int64_t bytes);
-/* Cumulative cache counters: out[0] capacity in slots, [1] hits, [2] misses loaded into a slot, [3] overflow rows (staged
- * without a slot: more misses in a set than it has ways), [4] dirty evictions written home.  Copies the first min(n, 5);
- * reset != 0 zeroes the counters [1..4] after the copy.  Synchronises the model stream. */
+/* The same cache on one rank of a row-sharded model (shard_world > 1): it holds the most recently used records of the rank's own
+ * host-placed shards (the rows it owns, in its shard row space) in its HBM, in front of the owner's stage-in and write-back.  Call
+ * per rank, after wd_model_create and before the first step or forward.  Results stay bit-identical to the uncached model and to
+ * the model with every shard in HBM, on both drivers (wd_shard_train_step_slot and wd_shard_phase).  Rules as
+ * wd_host_cache_enable: WD_ESTATE after the first step or forward or when a cache exists, WD_EINVAL for a negative budget or slots
+ * beyond 31-bit staging rows, WD_ENOMEM below the HBM reserve, a no-op (capacity 0) when this rank has no host-placed shard or the
+ * budget is below one set.  WD_EUNSUPPORTED when shard_world == 1 (use wd_host_cache_enable).  A model has at most one cache. */
+int wd_shard_cache_enable(WdModel *m, int64_t bytes);
+/* Cumulative counters of the model's cache (either kind): out[0] capacity in slots, [1] hits, [2] misses loaded into a slot,
+ * [3] overflow rows (staged without a slot: more misses in a set than it has ways), [4] dirty evictions written home.  All 0
+ * without a cache.  Copies the first min(n, 5); reset != 0 zeroes the counters [1..4] after the copy.  Synchronises the model
+ * stream. */
 int wd_host_cache_stats(WdModel *m, int64_t *out, int32_t n, int32_t reset);
 
 /* One training step: H2D copy, ids, forward, loss, backward, optimizers.  Replaces one

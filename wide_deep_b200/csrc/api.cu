@@ -668,8 +668,9 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         if (slot * tb.dim >= tb.stride) { set_error("table has no optimizer slot %d", slot); return WD_EINVAL; }
         float* dev = tb.data + slot * tb.dim;
         const size_t lw = (size_t)tb.dim_logical * 4;
-        // host records cached in HBM: dirty slots go home before either direction; a write then empties the cache
-        if (tb.host && m->cache_slots > 0) {
+        // host records cached in HBM (one GPU, or this rank's host shards): dirty slots go home before either direction; a write
+        // then empties the cache
+        if (tb.host) {
             const int rc = host_cache_sync(m, true, to_device != 0);
             if (rc) return rc;
         }
@@ -1245,7 +1246,7 @@ static int backward_eager(WdModel* m, bool join) {
 // The split step applies the embedding rows with the unfused kernels, which update host records through their mapped pointers:
 // with an HBM cache in front of those records the update would bypass it.
 static int refuse_split_step_with_cache(WdModel* m) {
-    if (m->cache_slots == 0) return WD_OK;
+    if (m->hcache.slots == 0) return WD_OK;
     set_error("the split step (wd_step_backward / wd_step_apply) is not supported on a model with a host-table cache");
     return WD_EUNSUPPORTED;
 }
@@ -1370,6 +1371,7 @@ extern "C" int wd_shard_phase(WdModel* m, int slot, int phase, int train) {
     if (m->shard.ipc) { set_error("wd_shard_phase is for ranks of one process; multi-process ranks call wd_shard_train_step_slot"); return WD_ESTATE; }
     if (train && !m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     if (phase < 0 || phase > 4) { set_error("wd_shard_phase: phase %d outside [0, 4]", phase); return WD_EINVAL; }
+    if (phase == 0) timer_begin(m);
     if ((rc = shard_step(m, train != 0, phase))) return rc;
     return train && phase == 4 ? mark_slot_used(m) : WD_OK;
 }
@@ -1389,6 +1391,7 @@ extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_train_step_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase)"); return WD_ESTATE; }
     if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
+    timer_begin(m);
     GraphRun how;
     if ((rc = run_train_graphed(m, m->slots[slot].shard, m->dbatch, [&](bool) { return shard_step(m, true, kAllSegments); }, &how))) return rc;
     if (how == GraphRun::captured) {

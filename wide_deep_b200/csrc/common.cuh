@@ -119,6 +119,23 @@ struct RecordSet {
     const int64_t* gs_off = nullptr;  // [ntab] float offset inside the small-table gradient block (-1: large table)
 };
 
+// HBM cache of the host records of one record set (host_tables.cu): the single-GPU cache in front of the replicated set
+// (WdModel::hcache, list 0, global rows) or an owner's cache of its host shards (ShardSpace::cache, list 2, shard rows).  The
+// set's staging buffer is then [slots | overflow rows]; a model has at most one cache.
+struct HostCache {
+    int64_t slots = 0;                       // C = 8 x 2^set_bits; 0: no cache (every staged row is an overflow row)
+    int set_bits = 0;
+    uint32_t* d_tag = nullptr;               // [C] row held by the slot (the set's row space), kInvalidRow: empty
+    uint32_t* d_stamp = nullptr;             // [C] stamp of the last call that used the slot (0: empty)
+    uint8_t* d_dirty = nullptr;              // [C] 1: the slot is newer than its host record
+    uint32_t* d_now = nullptr;               // device counter, bumped once per stage-in (the stamp of that call)
+    unsigned long long* d_stats = nullptr;   // [4] hits, loads, overflow rows, dirty evictions
+    int32_t* d_uslot = nullptr;              // [rows] staging row of unique row u; null without a cache (row u)
+    uint32_t* d_uvict = nullptr;             // [rows] row the slot of u held before u was loaded into it
+    uint8_t* d_uflag = nullptr;              // [rows] kLoad / kVictimDirty (host_tables.cu)
+    uint32_t *d_ck[2] = {}, *d_cv[2] = {};   // (set, u) pairs and their sort ping-pong buffers
+};
+
 struct DenseTensor {         // one trainable dense tensor inside the dense arena
     int64_t off;             // offset in arena (floats)
     int64_t count;           // physical element count
@@ -257,9 +274,10 @@ struct ShardSpace {           // one sharded table space on this rank: 0 = embed
     RecordSet set;
     uint32_t* d_adam_touched = nullptr;   // Adam: [ceil(local_rows / 32)] bit r: local row r was updated this step (sparse_dev.cuh)
     // host-placed shards (embedding space): the owner stages the records of the step's unique owned host rows (list 2) in HBM,
-    // record of unique row u at d_stage + u * stage_stride (set.rec.stage: 0 for an HBM slot)
+    // record of unique row u at staging row u (set.rec.stage: 0 for an HBM slot), or at cache.d_uslot[u] with a cache
     int stage_stride = 0;              // widest stride of the space's host slots; 0: every shard in HBM
-    float* d_stage = nullptr;          // [max_nnz + 1][stage_stride] owner staging buffer
+    float* d_stage = nullptr;          // [cache.slots + max_nnz + 1][stage_stride] owner staging buffer
+    HostCache cache;                   // wd_shard_cache_enable: HBM cache of this rank's host shard records
     float4* d_wide = nullptr;          // wide space: {w, n, z, -} per local row
     uint32_t* d_own = nullptr;         // [max_nnz] owner rank of entry j or kInvalidRow (not a sharded column)
     uint32_t* d_lrow = nullptr;        // [max_nnz] local row at the owner
@@ -380,18 +398,8 @@ struct WdModel {
     float* d_stage = nullptr;                // [max_nnz][stage_stride] records of the step's unique host rows, row u at u * stage_stride
     int stage_stride = 0;                    // largest stride of the host tables
     uint32_t* d_g_emb = nullptr;             // [max_nnz] ids the gather reads: e_emb, host-table entries replaced by their unique index u
-    // HBM cache of host records (wd_host_cache_enable): d_stage is then [cache_slots slots | max_nnz overflow rows]
-    int64_t cache_slots = 0;                 // C = 8 x 2^cache_set_bits; 0: no cache (every staged row is an overflow row)
-    int cache_set_bits = 0;
-    uint32_t* d_ctag = nullptr;              // [C] global row held by the slot, kInvalidRow: empty
-    uint32_t* d_cstamp = nullptr;            // [C] stamp of the last call that used the slot (0: empty)
-    uint8_t* d_cdirty = nullptr;             // [C] 1: the slot is newer than its host record
-    uint32_t* d_cnow = nullptr;              // device counter, bumped once per stage-in (the stamp of that call)
-    unsigned long long* d_cstats = nullptr;  // [4] hits, loads, overflow rows, dirty evictions
-    int32_t* d_uslot = nullptr;              // [max_nnz] staging row of unique row u; null without a cache (row u)
-    uint32_t* d_uvict = nullptr;             // [max_nnz] row the slot of u held before u was loaded into it
-    uint8_t* d_uflag = nullptr;              // [max_nnz] kLoad / kVictimDirty (host_tables.cu)
-    uint32_t *d_ck[2] = {}, *d_cv[2] = {};   // (set, u) pairs and their sort ping-pong buffers
+    // HBM cache of host records (wd_host_cache_enable): d_stage is then [hcache.slots slots | max_nnz overflow rows]
+    wd::HostCache hcache;
     bool stepped = false;                    // a forward or train step was issued (step graphs may exist)
 
     // numeric deep columns (device arrays)
@@ -535,9 +543,15 @@ int build_record_sets(WdModel* m);                               // host_tables.
 int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
 int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
 int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
-// host_tables.cu: records of the unique rows urow[0 .. *d_nuniq) of the staged tables of `rec` (tables found by row base) from
-// their host records into staging row u of rec.stage_base (in) or back (!in); S = stride of the staging rows
-int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, const RowRecords& rec, int S);
+// host_tables.cu, over any record set `rr` whose staged tables (found by row base) keep the records of the unique rows of list L
+// (urow[L][0 .. *d_nuniq[L])) in rr.stage_base at stride S, behind cache `c` (c.slots = 0: none, staging row u):
+//   stage_in_rows    cache keys -> sort -> assign (train: the used slots turn dirty), then dirty victims home and the records
+//                    to load -> their staging rows
+//   write_back_rows  overflow staging rows -> host records (every staged row without a cache)
+// `marks` names the phases (wd_last_timings): sort, assign, transfer in (null: the caller marks), write-back.
+struct CacheMarks { const char *sort, *assign, *in, *out; };
+int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, bool train, const CacheMarks& marks);
+int write_back_rows(WdModel* m, const HostCache& c, int L, const RowRecords& rr, int S, const CacheMarks& marks);
 int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d);  // shard.cu: HBM shard_build allocates (held back by auto placement)
 int64_t hbm_reserve_bytes(const WdModel* m);                     // api.cu: HBM the model keeps free for its later allocations
 // tsv.cu: device parse of n lines into the batch buffers on stream st, waiting for it; *status != 0: the buffers do not hold the

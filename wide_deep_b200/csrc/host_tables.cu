@@ -9,8 +9,11 @@
 //     WdModel::rtabs      large, then small                               small-table block (gs_off), stage-in / write-back /
 //                                                                         remap / flush of host tables and the cache, Adam's
 //                                                                         untouched pass (rows)
-//   shard                 slot order            this rank's shard rows    serve, combine, PeerEmb, the owner apply,
-//     ShardSpace::set                                                     host_rows_transfer, the shard's untouched pass
+//   shard                 slot order            this rank's shard rows    serve, combine, PeerEmb, the owner apply, stage-in /
+//     ShardSpace::set                                                     write-back / flush of host shards and their cache,
+//                                                                         the shard's untouched pass
+//   HostCache             per record set: WdModel::hcache in front of the replicated set (list 0), ShardSpace::cache in front
+//                         of the shard set (list 2); its uslot is the set's RowRecords::uslot
 //   gather view           per width,            global rows; a host       emb_pool_fwd_rows_kernel, emb_pool_fwd_kernel<G>
 //     WdModel::d_dim_desc table order           table at its staging row
 // A host table is staged in the by-table and replicated sets (stage[t] = stage_stride, records in d_stage) and read by the gather
@@ -33,8 +36,9 @@
 // model's bit for bit.  Updates that do not go through the fused kernels (data-parallel lists: wd_step_backward + wd_step_apply)
 // address the host records directly through their mapped pointers.
 // Row-sharded tables (shard_world > 1) keep a rank's shard here instead: its owner groups the rows it received (list 2) before
-// serving them and stages them into its own buffer through host_rows_transfer (the owner-side step is in shard.cu).  Only the
-// sharded tables may go to the host then; the replicated ones, the single-GPU staging buffer and the HBM cache stay out of it.
+// serving them and stages them into its own buffer through stage_in_rows / write_back_rows (the owner-side step is in shard.cu),
+// behind its own HBM cache when wd_shard_cache_enable made one.  Only the sharded tables may go to the host then; the replicated
+// ones, the single-GPU staging buffer and the single-GPU cache stay out of it.
 #include <algorithm>
 #include <type_traits>
 
@@ -44,10 +48,11 @@
 namespace wd {
 
 // ---------------------------------------------------------------------------------------------------------- HBM cache
-// wd_host_cache_enable turns the front of the staging buffer into an 8-way set-associative, write-back cache of host records:
-//   d_stage = [C cache slots | max_nnz overflow rows], stride stage_stride; slot s * 8 + w is way w of set s
-//   set of a row  Fibonacci hash of the global row (the hot rows of skewed id streams are the low ids of every table: a plain
-//                 modulo would put them into neighbouring sets)
+// wd_host_cache_enable (one GPU) and wd_shard_cache_enable (an owner's host shards) turn the front of a staging buffer into an
+// 8-way set-associative, write-back cache of host records (HostCache, common.cuh):
+//   stage = [C cache slots | overflow rows], one overflow row per unique row a call can stage; slot s * 8 + w is way w of set s
+//   set of a row  Fibonacci hash of the row in the set's row space (global rows / shard rows; the hot rows of skewed id streams
+//                 are the low ids of every table: a plain modulo would put them into neighbouring sets)
 //   stage-in      keys (set of every unique host row) -> stable radix sort by set -> assign (one thread per run of one set: hits
 //                 keep their slot, misses take the other ways by (last use, way index), empty ways first, and rows beyond the
 //                 ways overflow to staging row C + u) -> transfer (dirty victim home, then the new record in) -> remap
@@ -254,67 +259,72 @@ __global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32
     }
 }
 
-int host_tables_stage_in(WdModel* m, bool train) {
-    const int64_t C = m->cache_slots;
-    const int g = grid_for(m->max_nnz, 256);
-    const RowRecords& rr = m->rtabs.rec;
+int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, bool train, const CacheMarks& marks) {
+    const int64_t C = c.slots;
     if (C > 0) {
-        cache_keys_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], rr, m->cache_set_bits, m->d_ck[0], m->d_cv[0], m->d_cnow);
+        const int g = grid_for(m->max_nnz, 256);
+        cache_keys_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[L], m->d_urow[L], rr, c.set_bits, c.d_ck[0], c.d_cv[0], c.d_now);
         m->launches++;
-        int rc = radix_sort_pairs(m, &m->d_ck[0], &m->d_cv[0], &m->d_ck[1], &m->d_cv[1], m->cache_set_bits + 1, m->d_nuniq[0]);
+        int rc = radix_sort_pairs(m, &c.d_ck[0], &c.d_cv[0], &c.d_ck[1], &c.d_cv[1], c.set_bits + 1, m->d_nuniq[L]);
         if (rc) return rc;
-        mark(m, "cache_sort");
-        const CacheMeta cm{m->d_ctag, m->d_cstamp, m->d_cdirty, m->d_cnow, m->d_cstats};
-        cache_assign_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_ck[0], m->d_cv[0], m->d_urow[0], m->cache_set_bits, C, train ? 1 : 0, cm,
-                                                     m->d_uslot, m->d_uvict, m->d_uflag);
+        mark(m, marks.sort);
+        const CacheMeta cm{c.d_tag, c.d_stamp, c.d_dirty, c.d_now, c.d_stats};
+        cache_assign_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[L], c.d_ck[0], c.d_cv[0], m->d_urow[L], c.set_bits, C, train ? 1 : 0, cm,
+                                                     c.d_uslot, c.d_uvict, c.d_uflag);
         m->launches++;
-        mark(m, "cache_assign");
+        mark(m, marks.assign);
     }
-    const StageMap sm{m->d_uvict, m->d_uflag, C};
-    host_rows_kernel<true><<<grid_for(m->max_nnz * (m->stage_stride / 4) / kInFlight, 256), 256, 0, m->stream>>>(
-        m->d_nuniq[0], m->d_urow[0], rr, m->stage_stride, sm);
-    host_remap_kernel<<<g, 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], rr, m->d_g_emb);
-    m->launches += 2;
+    const StageMap sm{c.d_uvict, c.d_uflag, C};
+    host_rows_kernel<true><<<grid_for(m->max_nnz * (S / 4) / kInFlight, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_urow[L], rr, S, sm);
+    m->launches++;
+    if (marks.in) mark(m, marks.in);
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+
+int write_back_rows(WdModel* m, const HostCache& c, int L, const RowRecords& rr, int S, const CacheMarks& marks) {
+    const StageMap sm{c.d_uvict, c.d_uflag, c.slots};
+    host_rows_kernel<false><<<grid_for(m->max_nnz * (S / 4) / kInFlight, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_urow[L], rr, S, sm);
+    m->launches++;
+    mark(m, marks.out);
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+
+static const CacheMarks kHostMarks{"cache_sort", "cache_assign", nullptr, "write_back"};
+
+int host_tables_stage_in(WdModel* m, bool train) {
+    const RowRecords& rr = m->rtabs.rec;
+    int rc = stage_in_rows(m, m->hcache, 0, rr, m->stage_stride, train, kHostMarks);
+    if (rc) return rc;
+    host_remap_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], rr, m->d_g_emb);
+    m->launches++;
     mark(m, "stage_in");
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 
-int host_tables_write_back(WdModel* m) {
-    const StageMap sm{m->d_uvict, m->d_uflag, m->cache_slots};
-    host_rows_kernel<false><<<grid_for(m->max_nnz * (m->stage_stride / 4) / kInFlight, 256), 256, 0, m->stream>>>(
-        m->d_nuniq[0], m->d_urow[0], m->rtabs.rec, m->stage_stride, sm);
-    m->launches++;
-    mark(m, "write_back");
-    WD_CUDA(cudaGetLastError());
-    return WD_OK;
-}
-
-// The same transfer over another record set without a cache (staging row = u): the host-placed shards of a row-sharded space (shard.cu)
-int host_rows_transfer(WdModel* m, bool in, const int32_t* d_nuniq, const uint32_t* urow, const RowRecords& rec, int S) {
-    const StageMap sm{nullptr, nullptr, 0};
-    const int g = grid_for(m->max_nnz * (S / 4) / kInFlight, 256);
-    if (in) host_rows_kernel<true><<<g, 256, 0, m->stream>>>(d_nuniq, urow, rec, S, sm);
-    else host_rows_kernel<false><<<g, 256, 0, m->stream>>>(d_nuniq, urow, rec, S, sm);
-    m->launches++;
-    mark(m, in ? "shard_stage_in" : "shard_write_back");
-    WD_CUDA(cudaGetLastError());
-    return WD_OK;
-}
+int host_tables_write_back(WdModel* m) { return write_back_rows(m, m->hcache, 0, m->rtabs.rec, m->stage_stride, kHostMarks); }
 
 // Everything that reads or writes host records outside the step: flush = dirty slots home (they stay cached, now clean),
 // invalidate = empty every slot (after the host records were rewritten).  Enqueued on the model stream.
-int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
-    const int64_t C = m->cache_slots;
+static int cache_sync(WdModel* m, HostCache& c, const RowRecords& rr, int S, bool flush, bool invalidate) {
+    const int64_t C = c.slots;
     if (C == 0) return WD_OK;
     if (flush) {
-        cache_flush_kernel<<<grid_for(C * (m->stage_stride / 4), 256), 256, 0, m->stream>>>(C, m->stage_stride, m->d_ctag, m->d_cdirty, m->rtabs.rec);
+        cache_flush_kernel<<<grid_for(C * (S / 4), 256), 256, 0, m->stream>>>(C, S, c.d_tag, c.d_dirty, rr);
         m->launches++;
     }
-    cache_clear_kernel<<<grid_for(C, 256), 256, 0, m->stream>>>(C, m->d_ctag, m->d_cstamp, m->d_cdirty, invalidate ? 1 : 0);
+    cache_clear_kernel<<<grid_for(C, 256), 256, 0, m->stream>>>(C, c.d_tag, c.d_stamp, c.d_dirty, invalidate ? 1 : 0);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
+}
+// the model's cache, whichever it has (the single-GPU one or the owner's cache of its host shards)
+int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
+    ShardSpace& se = m->shard.sp[0];
+    int rc = cache_sync(m, m->hcache, m->rtabs.rec, m->stage_stride, flush, invalidate);
+    return rc ? rc : cache_sync(m, se.cache, se.set.rec, se.stage_stride, flush, invalidate);
 }
 
 // Allocates every embedding table — in HBM (WD_PLACE_HBM, and WD_PLACE_AUTO tables while they fit, largest first, with
@@ -405,8 +415,8 @@ static int upload_records(WdModel* m, RowRecords& r, const std::vector<int>& ids
 
 // Uploads the record sets and the gather view (table at the top of this file) from the tables as they stand.  build_model runs it
 // once every table and staging buffer exists and the shard layout is final (shard_build moves the sharded tables' row bases into
-// the shard's row space); wd_host_cache_enable runs it again after replacing the staging buffer: every array exists by then and is
-// overwritten in place.
+// the shard's row space); wd_host_cache_enable and wd_shard_cache_enable run it again after replacing a staging buffer: every array
+// exists by then and is overwritten in place.
 int build_record_sets(WdModel* m) {
     int rc;
     std::vector<int> all(m->tables.size()), slots;
@@ -418,18 +428,18 @@ int build_record_sets(WdModel* m) {
     auto rows_of = [](const EmbTable& tb) { return tb.arows; };
     if (!m->tables.empty()) {
         // by table
-        if ((rc = upload_records(m, m->tabs.rec, all, m->stage_stride, m->d_stage, m->d_uslot))) return rc;
+        if ((rc = upload_records(m, m->tabs.rec, all, m->stage_stride, m->d_stage, m->hcache.d_uslot))) return rc;
         if ((rc = upload_per_table(m, &m->tabs.x0, all, x0_of))) return rc;
         m->dplan.table_row_base = m->tabs.rec.row_base;
         // replicated, by row
-        if ((rc = upload_records(m, m->rtabs.rec, m->rtab_order, m->stage_stride, m->d_stage, m->d_uslot))) return rc;
+        if ((rc = upload_records(m, m->rtabs.rec, m->rtab_order, m->stage_stride, m->d_stage, m->hcache.d_uslot))) return rc;
         if ((rc = upload_per_table(m, &m->rtabs.rows, m->rtab_order, rows_of))) return rc;
         if ((rc = upload_per_table(m, &m->rtabs.gs_off, m->rtab_order, [](const EmbTable& tb) { return tb.gs_off; }))) return rc;
     }
     // shard: the embedding space's records; the wide space has only its columns' row bases
     ShardSpace& se = m->shard.sp[0];
     if (se.on) {
-        if ((rc = upload_records(m, se.set.rec, slots, se.stage_stride, se.d_stage, nullptr))) return rc;
+        if ((rc = upload_records(m, se.set.rec, slots, se.stage_stride, se.d_stage, se.cache.d_uslot))) return rc;
         if ((rc = upload_per_table(m, &se.set.x0, slots, x0_of))) return rc;
         if ((rc = upload_per_table(m, &se.set.rows, slots, rows_of))) return rc;
     }
@@ -451,79 +461,109 @@ int build_record_sets(WdModel* m) {
     return WD_OK;
 }
 
-// ------------------------------------------------------------------------------------------------------------ C-ABI
-extern "C" int wd_host_cache_enable(WdModel* m, int64_t bytes) {
-    if (!m) { set_error("null model"); return WD_EINVAL; }
-    if (bytes < 0) { set_error("host cache: negative budget %lld", (long long)bytes); return WD_EINVAL; }
-    WD_CUDA(cudaSetDevice(m->device));
-    if (m->stepped) { set_error("wd_host_cache_enable after the first step or forward: the step graphs are already captured"); return WD_ESTATE; }
-    if (m->cache_slots > 0) { set_error("wd_host_cache_enable: the cache is already enabled"); return WD_ESTATE; }
-    if (m->shard.world > 1 && m->host_bytes > 0) {
-        set_error("wd_host_cache_enable: the HBM cache is not supported for the host-placed shards of a row-sharded model");
-        return WD_EUNSUPPORTED;
-    }
-    if (m->n_host_tab == 0) return WD_OK;                                // nothing on the host: capacity 0
-    const int64_t S = m->stage_stride, slot_bytes = S * 4;
+// Turns the front of the staging buffer *stage (stride S, `rows` rows: one per unique row a call can stage) into cache `c` of at
+// most `bytes` of slots: *stage becomes [C slots | rows overflow rows] and the record sets are uploaded again.  Capacity 0 (nothing
+// allocated) when the budget is below one set.  `who` names the entry point in the error messages.
+static int cache_enable(WdModel* m, HostCache& c, int64_t bytes, int S, int64_t rows, float** stage, const char* who) {
+    const int64_t slot_bytes = (int64_t)S * 4;
     const int64_t sets = bytes / (kWays * slot_bytes);
     if (sets < 1) return WD_OK;
     int bits = 0;
     while (((int64_t)2 << bits) <= sets) ++bits;
     const int64_t C = (int64_t)kWays << bits;
-    if (C + m->max_nnz >= ((int64_t)1 << 31)) {
-        set_error("host cache: %lld slots + %lld overflow rows do not fit 31-bit staging rows", (long long)C, (long long)m->max_nnz);
+    if (C + rows >= ((int64_t)1 << 31)) {
+        set_error("%s: %lld slots + %lld overflow rows do not fit 31-bit staging rows", who, (long long)C, (long long)rows);
         return WD_EINVAL;
     }
     // HBM the cache adds: its slots, per-slot tag / stamp / dirty, and per unique row uslot / uvict / uflag + the (set, u) sort pairs
-    const int64_t meta = C * 9 + 4 + 4 * 8 + m->max_nnz * 9 + 4 * (m->max_nnz + 8) * 4;
+    const int64_t meta = C * 9 + 4 + 4 * 8 + rows * 9 + 4 * (m->max_nnz + 8) * 4;
     size_t free_b = 0, total_b = 0;
     WD_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const int64_t reserve = hbm_reserve_bytes(m);
     if ((int64_t)free_b - (C * slot_bytes + meta) < reserve) {
-        set_error("host cache of %lld bytes would leave %lld bytes of HBM free, less than the %lld the model keeps for its later allocations",
-                  (long long)(C * slot_bytes), (long long)((int64_t)free_b - C * slot_bytes - meta), (long long)reserve);
+        set_error("%s: a cache of %lld bytes would leave %lld bytes of HBM free, less than the %lld the model keeps for its later allocations",
+                  who, (long long)(C * slot_bytes), (long long)((int64_t)free_b - C * slot_bytes - meta), (long long)reserve);
         return WD_ENOMEM;
     }
-    // the staging buffer grows to [C slots | max_nnz overflow rows]: the old one is freed and every descriptor re-pointed
+    // the staging buffer grows to [C slots | rows overflow rows]: the old one is freed and every descriptor re-pointed
     WD_CUDA(cudaStreamSynchronize(m->stream));
-    auto it = std::find(m->allocs.begin(), m->allocs.end(), (void*)m->d_stage);
+    auto it = std::find(m->allocs.begin(), m->allocs.end(), (void*)*stage);
     if (it != m->allocs.end()) {
-        WD_CUDA(cudaFree(m->d_stage));
+        WD_CUDA(cudaFree(*stage));
         m->allocs.erase(it);
-        m->bytes_allocated -= m->max_nnz * slot_bytes;
+        m->bytes_allocated -= rows * slot_bytes;
     }
-    m->d_stage = nullptr;
+    *stage = nullptr;
     int rc;
-    if ((rc = dev_alloc(m, &m->d_stage, (C + m->max_nnz) * S, false))) return rc;
-    if ((rc = dev_alloc(m, &m->d_ctag, C, false))) return rc;
-    WD_CUDA(cudaMemsetAsync(m->d_ctag, 0xFF, C * 4, m->stream));       // kInvalidRow
-    if ((rc = dev_alloc(m, &m->d_cstamp, C))) return rc;
-    if ((rc = dev_alloc(m, &m->d_cdirty, C))) return rc;
-    if ((rc = dev_alloc(m, &m->d_cnow, 1))) return rc;
-    if ((rc = dev_alloc(m, &m->d_cstats, 4))) return rc;
-    if ((rc = dev_alloc(m, &m->d_uslot, m->max_nnz))) return rc;
-    if ((rc = dev_alloc(m, &m->d_uvict, m->max_nnz))) return rc;
-    if ((rc = dev_alloc(m, &m->d_uflag, m->max_nnz))) return rc;
+    if ((rc = dev_alloc(m, stage, (C + rows) * S, false))) return rc;
+    if ((rc = dev_alloc(m, &c.d_tag, C, false))) return rc;
+    WD_CUDA(cudaMemsetAsync(c.d_tag, 0xFF, C * 4, m->stream));         // kInvalidRow
+    if ((rc = dev_alloc(m, &c.d_stamp, C))) return rc;
+    if ((rc = dev_alloc(m, &c.d_dirty, C))) return rc;
+    if ((rc = dev_alloc(m, &c.d_now, 1))) return rc;
+    if ((rc = dev_alloc(m, &c.d_stats, 4))) return rc;
+    if ((rc = dev_alloc(m, &c.d_uslot, rows))) return rc;
+    if ((rc = dev_alloc(m, &c.d_uvict, rows))) return rc;
+    if ((rc = dev_alloc(m, &c.d_uflag, rows))) return rc;
     for (int k = 0; k < 2; ++k) {
-        if ((rc = dev_alloc(m, &m->d_ck[k], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_cv[k], m->max_nnz + 8))) return rc;
+        if ((rc = dev_alloc(m, &c.d_ck[k], m->max_nnz + 8))) return rc;
+        if ((rc = dev_alloc(m, &c.d_cv[k], m->max_nnz + 8))) return rc;
     }
-    m->cache_slots = C;
-    m->cache_set_bits = bits;
+    c.slots = C;
+    c.set_bits = bits;
     if ((rc = build_record_sets(m))) return rc;
     WD_CUDA(cudaStreamSynchronize(m->stream));
     return WD_OK;
+}
+
+// the checks both entry points share: arguments, and no step or forward issued and no cache yet
+static int cache_enable_check(WdModel* m, int64_t bytes, const char* who) {
+    if (!m) { set_error("null model"); return WD_EINVAL; }
+    if (bytes < 0) { set_error("%s: negative budget %lld", who, (long long)bytes); return WD_EINVAL; }
+    if (m->stepped) { set_error("%s after the first step or forward: the step graphs are already captured", who); return WD_ESTATE; }
+    if (m->hcache.slots > 0 || m->shard.sp[0].cache.slots > 0) { set_error("%s: the cache is already enabled", who); return WD_ESTATE; }
+    return WD_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------ C-ABI
+extern "C" int wd_host_cache_enable(WdModel* m, int64_t bytes) {
+    int rc = cache_enable_check(m, bytes, "wd_host_cache_enable");
+    if (rc) return rc;
+    WD_CUDA(cudaSetDevice(m->device));
+    if (m->shard.world > 1 && m->host_bytes > 0) {
+        set_error("wd_host_cache_enable: the host-placed shards of a row-sharded model are cached by their owner: use wd_shard_cache_enable");
+        return WD_EUNSUPPORTED;
+    }
+    if (m->n_host_tab == 0) return WD_OK;                                // nothing on the host: capacity 0
+    return cache_enable(m, m->hcache, bytes, m->stage_stride, m->max_nnz, &m->d_stage, "wd_host_cache_enable");
+}
+
+// The owner's cache of this rank's host shards: the rows of list 2 (every unique owned row of a call, max_nnz + 1 staging rows:
+// see the serve in shard.cu) in the shard set's row space.
+extern "C" int wd_shard_cache_enable(WdModel* m, int64_t bytes) {
+    int rc = cache_enable_check(m, bytes, "wd_shard_cache_enable");
+    if (rc) return rc;
+    if (m->shard.world <= 1) {
+        set_error("wd_shard_cache_enable: the model is not row-sharded (shard_world <= 1); its host tables are cached by wd_host_cache_enable");
+        return WD_EUNSUPPORTED;
+    }
+    WD_CUDA(cudaSetDevice(m->device));
+    ShardSpace& se = m->shard.sp[0];
+    if (se.stage_stride == 0) return WD_OK;                              // no host shard on this rank: capacity 0
+    return cache_enable(m, se.cache, bytes, se.stage_stride, m->max_nnz + 1, &se.d_stage, "wd_shard_cache_enable");
 }
 
 extern "C" int wd_host_cache_stats(WdModel* m, int64_t* out, int32_t n, int32_t reset) {
     if (!m || n < 0 || (n > 0 && !out)) { set_error("null argument"); return WD_EINVAL; }
     WD_CUDA(cudaSetDevice(m->device));
     WD_CUDA(cudaStreamSynchronize(m->stream));
+    const HostCache& c = m->hcache.slots > 0 ? m->hcache : m->shard.sp[0].cache;
     unsigned long long h[4] = {0, 0, 0, 0};
-    if (m->d_cstats) WD_CUDA(cudaMemcpy(h, m->d_cstats, sizeof(h), cudaMemcpyDeviceToHost));
-    const int64_t v[5] = {m->cache_slots, (int64_t)h[0], (int64_t)h[1], (int64_t)h[2], (int64_t)h[3]};
+    if (c.d_stats) WD_CUDA(cudaMemcpy(h, c.d_stats, sizeof(h), cudaMemcpyDeviceToHost));
+    const int64_t v[5] = {c.slots, (int64_t)h[0], (int64_t)h[1], (int64_t)h[2], (int64_t)h[3]};
     for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
-    if (reset && m->d_cstats) {
-        WD_CUDA(cudaMemsetAsync(m->d_cstats, 0, sizeof(h), m->stream));
+    if (reset && c.d_stats) {
+        WD_CUDA(cudaMemsetAsync(c.d_stats, 0, sizeof(h), m->stream));
         WD_CUDA(cudaStreamSynchronize(m->stream));
     }
     return WD_OK;

@@ -144,16 +144,17 @@ __device__ __forceinline__ bool shard_locate(int64_t f, const int32_t* __restric
 }
 
 // embedding space: 8 lanes per received entry; the lanes of a bag's first entry pool the whole run and store the partial sum.
-// slot_stage (null: every shard in HBM): a host slot's records are read from the owner staging buffer, row u = position of the
-// local row in the step's unique owned rows urow[0 .. *d_nuniq) (list 2, sorted ascending).  (Entries beyond the max_nnz the grouping
-// keeps — flagged as truncated — find u <= max_nnz: the staging buffer has one spare row.)
+// slot_stage (null: every shard in HBM): a host slot's records are read from the owner staging buffer, at uslot[u] (the owner's
+// cache) or row u without a cache, u = position of the local row in the step's unique owned rows urow[0 .. *d_nuniq) (list 2,
+// sorted ascending).  (Entries beyond the max_nnz the grouping keeps — flagged as truncated — find u <= max_nnz: the staging
+// buffer has one spare overflow row and uslot one spare entry.)
 __global__ void __launch_bounds__(256) shard_serve_emb_kernel(const uint2* __restrict__ inbox, const int32_t* __restrict__ cnt, int G, int me,
                                                               int64_t pair_cap, int n_slots, const int64_t* __restrict__ slot_base,
                                                               float* const* __restrict__ slot_data, const int32_t* __restrict__ slot_dim,
                                                               const int32_t* __restrict__ slot_stride, const ShardPeer* __restrict__ peers,
                                                               int64_t nbags_cap, int width, const int32_t* __restrict__ slot_stage,
                                                               const float* __restrict__ stage, const uint32_t* __restrict__ urow,
-                                                              const int32_t* __restrict__ d_nuniq) {
+                                                              const int32_t* __restrict__ d_nuniq, const int32_t* __restrict__ uslot) {
     const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
     int64_t total = 0;
     for (int r = 0; r < G; ++r) total += __ldcg(cnt + r);
@@ -171,7 +172,11 @@ __global__ void __launch_bounds__(256) shard_serve_emb_kernel(const uint2* __res
         const float* data = sst ? stage : slot_data[lo];
         const int64_t base = slot_base[lo];
         const int nu = sst ? *d_nuniq : 0;
-        auto rec = [&](uint32_t lrow) -> int64_t { return sst ? (int64_t)lower_bound_u32(urow, nu, lrow) : (int64_t)lrow - base; };
+        auto rec = [&](uint32_t lrow) -> int64_t {
+            if (!sst) return (int64_t)lrow - base;
+            const int u = lower_bound_u32(urow, nu, lrow);
+            return uslot ? (int64_t)__ldg(uslot + u) : (int64_t)u;
+        };
         const int n = __ldcg(cnt + r);
         float* dst = peers[r].recv + ((int64_t)me * nbags_cap + en.y) * width;
         for (int q = lig; q * 4 < dim; q += 8) {
@@ -590,9 +595,10 @@ static int shard_owner_group(WdModel* m, int s);
 
 // a space whose owner stages host-placed shards groups its received rows before serving them (the serve reads the staged records)
 static bool staged(const WdModel* m, int s) { return m->shard.sp[s].stage_stride > 0; }
+static const CacheMarks kShardMarks{"shard_cache_sort", "shard_cache_assign", "shard_stage_in", "shard_write_back"};
 
 // ---- owner: pooled partial sums of the received bags -> requesters' receive buffers
-static int shard_serve(WdModel* m, int s) {
+static int shard_serve(WdModel* m, int s, bool train) {
     ShardState& S = m->shard;
     ShardSpace& sp = S.sp[s];
     if (!sp.on) return WD_OK;
@@ -600,12 +606,12 @@ static int shard_serve(WdModel* m, int s) {
     int rc;
     if (staged(m, s)) {                          // unique owned rows (list 2), then the records of the host rows among them -> HBM
         if ((rc = shard_owner_group(m, s))) return rc;
-        if ((rc = host_rows_transfer(m, true, m->d_nuniq[2], m->d_urow[2], sp.set.rec, sp.stage_stride))) return rc;
+        if ((rc = stage_in_rows(m, sp.cache, 2, sp.set.rec, sp.stage_stride, train, kShardMarks))) return rc;
     }
     if (s == 0)
         shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, S.rank, sp.pair_cap,
             sp.n_slots, sp.set.rec.row_base, sp.set.rec.data, sp.set.rec.dim, sp.set.rec.stride, sp.d_peers, sp.nbags_cap, sp.width,
-            sp.set.rec.stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2]);
+            sp.set.rec.stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2], sp.cache.d_uslot);
     else
         shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, S.rank, sp.pair_cap,
             sp.d_wide, sp.d_peers, sp.nbags_cap);
@@ -660,8 +666,9 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
         if ((rc = list_apply_emb(m, L, sp.width, sp.set.rec, o))) return rc;
         // Adam: the shard's rows no rank touched, after its touched ones (no host-placed shards with Adam: no staged records)
         if ((rc = adam_untouched_emb(m, sp.set, sp.local_rows, o))) return rc;
-        // staged records home, on this stream: it joins the main stream before the step ends, so the next stage-in comes after
-        if (staged(m, s) && (rc = host_rows_transfer(m, false, m->d_nuniq[L], m->d_urow[L], sp.set.rec, sp.stage_stride))) return rc;
+        // staged records home (overflow rows only with a cache), on this stream: it joins the main stream before the step ends, so
+        // the next stage-in comes after
+        if (staged(m, s) && (rc = write_back_rows(m, sp.cache, L, sp.set.rec, sp.stage_stride, kShardMarks))) return rc;
     } else {
         const PeerWide src{m->d_sv[L], sp.d_rtag, sp.d_peers};
         wide_grad_sum_kernel<PeerWide, false><<<grid_for(m->max_nnz + m->cpart_cap, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],
@@ -713,19 +720,21 @@ static bool aux_split(WdModel* m) { return m->shard.sp[0].on && m->shard.sp[1].o
 
 // after barrier A: serve both spaces and run the local part of the forward (needed only by this rank's towers, while every peer's
 // barrier B waits for the serves)
-static int shard_serve_both(WdModel* m) {
+// (The embedding space's stage-in sorts its cache keys on the main stream while the aux stream and the side streams may be sorting
+// too: every stream has its own scan / sort scratch, on_stream.)
+static int shard_serve_both(WdModel* m, bool train) {
     ShardState& S = m->shard;
     int rc;
     if (aux_split(m)) {
         WD_CUDA(cudaEventRecord(S.ev_a2, m->stream));
         WD_CUDA(cudaStreamWaitEvent(S.aux, S.ev_a2, 0));
-        if ((rc = on_aux(m, [&] { int r = shard_serve(m, 1); return r ? r : sparse_forward(m); }))) return rc;
+        if ((rc = on_aux(m, [&] { int r = shard_serve(m, 1, train); return r ? r : sparse_forward(m); }))) return rc;
         WD_CUDA(cudaEventRecord(S.ev_aux_done, S.aux));
-        if ((rc = shard_serve(m, 0))) return rc;
+        if ((rc = shard_serve(m, 0, train))) return rc;
         WD_CUDA(cudaStreamWaitEvent(m->stream, S.ev_aux_done, 0));
         return WD_OK;
     }
-    for (int s = 0; s < 2; ++s) if ((rc = shard_serve(m, s))) return rc;
+    for (int s = 0; s < 2; ++s) if ((rc = shard_serve(m, s, train))) return rc;
     return sparse_forward(m);
 }
 
@@ -749,6 +758,7 @@ int shard_step(WdModel* m, bool train, int seg) {
     auto runs = [&](int k) { return seg == kAllSegments || seg == k; };
     int rc;
     if (runs(0)) {
+        m->stepped = true;
         if (S.d_trace) { shard_stamp_kernel<<<1, 1, 0, m->stream>>>(S.d_trace + 2 * (kBarriers - 1)); m->launches++; }   // step start
         if ((rc = ids_prepare(m))) return rc;
         const bool split = aux_split(m);
@@ -765,7 +775,7 @@ int shard_step(WdModel* m, bool train, int seg) {
         if ((rc = barrier(m, BAR_A))) return rc;
     }
     if (runs(1)) {
-        if ((rc = shard_serve_both(m))) return rc;
+        if ((rc = shard_serve_both(m, train))) return rc;
         if (train) {
             WD_CUDA(cudaEventRecord(S.ev_a, m->stream));
             for (int s = 0; s < 2; ++s) {

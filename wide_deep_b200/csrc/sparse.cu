@@ -711,7 +711,7 @@ int sparse_apply_which(WdModel* m, int which) {
     // the fused updates of host-table rows went to their staged copies: copy those home (the unfused kernels below update host
     // records in place, through their mapped pointers)
     if (done) return (which == 0 && m->n_host_tab > 0) ? host_tables_write_back(m) : WD_OK;
-    if (which == 0 && m->cache_slots > 0) {       // the unfused updates below would write host records behind the cache's back
+    if (which == 0 && m->hcache.slots > 0) {       // the unfused updates below would write host records behind the cache's back
         set_error("embedding rows of a model with a host-table cache are only updated by the fused single-GPU step");
         return WD_EUNSUPPORTED;
     }

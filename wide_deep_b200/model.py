@@ -77,6 +77,8 @@ class WideDeepModel(object):
         self.global_step = 0
         if getattr(plan, "host_cache_bytes", 0) > 0:
             check(self._lib.wd_host_cache_enable(self._h, int(plan.host_cache_bytes)))
+        if getattr(plan, "shard_cache_bytes", 0) > 0:
+            check(self._lib.wd_shard_cache_enable(self._h, int(plan.shard_cache_bytes)))
 
     def close(self):
         if getattr(self, "_h", None):
@@ -108,8 +110,9 @@ class WideDeepModel(object):
         return dev.value, host.value
 
     def host_cache_stats(self, reset=False):
-        """Cumulative counters of the HBM cache of host-table records: dict(capacity (slots), hits, loads (misses loaded into a
-        slot), overflow (rows staged without a slot), evictions (dirty records written home)).  All 0 without a cache."""
+        """Cumulative counters of the HBM cache of host-table records (one GPU) or of this rank's host shard records (a rank of a
+        row-sharded model): dict(capacity (slots), hits, loads (misses loaded into a slot), overflow (rows staged without a slot),
+        evictions (dirty records written home)).  All 0 without a cache."""
         out = (ctypes.c_int64 * 5)()
         check(self._lib.wd_host_cache_stats(self._h, out, 5, 1 if reset else 0))
         return dict(zip(("capacity", "hits", "loads", "overflow", "evictions"), (int(v) for v in out)))

@@ -149,7 +149,7 @@ class Plan(object):
     def __init__(self, feature_conf, cross_conf, model_conf, model_type="wide_deep", max_batch=8192,
                  embedding_dim_override=None, tf_compat_pad=False, gemm_engine="auto", max_nnz=0, max_keys=0,
                  dense_exchange_max_rows=0, shard_world=1, shard_rank=0, shard_capacity=0, shard_slack=2.0, host_tables=None,
-                 host_cache_bytes=0):
+                 host_cache_bytes=0, shard_cache_bytes=0):
         if model_type not in ("wide", "deep", "wide_deep"):
             raise ValueError("Invalid model type: {}, must be one of `wide`, `deep`, `wide_deep`".format(model_type))
         self.model_type, self.max_batch, self.tf_compat_pad = model_type, int(max_batch), bool(tf_compat_pad)
@@ -336,6 +336,14 @@ class Plan(object):
         if isinstance(host_cache_bytes, bool) or not isinstance(host_cache_bytes, (int, np.integer)) or host_cache_bytes < 0:
             raise ValueError("host_cache_bytes must be an int >= 0, got {!r}".format(host_cache_bytes))
         self.host_cache_bytes = int(host_cache_bytes)
+        # HBM budget (bytes, per rank) of the owner's write-back cache of its host-placed shard records (wd_shard_cache_enable);
+        # 0 = no cache.  Row-sharded plans only: one GPU caches its host tables through host_cache_bytes.
+        if isinstance(shard_cache_bytes, bool) or not isinstance(shard_cache_bytes, (int, np.integer)) or shard_cache_bytes < 0:
+            raise ValueError("shard_cache_bytes must be an int >= 0, got {!r}".format(shard_cache_bytes))
+        if shard_cache_bytes > 0 and self.shard_world <= 1:
+            raise ValueError("shard_cache_bytes caches the host shards of a row-sharded model (shard_world > 1); "
+                             "a single-GPU model caches its host tables through host_cache_bytes")
+        self.shard_cache_bytes = int(shard_cache_bytes)
 
         # ---- MLP
         hu = model_conf.get("dnn_hidden_units") or []

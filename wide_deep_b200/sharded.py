@@ -103,6 +103,10 @@ class LocalShardGroup(object):
         from .summary import LayerStats
         return LayerStats.merge_ranks([m.layer_statistics() for m in self.models])
 
+    def host_cache_stats(self, reset=False):
+        """Per rank, the counters of its cache of host shard records (WideDeepModel.host_cache_stats)."""
+        return [m.host_cache_stats(reset) for m in self.models]
+
     def get_tensor(self, name, slot=0):
         """Global tensor: row-sharded tensors are interleaved back from the ranks' shards."""
         plan = self.models[0].plan
@@ -184,6 +188,10 @@ class ShardedTrainer(object):
         """Collective: layer statistics of the last armed step over the global batch, on every rank."""
         from .summary import LayerStats
         return LayerStats.merge_ranks(self.gather(self.model.layer_statistics()))
+
+    def host_cache_stats(self, reset=False):
+        """Collective: every rank's counters of its cache of host shard records, in rank order."""
+        return self.gather(self.model.host_cache_stats(reset))
 
     def gather(self, obj):
         """Collective: every rank's `obj`, in rank order."""
