@@ -65,17 +65,7 @@ static std::vector<std::vector<int>> layer_sources(int mode, int L) {
 
 using namespace wd;
 
-struct WdModelExtra {   // host-only bookkeeping kept beside WdModel
-    std::vector<uint8_t> x0_real;            // [d0_phys] 1 where a physical deep-input column is a real feature
-    int d0_logical = 0;
-    std::vector<std::vector<int>> dense_index;   // [tower-layer id][sub] -> index into WdModel::dense, -1
-    std::vector<int> did_tower, did_layer;
-};
-static std::vector<std::pair<WdModel*, WdModelExtra*>> g_extra;
-static WdModelExtra* extra_of(WdModel* m) {
-    for (auto& p : g_extra) if (p.first == m) return p.second;
-    return nullptr;
-}
+static int ensure_slot(WdModel* m, int s);
 
 extern "C" const char* wd_last_error(void) { return wd::g_err; }
 extern "C" int wd_version(void) { return WD_API_VERSION; }
@@ -92,40 +82,25 @@ namespace wd { void tc_map_cache_clear(); }
 extern "C" int wd_model_destroy(WdModel* m) {
     if (!m) return WD_OK;
     cudaSetDevice(m->device);
-    if (m->stream) cudaStreamSynchronize(m->stream);
+    for (cudaStream_t s : m->streams) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    for (cudaEvent_t e : m->events) cudaEventDestroy(e);
     tc_map_cache_clear();
     for (auto& sl : m->slots) {
         sl.train.destroy();
         sl.bwd.destroy();
         sl.shard.destroy();
         sl.shard_eval.destroy();
-        if (sl.ev_up) cudaEventDestroy(sl.ev_up);
-        if (sl.ev_used) cudaEventDestroy(sl.ev_used);
     }
-    if (m->stream_up) { cudaStreamSynchronize(m->stream_up); cudaStreamDestroy(m->stream_up); }
-    tsv_dev_destroy(m);
     for (auto& g : m->merge_graph) g.destroy();
-    if (m->ev_bwd_done) cudaEventDestroy(m->ev_bwd_done);
-    for (void* p : m->allocs) cudaFree(p);
+    tsv_dev_destroy(m);
+    const ShardState& S = m->shard;
+    if (S.ipc)                                               // the peers' segments wd_shard_connect_ipc mapped
+        for (int r = 0; r < S.world; ++r)
+            if (r != S.rank && S.peer_seg[r]) cudaIpcCloseMemHandle(S.peer_seg[r]);
+    for (const DevAlloc& a : m->allocs) cudaFree(a.p);
     for (void* p : m->host_allocs) cudaFreeHost(p);
     if (m->h_loss_pinned) cudaFreeHost(m->h_loss_pinned);
-    for (auto& e : m->timer.ev) if (e) cudaEventDestroy(e);
-    if (m->shard.aux) { cudaStreamSynchronize(m->shard.aux); cudaStreamDestroy(m->shard.aux); }
-    for (cudaEvent_t ev : {m->shard.ev_a, m->shard.ev_ids2, m->shard.ev_routed1, m->shard.ev_a2, m->shard.ev_aux_done}) if (ev) cudaEventDestroy(ev);
-    for (int w = 0; w < 2; ++w) {
-        if (m->sstream[w]) { cudaStreamSynchronize(m->sstream[w]); cudaStreamDestroy(m->sstream[w]); }
-        if (m->ev_grouped[w]) cudaEventDestroy(m->ev_grouped[w]);
-        if (m->ev_done[w]) cudaEventDestroy(m->ev_done[w]);
-    }
-    if (m->ev_ids) cudaEventDestroy(m->ev_ids);
-    if (m->ev_wide_fwd) cudaEventDestroy(m->ev_wide_fwd);
-    if (m->ev_wgrad_rest) cudaEventDestroy(m->ev_wgrad_rest);
-    if (m->ev_head) cudaEventDestroy(m->ev_head);
-    if (m->ev_dx0) cudaEventDestroy(m->ev_dx0);
-    if (m->stream) cudaStreamDestroy(m->stream);
     delete m->summ;
-    for (size_t i = 0; i < g_extra.size(); ++i)
-        if (g_extra[i].first == m) { delete g_extra[i].second; g_extra.erase(g_extra.begin() + i); break; }
     delete m;
     return WD_OK;
 }
@@ -145,7 +120,7 @@ static int init_dense_slots(WdModel* m) {
     return WD_OK;
 }
 
-static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
+static int build_model(const WdPlanDesc* d, WdModel* m) {
     int rc;
     m->use_wide = d->model_type & 1;
     m->use_deep = (d->model_type & 2) != 0;
@@ -215,13 +190,9 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     if ((rc = upload(m, &m->d_num_a, d->num_norm_a, d->n_numeric))) return rc;
     if ((rc = upload(m, &m->d_num_b, d->num_norm_b, d->n_numeric))) return rc;
 
-    // ---- batch buffers
+    // ---- batch slot 0
     const int64_t Bm = m->max_batch;
-    if ((rc = dev_alloc(m, &m->d_cat_offsets, Bm * std::max(d->n_cat_fields, 1) + 1))) return rc;
-    if ((rc = dev_alloc(m, &m->d_cat_keys, m->keys_cap))) return rc;
-    if ((rc = dev_alloc(m, &m->d_dense, Bm * std::max(d->n_dense_fields, 1)))) return rc;
-    if ((rc = dev_alloc(m, &m->d_label, Bm))) return rc;
-    if ((rc = dev_alloc(m, &m->d_weight, Bm))) return rc;
+    if ((rc = ensure_slot(m, 0))) return rc;
     if ((rc = dev_alloc(m, &m->d_col_offs, Bm * std::max(C, 1) + 2))) return rc;
     if ((rc = dev_alloc(m, &m->d_e_wide, m->max_nnz))) return rc;
     if ((rc = dev_alloc(m, &m->d_e_emb, m->max_nnz))) return rc;
@@ -274,7 +245,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     }
 
     // ---- deep part
-    x->x0_real.assign(std::max(d->d0_phys, 1), 0);
+    m->x0_real.assign(std::max(d->d0_phys, 1), 0);
     if (m->use_deep) {
         int64_t row_base = 0;
         const int nslots = opt_nslots(m->dnn_opt);
@@ -292,7 +263,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
             tb.place = d->table_placement ? d->table_placement[t] : WD_PLACE_HBM;
             if (tb.place < WD_PLACE_HBM || tb.place > WD_PLACE_AUTO) { set_error("table %d: placement %d is not a WD_PLACE_*", t, tb.place); return WD_EINVAL; }
             tb.data = nullptr;                                       // allocated by place_tables, after every other buffer of the model
-            for (int i = 0; i < tb.dim_logical; ++i) x->x0_real[tb.x0_off + i] = 1;
+            for (int i = 0; i < tb.dim_logical; ++i) m->x0_real[tb.x0_off + i] = 1;
             m->emb_max_dim = std::max(m->emb_max_dim, tb.dim);
             m->tables.push_back(tb);
         }
@@ -318,10 +289,10 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
         m->emb_total_rows = row_base;
         if (m->dnn_opt.kind == WD_OPT_ADAM && (rc = dev_alloc(m, &m->d_adam_touched[0], (row_base + 31) / 32))) return rc;
         if (row_base >= (1ll << 31)) { set_error("more than 2^31 embedding rows on one device"); return WD_EUNSUPPORTED; }
-        for (int i = 0; i < d->n_numeric; ++i) x->x0_real[d->num_x0_off[i]] = 1;
+        for (int i = 0; i < d->n_numeric; ++i) m->x0_real[d->num_x0_off[i]] = 1;
         for (int c = 0; c < C; ++c)
-            if (d->col_ind_off[c] >= 0) for (int64_t i = 0; i < d->col_buckets[c]; ++i) x->x0_real[d->col_ind_off[c] + i] = 1;
-        for (auto v : x->x0_real) x->d0_logical += v;
+            if (d->col_ind_off[c] >= 0) for (int64_t i = 0; i < d->col_buckets[c]; ++i) m->x0_real[d->col_ind_off[c] + i] = 1;
+        for (auto v : m->x0_real) m->d0_logical += v;
         const int nt = (int)m->tables.size();
         // group the replicated tables by width (the gather view, build_record_sets)
         for (int t = 0; t < nt; ++t) {
@@ -363,7 +334,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
                     int src = srcs[l][s];
                     Seg sg{};
                     sg.src = src;
-                    sg.width = src < 0 ? x->d0_logical : hu[src];
+                    sg.width = src < 0 ? m->d0_logical : hu[src];
                     sg.width_phys = src < 0 ? d->d0_phys : pad_to(hu[src], 32);
                     sg.k_off = koff;
                     koff += sg.width_phys; klog += sg.width;
@@ -416,8 +387,8 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
                     L.t_bias = add_dense(1, 1, m->row_tiles, 1, 4, false);
                 }
                 idx[WD_D_KERNEL] = L.t_kernel; idx[WD_D_BIAS] = L.t_bias; idx[WD_D_GAMMA] = L.t_gamma; idx[WD_D_BETA] = L.t_beta;
-                x->dense_index.push_back(idx);
-                x->did_tower.push_back(t); x->did_layer.push_back(l);
+                m->dense_index.push_back(idx);
+                m->did_tower.push_back(t); m->did_layer.push_back(l);
                 ++did;
                 tw.layers.push_back(L);
             }
@@ -496,7 +467,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m, WdModelExtra* x) {
     if ((rc = metrics_setup())) return rc;
     if ((rc = init_sparse_tables(m, 0, 0))) return rc;           // slots = initial accumulator, weights 0
     if ((rc = init_dense_slots(m))) return rc;
-    for (auto& e : m->timer.ev) WD_CUDA(cudaEventCreate(&e));
+    for (auto& e : m->timer.ev) WD_CUDA(new_event(m, &e, cudaEventDefault));
     WD_CUDA(cudaStreamSynchronize(m->stream));
     return WD_OK;
 }
@@ -512,26 +483,16 @@ extern "C" int wd_model_create(const WdPlanDesc* d, int device, WdModel** out) {
     if (device < 0 || device >= ndev) { set_error("device %d out of range (%d devices)", device, ndev); return WD_EINVAL; }
     WD_CUDA(cudaSetDevice(device));
     WdModel* m = new WdModel();
-    WdModelExtra* x = new WdModelExtra();
-    g_extra.push_back({m, x});
     m->device = device;
-    memset(m->timer.ev, 0, sizeof(m->timer.ev));
-    cudaError_t e = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&m->stream_up, cudaStreamNonBlocking);
-    for (int w = 0; w < 2; ++w) {
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&m->sstream[w], cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_grouped[w], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_done[w], cudaEventDisableTiming);
-    }
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_ids, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_wide_fwd, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_wgrad_rest, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_head, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_dx0, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&m->ev_bwd_done, cudaEventDisableTiming);
+    cudaError_t e = cudaSuccess;
+    for (cudaStream_t* s : {&m->stream, &m->stream_up, &m->sstream[0], &m->sstream[1]})
+        if (e == cudaSuccess) e = new_stream(m, s);
+    for (cudaEvent_t* ev : {&m->ev_grouped[0], &m->ev_grouped[1], &m->ev_done[0], &m->ev_done[1], &m->ev_ids, &m->ev_wide_fwd,
+                            &m->ev_wgrad_rest, &m->ev_head, &m->ev_dx0, &m->ev_bwd_done})
+        if (e == cudaSuccess) e = new_event(m, ev, cudaEventDisableTiming);
     if (e != cudaSuccess) { set_error("cudaStreamCreate: %s", cudaGetErrorString(e)); wd_model_destroy(m); return WD_ECUDA; }
     m->graphs_enabled = getenv("WD_NO_GRAPH") == nullptr;
-    int rc = build_model(d, m, x);
+    int rc = build_model(d, m);
     if (rc) { wd_model_destroy(m); return rc; }
     *out = m;
     return WD_OK;
@@ -557,7 +518,7 @@ int64_t hbm_reserve_bytes(const WdModel* m) {
 }  // namespace wd
 
 // glorot-uniform kernels / zero biases / gamma 1 / beta 0 built on the host (dense part is ~1.5M floats)
-static int init_dense(WdModel* m, WdModelExtra* x, uint64_t seed) {
+static int init_dense(WdModel* m, uint64_t seed) {
     if (m->dense_count == 0) return WD_OK;
     std::vector<float> P(m->dense_count, 0.f), S1(m->dense_count, 0.f), S2(m->dense_count, 0.f);
     std::mt19937_64 rng(seed * 7919 + 17);
@@ -571,7 +532,7 @@ static int init_dense(WdModel* m, WdModelExtra* x, uint64_t seed) {
             for (int s = 0; s < L.n_in_segs; ++s) {
                 const Seg& sg = L.segs[s];
                 for (int j = 0; j < sg.width_phys; ++j) {
-                    bool real = sg.src < 0 ? (x->x0_real[j] != 0) : (j < sg.width);
+                    bool real = sg.src < 0 ? (m->x0_real[j] != 0) : (j < sg.width);
                     if (!real) continue;
                     float* prow = &P[tk.off + (int64_t)(sg.k_off + j) * L.N_phys];
                     for (int n = 0; n < L.N_param; ++n) {
@@ -600,7 +561,7 @@ extern "C" int wd_model_init(WdModel* m, uint64_t seed) {
     WD_CUDA(cudaSetDevice(m->device));
     int rc = init_sparse_tables(m, seed, 1);
     if (rc) return rc;
-    rc = init_dense(m, extra_of(m), seed);
+    rc = init_dense(m, seed);
     if (rc) return rc;
     WD_CUDA(cudaStreamSynchronize(m->stream));
     m->initialized = true;
@@ -608,18 +569,17 @@ extern "C" int wd_model_init(WdModel* m, uint64_t seed) {
 }
 
 // ---------------------------------------------------------------------------------------------- tensor IO
-static int resolve_dense(WdModel* m, WdModelExtra* x, int did, int sub, int* out) {
-    if (did < 0 || did >= (int)x->dense_index.size() || sub < 0 || sub > 3 || x->dense_index[did][sub] < 0) {
+static int resolve_dense(WdModel* m, int did, int sub, int* out) {
+    if (did < 0 || did >= (int)m->dense_index.size() || sub < 0 || sub > 3 || m->dense_index[did][sub] < 0) {
         set_error("no dense tensor (%d, %d)", did, sub);
         return WD_EINVAL;
     }
-    *out = x->dense_index[did][sub];
+    *out = m->dense_index[did][sub];
     return WD_OK;
 }
 
 extern "C" int64_t wd_tensor_size(WdModel* m, int kind, int index, int sub) {
     if (!m) return WD_EINVAL;
-    WdModelExtra* x = extra_of(m);
     if (kind == WD_T_WIDE_COL) {
         if (index < 0 || index >= m->n_columns) return WD_EINVAL;
         const ShardSpace& sw = m->shard.sp[1];
@@ -630,8 +590,8 @@ extern "C" int64_t wd_tensor_size(WdModel* m, int kind, int index, int sub) {
     if (kind == WD_T_EMB_TABLE) return (index >= 0 && index < (int)m->tables.size()) ? m->tables[index].arows * m->tables[index].dim_logical : WD_EINVAL;
     if (kind == WD_T_DENSE) {
         int di;
-        if (resolve_dense(m, x, index, sub, &di)) return WD_EINVAL;
-        Layer& L = m->towers[x->did_tower[index]].layers[x->did_layer[index]];
+        if (resolve_dense(m, index, sub, &di)) return WD_EINVAL;
+        Layer& L = m->towers[m->did_tower[index]].layers[m->did_layer[index]];
         return sub == WD_D_KERNEL ? (int64_t)L.K * L.N_param : (sub == WD_D_BIAS ? L.N_param : L.N);
     }
     return WD_EINVAL;
@@ -648,7 +608,6 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
     if (!m || !host) { set_error("null argument"); return WD_EINVAL; }
     WD_CUDA(cudaSetDevice(m->device));
     WD_CUDA(cudaStreamSynchronize(m->stream));
-    WdModelExtra* x = extra_of(m);
     int64_t want = wd_tensor_size(m, kind, index, sub);
     if (want < 0 || want != count) { set_error("tensor (%d,%d,%d): size %lld, caller passed %lld", kind, index, sub, (long long)want, (long long)count); return WD_EINVAL; }
     if (slot < 0 || slot > 2) { set_error("slot out of range"); return WD_EINVAL; }
@@ -687,10 +646,10 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         return WD_OK;
     }
     int di;
-    int rc = resolve_dense(m, x, index, sub, &di);
+    int rc = resolve_dense(m, index, sub, &di);
     if (rc) return rc;
     const DenseTensor& t = m->dense[di];
-    Layer& L = m->towers[x->did_tower[index]].layers[x->did_layer[index]];
+    Layer& L = m->towers[m->did_tower[index]].layers[m->did_layer[index]];
     std::vector<float> phys(t.count, 0.f);
     float* h = (float*)host;
     if (!to_device || slot > 0) {
@@ -702,7 +661,7 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         for (int s = 0; s < L.n_in_segs; ++s) {
             const Seg& sg = L.segs[s];
             for (int j = 0; j < sg.width_phys; ++j) {
-                bool real = sg.src < 0 ? (x->x0_real[j] != 0) : (j < sg.width);
+                bool real = sg.src < 0 ? (m->x0_real[j] != 0) : (j < sg.width);
                 if (!real) continue;
                 for (int n = 0; n < L.N_param; ++n) {
                     float& pv = phys[(int64_t)(sg.k_off + j) * L.N_phys + n];
@@ -746,14 +705,9 @@ static void timer_begin(WdModel* m) {
     mark(m, "start");
 }
 
-// make batch slot `s` current (allocating its buffers on first use); slot 0 aliases the model's own buffers
+// allocates the buffers of batch slots up to `s` on first use
 static int ensure_slot(WdModel* m, int s) {
     if (s < 0 || s >= 64) { set_error("batch slot %d out of range [0, 64)", s); return WD_EINVAL; }
-    if (m->slots.empty()) {
-        BatchSlot b0;
-        b0.off = m->d_cat_offsets; b0.keys = m->d_cat_keys; b0.dense = m->d_dense; b0.label = m->d_label; b0.weight = m->d_weight;
-        m->slots.push_back(b0);
-    }
     while ((int)m->slots.size() <= s) {
         BatchSlot b;
         int rc;
@@ -767,31 +721,47 @@ static int ensure_slot(WdModel* m, int s) {
     }
     return WD_OK;
 }
+// make batch slot `s` current (allocating its buffers on first use)
 static int select_slot(WdModel* m, int s) {
     int rc = ensure_slot(m, s);
     if (rc) return rc;
     BatchSlot& b = m->slots[s];
     m->cur_slot = s;
-    m->d_cat_offsets = b.off; m->d_cat_keys = b.keys; m->d_dense = b.dense; m->d_label = b.label; m->d_weight = b.weight;
-    if (b.filled) { m->dbatch = b.view; m->batch_has_label = b.has_label; }
+    if (b.filled) m->dbatch = b.view;
     if (b.up_pending) {                                     // a prefetch refilled this slot on the upload stream
         WD_CUDA(cudaStreamWaitEvent(m->stream, b.ev_up, 0));
         b.up_pending = false;
     }
     return WD_OK;
 }
+// the prologue of the entry points that run on a slot: makes `slot` current, refuses a slot never filled and, when the caller
+// needs labels (`needs_labels` names what it does with them), a batch without
+static int use_slot(WdModel* m, int slot, const char* needs_labels) {
+    int rc = select_slot(m, slot);
+    if (rc) return rc;
+    if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
+    if (needs_labels && !m->dbatch.label) { set_error("%s needs labels", needs_labels); return WD_EINVAL; }
+    return WD_OK;
+}
+// slot `s` now holds batch `view`; `pending`: its copies were issued on the upload stream, which the next step on it waits for
+static void fill_slot(WdModel* m, int s, const DevBatch& view, bool pending) {
+    BatchSlot& sl = m->slots[s];
+    sl.view = view;
+    sl.filled = true;
+    if (pending) sl.up_pending = true;
+    if (s == m->cur_slot) m->dbatch = view;
+}
 // the model stream has consumed the current slot up to here (a later prefetch into it must wait for this point)
 static int mark_slot_used(WdModel* m) {
-    if (m->slots.empty()) return WD_OK;
     BatchSlot& b = m->slots[m->cur_slot];
-    if (!b.ev_used) WD_CUDA(cudaEventCreateWithFlags(&b.ev_used, cudaEventDisableTiming));
+    if (!b.ev_used) WD_CUDA(new_event(m, &b.ev_used, cudaEventDisableTiming));
     WD_CUDA(cudaEventRecord(b.ev_used, m->stream));
     b.used_recorded = true;
     return WD_OK;
 }
 
 // copies a host batch into the buffers of slot `sl` on stream `st`; fills the device view of the batch
-static int upload_into(WdModel* m, BatchSlot& sl, const WdBatch* b, cudaStream_t st, DevBatch* view, bool* has_label) {
+static int upload_into(WdModel* m, BatchSlot& sl, const WdBatch* b, cudaStream_t st, DevBatch* view) {
     if (!b || b->batch_size <= 0 || b->batch_size > m->max_batch) { set_error("batch_size %d outside (0, %d]", b ? b->batch_size : -1, m->max_batch); return WD_EINVAL; }
     const int B = b->batch_size, F = m->n_cat_fields, Nd = m->n_dense_fields;
     int64_t nnz = b->cat_offsets ? b->nnz : (int64_t)B * F;
@@ -809,14 +779,14 @@ static int upload_into(WdModel* m, BatchSlot& sl, const WdBatch* b, cudaStream_t
     view->dense = sl.dense;
     view->label = b->label ? sl.label : nullptr;
     view->weight = b->weight ? sl.weight : nullptr;
-    *has_label = b->label != nullptr;
     return WD_OK;
 }
 
 static int upload_current(WdModel* m, const WdBatch* b) {
-    BatchSlot& sl = m->slots[m->cur_slot];
-    int rc = upload_into(m, sl, b, m->stream, &m->dbatch, &m->batch_has_label);
+    DevBatch view{};
+    int rc = upload_into(m, m->slots[m->cur_slot], b, m->stream, &view);
     if (rc) return rc;
+    fill_slot(m, m->cur_slot, view, false);
     mark(m, "h2d");
     return WD_OK;
 }
@@ -829,14 +799,12 @@ extern "C" int wd_batch_prefetch_slot(WdModel* m, int slot, const WdBatch* b) {
     if (rc) return rc;
     if ((rc = ensure_slot(m, slot))) return rc;
     BatchSlot& sl = m->slots[slot];
-    if (!sl.ev_up) WD_CUDA(cudaEventCreateWithFlags(&sl.ev_up, cudaEventDisableTiming));
+    if (!sl.ev_up) WD_CUDA(new_event(m, &sl.ev_up, cudaEventDisableTiming));
     if (sl.used_recorded) WD_CUDA(cudaStreamWaitEvent(m->stream_up, sl.ev_used, 0));
     DevBatch view{};
-    bool has_label = false;
-    if ((rc = upload_into(m, sl, b, m->stream_up, &view, &has_label))) return rc;
+    if ((rc = upload_into(m, sl, b, m->stream_up, &view))) return rc;
     WD_CUDA(cudaEventRecord(sl.ev_up, m->stream_up));
-    sl.view = view; sl.has_label = has_label; sl.filled = true; sl.up_pending = true;
-    if (slot == m->cur_slot) { m->dbatch = view; m->batch_has_label = has_label; }
+    fill_slot(m, slot, view, true);
     return WD_OK;
 }
 
@@ -849,12 +817,11 @@ extern "C" int wd_tsv_parse_slot(WdModel* m, int slot, const WdTsvSpec* sp, cons
     if (!sp || !text || !starts || n_lines < 0 || text_len < 0) { set_error("wd_tsv_parse_slot: bad arguments"); return WD_EINVAL; }
     if ((rc = ensure_slot(m, slot))) return rc;
     BatchSlot& sl = m->slots[slot];
-    if (!sl.ev_up) WD_CUDA(cudaEventCreateWithFlags(&sl.ev_up, cudaEventDisableTiming));
+    if (!sl.ev_up) WD_CUDA(new_event(m, &sl.ev_up, cudaEventDisableTiming));
     if (sl.used_recorded) WD_CUDA(cudaStreamWaitEvent(m->stream_up, sl.ev_used, 0));
     int status = 0;
     if ((rc = tsv_parse_device(m, sp, text, text_len, starts, n_lines, sl.off, sl.keys, sl.dense, sl.label, sl.weight, m->stream_up, &status))) return rc;
     DevBatch view{};
-    bool has_label = false;
     if (status == 0) {
         view.B = n_lines;
         view.cat_offsets = m->n_cat_fields > 0 ? sl.off : nullptr;
@@ -862,18 +829,16 @@ extern "C" int wd_tsv_parse_slot(WdModel* m, int slot, const WdTsvSpec* sp, cons
         view.dense = sl.dense;
         view.label = sp->has_label ? sl.label : nullptr;
         view.weight = (sp->use_weight && sp->has_label) ? sl.weight : nullptr;
-        has_label = sp->has_label != 0;
         m->tsv_device_batches++;
     } else {
         WdBatch hb{};
         if ((rc = tsv_parse_host(sp, text, starts, n_lines, &hb))) return rc;
-        if ((rc = upload_into(m, sl, &hb, m->stream_up, &view, &has_label))) return rc;
+        if ((rc = upload_into(m, sl, &hb, m->stream_up, &view))) return rc;
         m->tsv_host_batches++;
     }
     WD_CUDA(cudaEventRecord(sl.ev_up, m->stream_up));
     if (status != 0) WD_CUDA(cudaEventSynchronize(sl.ev_up));      // the host batch lives in per-thread buffers
-    sl.view = view; sl.has_label = has_label; sl.filled = true; sl.up_pending = true;
-    if (slot == m->cur_slot) { m->dbatch = view; m->batch_has_label = has_label; }
+    fill_slot(m, slot, view, true);
     return WD_OK;
 }
 
@@ -889,11 +854,7 @@ extern "C" int wd_batch_upload_slot(WdModel* m, int slot, const WdBatch* b) {
     int rc = check_ready(m);
     if (rc) return rc;
     if ((rc = select_slot(m, slot))) return rc;
-    if ((rc = upload_current(m, b))) return rc;
-    m->slots[slot].view = m->dbatch;
-    m->slots[slot].has_label = m->batch_has_label;
-    m->slots[slot].filled = true;
-    return WD_OK;
+    return upload_current(m, b);
 }
 extern "C" int wd_batch_upload(WdModel* m, const WdBatch* b) { return wd_batch_upload_slot(m, 0, b); }
 
@@ -924,7 +885,7 @@ static int finish_step(WdModel* m, float* loss_out, float* logits_out) {
         set_error("row-sharded exchange: a peer rank did not reach a barrier within 20 s (ranks out of step, or a rank failed)");
         return WD_ESTATE;
     }
-    if (loss_out) *loss_out = m->batch_has_label ? m->h_loss_pinned[0] : 0.f;
+    if (loss_out) *loss_out = m->dbatch.label ? m->h_loss_pinned[0] : 0.f;
     if (m->timer.enabled) {
         PhaseTimer& t = m->timer;
         for (int i = 1; i < t.n; ++i) cudaEventElapsedTime(&t.ms[i], t.ev[i - 1], t.ev[i]);
@@ -1169,16 +1130,29 @@ static int run_train_graphed(WdModel* m, StepGraph<Key>& g, const Key& key, F is
     return run_graphed(m, g, key, m->stream, issue, how);
 }
 
+// After a graph ran in place of the issuing code, the host state that code leaves behind (a replay runs none of it): a whole step
+// leaves nothing pending; the split step (`bwd`: its slot) leaves the lists' sums on the side streams the captured backward left
+// them on, and those streams continue behind the graph.
+static int after_graph(WdModel* m, GraphRun how, BatchSlot* bwd) {
+    if (how == GraphRun::eager) return WD_OK;
+    if (bwd && how == GraphRun::captured)
+        for (int w = 0; w < 2; ++w) bwd->bwd_side_active[w] = m->side_active[w];
+    if (bwd) WD_CUDA(cudaEventRecord(m->ev_bwd_done, m->stream));
+    for (int w = 0; w < 2; ++w) {
+        m->side_pending[w] = false;
+        m->side_active[w] = bwd && bwd->bwd_side_active[w];
+        if (m->side_active[w]) WD_CUDA(cudaStreamWaitEvent(m->sstream[w], m->ev_bwd_done, 0));
+    }
+    m->grads_pending = bwd != nullptr;
+    return WD_OK;
+}
+
 // One whole train step on the current slot (three streams, ~55 kernels, no host sync), graphed per slot.
 static int train_current(WdModel* m, float* loss_out) {
-    if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     GraphRun how;
     int rc = run_train_graphed(m, m->slots[m->cur_slot].train, m->dbatch, [&](bool) { return train_eager(m); }, &how);
     if (rc) return rc;
-    if (how != GraphRun::eager) {                           // a graphed step ends as an eager one does: nothing left pending
-        m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
-        m->grads_pending = false;
-    }
+    if ((rc = after_graph(m, how, nullptr))) return rc;
     if ((rc = mark_slot_used(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);
     return WD_OK;
@@ -1187,8 +1161,7 @@ static int train_current(WdModel* m, float* loss_out) {
 extern "C" int wd_train_step_slot(WdModel* m, int slot, float* loss_out) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if ((rc = select_slot(m, slot))) return rc;
-    if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
+    if ((rc = use_slot(m, slot, "training"))) return rc;
     timer_begin(m);
     return train_current(m, loss_out);
 }
@@ -1200,7 +1173,7 @@ extern "C" int wd_train_step(WdModel* m, const WdBatch* b, float* loss_out) {
     if ((rc = select_slot(m, 0))) return rc;
     timer_begin(m);
     if ((rc = upload_current(m, b))) return rc;
-    m->slots[0].view = m->dbatch; m->slots[0].has_label = m->batch_has_label; m->slots[0].filled = true;
+    if ((rc = use_slot(m, 0, "training"))) return rc;
     float dummy;
     return train_current(m, loss_out ? loss_out : &dummy);
 }
@@ -1220,7 +1193,6 @@ extern "C" int wd_forward(WdModel* m, const WdBatch* b, float* logits_out, float
     if ((rc = select_slot(m, 0))) return rc;
     timer_begin(m);
     if ((rc = upload_current(m, b))) return rc;
-    m->slots[0].view = m->dbatch; m->slots[0].has_label = m->batch_has_label; m->slots[0].filled = true;
     if ((rc = forward_core(m, false))) return rc;
     return finish_step(m, loss_out, logits_out);
 }
@@ -1254,25 +1226,13 @@ static int refuse_split_step_with_cache(WdModel* m) {
 extern "C" int wd_step_backward_slot(WdModel* m, int slot, float* loss_out) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if ((rc = select_slot(m, slot))) return rc;
-    if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
-    if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
+    if ((rc = use_slot(m, slot, "training"))) return rc;
     if ((rc = refuse_split_step_with_cache(m))) return rc;
     timer_begin(m);
     BatchSlot& sl = m->slots[slot];
     GraphRun how;
     if ((rc = run_train_graphed(m, sl.bwd, m->dbatch, [&](bool capturing) { return backward_eager(m, capturing); }, &how))) return rc;
-    if (how == GraphRun::captured)
-        for (int w = 0; w < 2; ++w) sl.bwd_side_active[w] = m->side_active[w];
-    if (how != GraphRun::eager) {
-        WD_CUDA(cudaEventRecord(m->ev_bwd_done, m->stream));
-        for (int w = 0; w < 2; ++w) {
-            m->side_pending[w] = false;
-            m->side_active[w] = sl.bwd_side_active[w];
-            if (m->side_active[w]) WD_CUDA(cudaStreamWaitEvent(m->sstream[w], m->ev_bwd_done, 0));
-        }
-        m->grads_pending = true;
-    }
+    if ((rc = after_graph(m, how, &sl))) return rc;
     if ((rc = mark_slot_used(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);
     return WD_OK;
@@ -1292,7 +1252,7 @@ extern "C" int wd_step_backward(WdModel* m, const WdBatch* b, float* loss_out) {
     if ((rc = refuse_split_step_with_cache(m))) return rc;
     if (b && (rc = wd_batch_upload(m, b))) return rc;
     timer_begin(m);
-    if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
+    if (!m->dbatch.label) { set_error("training needs labels"); return WD_EINVAL; }
     if ((rc = forward_core(m, true))) return rc;
     if ((rc = backward_core(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);
@@ -1354,22 +1314,19 @@ extern "C" int wd_sparse_set_sorted(WdModel* m, int which, const void* rows_dev,
 }
 
 // ------------------------------------------------------------------------------------- row-sharded tables
-static int shard_ready(WdModel* m, int slot) {
+static int shard_ready(WdModel* m, int slot, const char* needs_labels) {
     int rc = check_ready(m);
     if (rc) return rc;
     if (m->shard.world <= 1) { set_error("model has no row-sharded tables (shard_world <= 1)"); return WD_ESTATE; }
     if (!m->shard.connected) { set_error("row-sharded model is not connected to its peers (wd_shard_connect_ipc / wd_shard_connect_local)"); return WD_ESTATE; }
-    if ((rc = select_slot(m, slot))) return rc;
-    if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
-    return WD_OK;
+    return use_slot(m, slot, needs_labels);
 }
 
 // Segment `phase` of the rank-step (ranks driven by ONE process: the caller runs segment k on every rank, then wd_shard_local_sync).
 extern "C" int wd_shard_phase(WdModel* m, int slot, int phase, int train) {
-    int rc = shard_ready(m, slot);
+    int rc = shard_ready(m, slot, train ? "training" : nullptr);
     if (rc) return rc;
     if (m->shard.ipc) { set_error("wd_shard_phase is for ranks of one process; multi-process ranks call wd_shard_train_step_slot"); return WD_ESTATE; }
-    if (train && !m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     if (phase < 0 || phase > 4) { set_error("wd_shard_phase: phase %d outside [0, 4]", phase); return WD_EINVAL; }
     if (phase == 0) timer_begin(m);
     if ((rc = shard_step(m, train != 0, phase))) return rc;
@@ -1387,17 +1344,13 @@ extern "C" int wd_shard_finish(WdModel* m, float* loss_out, float* logits_out) {
 // optimizers, with flag barriers in peer memory between the segments.  Every rank must call it once per step (it is a collective).
 // Graphed per batch slot, barrier kernels included.
 extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
-    int rc = shard_ready(m, slot);
+    int rc = shard_ready(m, slot, "training");
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_train_step_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase)"); return WD_ESTATE; }
-    if (!m->batch_has_label) { set_error("training needs labels"); return WD_EINVAL; }
     timer_begin(m);
     GraphRun how;
     if ((rc = run_train_graphed(m, m->slots[slot].shard, m->dbatch, [&](bool) { return shard_step(m, true, kAllSegments); }, &how))) return rc;
-    if (how == GraphRun::captured) {
-        m->side_pending[0] = m->side_pending[1] = m->side_active[0] = m->side_active[1] = false;
-        m->grads_pending = false;
-    }
+    if ((rc = after_graph(m, how, nullptr))) return rc;
     if ((rc = mark_slot_used(m))) return rc;
     if (loss_out) return finish_step(m, loss_out, nullptr);
     return WD_OK;
@@ -1405,7 +1358,7 @@ extern "C" int wd_shard_train_step_slot(WdModel* m, int slot, float* loss_out) {
 
 // Forward only on a sharded model (collective, multi-process ranks): logits of this rank's batch shard.
 extern "C" int wd_shard_forward_slot(WdModel* m, int slot, float* logits_out, float* loss_out) {
-    int rc = shard_ready(m, slot);
+    int rc = shard_ready(m, slot, nullptr);
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_forward_slot needs wd_shard_connect_ipc"); return WD_ESTATE; }
     if ((rc = shard_step(m, false, kAllSegments))) return rc;
@@ -1418,7 +1371,7 @@ namespace wd { int shard_metrics_reduce(WdModel* m); }
 
 static int check_eval_rows(WdModel* m, int32_t n_valid) {
     if (n_valid < 0 || n_valid > m->dbatch.B) { set_error("n_valid %d outside [0, batch size %d]", n_valid, m->dbatch.B); return WD_EINVAL; }
-    if (n_valid > 0 && !m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
+    if (n_valid > 0 && !m->dbatch.label) { set_error("evaluation needs labels"); return WD_EINVAL; }
     return WD_OK;
 }
 
@@ -1426,7 +1379,7 @@ static int check_eval_rows(WdModel* m, int32_t n_valid) {
 // device.  A rank without rows left enters with any one-row batch and n_valid = 0: its forward still serves its peers.  Graphed per
 // batch slot and n_valid.
 extern "C" int wd_shard_eval_accumulate_slot(WdModel* m, int slot, int32_t n_valid) {
-    int rc = shard_ready(m, slot);
+    int rc = shard_ready(m, slot, nullptr);
     if (rc) return rc;
     if (!m->shard.ipc) { set_error("wd_shard_eval_accumulate_slot needs wd_shard_connect_ipc (ranks of one process use wd_shard_phase + wd_shard_eval_accumulate_phase)"); return WD_ESTATE; }
     if ((rc = check_eval_rows(m, n_valid))) return rc;
@@ -1441,7 +1394,7 @@ extern "C" int wd_shard_eval_accumulate_slot(WdModel* m, int slot, int32_t n_val
 // Ranks of one process: after segments 0..2 of wd_shard_phase(train = 0) on every rank, the metrics of the first n_valid rows of
 // this rank's logits.
 extern "C" int wd_shard_eval_accumulate_phase(WdModel* m, int32_t n_valid) {
-    int rc = shard_ready(m, m->cur_slot);
+    int rc = shard_ready(m, m->cur_slot, nullptr);
     if (rc) return rc;
     if (m->shard.ipc) { set_error("wd_shard_eval_accumulate_phase is for ranks of one process; multi-process ranks call wd_shard_eval_accumulate_slot"); return WD_ESTATE; }
     if ((rc = check_eval_rows(m, n_valid))) return rc;
@@ -1472,7 +1425,7 @@ extern "C" int wd_eval_reset(WdModel* m) {
 extern "C" int wd_eval_accumulate(WdModel* m, const WdBatch* b) {
     int rc = wd_batch_upload(m, b);
     if (rc) return rc;
-    if (!m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
+    if (!m->dbatch.label) { set_error("evaluation needs labels"); return WD_EINVAL; }
     if ((rc = forward_core(m, false))) return rc;
     if ((rc = metrics_accumulate(m, m->dbatch.B))) return rc;
     return finish_step(m, nullptr, nullptr);
@@ -1480,9 +1433,7 @@ extern "C" int wd_eval_accumulate(WdModel* m, const WdBatch* b) {
 extern "C" int wd_eval_accumulate_slot(WdModel* m, int slot) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if ((rc = select_slot(m, slot))) return rc;
-    if (!m->slots[slot].filled) { set_error("batch slot %d was never uploaded", slot); return WD_ESTATE; }
-    if (!m->batch_has_label) { set_error("evaluation needs labels"); return WD_EINVAL; }
+    if ((rc = use_slot(m, slot, "evaluation"))) return rc;
     if ((rc = forward_core(m, false))) return rc;
     if ((rc = metrics_accumulate(m, m->dbatch.B))) return rc;
     if ((rc = mark_slot_used(m))) return rc;
@@ -1575,7 +1526,7 @@ extern "C" int64_t wd_launch_count(WdModel* m) { return m ? m->launches : 0; }
 extern "C" int wd_summary_segments(WdModel* m, int32_t* kind, int32_t* tower, int32_t* layer, int32_t cap) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if ((rc = summary_prepare(m, extra_of(m)->x0_real))) return rc;
+    if ((rc = summary_prepare(m, m->x0_real))) return rc;
     const SummaryState* S = m->summ;
     const int n = (int)S->h.size();
     for (int i = 0; i < n && i < cap; ++i) {
@@ -1588,7 +1539,7 @@ extern "C" int wd_summary_segments(WdModel* m, int32_t* kind, int32_t* tower, in
 extern "C" int wd_summary_arm(WdModel* m) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if ((rc = summary_prepare(m, extra_of(m)->x0_real))) return rc;
+    if ((rc = summary_prepare(m, m->x0_real))) return rc;
     m->summary_armed = true;
     return WD_OK;
 }

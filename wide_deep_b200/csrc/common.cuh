@@ -234,7 +234,7 @@ struct BatchSlot {           // one device-resident batch (ring used by benchmar
     uint64_t* keys = nullptr;
     float *dense = nullptr, *label = nullptr, *weight = nullptr;
     DevBatch view{};
-    bool has_label = false, filled = false;
+    bool filled = false;
     // asynchronous refill (wd_batch_prefetch_slot): copies run on the upload stream between these two events
     cudaEvent_t ev_up = nullptr;             // recorded on the upload stream after the slot's copies
     cudaEvent_t ev_used = nullptr;           // recorded on the model stream after the last step that read the slot
@@ -340,6 +340,8 @@ struct SummaryState {
 
 struct TsvDev;                                 // device TSV parser: spec copy and scratch (tsv.cu)
 
+struct DevAlloc { void* p; int64_t bytes; };   // one cudaMalloc of the model (dev_alloc / dev_free)
+
 }  // namespace wd
 
 struct WdModel {
@@ -388,7 +390,11 @@ struct WdModel {
     int32_t* d_nubig[2] = {nullptr, nullptr};   // unique rows below small_base (what stays in the list)
     wd::ShardState shard;                    // row-sharded tables (world == 1: unused)
     wd::DevPlan dplan{};
-    std::vector<void*> allocs;               // everything cudaMalloc'ed (freed in destroy)
+    // what the model owns on the device, released by wd_model_destroy: streams and events (new_stream / new_event), and
+    // everything cudaMalloc'ed (dev_alloc; bytes_allocated is their sum)
+    std::vector<cudaStream_t> streams;
+    std::vector<cudaEvent_t> events;
+    std::vector<wd::DevAlloc> allocs;
     int64_t bytes_allocated = 0;
     // ---- host-placed embedding tables (host_tables.cu)
     std::vector<void*> host_allocs;          // cudaHostAlloc'ed table records (freed in destroy)
@@ -406,13 +412,9 @@ struct WdModel {
     int32_t *d_num_field = nullptr, *d_num_norm_kind = nullptr, *d_num_x0_off = nullptr;
     float *d_num_a = nullptr, *d_num_b = nullptr;
 
-    // ---- batch buffers
-    int32_t* d_cat_offsets = nullptr;
-    uint64_t* d_cat_keys = nullptr;
+    // ---- the batch of the current slot (slots, cur_slot)
     int64_t keys_cap = 0;
-    float *d_dense = nullptr, *d_label = nullptr, *d_weight = nullptr;
     wd::DevBatch dbatch{};
-    bool batch_has_label = false;
 
     // ---- column ids (CSR over (row, column)) and per-entry arrays
     int32_t* d_col_offs = nullptr;           // [max_batch * n_columns + 1]
@@ -504,7 +506,7 @@ struct WdModel {
     bool graphs_enabled = true;              // WD_NO_GRAPH=1 disables step graphs
     int cur_layer = 0;                       // layer being launched (names the profiling marks)
     wd::PhaseTimer timer;
-    std::vector<wd::BatchSlot> slots;        // slot 0 aliases the d_cat_* buffers above
+    std::vector<wd::BatchSlot> slots;        // batch slots, allocated up to the highest one used (slot 0 by wd_model_create)
     wd::TsvDev* tsv = nullptr;               // device TSV parser (wd_tsv_parse_slot), created on first use
     int64_t tsv_device_batches = 0, tsv_host_batches = 0;   // batches wd_tsv_parse_slot parsed on the device / on the host
     bool initialized = false;
@@ -512,6 +514,12 @@ struct WdModel {
     // layer summaries (summary.cu): the next train step takes the statistics (wd_summary_arm); they await wd_summary_read
     wd::SummaryState* summ = nullptr;
     bool summary_armed = false, summary_ready = false;
+
+    // ---- host-only plan bookkeeping (tensor IO, initialisation, summaries)
+    std::vector<uint8_t> x0_real;            // [d0_phys] 1 where a physical deep-input column is a real feature
+    int d0_logical = 0;
+    std::vector<std::vector<int>> dense_index;   // [tower-layer id][sub] -> index into dense, -1
+    std::vector<int> did_tower, did_layer;
 };
 
 namespace wd {
@@ -587,10 +595,32 @@ int dev_alloc(WdModel* m, T** p, int64_t count, bool zero = true) {
         e = cudaMemsetAsync(q, 0, (size_t)count * sizeof(T), m->stream);
         if (e != cudaSuccess) { set_error("cudaMemset failed: %s", cudaGetErrorString(e)); return WD_ECUDA; }
     }
-    m->allocs.push_back(q);
+    m->allocs.push_back({q, count * (int64_t)sizeof(T)});
     m->bytes_allocated += count * (int64_t)sizeof(T);
     *p = (T*)q;
     return WD_OK;
+}
+// frees an allocation of dev_alloc before the model dies, and takes its bytes off bytes_allocated
+inline int dev_free(WdModel* m, void* p) {
+    for (size_t i = 0; i < m->allocs.size(); ++i) {
+        if (m->allocs[i].p != p) continue;
+        WD_CUDA(cudaFree(p));
+        m->bytes_allocated -= m->allocs[i].bytes;
+        m->allocs.erase(m->allocs.begin() + i);
+        break;
+    }
+    return WD_OK;
+}
+// a stream / an event the model owns (wd_model_destroy synchronises and destroys it)
+inline cudaError_t new_stream(WdModel* m, cudaStream_t* s) {
+    const cudaError_t e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+    if (e == cudaSuccess) m->streams.push_back(*s);
+    return e;
+}
+inline cudaError_t new_event(WdModel* m, cudaEvent_t* ev, unsigned flags) {
+    const cudaError_t e = cudaEventCreateWithFlags(ev, flags);
+    if (e == cudaSuccess) m->events.push_back(*ev);
+    return e;
 }
 // copies src[0 .. n) to the device array *dst, allocated here while *dst is null; an existing array is overwritten in place (a
 // second upload of the same descriptor allocates nothing)

@@ -487,14 +487,9 @@ static int cache_enable(WdModel* m, HostCache& c, int64_t bytes, int S, int64_t 
     }
     // the staging buffer grows to [C slots | rows overflow rows]: the old one is freed and every descriptor re-pointed
     WD_CUDA(cudaStreamSynchronize(m->stream));
-    auto it = std::find(m->allocs.begin(), m->allocs.end(), (void*)*stage);
-    if (it != m->allocs.end()) {
-        WD_CUDA(cudaFree(*stage));
-        m->allocs.erase(it);
-        m->bytes_allocated -= rows * slot_bytes;
-    }
-    *stage = nullptr;
     int rc;
+    if ((rc = dev_free(m, *stage))) return rc;
+    *stage = nullptr;
     if ((rc = dev_alloc(m, stage, (C + rows) * S, false))) return rc;
     if ((rc = dev_alloc(m, &c.d_tag, C, false))) return rc;
     WD_CUDA(cudaMemsetAsync(c.d_tag, 0xFF, C * 4, m->stream));         // kInvalidRow

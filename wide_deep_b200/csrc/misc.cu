@@ -122,7 +122,7 @@ int metrics_setup() {
 }
 
 int metrics_accumulate(WdModel* m, int rows) {
-    metrics_kernel<<<grid_for(rows, 256, kNumSms), 256, 0, m->stream>>>(rows, m->d_logits, m->d_label, m->dbatch.weight, m->d_metrics);
+    metrics_kernel<<<grid_for(rows, 256, kNumSms), 256, 0, m->stream>>>(rows, m->d_logits, m->dbatch.label, m->dbatch.weight, m->d_metrics);
     m->launches++;
     m->eval_batches++;
     WD_CUDA(cudaGetLastError());

@@ -866,7 +866,7 @@ int loss_forward(WdModel* m, bool need_grad) {
         in.tower_logit[t] = tw.logit;
     }
     const int blocks = grid_for((int64_t)B * 8, 256, 512);               // eight lanes per example (loss_part holds 512 block partials)
-    logits_head_kernel<<<blocks, 256, 0, m->stream>>>(in, B, m->use_wide ? m->d_wide_logit : nullptr, m->batch_has_label ? m->d_label : nullptr,
+    logits_head_kernel<<<blocks, 256, 0, m->stream>>>(in, B, m->use_wide ? m->d_wide_logit : nullptr, m->dbatch.label,
                                                      m->dbatch.weight, m->d_logits, need_grad ? m->d_dlogit : nullptr, m->d_loss_part,
                                                      m->d_head_counter, m->d_loss);
     m->launches++;

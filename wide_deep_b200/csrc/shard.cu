@@ -468,13 +468,7 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     S.off_gred = take(std::max<int64_t>(S.ar_count, 4) * 4);
     S.off_metrics = take(kMetricsDoubles * 8);
     S.seg_bytes = off;
-    void* seg = nullptr;
-    cudaError_t e = cudaMalloc(&seg, (size_t)S.seg_bytes);
-    if (e != cudaSuccess) { set_error("cudaMalloc of the %lld-byte exchange segment failed: %s", (long long)S.seg_bytes, cudaGetErrorString(e)); return WD_ENOMEM; }
-    m->allocs.push_back(seg);
-    m->bytes_allocated += S.seg_bytes;
-    WD_CUDA(cudaMemsetAsync(seg, 0, (size_t)S.seg_bytes, m->stream));
-    S.seg = (uint8_t*)seg;
+    if ((rc = dev_alloc(m, &S.seg, S.seg_bytes))) return rc;
     m->d_dX0 = reinterpret_cast<float*>(S.seg + S.sp[0].off_grad);
     m->d_dlogit = reinterpret_cast<float*>(S.seg + S.sp[1].off_grad);
     m->d_G = reinterpret_cast<float*>(S.seg + S.off_G);
@@ -486,12 +480,8 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     if (getenv("WD_SHARD_TRACE") && (rc = dev_alloc(m, &S.d_trace, 2 * kBarriers))) return rc;
     if ((rc = dev_alloc(m, &S.d_peer_G, kMaxRanks))) return rc;
     if ((rc = dev_alloc(m, &S.d_peer_gred, kMaxRanks))) return rc;
-    WD_CUDA(cudaEventCreateWithFlags(&S.ev_a, cudaEventDisableTiming));
-    WD_CUDA(cudaEventCreateWithFlags(&S.ev_ids2, cudaEventDisableTiming));
-    WD_CUDA(cudaEventCreateWithFlags(&S.ev_routed1, cudaEventDisableTiming));
-    WD_CUDA(cudaEventCreateWithFlags(&S.ev_a2, cudaEventDisableTiming));
-    WD_CUDA(cudaEventCreateWithFlags(&S.ev_aux_done, cudaEventDisableTiming));
-    WD_CUDA(cudaStreamCreateWithFlags(&S.aux, cudaStreamNonBlocking));
+    for (cudaEvent_t* ev : {&S.ev_a, &S.ev_ids2, &S.ev_routed1, &S.ev_a2, &S.ev_aux_done}) WD_CUDA(new_event(m, ev, cudaEventDisableTiming));
+    WD_CUDA(new_stream(m, &S.aux));
     return WD_OK;
 }
 
@@ -864,6 +854,8 @@ extern "C" int wd_shard_ipc_handle(WdModel* m, void* handle_out64) {
     return WD_OK;
 }
 
+// Maps every peer's exchange segment into this process.  wd_model_destroy closes these mappings and frees this rank's segment,
+// which its peers write into: ranks should destroy their models only after their last collective call.
 extern "C" int wd_shard_connect_ipc(WdModel* m, const void* handles, int32_t n_ranks) {
     if (!m || !handles) { set_error("null argument"); return WD_EINVAL; }
     ShardState& S = m->shard;
