@@ -327,6 +327,9 @@ int64_t wd_launch_count(WdModel *m);
  * covered by the wgmma kernel.  0 for every plan the library builds itself (all widths are padded to whole k-blocks); the
  * tests assert 0 so a silent downgrade cannot hide. */
 int64_t wd_gemm_fallback_count(WdModel *m);
+/* Step graphs since creation: out[0] = captures, out[1] = replays (launches of a graph captured by an earlier call).  A capture
+ * that fails leaves the model eager for good without an error, so tests that mean to run a graph read these. */
+int wd_graph_stats(WdModel *m, int64_t *out, int32_t n);
 /* Per-phase device timings of the last synchronised step in milliseconds (CUDA events recorded on the model
  * stream between the stages, enabled by wd_set_profile).  Returns the number of phases n and fills
  * ms_out[0..min(n,cap)): [0] = whole step, [i] = the phase ending at mark wd_timing_name(m, i). */

@@ -1,7 +1,9 @@
 """Sparse gradient sums and row updates (csrc/sparse.cu, shard.cu, sparse_dev.cuh) held bit for bit.
 
-The other bitwise tests compare two models that run the same sparse kernels (host against HBM tables, host against HBM shards),
-so a rounding change shared by both would pass them.  These cases hold the losses and every trained tensor and optimizer slot
+Whether the updates are right is tests/test_gpu_optimizer_parity.py's question: it holds every element of every update kernel to a
+float64 reference under a derived bound.  These digests catch a change, not an error.  The other bitwise tests compare two models
+that run the same sparse kernels (host against HBM tables, host against HBM shards), so a rounding change shared by both would
+pass them.  These cases hold the losses and every trained tensor and optimizer slot
 after four train steps to SHA-256 digests recorded on an H100 80GB HBM3, per rank for the sharded runs.  Every case has rows
 touched more than kChunk = 16 times in a step, so both the direct sums and the chunked hot-row combine run:
 

@@ -88,6 +88,7 @@ SYMBOLS = {
     "wd_debug_hidden": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, _vp, _i64]),
     "wd_launch_count": (_i64, [_vp]),
     "wd_gemm_fallback_count": (_i64, [_vp]),
+    "wd_graph_stats": (ctypes.c_int, [_vp, ctypes.POINTER(_i64), _i32]),
     "wd_last_timings": (ctypes.c_int, [_vp, _vp, ctypes.c_int]),
     "wd_timing_name": (ctypes.c_char_p, [_vp, ctypes.c_int]),
     "wd_batch_upload_slot": (ctypes.c_int, [_vp, ctypes.c_int, _vp]),

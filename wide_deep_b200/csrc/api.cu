@@ -1086,6 +1086,7 @@ static int run_graphed(WdModel* m, StepGraph<Key>& g, const Key& key, cudaStream
     if (!m->graphs_enabled || m->timer.enabled) return issue(false);
     if (g.exec && g.key == key) {
         *how = GraphRun::replayed;
+        m->graph_replays++;
     } else if (g.eager < 2) {
         const int rc = issue(false);
         if (rc == WD_OK) g.eager++;
@@ -1112,6 +1113,7 @@ static int run_graphed(WdModel* m, StepGraph<Key>& g, const Key& key, cudaStream
         g.launches = m->launches - l0;                      // counted again on every launch of the graph
         m->launches = l0;
         *how = GraphRun::captured;
+        m->graph_captures++;
     }
     WD_CUDA(cudaGraphLaunch(g.exec, st));
     m->launches += g.launches;
@@ -1544,6 +1546,12 @@ extern "C" int wd_summary_arm(WdModel* m) {
     return WD_OK;
 }
 extern "C" int64_t wd_gemm_fallback_count(WdModel* m) { return m ? m->gemm_fallbacks : 0; }
+extern "C" int wd_graph_stats(WdModel* m, int64_t* out, int32_t n) {
+    if (!m || !out || n < 2) { wd::set_error("wd_graph_stats: bad arguments"); return WD_EINVAL; }
+    out[0] = m->graph_captures;
+    out[1] = m->graph_replays;
+    return WD_OK;
+}
 extern "C" int wd_last_timings(WdModel* m, float* ms_out, int cap) {
     if (!m) return WD_EINVAL;
     int n = m->timer.n_last;

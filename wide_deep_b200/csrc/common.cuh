@@ -497,6 +497,7 @@ struct WdModel {
     int64_t eval_batches = 0;
 
     int64_t launches = 0;
+    int64_t graph_captures = 0, graph_replays = 0;   // step graphs captured / replayed (wd_graph_stats)
     float dropout_rate = 0.f;               // dnn_dropout: tf.layers.dropout after every hidden layer's activation, train steps only
     unsigned long long dropout_seed = 0;
     unsigned int* d_step = nullptr;         // device: train steps completed (dropout counter; advances at the end of every step)

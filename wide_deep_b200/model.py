@@ -290,6 +290,12 @@ class WideDeepModel(object):
         """Tensor-core-engine GEMMs that ran on the FFMA kernel instead (must stay 0)."""
         return int(self._lib.wd_gemm_fallback_count(self._h))
 
+    def graph_stats(self):
+        """dict(captures, replays) of the model's step graphs since creation (a failed capture leaves the model eager, silently)."""
+        out = (ctypes.c_int64 * 2)()
+        check(self._lib.wd_graph_stats(self._h, out, 2))
+        return dict(captures=int(out[0]), replays=int(out[1]))
+
     def set_profile(self, on=True):
         check(self._lib.wd_set_profile(self._h, 1 if on else 0))
 
