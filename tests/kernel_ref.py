@@ -291,13 +291,11 @@ class StepRef(object):
         return out
 
     # ---- backward
-    def gradients(self):
-        """-> (ref, M, R, C) dicts by tensor name: float64 gradients of every parameter the step touches, their magnitudes, the
-        root-sum-squares of their last reduction (None where not a reduction) and the criterion-1 constant."""
-        ref, M, R, Cd = {}, {}, {}, {}
+    def head(self):
+        """-> (logit, Mlogit, Rlogit2, Khead, wide): float64 logits from the GPU's last inputs, the same sum on absolute values, the
+        sum of squared products, the longest fp32 accumulation of the head (wide ids + logits-layer inputs) and, per wide column,
+        (column, example of each id, id)."""
         plan, B = self.plan, self.B
-        w_abs = np.abs(self.weight)
-        # logits from the GPU's last inputs (the head is an fp32 FFMA kernel: its error enters dlogit through sigmoid' <= 1/4)
         logit, Mlogit, Rlogit2, Khead = np.zeros(B), np.zeros(B), np.zeros(B), 1
         wide = []
         if plan.use_wide:
@@ -321,6 +319,16 @@ class StepRef(object):
             Mlogit += (np.abs(inp) @ np.abs(W) + np.abs(b))[:, 0]
             Rlogit2 += ((inp * inp) @ (W * W))[:, 0]
             Khead += inp.shape[1]
+        return logit, Mlogit, Rlogit2, Khead, wide
+
+    def gradients(self):
+        """-> (ref, M, R, C) dicts by tensor name: float64 gradients of every parameter the step touches, their magnitudes, the
+        root-sum-squares of their last reduction (None where not a reduction) and the criterion-1 constant."""
+        ref, M, R, Cd = {}, {}, {}, {}
+        plan, B = self.plan, self.B
+        w_abs = np.abs(self.weight)
+        # logits from the GPU's last inputs (the head is an fp32 FFMA kernel: its error enters dlogit through sigmoid' <= 1/4)
+        logit, Mlogit, Rlogit2, Khead, wide = self.head()
         sig = 1.0 / (1.0 + np.exp(-logit))
         dlogit = (sig - self.label) * self.weight
         Rd = sig * (1 - sig) * w_abs * np.sqrt(Rlogit2)          # (the head's products, through sigmoid')
