@@ -30,15 +30,9 @@ int refresh_weight_copies(WdModel* m);
 int wide_bias_grad(WdModel* m);
 int metrics_setup();
 int merge_sparse(WdModel* m, int which, const void* rows, const void* grads, int64_t n);
-int shard_build(WdModel* m, const WdPlanDesc* d);
 int shard_step(WdModel* m, bool train, int seg);
 
 static int pad_to(int n, int k) { return (n + k - 1) / k * k; }
-static int bits_for(int64_t n) {
-    int b = 1;
-    while ((1ll << b) < n) ++b;
-    return b;
-}
 
 // sources of each layer input, in concat order (reference dnn.py:92-193); -1 = deep input x
 static std::vector<std::vector<int>> layer_sources(int mode, int L) {
@@ -200,14 +194,11 @@ static int build_model(const WdPlanDesc* d, WdModel* m) {
     if ((rc = dev_alloc(m, &m->d_e_id, m->max_nnz))) return rc;
     if ((rc = dev_alloc(m, &m->d_nnz, 4))) return rc;
     if ((rc = dev_alloc(m, &m->d_flags, 4))) return rc;
-    for (int k = 0; k < 4; ++k) if ((rc = dev_alloc(m, &m->d_sort_counter_s[k], 4))) return rc;
-    {
-        int64_t n = std::max<int64_t>(Bm * std::max(C, 1) + 2, m->max_nnz + 2);
-        for (int k = 0; k < 4; ++k) {
-            int32_t* t;
-            if ((rc = dev_alloc(m, &t, n / 4096 + 8))) return rc;
-            m->d_scan_tmp_s[k] = t;
-        }
+    m->sort_hist_cap = 1024 * ((m->max_nnz + kSortTile - 1) / kSortTile + 1) + 4 * 1024 + 64;
+    for (SortScratch& sc : m->scratch) {
+        if ((rc = dev_alloc(m, &sc.counter, 4))) return rc;
+        if ((rc = dev_alloc(m, &sc.scan, std::max<int64_t>(Bm * std::max(C, 1) + 2, m->max_nnz + 2) / 4096 + 8))) return rc;
+        if ((rc = dev_alloc(m, &sc.hist, m->sort_hist_cap))) return rc;
     }
     if ((rc = dev_alloc(m, &m->d_logits, Bm))) return rc;
     if (G == 1 && (rc = dev_alloc(m, &m->d_dlogit, Bm))) return rc;
@@ -423,36 +414,13 @@ static int build_model(const WdPlanDesc* d, WdModel* m) {
         if ((rc = upload(m, &m->d_dense_desc, m->dense))) return rc;
     }
 
-    // ---- sparse backward scratch
-    m->sort_bits[0] = bits_for(std::max<int64_t>(m->emb_total_rows, 2));
-    m->sort_bits[1] = bits_for(std::max<int64_t>(m->wide_rows, 2));
-    if (m->sort_bits[0] > 30 || m->sort_bits[1] > 30) { set_error("more than 2^30 rows in one table space on one device"); return WD_EUNSUPPORTED; }
-    const int which_lo = (m->use_deep && !m->tables.empty()) ? 0 : 1, which_hi = m->use_wide ? 1 : 0;
-    for (int w = which_lo; w <= which_hi; ++w) {
-        if ((rc = dev_alloc(m, &m->d_sk[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_sv[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_sk2[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_sv2[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_urow[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_ustart[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_ugrad[w], (m->max_nnz + 8) * (w == 0 ? std::max(m->emb_max_dim, 4) : 1)))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nuniq[w], 4))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nubig[w], 4))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nvalid[w], 4))) return rc;
-        m->cpart_cap = 2 * (m->max_nnz / 16) + 64;        // kChunk = 16 (sparse.cu)
-        if ((rc = dev_alloc(m, &m->d_choff[w], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nchunks[w], 4))) return rc;
-        if ((rc = dev_alloc(m, &m->d_cpart[w], m->cpart_cap * (w == 0 ? std::max(m->emb_max_dim, 4) : 1)))) return rc;
-        m->sparse_cap[w] = m->max_nnz;
-    }
-    m->sort_hist_cap = 1024 * ((m->max_nnz + kSortTile - 1) / kSortTile + 1) + 4 * 1024 + 64;
-    for (int k = 0; k < 4; ++k) if ((rc = dev_alloc(m, &m->d_sort_hist_s[k], m->sort_hist_cap))) return rc;
-    if (m->use_deep) {
-        // Embedding tables come last, so an auto-placed table competes only with what is allocated after wd_model_create returns
-        // (and, in a row-sharded model, with what shard_build allocates right below).
-        if ((rc = place_tables(m, hbm_reserve_bytes(m) + (G > 1 ? shard_hbm_bytes(m, d) : 0)))) return rc;
-    }
+    // ---- sparse backward scratch: lists 0 (embedding rows) and 1 (wide rows); a row-sharded model's lists 2 - 5 in shard_build
+    if (std::max(m->emb_total_rows, m->wide_rows) > (1ll << 30)) { set_error("more than 2^30 rows in one table space on one device"); return WD_EUNSUPPORTED; }
+    if (m->use_deep && !m->tables.empty() && (rc = list_alloc(m, 0, m->emb_total_rows, m->emb_max_dim, false))) return rc;
+    if (m->use_wide && (rc = list_alloc(m, 1, m->wide_rows, 1, false))) return rc;
     if (G > 1 && (rc = shard_build(m, d))) return rc;
+    // Embedding tables come last, so an auto-placed table competes only with what is allocated after wd_model_create returns.
+    if (m->use_deep && (rc = place_tables(m, hbm_reserve_bytes(m)))) return rc;
     if ((rc = build_record_sets(m))) return rc;               // every table, staging buffer and shard row base is final now
     if (G > 1) {
         DevPlan& dp = m->dplan;
@@ -502,7 +470,8 @@ namespace wd {
 // HBM kept free for what is allocated after the embedding tables (see ensure_slot, place_tables and the step graphs): the auto
 // tables are placed with it held back, and wd_host_cache_enable refuses a cache that would eat into it.
 //   kReserveSlots batch slots beyond slot 0 (cat offsets, keys, dense, label, weight each; bench.py and the estimator use at most 10),
-//   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table) and the record sets
+//   the staging buffer + gather ids of the host tables (at most max_nnz records of the widest table), or a row-sharded model's
+//   owner staging buffer of its host shards (max_nnz + 1 records, inside the same bound), and the record sets
 //   (build_record_sets: a few hundred bytes per table, inside the kGraphReserve margin),
 //   kGraphReserve for the instantiated step graphs (one train and one backward graph per slot) and the runtime's growth.
 int64_t hbm_reserve_bytes(const WdModel* m) {
@@ -1274,18 +1243,19 @@ extern "C" void* wd_dense_grad_ptr(WdModel* m) { return m ? m->d_G : nullptr; }
 extern "C" int wd_sparse_grads(WdModel* m, int which, void** rows, void** grads, int64_t* n, int32_t* width, int64_t* capacity) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if (which < 0 || which > 1 || !m->d_urow[which]) { set_error("no sparse gradient list %d", which); return WD_EINVAL; }
+    if (which < 0 || which > 1 || !m->lists[which].urow) { set_error("no sparse gradient list %d", which); return WD_EINVAL; }
+    const RowList& l = m->lists[which];
     if (n) {                                   // the count needs a sync; pass n = NULL for the asynchronous fixed-size exchange
         int32_t nu = 0;
         WD_CUDA(cudaStreamSynchronize(m->stream));
         WD_CUDA(cudaStreamSynchronize(m->sstream[which]));
-        WD_CUDA(cudaMemcpy(&nu, m->d_nuniq[which], 4, cudaMemcpyDeviceToHost));
+        WD_CUDA(cudaMemcpy(&nu, l.nuniq, 4, cudaMemcpyDeviceToHost));
         *n = nu;
     }
-    if (rows) *rows = m->d_urow[which];
-    if (grads) *grads = m->d_ugrad[which];
-    if (width) *width = which == 0 ? m->emb_max_dim : 1;
-    if (capacity) *capacity = m->sparse_cap[which];
+    if (rows) *rows = l.urow;
+    if (grads) *grads = l.ugrad;
+    if (width) *width = l.width;
+    if (capacity) *capacity = m->max_nnz;
     return WD_OK;
 }
 
@@ -1293,7 +1263,7 @@ extern "C" int wd_sparse_grads(WdModel* m, int which, void** rows, void** grads,
 static int sparse_set_impl(WdModel* m, int which, const void* rows_dev, const void* grads_dev, int64_t n, int n_lists, int64_t list_len) {
     int rc = check_ready(m);
     if (rc) return rc;
-    if (which < 0 || which > 1 || !m->d_urow[which]) { set_error("no sparse gradient list %d", which); return WD_EINVAL; }
+    if (which < 0 || which > 1 || !m->lists[which].urow) { set_error("no sparse gradient list %d", which); return WD_EINVAL; }
     const bool side = m->side_active[which];
     auto merge = [&]() -> int {
         return n_lists > 0 ? merge_sparse_sorted(m, which, rows_dev, grads_dev, n_lists, list_len) : merge_sparse(m, which, rows_dev, grads_dev, n);

@@ -29,7 +29,7 @@ constexpr int kMaxSegs = 8;      // sources concatenated into one MLP layer inpu
 constexpr int kMaxTowers = 8;    // deep towers per model: the head kernel takes all of their logits layers as one parameter block
 constexpr int kNumSms = 132;     // SMs of an H100 SXM: the grid caps of the grid-stride kernels are sized by it
 constexpr int kMaxDims = 8;      // distinct embedding widths per model
-// sort / unique-row scratch sets ("lists"): 0 embedding rows and 1 wide rows of the replicated tables; row-sharded tables add
+// sparse row lists (RowList, WdModel::lists): 0 embedding rows and 1 wide rows of the replicated tables; row-sharded tables add
 // 2 / 3 = rows this rank OWNS that were touched by any rank this step (embedding / wide) and 4 / 5 = this rank's own ids
 // grouped by owner rank (routing; only the key / value ping-pong buffers exist)
 constexpr int kLists = 6;
@@ -135,6 +135,24 @@ struct HostCache {
     uint8_t* d_uflag = nullptr;              // [rows] kLoad / kVictimDirty (host_tables.cu)
     uint32_t *d_ck[2] = {}, *d_cv[2] = {};   // (set, u) pairs and their sort ping-pong buffers
 };
+
+// The sort and unique-row scratch of one set of touched rows (kLists), allocated by list_alloc; a routing list's non-key pointers stay null
+struct RowList {
+    uint32_t *keys = nullptr, *vals = nullptr;     // [max_nnz + 8] (row, occurrence) pairs; sorted pairs end here
+    uint32_t *keys2 = nullptr, *vals2 = nullptr;   // their ping-pong copies
+    uint32_t* urow = nullptr;                      // unique rows, ascending
+    int32_t* ustart = nullptr;                     // segment starts in the sorted list (+1 sentinel)
+    int32_t* choff = nullptr;                      // chunk offsets of hot rows (exclusive scan)
+    float* ugrad = nullptr;                        // [max_nnz + 8][width] summed gradient of each unique row
+    float* cpart = nullptr;                        // [chunk_cap(max_nnz)][width] chunk partial sums
+    // device scalars: unique rows, entries of a merged external list, hot-row chunks, and (lists 0 / 1) unique rows below
+    // small_base (what stays in the list)
+    int32_t *nuniq = nullptr, *nvalid = nullptr, *nchunks = nullptr, *nubig = nullptr;
+    int bits = 0, width = 0;                       // key bits of the row space (the invalid key 1 << bits sorts last); floats per ugrad row
+    bool fused = false;                            // this step's rows were updated by the list's gradient-sum / combine launches (sparse.cu)
+};
+// one stream's scan / sort scratch (on_stream): scan chunk sums, radix-sort histograms [sort_hist_cap], finished scan blocks
+struct SortScratch { int32_t *scan = nullptr, *hist = nullptr, *counter = nullptr; };
 
 struct DenseTensor {         // one trainable dense tensor inside the dense arena
     int64_t off;             // offset in arena (floats)
@@ -275,8 +293,8 @@ struct ShardSpace {           // one sharded table space on this rank: 0 = embed
     uint32_t* d_adam_touched = nullptr;   // Adam: [ceil(local_rows / 32)] bit r: local row r was updated this step (sparse_dev.cuh)
     // host-placed shards (embedding space): the owner stages the records of the step's unique owned host rows (list 2) in HBM,
     // record of unique row u at staging row u (set.rec.stage: 0 for an HBM slot), or at cache.d_uslot[u] with a cache
-    int stage_stride = 0;              // widest stride of the space's host slots; 0: every shard in HBM
-    float* d_stage = nullptr;          // [cache.slots + max_nnz + 1][stage_stride] owner staging buffer
+    int stage_stride = 0;              // widest stride of the space's host slots; 0: every shard in HBM (place_tables)
+    float* d_stage = nullptr;          // [cache.slots + max_nnz + 1][stage_stride] owner staging buffer (place_tables)
     HostCache cache;                   // wd_shard_cache_enable: HBM cache of this rank's host shard records
     float4* d_wide = nullptr;          // wide space: {w, n, z, -} per local row
     uint32_t* d_own = nullptr;         // [max_nnz] owner rank of entry j or kInvalidRow (not a sharded column)
@@ -370,7 +388,6 @@ struct WdModel {
     cudaEvent_t ev_ids = nullptr, ev_head = nullptr, ev_dx0 = nullptr, ev_bwd_done = nullptr, ev_wide_fwd = nullptr, ev_wgrad_rest = nullptr;
     bool sort_smem_opt_in = false;               // rs_scatter_kernel<RS_BIG_TILE, true> was granted its dynamic shared memory on this device
     bool crelu = false;                          // dnn_activation_function crelu: relu on mirrored kernels (mlp.cu crelu_fold / crelu_mirror)
-    bool list_apply_fused[2] = {false, false};   // this step's rows of the list were updated by its gradient-sum / combine launches (sparse.cu)
     bool record_wgrad_rest = false;           // mlp_backward: record ev_wgrad_rest before the first layer's weight gradient
     int dense_split_tensor = -1, dense_part = 0;   // dense_apply: see mlp.cu (single-GPU step, split dense optimizer)
     cudaEvent_t ev_grouped[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
@@ -387,7 +404,6 @@ struct WdModel {
     // Adam: bitmaps of the replicated record sets (0: embedding rows, emb_total_rows bits; 1: wide rows, wide_rows bits), bit r set
     // when row r was updated this step, cleared by the set's untouched pass (sparse_dev.cuh); null unless that optimizer is Adam
     uint32_t* d_adam_touched[2] = {nullptr, nullptr};
-    int32_t* d_nubig[2] = {nullptr, nullptr};   // unique rows below small_base (what stays in the list)
     wd::ShardState shard;                    // row-sharded tables (world == 1: unused)
     wd::DevPlan dplan{};
     // what the model owns on the device, released by wd_model_destroy: streams and events (new_stream / new_event), and
@@ -424,8 +440,9 @@ struct WdModel {
     int32_t* d_e_id = nullptr;               // [max_nnz] column-local id (debug / parity)
     int32_t* d_nnz = nullptr;                // device scalar: entries this step
     int32_t* d_flags = nullptr;              // device error flags [4]
-    void* d_scan_tmp_s[4] = {nullptr, nullptr, nullptr, nullptr};   // scan / sort scratch, one set per stream (0 main, 1 + list for the side streams, 3 aux)
+    wd::SortScratch scratch[4];              // scan / sort scratch, one set per stream (0 main, 1 + list for the side streams, 3 aux)
     int scratch_sel = 0;
+    int64_t sort_hist_cap = 0;
 
     // ---- wide part: record {w, n, z, 0} per row
     float4* d_wide = nullptr;
@@ -472,25 +489,7 @@ struct WdModel {
     float* d_bpow = nullptr;                 // Adam: {linear beta1^t, linear beta2^t, dnn beta1^t, dnn beta2^t}, multiplied in fp32 after every step (AdamOptimizer._finish)
     float* h_loss_pinned = nullptr;
 
-    // ---- sparse backward scratch (two sorts: 0 = embedding rows, 1 = wide rows)
-    uint32_t *d_sk[wd::kLists] = {}, *d_sv[wd::kLists] = {};     // ping-pong keys / values
-    uint32_t *d_sk2[wd::kLists] = {}, *d_sv2[wd::kLists] = {};
-    int32_t* d_sort_hist_s[4] = {nullptr, nullptr, nullptr, nullptr};
-    int64_t sort_hist_cap = 0;
-    int32_t* d_sort_counter_s[4] = {nullptr, nullptr, nullptr, nullptr};
-    uint32_t* d_urow[wd::kLists] = {};   // unique rows
-    int32_t* d_ustart[wd::kLists] = {};  // segment starts in the sorted list (+1 sentinel)
-    float* d_ugrad[wd::kLists] = {};     // [cap, width]
-    int32_t* d_nuniq[wd::kLists] = {};   // device scalars
-    int32_t* d_nvalid[wd::kLists] = {};
-    int32_t* d_choff[wd::kLists] = {};   // chunk offsets of hot rows (exclusive scan)
-    int32_t* d_nchunks[wd::kLists] = {};
-    float* d_cpart[wd::kLists] = {};     // chunk partial sums
-    int64_t cpart_cap = 0;
-    int64_t sparse_cap[2] = {0, 0};
-    bool sparse_overridden[2] = {false, false};
-    int64_t sparse_override_n[2] = {0, 0};
-    int sort_bits[wd::kLists] = {};
+    wd::RowList lists[wd::kLists];           // sparse backward scratch: the sparse row lists
 
     // ---- eval metrics
     double* d_metrics = nullptr;             // accumulators
@@ -529,12 +528,12 @@ int ids_prepare(WdModel* m);                                     // ids.cu
 int sparse_forward(WdModel* m);                                  // sparse.cu: wide logit + embedding pooling + numerics
 int sparse_forward_wide(WdModel* m);                             //   the wide half alone
 int sparse_forward_emb(WdModel* m);                              //   the deep half alone
-int sparse_group(WdModel* m);                                    // sparse.cu: sort (row, occurrence) pairs, unique rows, chunks
 int sparse_reduce_emb(WdModel* m);                               // sparse.cu: per-row gradient sums (needs dX0)
 int sparse_reduce_wide(WdModel* m);                              // sparse.cu: per-row gradient sums (needs dlogit only)
-int sparse_apply(WdModel* m);                                    // sparse.cu: optimizer on the touched rows (both lists)
-int sparse_apply_which(WdModel* m, int which);                   // sparse.cu: one list (0 = embedding rows, 1 = wide rows)
-int sparse_group_which(WdModel* m, int which);                   // sparse.cu: grouping of one list
+int sparse_apply_which(WdModel* m, int which);                   // sparse.cu: optimizer on the touched rows of list 0 (embedding rows) / 1 (wide rows)
+int sparse_group_which(WdModel* m, int which);                   // sparse.cu: sort (row, occurrence) pairs of one list, unique rows, chunks
+// sparse.cu: list L over a space of `rows` rows, ugrad / cpart rows of `width` floats; sort_only: keys / values alone (routing)
+int list_alloc(WdModel* m, int L, int64_t rows, int width, bool sort_only);
 int merge_sparse_sorted(WdModel* m, int which, const void* rows, const void* grads, int n_lists, int64_t list_len);   // sparse.cu
 int small_scatter(WdModel* m, int which);                        // sparse.cu: small-table rows of list `which` -> dense block
 int small_apply(WdModel* m);                                     // sparse.cu: optimizer over the dense block (after its all-reduce)
@@ -547,13 +546,14 @@ int loss_forward(WdModel* m, bool need_grad);                    // mlp.cu: logi
 int model_init_params(WdModel* m, uint64_t seed);                // init.cu
 int step_tick(WdModel* m);                                       // misc.cu: train-step counter on the device (dropout)
 int adam_tick(WdModel* m);                                       // misc.cu: beta powers advance (after every optimizer of the step)
-int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host) and staging buffer
+int shard_build(WdModel* m, const WdPlanDesc* d);                // shard.cu: sharded spaces, their lists and the exchange segment
+int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host) and staging buffers
 int build_record_sets(WdModel* m);                               // host_tables.cu: upload the record sets and the gather view
 int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
 int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
 int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
 // host_tables.cu, over any record set `rr` whose staged tables (found by row base) keep the records of the unique rows of list L
-// (urow[L][0 .. *d_nuniq[L])) in rr.stage_base at stride S, behind cache `c` (c.slots = 0: none, staging row u):
+// (lists[L].urow[0 .. *lists[L].nuniq)) in rr.stage_base at stride S, behind cache `c` (c.slots = 0: none, staging row u):
 //   stage_in_rows    cache keys -> sort -> assign (train: the used slots turn dirty), then dirty victims home and the records
 //                    to load -> their staging rows
 //   write_back_rows  overflow staging rows -> host records (every staged row without a cache)
@@ -561,7 +561,6 @@ int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.
 struct CacheMarks { const char *sort, *assign, *in, *out; };
 int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, bool train, const CacheMarks& marks);
 int write_back_rows(WdModel* m, const HostCache& c, int L, const RowRecords& rr, int S, const CacheMarks& marks);
-int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d);  // shard.cu: HBM shard_build allocates (held back by auto placement)
 int64_t hbm_reserve_bytes(const WdModel* m);                     // api.cu: HBM the model keeps free for its later allocations
 // tsv.cu: device parse of n lines into the batch buffers on stream st, waiting for it; *status != 0: the buffers do not hold the
 // batch (parse it on the host)
@@ -647,7 +646,7 @@ inline void mark(WdModel* m, const char* name) {
     t.n++;
 }
 
-// run `fn` with the model's launches going to `stream` and its scan / sort scratch set `scratch_sel` (d_scan_tmp_s)
+// run `fn` with the model's launches going to `stream` and its scan / sort scratch set `scratch_sel` (WdModel::scratch)
 template <typename F>
 int on_stream(WdModel* m, cudaStream_t stream, int scratch_sel, F fn) {
     cudaStream_t main_stream = m->stream;

@@ -260,22 +260,23 @@ __global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32
 }
 
 int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, bool train, const CacheMarks& marks) {
+    const RowList& l = m->lists[L];
     const int64_t C = c.slots;
     if (C > 0) {
         const int g = grid_for(m->max_nnz, 256);
-        cache_keys_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[L], m->d_urow[L], rr, c.set_bits, c.d_ck[0], c.d_cv[0], c.d_now);
+        cache_keys_kernel<<<g, 256, 0, m->stream>>>(l.nuniq, l.urow, rr, c.set_bits, c.d_ck[0], c.d_cv[0], c.d_now);
         m->launches++;
-        int rc = radix_sort_pairs(m, &c.d_ck[0], &c.d_cv[0], &c.d_ck[1], &c.d_cv[1], c.set_bits + 1, m->d_nuniq[L]);
+        int rc = radix_sort_pairs(m, &c.d_ck[0], &c.d_cv[0], &c.d_ck[1], &c.d_cv[1], c.set_bits + 1, l.nuniq);
         if (rc) return rc;
         mark(m, marks.sort);
         const CacheMeta cm{c.d_tag, c.d_stamp, c.d_dirty, c.d_now, c.d_stats};
-        cache_assign_kernel<<<g, 256, 0, m->stream>>>(m->d_nuniq[L], c.d_ck[0], c.d_cv[0], m->d_urow[L], c.set_bits, C, train ? 1 : 0, cm,
+        cache_assign_kernel<<<g, 256, 0, m->stream>>>(l.nuniq, c.d_ck[0], c.d_cv[0], l.urow, c.set_bits, C, train ? 1 : 0, cm,
                                                      c.d_uslot, c.d_uvict, c.d_uflag);
         m->launches++;
         mark(m, marks.assign);
     }
     const StageMap sm{c.d_uvict, c.d_uflag, C};
-    host_rows_kernel<true><<<grid_for(m->max_nnz * (S / 4) / kInFlight, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_urow[L], rr, S, sm);
+    host_rows_kernel<true><<<grid_for(m->max_nnz * (S / 4) / kInFlight, 256), 256, 0, m->stream>>>(l.nuniq, l.urow, rr, S, sm);
     m->launches++;
     if (marks.in) mark(m, marks.in);
     WD_CUDA(cudaGetLastError());
@@ -283,8 +284,9 @@ int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, 
 }
 
 int write_back_rows(WdModel* m, const HostCache& c, int L, const RowRecords& rr, int S, const CacheMarks& marks) {
+    const RowList& l = m->lists[L];
     const StageMap sm{c.d_uvict, c.d_uflag, c.slots};
-    host_rows_kernel<false><<<grid_for(m->max_nnz * (S / 4) / kInFlight, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_urow[L], rr, S, sm);
+    host_rows_kernel<false><<<grid_for(m->max_nnz * (S / 4) / kInFlight, 256), 256, 0, m->stream>>>(l.nuniq, l.urow, rr, S, sm);
     m->launches++;
     mark(m, marks.out);
     WD_CUDA(cudaGetLastError());
@@ -297,7 +299,7 @@ int host_tables_stage_in(WdModel* m, bool train) {
     const RowRecords& rr = m->rtabs.rec;
     int rc = stage_in_rows(m, m->hcache, 0, rr, m->stage_stride, train, kHostMarks);
     if (rc) return rc;
-    host_remap_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->d_nuniq[0], m->d_urow[0], rr, m->d_g_emb);
+    host_remap_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nnz, m->d_e_emb, m->lists[0].nuniq, m->lists[0].urow, rr, m->d_g_emb);
     m->launches++;
     mark(m, "stage_in");
     WD_CUDA(cudaGetLastError());
@@ -329,8 +331,9 @@ int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
 
 // Allocates every embedding table — in HBM (WD_PLACE_HBM, and WD_PLACE_AUTO tables while they fit, largest first, with
 // `hbm_reserve` bytes held back for the buffers allocated after wd_model_create) or in mapped page-locked host memory — and the
-// staging buffer of the host tables.  The descriptors that point at them come later (build_record_sets).  A row-sharded model (shard_world > 1) may place only its sharded tables on the host: this rank's shard lives there
-// and is staged by its owner-side step (shard.cu), nothing here stages it.
+// staging buffer of the host tables.  The descriptors that point at them come later (build_record_sets).  A row-sharded model
+// (shard_world > 1) may place only its sharded tables on the host: this rank's shard lives there and its owner-side step
+// (shard.cu) stages it through the owner staging buffer allocated here.
 int place_tables(WdModel* m, int64_t hbm_reserve) {
     const int nt = (int)m->tables.size();
     auto host_ok = [&](const EmbTable& tb) {
@@ -378,9 +381,9 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
         void* dp = nullptr;
         WD_CUDA(cudaHostGetDevicePointer(&dp, p, 0));
         tb.data = (float*)dp;                // every element is written by init_sparse_tables before first use
-        if (tb.sharded) continue;            // staged by its owner (shard_build sizes that buffer)
-        m->n_host_tab++;
-        m->stage_stride = std::max(m->stage_stride, tb.stride);
+        if (!tb.sharded) m->n_host_tab++;    // (a host shard is staged by its owner, in the shard's own buffer)
+        int& stage_stride = tb.sharded ? m->shard.sp[0].stage_stride : m->stage_stride;
+        stage_stride = std::max(stage_stride, tb.stride);
     }
 
     if (m->n_host_tab > 0) {
@@ -389,6 +392,9 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
     } else {
         m->d_g_emb = m->d_e_emb;             // nothing on the host: the gather reads the step's own ids
     }
+    // host shards: the owner's staging rows of the step's unique owned rows (+1: see the serve in shard.cu)
+    ShardSpace& se = m->shard.sp[0];
+    if (se.stage_stride > 0 && (rc = dev_alloc(m, &se.d_stage, (m->max_nnz + 1) * (int64_t)se.stage_stride, false))) return rc;
     return WD_OK;
 }
 

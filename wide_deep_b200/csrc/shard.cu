@@ -351,12 +351,13 @@ __global__ void __launch_bounds__(256) shard_metrics_reduce_kernel(PeerMetrics p
 }
 
 // ================================================================================================== host side
-static int bits_for64(int64_t n) { int b = 1; while ((1ll << b) < n) ++b; return b; }
 static int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
-// Lays out the sharded spaces and the exchange segment.  Called at the end of build_model (world > 1): by then the dense arena
-// size is known; d_dX0 / d_dlogit / d_G live INSIDE the segment so that peers can read them.  The sharded tables' row bases move
-// into the shard's row space here; the shard set that describes them is uploaded after (build_record_sets).
+// Lays out the sharded spaces and the exchange segment and allocates their scratch and lists 2 - 5.  Called by build_model (world
+// > 1) before the embedding tables are placed, so that their auto placement finds this HBM taken: by then the dense arena size is
+// known; d_dX0 / d_dlogit / d_G live INSIDE the segment so that peers can read them.  The sharded tables' row bases move into the
+// shard's row space here; the shard set that describes them is uploaded after (build_record_sets).  The owner staging buffer of
+// host-placed shards is place_tables' (which shards go to the host is known there).
 int shard_build(WdModel* m, const WdPlanDesc* d) {
     ShardState& S = m->shard;
     S.world = d->shard_world; S.rank = d->shard_rank;
@@ -374,7 +375,6 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
             if (!tb.sharded) continue;
             col_slot[tb.col] = sp.n_slots++;
             base.push_back(rows);
-            if (tb.host) sp.stage_stride = std::max(sp.stage_stride, tb.stride);
             tb.row_base = rows;
             rows += (tb.rows + G - 1) / G;            // the SAME layout on every rank (a requester computes the owner's local row): ceil(rows / G) per table
             sp.width = std::max(sp.width, tb.dim);
@@ -384,8 +384,6 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
         sp.bags_per_row = sp.n_slots;
         sp.h_col_slot = col_slot; sp.h_slot_base = base;
         if (sp.on && (rc = upload(m, &sp.d_col_slot, col_slot))) return rc;
-        // host-placed shards: staging rows of the step's unique owned rows (+1: see the serve)
-        if (sp.stage_stride > 0 && (rc = dev_alloc(m, &sp.d_stage, (m->max_nnz + 1) * (int64_t)sp.stage_stride, false))) return rc;
     }
     // ---- wide space
     {
@@ -430,23 +428,8 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
         if ((rc = dev_alloc(m, &sp.d_rrow, m->max_nnz + 8))) return rc;
         if ((rc = dev_alloc(m, &sp.d_nrecv, 4))) return rc;
         if ((rc = dev_alloc(m, &sp.d_peers, kMaxRanks))) return rc;
-        const int Lo = 2 + s, Lr = 4 + s, w = s == 0 ? std::max(sp.width, 4) : 1;
-        for (int L : {Lo, Lr}) {
-            if ((rc = dev_alloc(m, &m->d_sk[L], m->max_nnz + 8))) return rc;
-            if ((rc = dev_alloc(m, &m->d_sv[L], m->max_nnz + 8))) return rc;
-            if ((rc = dev_alloc(m, &m->d_sk2[L], m->max_nnz + 8))) return rc;
-            if ((rc = dev_alloc(m, &m->d_sv2[L], m->max_nnz + 8))) return rc;
-        }
-        if ((rc = dev_alloc(m, &m->d_urow[Lo], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_ustart[Lo], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_ugrad[Lo], (m->max_nnz + 8) * w))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nuniq[Lo], 4))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nvalid[Lo], 4))) return rc;
-        if ((rc = dev_alloc(m, &m->d_choff[Lo], m->max_nnz + 8))) return rc;
-        if ((rc = dev_alloc(m, &m->d_nchunks[Lo], 4))) return rc;
-        if ((rc = dev_alloc(m, &m->d_cpart[Lo], m->cpart_cap * w))) return rc;
-        m->sort_bits[Lo] = bits_for64(std::max<int64_t>(sp.local_rows, 2));
-        m->sort_bits[Lr] = bits_for64(std::max(G, 2));
+        if ((rc = list_alloc(m, 2 + s, sp.local_rows, sp.width, false))) return rc;     // owned rows, in the shard's row space
+        if ((rc = list_alloc(m, 4 + s, G, 1, true))) return rc;                         // routing: keys are owner ranks
     }
     // ---- exchange segment layout (identical on every rank)
     int64_t off = 0;
@@ -483,36 +466,6 @@ int shard_build(WdModel* m, const WdPlanDesc* d) {
     for (cudaEvent_t* ev : {&S.ev_a, &S.ev_ids2, &S.ev_routed1, &S.ev_a2, &S.ev_aux_done}) WD_CUDA(new_event(m, ev, cudaEventDisableTiming));
     WD_CUDA(new_stream(m, &S.aux));
     return WD_OK;
-}
-
-// HBM that shard_build allocates after the embedding tables, for their auto placement to hold back: the wide shard, the per-space
-// scratch and sort lists 2 + s / 4 + s, the exchange segment, and 1 MB for descriptors, flags and alignment.  (The owner staging
-// buffer is covered by hbm_reserve_bytes, whose single-GPU staging buffer a sharded model never allocates.)
-int64_t shard_hbm_bytes(const WdModel* m, const WdPlanDesc* d) {
-    const int G = std::max(d->shard_world, 1);
-    const int64_t n = m->max_nnz + 8;
-    int emb_width = 0, n_slots = 0;
-    for (const EmbTable& tb : m->tables)
-        if (tb.sharded) { emb_width = std::max(emb_width, tb.dim); n_slots++; }
-    int64_t wide_rows = 0;
-    bool wide_on = false;
-    if (m->use_wide && d->col_wide_sharded)
-        for (int c = 0; c < m->n_columns; ++c)
-            if (d->col_wide_sharded[c]) { wide_on = true; wide_rows += (d->col_buckets[c] + G - 1) / G; }
-    int64_t bytes = (1 << 20) + wide_rows * 16;
-    for (int s = 0; s < 2; ++s) {
-        if (s == 0 ? n_slots == 0 : !wide_on) continue;
-        const int64_t width = s == 0 ? emb_width : 1, w = s == 0 ? std::max(emb_width, 4) : 1;
-        const int64_t nbags = (int64_t)m->max_batch * (s == 0 ? n_slots : 1);
-        bytes += 4 * (4 * n + nbags + 8)                              // own, lrow, rtag, rrow, bagmask
-                 + 4 * 8 * n                                          // keys / values (+ ping-pong) of lists 2 + s and 4 + s
-                 + 4 * (3 * n + n * w + m->cpart_cap * w)             // urow, ustart, choff, ugrad, cpart
-                 + (int64_t)G * m->max_nnz * 8                        // inbox
-                 + (int64_t)G * nbags * width * 4 + nbags * 4;        // recv, bagscale
-    }
-    const int64_t x0n = m->use_deep ? (int64_t)m->max_batch_pad * std::max(m->d0_phys, 1) : 4;
-    bytes += x0n * 4 + (int64_t)m->max_batch * 4 + 2 * align_up(m->dense_count + m->gs_count + 4, 4) * 4 + 2 * kMetricsDoubles * 8;
-    return bytes;
 }
 
 // peer segment bases known: fill the per-peer pointer tables
@@ -562,19 +515,20 @@ static int shard_route_send(WdModel* m, int s) {
     ShardState& S = m->shard;
     ShardSpace& sp = S.sp[s];
     if (!sp.on) return WD_OK;
-    const int G = S.world, L = 4 + s;
+    const int G = S.world;
+    RowList& l = m->lists[4 + s];
     int rc;
     WD_CUDA(cudaMemsetAsync(sp.d_bagmask, 0, (size_t)(m->dbatch.B * (int64_t)sp.bags_per_row) * 4, m->stream));
     // keys = owner (or "not sharded" = 1 << bits, sorts last), values = entry index; one stable radix pass
-    if ((rc = list_sort_by_key(m, L, m->d_nnz, sp.d_own))) return rc;
-    shard_starts_kernel<<<1, 32, 0, m->stream>>>(m->d_nnz, m->d_sk[L], G, sp.d_ostart);
+    if ((rc = list_sort_by_key(m, l, m->d_nnz, sp.d_own))) return rc;
+    shard_starts_kernel<<<1, 32, 0, m->stream>>>(m->d_nnz, l.keys, G, sp.d_ostart);
     float* bagscale = const_cast<float*>(sp.peers[S.rank].bagscale);
     const int g = grid_for(m->max_nnz, 256);
     if (s == 0)
-        shard_send_kernel<true><<<g, 256, 0, m->stream>>>(sp.d_ostart, m->d_sk[L], m->d_sv[L], sp.d_lrow, m->d_e_bc, m->d_col_offs, m->n_columns,
+        shard_send_kernel<true><<<g, 256, 0, m->stream>>>(sp.d_ostart, l.keys, l.vals, sp.d_lrow, m->d_e_bc, m->d_col_offs, m->n_columns,
             sp.n_slots, sp.d_col_slot, sp.d_peers, G, S.rank, sp.pair_cap, sp.d_bagmask, bagscale, m->d_flags);
     else
-        shard_send_kernel<false><<<g, 256, 0, m->stream>>>(sp.d_ostart, m->d_sk[L], m->d_sv[L], sp.d_lrow, m->d_e_bc, m->d_col_offs, m->n_columns,
+        shard_send_kernel<false><<<g, 256, 0, m->stream>>>(sp.d_ostart, l.keys, l.vals, sp.d_lrow, m->d_e_bc, m->d_col_offs, m->n_columns,
             sp.n_slots, sp.d_col_slot, sp.d_peers, G, S.rank, sp.pair_cap, sp.d_bagmask, bagscale, m->d_flags);
     m->launches += 2;
     WD_CUDA(cudaGetLastError());
@@ -601,7 +555,7 @@ static int shard_serve(WdModel* m, int s, bool train) {
     if (s == 0)
         shard_serve_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, S.rank, sp.pair_cap,
             sp.n_slots, sp.set.rec.row_base, sp.set.rec.data, sp.set.rec.dim, sp.set.rec.stride, sp.d_peers, sp.nbags_cap, sp.width,
-            sp.set.rec.stage, sp.d_stage, m->d_urow[2], m->d_nuniq[2], sp.cache.d_uslot);
+            sp.set.rec.stage, sp.d_stage, m->lists[2].urow, m->lists[2].nuniq, sp.cache.d_uslot);
     else
         shard_serve_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(me.inbox, me.inbox_cnt, S.world, S.rank, sp.pair_cap,
             sp.d_wide, sp.d_peers, sp.nbags_cap);
@@ -620,7 +574,7 @@ static int shard_owner_group(WdModel* m, int s) {
                                                                             sp.d_nrecv, m->max_nnz, m->d_flags);
     m->launches++;
     WD_CUDA(cudaGetLastError());
-    return list_group(m, 2 + s, sp.d_nrecv, sp.d_rrow);
+    return list_group(m, m->lists[2 + s], sp.d_nrecv, sp.d_rrow);
 }
 
 static int shard_combine(WdModel* m, int s) {
@@ -645,28 +599,30 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
     ShardSpace& sp = S.sp[s];
     if (!sp.on) return WD_OK;
     const int L = 2 + s;
+    const RowList& l = m->lists[L];
+    const int64_t ncap = m->max_nnz + chunk_cap(m->max_nnz);     // unique rows + hot-row chunks
     int rc;
     if (s == 0) {
-        const PeerEmb src{m->d_sv[L], sp.d_rtag, sp.d_peers, sp.n_slots, sp.set.rec.dim, sp.set.x0, m->d0_phys};
-        emb_grad_sum_kernel<PeerEmb, false><<<grid_for((m->max_nnz + m->cpart_cap) * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],
-            m->d_ustart[L], m->d_choff[L], src, m->d_ugrad[L], m->d_cpart[L], sp.width, RowApply{});
+        const PeerEmb src{l.vals, sp.d_rtag, sp.d_peers, sp.n_slots, sp.set.rec.dim, sp.set.x0, m->d0_phys};
+        emb_grad_sum_kernel<PeerEmb, false><<<grid_for(ncap * 8, 256), 256, 0, m->stream>>>(l.nuniq, l.nchunks, l.ustart, l.choff, src, l.ugrad,
+                                                                                            l.cpart, l.width, RowApply{});
         m->launches++;
-        if ((rc = list_chunk_combine(m, L, sp.width))) return rc;
+        if ((rc = list_chunk_combine(m, l))) return rc;
         const OptParams o = space_opt(m, 0, sp.d_adam_touched);
-        if ((rc = list_apply_emb(m, L, sp.width, sp.set.rec, o))) return rc;
+        if ((rc = list_apply_emb(m, l, sp.set.rec, o))) return rc;
         // Adam: the shard's rows no rank touched, after its touched ones (no host-placed shards with Adam: no staged records)
         if ((rc = adam_untouched_emb(m, sp.set, sp.local_rows, o))) return rc;
         // staged records home (overflow rows only with a cache), on this stream: it joins the main stream before the step ends, so
         // the next stage-in comes after
         if (staged(m, s) && (rc = write_back_rows(m, sp.cache, L, sp.set.rec, sp.stage_stride, kShardMarks))) return rc;
     } else {
-        const PeerWide src{m->d_sv[L], sp.d_rtag, sp.d_peers};
-        wide_grad_sum_kernel<PeerWide, false><<<grid_for(m->max_nnz + m->cpart_cap, 256), 256, 0, m->stream>>>(m->d_nuniq[L], m->d_nchunks[L],
-            m->d_ustart[L], m->d_choff[L], src, m->d_ugrad[L], m->d_cpart[L], RowApply{});
+        const PeerWide src{l.vals, sp.d_rtag, sp.d_peers};
+        wide_grad_sum_kernel<PeerWide, false><<<grid_for(ncap, 256), 256, 0, m->stream>>>(l.nuniq, l.nchunks, l.ustart, l.choff, src, l.ugrad, l.cpart,
+                                                                                          RowApply{});
         m->launches++;
-        if ((rc = list_chunk_combine(m, L, 1))) return rc;
+        if ((rc = list_chunk_combine(m, l))) return rc;
         const OptParams o = space_opt(m, 1, sp.d_adam_touched);
-        if ((rc = list_apply_wide(m, L, sp.d_wide, o))) return rc;
+        if ((rc = list_apply_wide(m, l, sp.d_wide, o))) return rc;
         if ((rc = adam_untouched_wide(m, sp.d_wide, sp.local_rows, o))) return rc;
     }
     WD_CUDA(cudaGetLastError());

@@ -105,9 +105,9 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_add_kernel(int32_t* data, i
 int exclusive_scan_i32(WdModel* m, int32_t* data, int64_t n, int32_t* total_out) {
     int nchunks = (int)((n + SCAN_CHUNK - 1) / SCAN_CHUNK);
     if (nchunks < 1) nchunks = 1;
-    int32_t* sums = (int32_t*)m->d_scan_tmp_s[m->scratch_sel];
-    scan_chunks_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(data, n, sums, m->d_sort_counter_s[m->scratch_sel]);
-    scan_add_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(data, n, sums, nchunks, total_out);
+    const SortScratch& sc = m->scratch[m->scratch_sel];
+    scan_chunks_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(data, n, sc.scan, sc.counter);
+    scan_add_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(data, n, sc.scan, nchunks, total_out);
     m->launches += 2;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -204,10 +204,10 @@ int seg_heads(WdModel* m, const int32_t* d_n, const uint32_t* keys, uint32_t inv
               int32_t* d_nuniq) {
     int nchunks = (int)((cap + SCAN_CHUNK - 1) / SCAN_CHUNK);
     if (nchunks < 1) nchunks = 1;
-    int32_t* sums = (int32_t*)m->d_scan_tmp_s[m->scratch_sel];
+    const SortScratch& sc = m->scratch[m->scratch_sel];
     const ScanGen g{d_n, keys, invalid, nullptr, nullptr, 0};
-    scan_gen_chunks_kernel<0><<<nchunks, SCAN_THREADS, 0, m->stream>>>(g, pos, cap, sums, m->d_sort_counter_s[m->scratch_sel]);
-    seg_add_compact_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(g, pos, sums, nchunks, ustart, urow, d_nuniq);
+    scan_gen_chunks_kernel<0><<<nchunks, SCAN_THREADS, 0, m->stream>>>(g, pos, cap, sc.scan, sc.counter);
+    seg_add_compact_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(g, pos, sc.scan, nchunks, ustart, urow, d_nuniq);
     m->launches += 2;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -217,10 +217,10 @@ int seg_heads(WdModel* m, const int32_t* d_n, const uint32_t* keys, uint32_t inv
 int chunk_offsets(WdModel* m, const int32_t* d_nuniq, const int32_t* ustart, uint32_t* urow, int32_t* choff, int64_t cap, int chunk, int32_t* d_nchunks) {
     int nchunks = (int)((cap + SCAN_CHUNK - 1) / SCAN_CHUNK);
     if (nchunks < 1) nchunks = 1;
-    int32_t* sums = (int32_t*)m->d_scan_tmp_s[m->scratch_sel];
+    const SortScratch& sc = m->scratch[m->scratch_sel];
     const ScanGen g{d_nuniq, nullptr, 0u, ustart, urow, chunk};
-    scan_gen_chunks_kernel<1><<<nchunks, SCAN_THREADS, 0, m->stream>>>(g, choff, cap, sums, m->d_sort_counter_s[m->scratch_sel]);
-    scan_add_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(choff, cap, sums, nchunks, d_nchunks);
+    scan_gen_chunks_kernel<1><<<nchunks, SCAN_THREADS, 0, m->stream>>>(g, choff, cap, sc.scan, sc.counter);
+    scan_add_kernel<<<nchunks, SCAN_THREADS, 0, m->stream>>>(choff, cap, sc.scan, nchunks, d_nchunks);
     m->launches += 2;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -435,7 +435,7 @@ int radix_sort_pairs(WdModel* m, uint32_t** keys, uint32_t** vals, uint32_t** ke
         set_error("radix sort histogram capacity too small");
         return WD_ESTATE;
     }
-    int32_t* hist = m->d_sort_hist_s[m->scratch_sel];
+    int32_t* hist = m->scratch[m->scratch_sel].hist;
     int32_t* gtot = hist + (int64_t)bins * ntiles_cap;                  // [passes][bins]
     for (int p = 0; p < passes; ++p) {
         int shift = p * per;

@@ -400,22 +400,46 @@ __global__ void __launch_bounds__(256) adam_untouched_wide_kernel(float4* __rest
 }
 
 
-// sort (row, occurrence) pairs by row and find the unique rows; e_row: per-occurrence row ids (kInvalidRow = skip)
-static int group_tail(WdModel* m, int which, const int32_t* d_n);
-static int group_rows(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row, const int32_t* val_src = nullptr) {
-    const uint32_t invalid = 1u << m->sort_bits[which];
-    int g = grid_for(m->max_nnz, 256);
-    sort_keys_kernel<<<g, 256, 0, m->stream>>>(d_n, e_row, invalid, m->d_sk[which], m->d_sv[which], val_src);
-    m->launches++;
-    int rc = radix_sort_pairs(m, &m->d_sk[which], &m->d_sv[which], &m->d_sk2[which], &m->d_sv2[which], m->sort_bits[which] + 1, d_n);
-    if (rc) return rc;
-    return group_tail(m, which, d_n);
+static int bits_for(int64_t n) {
+    int b = 1;
+    while ((1ll << b) < n) ++b;
+    return b;
 }
-// unique rows + segment starts of the sorted (row, occurrence) pairs in d_sk / d_sv
-static int group_tail(WdModel* m, int which, const int32_t* d_n) {
-    const uint32_t invalid = 1u << m->sort_bits[which];
-    int32_t* pos = (int32_t*)m->d_sk2[which];                 // ping-pong buffer is free after the sort
-    return seg_heads(m, d_n, m->d_sk[which], invalid, pos, m->max_nnz, m->d_ustart[which], m->d_urow[which], m->d_nuniq[which]);
+
+int list_alloc(WdModel* m, int L, int64_t rows, int width, bool sort_only) {
+    RowList& l = m->lists[L];
+    const int64_t n = m->max_nnz + 8;
+    l.bits = bits_for(rows);
+    l.width = width;
+    int rc;
+    for (uint32_t** p : {&l.keys, &l.vals, &l.keys2, &l.vals2})
+        if ((rc = dev_alloc(m, p, n))) return rc;
+    if (sort_only) return WD_OK;
+    if ((rc = dev_alloc(m, &l.urow, n))) return rc;
+    if ((rc = dev_alloc(m, &l.ustart, n))) return rc;
+    if ((rc = dev_alloc(m, &l.ugrad, n * width))) return rc;
+    if ((rc = dev_alloc(m, &l.nuniq, 4))) return rc;
+    if (L < 2 && (rc = dev_alloc(m, &l.nubig, 4))) return rc;     // (only the replicated lists hand rows to the small-table block)
+    if ((rc = dev_alloc(m, &l.nvalid, 4))) return rc;
+    if ((rc = dev_alloc(m, &l.choff, n))) return rc;
+    if ((rc = dev_alloc(m, &l.nchunks, 4))) return rc;
+    return dev_alloc(m, &l.cpart, chunk_cap(m->max_nnz) * width);
+}
+
+// sort (row, occurrence) pairs by row and find the unique rows; e_row: per-occurrence row ids (kInvalidRow = skip)
+static int group_tail(WdModel* m, RowList& l, const int32_t* d_n);
+static int group_rows(WdModel* m, RowList& l, const int32_t* d_n, const uint32_t* e_row, const int32_t* val_src = nullptr) {
+    int g = grid_for(m->max_nnz, 256);
+    sort_keys_kernel<<<g, 256, 0, m->stream>>>(d_n, e_row, 1u << l.bits, l.keys, l.vals, val_src);
+    m->launches++;
+    int rc = radix_sort_pairs(m, &l.keys, &l.vals, &l.keys2, &l.vals2, l.bits + 1, d_n);
+    if (rc) return rc;
+    return group_tail(m, l, d_n);
+}
+// unique rows + segment starts of the sorted (row, occurrence) pairs in keys / vals
+static int group_tail(WdModel* m, RowList& l, const int32_t* d_n) {
+    int32_t* pos = (int32_t*)l.keys2;                          // ping-pong buffer is free after the sort
+    return seg_heads(m, d_n, l.keys, 1u << l.bits, pos, m->max_nnz, l.ustart, l.urow, l.nuniq);
 }
 
 // out[u] = sum over the segment of in[sv[j]] (rows of `width` floats); one thread per (unique row, float4 chunk)
@@ -436,14 +460,14 @@ __global__ void set_count_kernel(int32_t* dst, int32_t v) { *dst = v; }
 // Replace the gradient list `which` by the row-wise sum of an external (rows, grads) list, e.g. the
 // all-gathered lists of every rank: keeps "sum duplicates, apply once" across data-parallel replicas.
 int merge_sparse(WdModel* m, int which, const void* rows, const void* grads, int64_t n) {
+    RowList& l = m->lists[which];
     if (n > m->max_nnz) { set_error("merged sparse list has %lld rows, capacity %lld", (long long)n, (long long)m->max_nnz); return WD_EINVAL; }
-    set_count_kernel<<<1, 1, 0, m->stream>>>(m->d_nvalid[which], (int32_t)n);     // (a kernel, not a memcpy: capturable into a graph)
+    set_count_kernel<<<1, 1, 0, m->stream>>>(l.nvalid, (int32_t)n);     // (a kernel, not a memcpy: capturable into a graph)
     m->launches++;
-    int rc = group_rows(m, which, m->d_nvalid[which], (const uint32_t*)rows);
+    int rc = group_rows(m, l, l.nvalid, (const uint32_t*)rows);
     if (rc) return rc;
-    const int width = which == 0 ? m->emb_max_dim : 1;
-    merged_sum_kernel<<<grid_for(std::max<int64_t>(n, 1) * width, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_ustart[which], m->d_sv[which],
-                                                                                           (const float*)grads, m->d_ugrad[which], width);
+    merged_sum_kernel<<<grid_for(std::max<int64_t>(n, 1) * l.width, 256), 256, 0, m->stream>>>(l.nuniq, l.ustart, l.vals, (const float*)grads,
+                                                                                              l.ugrad, l.width);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -479,18 +503,18 @@ __global__ void list_len_check_kernel(const int32_t* __restrict__ d_nuniq, int64
     if ((int64_t)*d_nuniq > list_len) atomicOr(flags, 8);
 }
 int merge_sparse_sorted(WdModel* m, int which, const void* rows, const void* grads, int n_lists, int64_t list_len) {
+    RowList& l = m->lists[which];
     const int64_t n = (int64_t)n_lists * list_len;
     if (n_lists < 1 || list_len < 1 || list_len > 0x7fffffff) { set_error("merge: bad list shape"); return WD_EINVAL; }
     if (n > m->max_nnz) { set_error("merged sparse list has %lld rows, capacity %lld", (long long)n, (long long)m->max_nnz); return WD_EINVAL; }
-    list_len_check_kernel<<<1, 1, 0, m->stream>>>(m->d_nuniq[which], list_len, m->d_flags);   // (d_nuniq still holds the local count)
+    list_len_check_kernel<<<1, 1, 0, m->stream>>>(l.nuniq, list_len, m->d_flags);   // (nuniq still holds the local count)
     m->launches++;
-    merge_rank_kernel<<<grid_for(n, 256), 256, 0, m->stream>>>((const uint32_t*)rows, n_lists, (int)list_len, m->d_sk[which], m->d_sv[which], m->d_nvalid[which]);
+    merge_rank_kernel<<<grid_for(n, 256), 256, 0, m->stream>>>((const uint32_t*)rows, n_lists, (int)list_len, l.keys, l.vals, l.nvalid);
     m->launches++;
-    int rc = group_tail(m, which, m->d_nvalid[which]);
+    int rc = group_tail(m, l, l.nvalid);
     if (rc) return rc;
-    const int width = which == 0 ? m->emb_max_dim : 1;
-    merged_sum_kernel<<<grid_for(std::max<int64_t>(n, 1) * width, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_ustart[which], m->d_sv[which],
-                                                                                           (const float*)grads, m->d_ugrad[which], width);
+    merged_sum_kernel<<<grid_for(std::max<int64_t>(n, 1) * l.width, 256), 256, 0, m->stream>>>(l.nuniq, l.ustart, l.vals, (const float*)grads,
+                                                                                              l.ugrad, l.width);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -502,54 +526,48 @@ int merge_sparse_sorted(WdModel* m, int which, const void* rows, const void* gra
 // concurrently with the towers' forward/backward.
 int sparse_group_which(WdModel* m, int which) {
     int rc;
-    const int g = grid_for(m->max_nnz, 256);
+    RowList& l = m->lists[which];
     const bool present = which == 0 ? (m->use_deep && !m->tables.empty()) : m->use_wide;
     if (present) {
-        if ((rc = group_rows(m, which, m->d_nnz, which == 0 ? m->d_e_emb : m->d_e_wide, m->d_e_bc))) return rc;     // values = cell indices
-        if ((rc = chunk_offsets(m, m->d_nuniq[which], m->d_ustart[which], m->d_urow[which], m->d_choff[which], m->max_nnz, kChunk, m->d_nchunks[which]))) return rc;
+        if ((rc = group_rows(m, l, m->d_nnz, which == 0 ? m->d_e_emb : m->d_e_wide, m->d_e_bc))) return rc;     // values = cell indices
+        if ((rc = chunk_offsets(m, l.nuniq, l.ustart, l.urow, l.choff, m->max_nnz, kChunk, l.nchunks))) return rc;
         mark(m, which == 0 ? "emb_group" : "wide_group");
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int sparse_group(WdModel* m) {
-    int rc = sparse_group_which(m, 0);
-    return rc ? rc : sparse_group_which(m, 1);
-}
 
 // Stage 2: per-row gradient sums; leaves (urow, ugrad, nuniq) ready for exchange / apply.
 // Single-GPU step (train_eager: nothing exchanges the sums between backward and optimizer) with a row-local optimizer (everything
 // but Adam, whose moments decay over whole tables): the rows are updated inside these two launches and sparse_apply_which has
-// nothing left to launch for the list (m->list_apply_fused).
+// nothing left to launch for the list (RowList::fused).
 static bool fuse_row_apply(const WdModel* m, const WdOptimizer& o) {
     return m->fuse_dense && o.kind != WD_OPT_ADAM && m->gs_count == 0;
 }
 int sparse_reduce_emb(WdModel* m) {
     const int g = grid_for(m->max_nnz, 256);
     if (m->use_deep && !m->tables.empty()) {
-        const int width = m->emb_max_dim, G4 = width >> 2;
-        const int ge = grid_for((m->max_nnz + m->cpart_cap) * 8, 256);
+        RowList& l = m->lists[0];
+        const int width = l.width, G4 = width >> 2;
+        const int ge = grid_for((m->max_nnz + chunk_cap(m->max_nnz)) * 8, 256);
         // the hot rows' update lives in the lane-group branch of chunk_combine_kernel: widths 4, 8, ..., 128
         const bool fused = fuse_row_apply(m, m->dnn_opt) && width >= 4 && (G4 & (G4 - 1)) == 0 && G4 <= 32;
         // the direct rows' records by table in plan order (a sum knows its table from the column), the hot rows' by table in row
         // order; host tables: the fused updates go to the staged records, host_tables_write_back copies them home after the list's apply
         const OptParams o = make_opt(m->dnn_opt);
-        const RowApply ra{m->d_urow[0], m->tabs.rec, nullptr, o};
-        const RowApply ha{m->d_urow[0], m->rtabs.rec, nullptr, o};
-        const LocalEmb src{m->d_sv[0], m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->tabs.rec.dim, m->tabs.x0, m->d_dX0, m->d0_phys};
+        const RowApply ra{l.urow, m->tabs.rec, nullptr, o};
+        const RowApply ha{l.urow, m->rtabs.rec, nullptr, o};
+        const LocalEmb src{l.vals, m->d_col_offs, m->n_columns, m->dplan.col_emb_table, m->tabs.rec.dim, m->tabs.x0, m->d_dX0, m->d0_phys};
         if (fused) {
-            emb_grad_sum_kernel<LocalEmb, true><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], src,
-                                                                          m->d_ugrad[0], m->d_cpart[0], width, ra);
-            chunk_combine_kernel<1><<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_choff[0], m->d_cpart[0], m->d_ugrad[0], width, ha);
+            emb_grad_sum_kernel<LocalEmb, true><<<ge, 256, 0, m->stream>>>(l.nuniq, l.nchunks, l.ustart, l.choff, src, l.ugrad, l.cpart, width, ra);
+            chunk_combine_kernel<1><<<g, 256, 0, m->stream>>>(l.nuniq, l.choff, l.cpart, l.ugrad, width, ha);
         } else {
-            emb_grad_sum_kernel<LocalEmb, false><<<ge, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_nchunks[0], m->d_ustart[0], m->d_choff[0], src,
-                                                                           m->d_ugrad[0], m->d_cpart[0], width, ra);
-            chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(m->d_nuniq[0], m->d_choff[0], m->d_cpart[0], m->d_ugrad[0], width, ha);
+            emb_grad_sum_kernel<LocalEmb, false><<<ge, 256, 0, m->stream>>>(l.nuniq, l.nchunks, l.ustart, l.choff, src, l.ugrad, l.cpart, width, ra);
+            chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(l.nuniq, l.choff, l.cpart, l.ugrad, width, ha);
         }
-        m->list_apply_fused[0] = fused;
+        l.fused = fused;
         m->launches += 2;
         mark(m, "emb_grad_sum");
-        m->sparse_overridden[0] = false;
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -558,23 +576,21 @@ int sparse_reduce_emb(WdModel* m) {
 int sparse_reduce_wide(WdModel* m) {
     const int g = grid_for(m->max_nnz, 256);
     if (m->use_wide) {
+        RowList& l = m->lists[1];
         const bool fused = fuse_row_apply(m, m->lin_opt);
-        const RowApply ra{m->d_urow[1], RowRecords{}, m->d_wide, make_opt(m->lin_opt)};
-        const LocalWide src{m->d_sv[1], m->n_columns, m->d_dlogit};
-        const int gw = grid_for(m->max_nnz + m->cpart_cap, 256);
+        const RowApply ra{l.urow, RowRecords{}, m->d_wide, make_opt(m->lin_opt)};
+        const LocalWide src{l.vals, m->n_columns, m->d_dlogit};
+        const int gw = grid_for(m->max_nnz + chunk_cap(m->max_nnz), 256);
         if (fused) {
-            wide_grad_sum_kernel<LocalWide, true><<<gw, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_nchunks[1], m->d_ustart[1], m->d_choff[1], src,
-                                                                            m->d_ugrad[1], m->d_cpart[1], ra);
-            chunk_combine_kernel<2><<<g, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_choff[1], m->d_cpart[1], m->d_ugrad[1], 1, ra);
+            wide_grad_sum_kernel<LocalWide, true><<<gw, 256, 0, m->stream>>>(l.nuniq, l.nchunks, l.ustart, l.choff, src, l.ugrad, l.cpart, ra);
+            chunk_combine_kernel<2><<<g, 256, 0, m->stream>>>(l.nuniq, l.choff, l.cpart, l.ugrad, 1, ra);
         } else {
-            wide_grad_sum_kernel<LocalWide, false><<<gw, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_nchunks[1], m->d_ustart[1], m->d_choff[1], src,
-                                                                             m->d_ugrad[1], m->d_cpart[1], ra);
-            chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(m->d_nuniq[1], m->d_choff[1], m->d_cpart[1], m->d_ugrad[1], 1, ra);
+            wide_grad_sum_kernel<LocalWide, false><<<gw, 256, 0, m->stream>>>(l.nuniq, l.nchunks, l.ustart, l.choff, src, l.ugrad, l.cpart, ra);
+            chunk_combine_kernel<0><<<g, 256, 0, m->stream>>>(l.nuniq, l.choff, l.cpart, l.ugrad, 1, ra);
         }
-        m->list_apply_fused[1] = fused;
+        l.fused = fused;
         m->launches += 2;
         mark(m, "wide_grad_sum");
-        m->sparse_overridden[1] = false;
     }
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -625,18 +641,19 @@ __global__ void copy_count_kernel(int32_t* dst, const int32_t* src) { *dst = *sr
 
 int small_scatter(WdModel* m, int which) {
     if (m->gs_count == 0) return WD_OK;
+    const RowList& l = m->lists[which];
     float* block = m->d_G + m->dense_count;
     if (which == 0) {
         if (m->n_small_tab == 0 || !(m->use_deep && !m->tables.empty())) return WD_OK;
-        small_scatter_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(m->d_nuniq[0], m->d_urow[0], m->d_ugrad[0], m->emb_max_dim,
+        small_scatter_emb_kernel<<<grid_for(m->max_nnz * 8, 256, kNumSms * 8), 256, 0, m->stream>>>(l.nuniq, l.urow, l.ugrad, l.width,
             (uint32_t)m->small_base[0], m->rtabs.rec.ntab, m->rtabs.rec.row_base, m->rtabs.rec.dim, m->rtabs.gs_off, block,
-            block + m->gs_touch_off[0], m->d_nubig[0]);
+            block + m->gs_touch_off[0], l.nubig);
     } else {
         if (!m->use_wide || m->small_base[1] >= m->wide_rows) return WD_OK;
-        small_scatter_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(m->d_nuniq[1], m->d_urow[1], m->d_ugrad[1],
-            (uint32_t)m->small_base[1], block + m->gs_emb_floats, block + m->gs_touch_off[1], m->d_nubig[1]);
+        small_scatter_wide_kernel<<<grid_for(m->max_nnz, 256, kNumSms * 8), 256, 0, m->stream>>>(l.nuniq, l.urow, l.ugrad,
+            (uint32_t)m->small_base[1], block + m->gs_emb_floats, block + m->gs_touch_off[1], l.nubig);
     }
-    copy_count_kernel<<<1, 1, 0, m->stream>>>(m->d_nuniq[which], m->d_nubig[which]);
+    copy_count_kernel<<<1, 1, 0, m->stream>>>(l.nuniq, l.nubig);
     m->launches += 2;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -705,9 +722,10 @@ static RowRecords in_place(RowRecords r) {
 
 int sparse_apply_which(WdModel* m, int which) {
     int rc;
-    // rows already updated by the gradient-sum / combine launches of this step (single-GPU step), unless a caller replaced the list since
-    const bool done = m->list_apply_fused[which] && !m->sparse_overridden[which];
-    m->list_apply_fused[which] = false;
+    RowList& l = m->lists[which];
+    // rows already updated by the gradient-sum / combine launches of this step (single-GPU step)
+    const bool done = l.fused;
+    l.fused = false;
     // the fused updates of host-table rows went to their staged copies: copy those home (the unfused kernels below update host
     // records in place, through their mapped pointers)
     if (done) return (which == 0 && m->n_host_tab > 0) ? host_tables_write_back(m) : WD_OK;
@@ -715,40 +733,40 @@ int sparse_apply_which(WdModel* m, int which) {
         set_error("embedding rows of a model with a host-table cache are only updated by the fused single-GPU step");
         return WD_EUNSUPPORTED;
     }
-    if (which == 0 && m->use_deep && !m->tables.empty() && (rc = list_apply_emb(m, 0, m->emb_max_dim, in_place(m->rtabs.rec), space_opt(m, 0, m->d_adam_touched[0]))))
+    if (which == 0 && m->use_deep && !m->tables.empty() && (rc = list_apply_emb(m, l, in_place(m->rtabs.rec), space_opt(m, 0, m->d_adam_touched[0]))))
         return rc;
-    if (which == 1 && m->use_wide && (rc = list_apply_wide(m, 1, m->d_wide, space_opt(m, 1, m->d_adam_touched[1])))) return rc;
+    if (which == 1 && m->use_wide && (rc = list_apply_wide(m, l, m->d_wide, space_opt(m, 1, m->d_adam_touched[1])))) return rc;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
 // ---- wrappers used by shard.cu (rows this rank owns in a row-sharded table space)
-// stable sort of (e_key[i], i) pairs, i < *d_n, by key; keys equal to kInvalidRow sort last; result in d_sk / d_sv of list `which`
-int list_sort_by_key(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_key) {
-    sort_keys_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(d_n, e_key, 1u << m->sort_bits[which], m->d_sk[which], m->d_sv[which], nullptr);
+// stable sort of (e_key[i], i) pairs, i < *d_n, by key; keys equal to kInvalidRow sort last; result in the list's keys / vals
+int list_sort_by_key(WdModel* m, RowList& l, const int32_t* d_n, const uint32_t* e_key) {
+    sort_keys_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(d_n, e_key, 1u << l.bits, l.keys, l.vals, nullptr);
     m->launches++;
-    return radix_sort_pairs(m, &m->d_sk[which], &m->d_sv[which], &m->d_sk2[which], &m->d_sv2[which], m->sort_bits[which] + 1, d_n);
+    return radix_sort_pairs(m, &l.keys, &l.vals, &l.keys2, &l.vals2, l.bits + 1, d_n);
 }
-int list_group(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row) {
-    int rc = group_rows(m, which, d_n, e_row);
+int list_group(WdModel* m, RowList& l, const int32_t* d_n, const uint32_t* e_row) {
+    int rc = group_rows(m, l, d_n, e_row);
     if (rc) return rc;
-    if ((rc = chunk_offsets(m, m->d_nuniq[which], m->d_ustart[which], m->d_urow[which], m->d_choff[which], m->max_nnz, kChunk, m->d_nchunks[which]))) return rc;
+    if ((rc = chunk_offsets(m, l.nuniq, l.ustart, l.urow, l.choff, m->max_nnz, kChunk, l.nchunks))) return rc;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int list_chunk_combine(WdModel* m, int which, int width) {
-    chunk_combine_kernel<0><<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_choff[which], m->d_cpart[which], m->d_ugrad[which], width, RowApply{});
+int list_chunk_combine(WdModel* m, const RowList& l) {
+    chunk_combine_kernel<0><<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(l.nuniq, l.choff, l.cpart, l.ugrad, l.width, RowApply{});
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const OptParams& o) {
-    emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], width, rec, o);
+int list_apply_emb(WdModel* m, const RowList& l, const RowRecords& rec, const OptParams& o) {
+    emb_apply_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(l.nuniq, l.urow, l.ugrad, l.width, rec, o);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
-int list_apply_wide(WdModel* m, int which, float4* wide, const OptParams& o) {
-    wide_apply_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(m->d_nuniq[which], m->d_urow[which], m->d_ugrad[which], wide, o);
+int list_apply_wide(WdModel* m, const RowList& l, float4* wide, const OptParams& o) {
+    wide_apply_kernel<<<grid_for(m->max_nnz, 256), 256, 0, m->stream>>>(l.nuniq, l.urow, l.ugrad, wide, o);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -773,11 +791,6 @@ int adam_untouched_replicated(WdModel* m) {
     if (m->use_deep && (rc = adam_untouched_emb(m, m->rtabs, m->emb_total_rows, space_opt(m, 0, m->d_adam_touched[0]))))
         return rc;
     return m->use_wide ? adam_untouched_wide(m, m->d_wide, m->wide_rows, space_opt(m, 1, m->d_adam_touched[1])) : WD_OK;
-}
-
-int sparse_apply(WdModel* m) {
-    int rc = sparse_apply_which(m, 0);
-    return rc ? rc : sparse_apply_which(m, 1);
 }
 
 }  // namespace wd

@@ -22,6 +22,8 @@ __device__ __forceinline__ float warp_sum(float v) {
 // Rows touched at most kChunk times are summed by one lane group directly.  Hotter rows (small tables, skewed ids) are split into
 // chunks of kChunk occurrences that are summed in parallel and then combined in chunk order (deterministic).
 constexpr int kChunk = 16;
+// rows of a list's chunk partials (RowList::cpart): a row of len > kChunk entries has ceil(len / kChunk) <= 2 len / kChunk chunks
+inline int64_t chunk_cap(int64_t max_nnz) { return 2 * (max_nnz / kChunk) + 64; }
 
 __device__ __forceinline__ int chunk_owner(const int32_t* __restrict__ choff, int nu, int c) {
     int lo = 0, hi = nu;                         // last u with choff[u] <= c
@@ -260,14 +262,14 @@ __global__ void wide_grad_sum_kernel(const int32_t* __restrict__ d_nuniq, const 
 }
 
 // ---- list machinery implemented in sparse.cu, used by shard.cu for the rows a rank owns
-// sort (row, occurrence) pairs of e_row[0 .. *d_n) by row, unique rows, segment starts, hot-row chunk layout -> list `which`
-int list_group(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_row);
-int list_sort_by_key(WdModel* m, int which, const int32_t* d_n, const uint32_t* e_key);
+// sort (row, occurrence) pairs of e_row[0 .. *d_n) by row, unique rows, segment starts, hot-row chunk layout -> list l
+int list_group(WdModel* m, RowList& l, const int32_t* d_n, const uint32_t* e_row);
+int list_sort_by_key(WdModel* m, RowList& l, const int32_t* d_n, const uint32_t* e_key);
 // ugrad[u] = fixed-order sum of the chunk partials of multi-chunk rows (after the two gradient-sum passes)
-int list_chunk_combine(WdModel* m, int which, int width);
-// optimizer over the unique rows of list `which`: embedding records as `rec` says (tables in row order) / one wide record array
-int list_apply_emb(WdModel* m, int which, int width, const RowRecords& rec, const OptParams& o);
-int list_apply_wide(WdModel* m, int which, float4* wide, const OptParams& o);
+int list_chunk_combine(WdModel* m, const RowList& l);
+// optimizer over the unique rows of list l: embedding records as `rec` says (tables in row order) / one wide record array
+int list_apply_emb(WdModel* m, const RowList& l, const RowRecords& rec, const OptParams& o);
+int list_apply_wide(WdModel* m, const RowList& l, float4* wide, const OptParams& o);
 // the optimizer of table space `space` (0 embedding rows: dnn_optimizer, 1 wide rows: linear_optimizer); Adam: with its beta powers
 // and the bitmap `touched` of the record set it updates
 OptParams space_opt(const WdModel* m, int space, uint32_t* touched);
