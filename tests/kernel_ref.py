@@ -228,6 +228,10 @@ class StepRef(object):
         pos = np.concatenate([np.arange(a, b) for a, b in zip(s, e)]) if len(s) else np.zeros(0, dtype=np.int64)
         return rows, self.ids[pos.astype(np.int64)], cnt
 
+    def _bag_scale(self, cnt):
+        """The mean combiner's factor of each bag, from its id count."""
+        return 1.0 / np.maximum(cnt, 1)
+
     def _keep(self, t, l, width):
         if self.rate <= 0:
             return None
@@ -357,7 +361,7 @@ class StepRef(object):
                 name = "dnn/input_from_feature_columns/input_layer/%s/embedding_weights" % tb["name"]
                 lo, po, w = plan.deep_layout[tb["name"]]
                 rows, ids, cnt = self._col_ids(tb["column"])
-                mw = (1.0 / np.maximum(cnt, 1))[rows][:, None]
+                mw = self._bag_scale(cnt)[rows][:, None]
                 g, m, r = (np.zeros((tb["rows"], tb["dim"])) for _ in range(3))
                 np.add.at(g, ids, mw * dX[rows, lo:lo + w])
                 np.add.at(m, ids, mw * MdX[rows, lo:lo + w])

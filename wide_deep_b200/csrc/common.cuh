@@ -342,6 +342,7 @@ struct SummarySeg {          // one segment of the statistics kernel: a [B, cols
     const uint8_t* mask;     // [cols] 1 = a real column (the deep input's logical columns), null: every column
     const float *gamma, *beta; int bn;   // hidden layers: BN affine
     float drop_rate; int layer_id;       //   and dropout (DropArgs)
+    unsigned int drop_row0;
     int blk0, nblk;          // the segment's blocks in the grid
 };
 struct SummaryState {
@@ -545,6 +546,8 @@ int dense_apply(WdModel* m);                                     // mlp.cu
 int loss_forward(WdModel* m, bool need_grad);                    // mlp.cu: logits = wide + deep, loss, dlogit
 int model_init_params(WdModel* m, uint64_t seed);                // init.cu
 int step_tick(WdModel* m);                                       // misc.cu: train-step counter on the device (dropout)
+// first row of this rank's batch in the global batch the dropout mask is drawn over (DropArgs::row0): rank * max_batch
+inline unsigned int drop_row0(const WdModel* m) { return m->shard.world > 1 ? (unsigned int)m->shard.rank * (unsigned int)m->max_batch : 0u; }
 int adam_tick(WdModel* m);                                       // misc.cu: beta powers advance (after every optimizer of the step)
 int shard_build(WdModel* m, const WdPlanDesc* d);                // shard.cu: sharded spaces, their lists and the exchange segment
 int place_tables(WdModel* m, int64_t hbm_reserve);               // host_tables.cu: allocate the tables (HBM / host) and staging buffers

@@ -84,7 +84,9 @@ int make_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, const void* ptr
 // (oracle/model.py drop_keep): element (m, n) of layer `layer_id` in train step `step` is kept iff
 //   u >= rate,  u = top 24 bits of splitmix64(key ^ (m * 65536 + n)) / 2^24,  key = splitmix64(seed ^ step * GOLDEN ^ layer_id << 48)
 // and kept elements are scaled by 1 / (1 - rate).  Nothing is stored: the backward regenerates the mask.
-struct DropArgs { float rate; unsigned long long seed; const unsigned int* step; int layer_id; };
+// m is the row of the global batch: row0 + the local row, row0 = rank * max_batch on a row-sharded rank (drop_row0) and 0 on one
+// GPU.  So no two ranks share a mask, and G ranks with full batches draw the mask one GPU draws on their concatenated batch.
+struct DropArgs { float rate; unsigned long long seed; const unsigned int* step; int layer_id; unsigned int row0; };
 __device__ __forceinline__ unsigned long long splitmix64_dev(unsigned long long x) {
     x += 0x9E3779B97F4A7C15ULL;
     x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;

@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256) dropout_fwd_kernel(int B, int N, int n_lo
         const int mrow = (int)(t / N), n = (int)(t % N);
         float h = 0.f;
         if (n < n_logical) {
-            const float a = A[(int64_t)mrow * ld + n] * drop_mult(key, (unsigned)mrow, (unsigned)n, dr.rate, inv_keep);
+            const float a = A[(int64_t)mrow * ld + n] * drop_mult(key, dr.row0 + (unsigned)mrow, (unsigned)n, dr.rate, inv_keep);
             h = bn_out(a, gamma, beta, n, bn);
         }
         if (H) H[(int64_t)mrow * ld + n] = h;
@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(256) act_bn_bwd_kernel(int B, int N, int n_log
             float dz = 0.f;
             if (mm < B && n < n_logical) {
                 float dh = dH[(int64_t)mm * ld + n], a = Aact[(int64_t)mm * ld + n];
-                const float dm = dr.rate > 0.f ? drop_mult(dkey, (unsigned)mm, (unsigned)n, dr.rate, inv_keep) : 1.f;
+                const float dm = dr.rate > 0.f ? drop_mult(dkey, dr.row0 + (unsigned)mm, (unsigned)n, dr.rate, inv_keep) : 1.f;
                 dz = dh * gsc * dm * act_bwd(act, a);
                 sb += dz; sg += dh * (a * dm) * inv; sbe += dh;
             }
@@ -456,7 +456,7 @@ __global__ void __launch_bounds__(256) act_bn_bwd_q_kernel(int B, int N, int n_l
             for (int j = 0; j < 4; ++j) {
                 dz[j] = 0.f;
                 if (n0 + j < n_logical) {
-                    const float dm = dr.rate > 0.f ? drop_mult(dkey, (unsigned)mm, (unsigned)(n0 + j), dr.rate, inv_keep) : 1.f;
+                    const float dm = dr.rate > 0.f ? drop_mult(dkey, dr.row0 + (unsigned)mm, (unsigned)(n0 + j), dr.rate, inv_keep) : 1.f;
                     dz[j] = dh[j] * gsc[j] * dm * act_bwd(act, a[j]);
                     sb[j] += dz[j]; sg[j] += dh[j] * (a[j] * dm) * inv; sbe[j] += dh[j];
                 }
@@ -835,7 +835,7 @@ int mlp_forward(WdModel* m, bool train) {
             int rc = run_gemm(m, EPI_FWD, A, W, B, L.N_phys, ep);
             if (rc) return rc;
             if (train && m->dropout_rate > 0.f) {              // tf.layers.dropout(training=True): TRAIN steps only (dnn.py:111-112)
-                const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l};
+                const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l, drop_row0(m)};
                 dropout_fwd_kernel<<<grid_for((int64_t)B * L.N_phys, 256), 256, 0, m->stream>>>(B, L.N_phys, L.N, L.A, L.N_phys, ep.gamma, ep.beta, m->batch_norm,
                     L.H, L.Hs[0], L.Hs[1], ep.HT, m->ldt, dr);
                 m->launches++;
@@ -938,7 +938,7 @@ int mlp_backward(WdModel* m) {
                 WD_CUDA(cudaMemsetAsync(L.dH, 0, (size_t)m->max_batch_pad * L.N_phys * sizeof(float), m->stream));
             }
             dim3 g((L.N_phys + 31) / 32, rts);
-            const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l};
+            const DropArgs dr{m->dropout_rate, m->dropout_seed, m->d_step, (int)(&tw - &m->towers[0]) * 64 + l, drop_row0(m)};
             if (fused[l]) {
                 // dZ and the partials of this layer were written by logits_act_bwd_q_kernel
             } else if (bf16_ops)

@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(kSummaryThreads) summary_stats_kernel(const Su
 
     const bool hidden = sg.kind == WD_SEG_HIDDEN;
     const bool drop = hidden && sg.drop_rate > 0.f;
-    const unsigned long long key = drop ? drop_key(DropArgs{sg.drop_rate, seed, step, sg.layer_id}) : 0ull;
+    const unsigned long long key = drop ? drop_key(DropArgs{sg.drop_rate, seed, step, sg.layer_id, sg.drop_row0}) : 0ull;
     const float inv_keep = drop ? 1.f / (1.f - sg.drop_rate) : 1.f;
     double sum = 0.0, sumsq = 0.0, mn = DBL_MAX, mx = -DBL_MAX;
     long long num = 0, zeros = 0, bad = 0;
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(kSummaryThreads) summary_stats_kernel(const Su
         if (sg.mask && !sg.mask[col]) continue;
         float v = sg.ptr[(int64_t)row * sg.ld + col];
         if (hidden) {
-            if (drop) v *= drop_mult(key, row, col, sg.drop_rate, inv_keep);
+            if (drop) v *= drop_mult(key, sg.drop_row0 + row, col, sg.drop_rate, inv_keep);
             v = bn_out(v, sg.gamma, sg.beta, col, sg.bn);
         }
         ++num;
@@ -157,6 +157,7 @@ int summary_prepare(WdModel* m, const std::vector<uint8_t>& x0_real) {
                 g.beta = L.t_beta >= 0 ? m->d_P + m->dense[L.t_beta].off : nullptr;
                 g.drop_rate = m->dropout_rate;
                 g.layer_id = (int)t * 64 + l;                              // as mlp_forward's DropArgs
+                g.drop_row0 = drop_row0(m);
             }
             if ((rc = add(WD_SEG_TOWER_LOGITS, (int)t, -1, tw.logit, 1, 1))) return rc;
         }
