@@ -50,7 +50,8 @@ enum { WD_GEMM_AUTO = 0, WD_GEMM_FFMA = 1, WD_GEMM_TC3X = 2 /* wgmma tf32, 3-pas
        WD_GEMM_BF16X3 = 4 /* wgmma on bf16 hi/lo copies written by the producing kernels, 3 passes */ };
 /* where an embedding table's records live (WdPlanDesc::table_placement) */
 enum { WD_PLACE_HBM = 0, WD_PLACE_HOST = 1 /* mapped, page-locked host memory */,
-       WD_PLACE_AUTO = 2 /* HBM if it fits, else host memory (resolved once by wd_model_create) */ };
+       WD_PLACE_AUTO = 2 /* HBM if it fits, else host memory (resolved once by wd_model_create) */,
+       WD_PLACE_DEFER_ADAM = 4 /* flag OR'ed into WD_PLACE_HOST / WD_PLACE_AUTO: Adam's untouched rows catch up when next read */ };
 
 typedef struct WdOptimizer {
     int32_t kind;        /* WD_OPT_* */
@@ -141,7 +142,13 @@ typedef struct WdPlanDesc {
      * shard lives in its own host memory and its owner stages the rows it owns (results bit-identical to the shards in HBM); the
      * auto placement then also keeps room for the sharded exchange buffers.  Host placement is refused (WD_EUNSUPPORTED) for a
      * replicated table of a sharded model, with dense_exchange_max_rows > 0 and shard_world <= 1, or with Adam as the dnn
-     * optimizer; auto tables stay in HBM in those cases. */
+     * optimizer; auto tables stay in HBM in those cases.
+     * Adam: sparse Adam moves every row of a table every step (decay of m and v, then a step of w), which would stream a host
+     * table over PCIe twice per step.  WD_PLACE_DEFER_ADAM OR'ed into a WD_PLACE_HOST / WD_PLACE_AUTO entry lifts the Adam
+     * refusal for that table: its records become [w | m | v | stamp] (the stamp: the last Adam step the record reflects, in a
+     * trailing float4) and a row that no gradient touched is brought up to date when it is next staged, by replaying the
+     * steps it missed in order with the same fp32 operations, so results stay bit-identical to the table in HBM.  The replay
+     * costs up to one step per missed step and row, until the row's values stop changing.  Ignored for other optimizers. */
     const uint8_t *table_placement;
 } WdPlanDesc;
 
@@ -174,7 +181,9 @@ int wd_model_destroy(WdModel *m);
 /* Device-side initialisation with the TF initialisers (truncated normal / glorot uniform / zeros). */
 int wd_model_init(WdModel *m, uint64_t seed);
 /* Number of optimizer steps already taken (checkpoint resume): restores Adam's beta1^t / beta2^t (the non-slot variables of
- * tf.train.AdamOptimizer); a no-op for the other optimizers. */
+ * tf.train.AdamOptimizer); a no-op for the other optimizers.  Rows of WD_PLACE_DEFER_ADAM tables keep their step stamps: the
+ * call moves "now", so a row stamped s then owes steps s+1 .. steps (none when s >= steps).  Writing a table's tensor
+ * (wd_tensor_io) stamps every row with the current step. */
 int wd_set_opt_step(WdModel *m, int64_t steps);
 /* Copy a parameter or optimizer slot to/from host.  slot 0 = value, 1.. = optimizer accumulators
  * (Adagrad: acc; FTRL: n, z).  Logical (unpadded) shapes; kernels are [in, out] like tf.layers.dense. */
@@ -207,6 +216,11 @@ int wd_shard_cache_enable(WdModel *m, int64_t bytes);
  * without a cache.  Copies the first min(n, 5); reset != 0 zeroes the counters [1..4] after the copy.  Synchronises the model
  * stream. */
 int wd_host_cache_stats(WdModel *m, int64_t *out, int32_t n, int32_t reset);
+/* Cumulative counters of the catch-up of WD_PLACE_DEFER_ADAM tables: out[0] rows caught up (staged or settled with at least one
+ * missed step), [1] steps replayed, [2] steps skipped because a row's values had stopped changing (past the last step whose
+ * lr_t differs from lr), [3] the longest gap (missed steps of one row) seen.  Same conventions as wd_host_cache_stats: copies the
+ * first min(n, 4), reset != 0 zeroes them after the copy, synchronises the model stream; all 0 without deferred tables. */
+int wd_deferred_adam_stats(WdModel *m, int64_t *out, int32_t n, int32_t reset);
 
 /* One training step: H2D copy, ids, forward, loss, backward, optimizers.  Replaces one
  * sess.run(train_op) of Estimator.train (reference python/train.py:128-133; joint.py:224-262).

@@ -16,7 +16,13 @@ distribution (synthetic.criteo_batch_arrays(zipf=...)); multihot ids stay unifor
   * GPU name, power limit and max SM clock (read-only nvidia-smi query).
 Afterwards every parameter and optimizer slot of B and C is compared byte for byte with A's.
 
-    python tools/host_tables_bench.py [--workloads criteo,multihot] [--steps 50] [--ring 64] [--zipf 1.05] [--cache-bytes N] [--out FILE]
+--dnn-opt OPT replaces the workload's dnn_optimizer (e.g. Adam).  With Adam, B and C are deferred Adam tables
+(Plan(defer_adam=True)): rows no gradient touched catch up on their missed steps when next staged.  Then also reported: the
+catch-up counters per timed step of B and C (rows caught up, steps replayed, steps skipped by the early exit, longest gap), and
+the time of one settling read of B's largest host table (a whole-table read first replays every row's missed steps).
+
+    python tools/host_tables_bench.py [--workloads criteo,multihot] [--steps 50] [--ring 64] [--zipf 1.05] [--cache-bytes N]
+                                      [--dnn-opt Adam] [--out FILE]
 """
 import argparse
 import json
@@ -67,10 +73,17 @@ def build(wl, B, host_tables, cache_bytes=0):
     from wide_deep_b200.plan import Plan
     return Plan(wl["fc"], wl["cross"], wl["model"], wl["model_type"], max_batch=B, embedding_dim_override=wl["emb"],
                 gemm_engine="bf16x3", max_keys=B * wl["keys_per_row"], max_nnz=B * wl["ids_per_row"], host_tables=host_tables,
-                host_cache_bytes=cache_bytes)
+                host_cache_bytes=cache_bytes, defer_adam=bool(host_tables))
 
 
-def workload(name, zipf=None):
+def workload(name, zipf=None, dnn_opt=None):
+    wl = _workload(name, zipf)
+    if dnn_opt:
+        wl["model"] = dict(wl["model"], dnn_optimizer=dnn_opt)
+    return wl
+
+
+def _workload(name, zipf=None):
     from wide_deep_b200 import synthetic
     if name == "criteo":
         fc, cross, model, emb = synthetic.criteo_conf()
@@ -102,9 +115,9 @@ def all_equal(a, b):
     return True, None
 
 
-def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed=7):
+def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed=7, dnn_opt=None):
     from wide_deep_b200.model import WideDeepModel
-    wl = workload(name, zipf)
+    wl = workload(name, zipf, dnn_opt)
     B = wl["batch"]
     plan_a = build(wl, B, [])
     host = [t["name"] for t in plan_a.tables if t["rows"] > host_min_rows]
@@ -124,9 +137,10 @@ def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed
     host_cols = [ci for ci, c in enumerate(plan_a.columns) if c.emb_table >= 0 and by_table[c.emb_table]["name"] in host]
     rec_bytes = {}
     nslots = {"sgd": 0, "adagrad": 1, "ftrl": 2, "adam": 2, "rmsprop": 2}[plan_a.dnn_opt["kind"]]
+    adam = plan_a.dnn_opt["kind"] == "adam"
     for ci in host_cols:
         t = by_table[plan_a.columns[ci].emb_table]
-        rec_bytes[ci] = ((t["dim"] + 3) // 4 * 4) * (1 + nslots) * 4
+        rec_bytes[ci] = (((t["dim"] + 3) // 4 * 4) * (1 + nslots) + (4 if adam else 0)) * 4     # (deferred Adam: + the stamp)
     u_host, bytes_way, nuniq = [], [], []
     step = 0
     for i in range(warmup):                      # same steps on every model; the first steps also count the rows
@@ -147,6 +161,8 @@ def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed
         step += 1
     if "cache" in models:
         models["cache"].host_cache_stats(reset=True)
+    for m in models.values():
+        m.deferred_adam_stats(reset=True)
     times = {k: [] for k in models}
     for w in range(2):                            # A / B / C / A / B / C, each window on the same steps
         for key, m in models.items():
@@ -158,6 +174,8 @@ def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed
             times[key].append(time.perf_counter() - t)
         step += steps
     rate = {k: B * steps / min(v) for k, v in times.items()}
+    catch_up = {k: {c: (v if c == "max_gap" else v / (2 * steps)) for c, v in m.deferred_adam_stats().items()}
+                for k, m in models.items() if k != "hbm"}
     phases = {}
     for key, m in models.items():                 # one profiled (eager) step per model, the same step on each: phase times in ms
         m.set_profile(True)
@@ -185,6 +203,21 @@ def run(name, steps, warmup, host_min_rows, ring, zipf=None, cache_bytes=0, seed
                    pcie_records_out_per_step=(c["evictions"] + c["overflow"]) / n,
                    pcie_bytes_in_per_step=(c["loads"] + c["overflow"]) / n * rec,
                    pcie_bytes_out_per_step=(c["evictions"] + c["overflow"]) / n * rec)
+    if adam and host:
+        res["catch_up_per_step"] = catch_up
+        largest = max((t for t in plan_a.tables if t["name"] in host), key=lambda t: t["rows"] * t["dim"])
+        from wide_deep_b200.plan import T_EMB_TABLE
+        tname = [n for n, v in plan_a.tensor_names.items() if v[0] == T_EMB_TABLE and plan_a.tables[v[1]]["name"] == largest["name"]][0]
+        mb = models["host"]
+        mb.sync()
+        mb.deferred_adam_stats(reset=True)
+        t = time.perf_counter()
+        mb.get_tensor(tname)
+        res["settle_read_s"] = time.perf_counter() - t
+        res["settle_table"] = dict(name=largest["name"], rows=largest["rows"], dim=largest["dim"], counters=mb.deferred_adam_stats())
+        t = time.perf_counter()
+        mb.get_tensor(tname)
+        res["second_read_s"] = time.perf_counter() - t
     for k in models:
         if k == "hbm":
             continue
@@ -206,6 +239,7 @@ def main():
     ap.add_argument("--zipf", type=float, default=None, help="Criteo ids from Zipf(ALPHA) instead of uniform")
     ap.add_argument("--cache-bytes", type=int, default=0, help="also run the host model with an HBM cache of this many bytes")
     ap.add_argument("--host-min-rows", type=int, default=16384, help="tables with more rows than this go to host memory")
+    ap.add_argument("--dnn-opt", default=None, help="dnn optimizer of every workload (e.g. Adam: deferred Adam host tables)")
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
     args = ap.parse_args()
     info = gpu_info()
@@ -214,7 +248,7 @@ def main():
     ok = True
     for name in args.workloads.split(","):
         r = run(name, args.steps, 3 * args.ring if args.warmup is None else args.warmup, args.host_min_rows, args.ring,
-                zipf=args.zipf, cache_bytes=args.cache_bytes)
+                zipf=args.zipf, cache_bytes=args.cache_bytes, dnn_opt=args.dnn_opt)
         extra = (r["step_ms_host"] - r["step_ms_hbm"]) / 1e3
         by = r["pcie_bytes_per_step_each_way"]
         r.update(info)

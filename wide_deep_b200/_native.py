@@ -48,6 +48,7 @@ SYMBOLS = {
     "wd_host_cache_enable": (ctypes.c_int, [_vp, _i64]),
     "wd_shard_cache_enable": (ctypes.c_int, [_vp, _i64]),
     "wd_host_cache_stats": (ctypes.c_int, [_vp, ctypes.POINTER(_i64), _i32, _i32]),
+    "wd_deferred_adam_stats": (ctypes.c_int, [_vp, ctypes.POINTER(_i64), _i32, _i32]),
     "wd_train_step": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(ctypes.c_float)]),
     "wd_forward": (ctypes.c_int, [_vp, _vp, _vp, ctypes.POINTER(ctypes.c_float)]),
     "wd_batch_upload": (ctypes.c_int, [_vp, _vp]),

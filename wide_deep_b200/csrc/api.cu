@@ -208,6 +208,7 @@ static int build_model(const WdPlanDesc* d, WdModel* m) {
     if (getenv("WD_STEP_TRACE") && (rc = dev_alloc(m, &m->d_step_trace, 16))) return rc;
     if ((rc = dev_alloc(m, &m->d_step, 4))) return rc;
     if ((rc = dev_alloc(m, &m->d_bpow, 4))) return rc;
+    if ((rc = dev_alloc(m, &m->d_adam_step, 1))) return rc;
     {
         const float bp[4] = {m->lin_opt.beta1, m->lin_opt.beta2, m->dnn_opt.beta1, m->dnn_opt.beta2};     // beta^1: state before the first step
         WD_CUDA(cudaMemcpyAsync(m->d_bpow, bp, sizeof(bp), cudaMemcpyHostToDevice, m->stream));
@@ -245,14 +246,16 @@ static int build_model(const WdPlanDesc* d, WdModel* m) {
             tb.rows = d->table_rows[t]; tb.dim = d->table_dim[t]; tb.x0_off = d->table_x0_off[t];
             tb.dim_logical = d->table_dim_logical[t];
             if (tb.dim_logical < 1 || tb.dim_logical > tb.dim) { set_error("table %d: bad logical width", t); return WD_EINVAL; }
-            tb.row_base = 0; tb.gs_off = -1; tb.stride = tb.dim * (1 + nslots); tb.col = -1;
+            const int place = d->table_placement ? d->table_placement[t] : WD_PLACE_HBM;
+            tb.place = place & ~WD_PLACE_DEFER_ADAM;
+            if (tb.place < WD_PLACE_HBM || tb.place > WD_PLACE_AUTO) { set_error("table %d: placement %d is not a WD_PLACE_*", t, place); return WD_EINVAL; }
+            tb.defer = (place & WD_PLACE_DEFER_ADAM) && tb.place != WD_PLACE_HBM && m->dnn_opt.kind == WD_OPT_ADAM;
+            tb.row_base = 0; tb.gs_off = -1; tb.stride = tb.dim * (1 + nslots) + (tb.defer ? 4 : 0); tb.col = -1;
             tb.sharded = G > 1 && d->table_sharded && d->table_sharded[t];
             tb.arows = tb.sharded ? (tb.rows - m->shard.rank + G - 1) / G : tb.rows;
             if (tb.dim % 4 || tb.x0_off % 4) { set_error("table %d: dim and deep-input offset must be multiples of 4", t); return WD_EINVAL; }
             for (int c = 0; c < C; ++c) if (d->col_emb_table[c] == t) tb.col = c;
             if (tb.col < 0) { set_error("table %d has no producing column", t); return WD_EINVAL; }
-            tb.place = d->table_placement ? d->table_placement[t] : WD_PLACE_HBM;
-            if (tb.place < WD_PLACE_HBM || tb.place > WD_PLACE_AUTO) { set_error("table %d: placement %d is not a WD_PLACE_*", t, tb.place); return WD_EINVAL; }
             tb.data = nullptr;                                       // allocated by place_tables, after every other buffer of the model
             for (int i = 0; i < tb.dim_logical; ++i) m->x0_real[tb.x0_off + i] = 1;
             m->emb_max_dim = std::max(m->emb_max_dim, tb.dim);
@@ -602,9 +605,18 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
             const int rc = host_cache_sync(m, true, to_device != 0);
             if (rc) return rc;
         }
+        // a deferred table's rows are brought up to the current step before a read; a write makes them current
+        if (deferred(tb) && !to_device) {
+            const int rc = deferred_adam_settle(m, tb, false);
+            if (rc) return rc;
+        }
         const cudaMemcpyKind dir = tb.host ? cudaMemcpyDefault : (to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost);
         if (to_device) WD_CUDA(cudaMemcpy2DAsync(dev, (size_t)tb.stride * 4, host, lw, lw, tb.arows, dir, m->stream));
         else WD_CUDA(cudaMemcpy2DAsync(host, lw, dev, (size_t)tb.stride * 4, lw, tb.arows, dir, m->stream));
+        if (deferred(tb) && to_device) {
+            const int rc = deferred_adam_settle(m, tb, true);
+            if (rc) return rc;
+        }
         WD_CUDA(cudaStreamSynchronize(m->stream));
         return WD_OK;
     }
@@ -1187,10 +1199,11 @@ static int backward_eager(WdModel* m, bool join) {
 // is ~65 launches on three streams, graphed per batch slot.  Inside the graph the streams overlap as in the eager schedule; after
 // it the sparse lists continue on their side streams, which wait for the graph through ev_bwd_done.
 // The split step applies the embedding rows with the unfused kernels, which update host records through their mapped pointers:
-// with an HBM cache in front of those records the update would bypass it.
+// with an HBM cache in front of those records the update would bypass it, and a deferred Adam table's records lag behind the step.
 static int refuse_split_step_with_cache(WdModel* m) {
-    if (m->hcache.slots == 0) return WD_OK;
-    set_error("the split step (wd_step_backward / wd_step_apply) is not supported on a model with a host-table cache");
+    if (m->hcache.slots == 0 && m->n_defer_tab == 0) return WD_OK;
+    set_error("the split step (wd_step_backward / wd_step_apply) is not supported on a model with a host-table cache or with "
+              "deferred Adam tables (WD_PLACE_DEFER_ADAM)");
     return WD_EUNSUPPORTED;
 }
 

@@ -83,13 +83,17 @@ struct EmbTable {
     int col;                 // producing column
     int64_t row_base;        // global row id base
     int64_t gs_off;          // small (dense-exchanged) table: float offset of its gradients in the small-table block; else -1
-    float* data;            // arows * stride floats; record = [w[dim] | slot1[dim] | slot2[dim]]
-    int stride;              // dim * (1 + nslots)
+    float* data;            // arows * stride floats; record = [w[dim] | slot1[dim] | slot2[dim]] (+ stamp: see defer)
+    int stride;              // dim * (1 + nslots), + 4 with defer
     bool sharded;            // row-sharded over the ranks: this rank holds rows r with r mod G == rank at local index r / G
     int64_t arows;           // rows allocated on this rank (= rows unless sharded); row_base then counts in the shard's row space
     int place;               // requested placement WD_PLACE_*
     bool host;               // records live in mapped page-locked host memory (staged through HBM every step, host_tables.cu)
+    // WD_PLACE_DEFER_ADAM with the Adam dnn optimizer: record [w | m | v | stamp float4], lane 0 of the stamp = the last Adam step
+    // the record reflects; on the host (deferred()) the untouched pass skips the table and rows catch up when staged (host_tables.cu)
+    bool defer;
 };
+inline bool deferred(const EmbTable& tb) { return tb.host && tb.defer; }
 
 struct TabDesc {            // per-table descriptor grouped by width (one 32-byte load in the gather kernels)
     float* data;
@@ -423,6 +427,12 @@ struct WdModel {
     uint32_t* d_g_emb = nullptr;             // [max_nnz] ids the gather reads: e_emb, host-table entries replaced by their unique index u
     // HBM cache of host records (wd_host_cache_enable): d_stage is then [hcache.slots slots | max_nnz overflow rows]
     wd::HostCache hcache;
+    // Adam on deferred host tables (host_tables.cu): tables with deferred() (host shards included), lr_t[j] of steps j = 1 ..
+    // lr_t_last (later steps: lr), counters [rows caught up, steps replayed, steps skipped, longest gap]
+    int n_defer_tab = 0;
+    float* d_lr_t = nullptr;
+    int64_t lr_t_last = 0;
+    unsigned long long* d_defer_stats = nullptr;
     bool stepped = false;                    // a forward or train step was issued (step graphs may exist)
 
     // numeric deep columns (device arrays)
@@ -488,6 +498,7 @@ struct WdModel {
     unsigned long long* d_step_trace = nullptr;   // WD_STEP_TRACE=1: globaltimer stamps of the last step (wd_debug_step_trace)
     int32_t* d_head_counter = nullptr;       // blocks of the head kernel that have finished (last one sums the loss)
     float* d_bpow = nullptr;                 // Adam: {linear beta1^t, linear beta2^t, dnn beta1^t, dnn beta2^t}, multiplied in fp32 after every step (AdamOptimizer._finish)
+    uint32_t* d_adam_step = nullptr;         // Adam: steps completed (advances with d_bpow; the "now" of deferred tables' stamps)
     float* h_loss_pinned = nullptr;
 
     wd::RowList lists[wd::kLists];           // sparse backward scratch: the sparse row lists
@@ -555,6 +566,8 @@ int build_record_sets(WdModel* m);                               // host_tables.
 int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
 int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
 int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
+// host_tables.cu: every host record of deferred table tb caught up to the current Adam step in place (stamp_only: just stamped)
+int deferred_adam_settle(WdModel* m, const EmbTable& tb, bool stamp_only);
 // host_tables.cu, over any record set `rr` whose staged tables (found by row base) keep the records of the unique rows of list L
 // (lists[L].urow[0 .. *lists[L].nuniq)) in rr.stage_base at stride S, behind cache `c` (c.slots = 0: none, staging row u):
 //   stage_in_rows    cache keys -> sort -> assign (train: the used slots turn dirty), then dirty victims home and the records

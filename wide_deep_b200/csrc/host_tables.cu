@@ -39,6 +39,16 @@
 // serving them and stages them into its own buffer through stage_in_rows / write_back_rows (the owner-side step is in shard.cu),
 // behind its own HBM cache when wd_shard_cache_enable made one.  Only the sharded tables may go to the host then; the replicated
 // ones, the single-GPU staging buffer and the single-GPU cache stay out of it.
+//
+// Adam (WD_PLACE_DEFER_ADAM).  Sparse Adam moves every row every step; for a row no gradient touched that step is a fixed
+// function of the record and the step's lr_t (m *= b1, v *= b2, w -= lr_t m / (sqrt(v) + eps)).  A deferred table skips the
+// untouched pass (its RecordSet::rows are 0) and carries a stamp in its record, [w | m | v | stamp float4]: the last Adam step the
+// record reflects.  The stamp travels inside the stride through every transfer above.  Invariant: wherever a deferred record lives
+// (host, staging row, cache slot), it is the exact state as of its stamp.  stage_in_rows then catches every staged row up
+// (adam_catch_up_kernel): steps s+1 .. g (g = WdModel::d_adam_step) in order, with lr_t[j] from the table deferred_adam_setup
+// builds with with_lr_t's own expression, so the values are bit-identical to the untouched passes of the table in HBM.  A train
+// call stamps g + 1 (the list's update follows, on the staged record, then the write-back); a forward-only call stamps g.  Reads
+// of the whole table (wd_tensor_io) settle every host record first; writes stamp every record with g.
 #include <algorithm>
 #include <type_traits>
 
@@ -259,6 +269,174 @@ __global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32
     }
 }
 
+// ---------------------------------------------------------------------------------------------------- deferred Adam
+// Steps past lr_t_last have lr_t == lr exactly (both 1 - beta^j round to 1).  The table must end there: betas so close to 1 that it
+// would be longer than this are refused.
+constexpr int64_t kMaxLrT = 1 << 22;
+struct AdamReplay { const float* lr_t; int64_t last; const uint32_t* now; unsigned long long* stats; };
+
+// Steps s+1 .. g of Adam's untouched update on four consecutive elements of a record [w | m | v] (gap floats apart); returns the
+// steps run.  Past `last` every step is the same map, so once a step leaves all twelve values' bits unchanged the rest are skipped.
+__device__ __forceinline__ uint32_t adam_replay4(OptParams o, const AdamReplay& ar, float* w, int gap, uint32_t s, uint32_t g) {
+    float4 x = *reinterpret_cast<float4*>(w), mm = *reinterpret_cast<float4*>(w + gap), vv = *reinterpret_cast<float4*>(w + 2 * gap);
+    uint32_t j = s + 1;
+    for (; j <= g; ++j) {
+        o.lr_t = (int64_t)j <= ar.last ? ar.lr_t[j] : o.lr;
+        const float4 x0 = x, m0 = mm, v0 = vv;
+        adam_decay(o, mm.x, vv.x); adam_step(o, x.x, mm.x, vv.x);
+        adam_decay(o, mm.y, vv.y); adam_step(o, x.y, mm.y, vv.y);
+        adam_decay(o, mm.z, vv.z); adam_step(o, x.z, mm.z, vv.z);
+        adam_decay(o, mm.w, vv.w); adam_step(o, x.w, mm.w, vv.w);
+        if ((int64_t)j > ar.last) {
+            const bool same = __float_as_uint(x.x) == __float_as_uint(x0.x) && __float_as_uint(x.y) == __float_as_uint(x0.y) &&
+                              __float_as_uint(x.z) == __float_as_uint(x0.z) && __float_as_uint(x.w) == __float_as_uint(x0.w) &&
+                              __float_as_uint(mm.x) == __float_as_uint(m0.x) && __float_as_uint(mm.y) == __float_as_uint(m0.y) &&
+                              __float_as_uint(mm.z) == __float_as_uint(m0.z) && __float_as_uint(mm.w) == __float_as_uint(m0.w) &&
+                              __float_as_uint(vv.x) == __float_as_uint(v0.x) && __float_as_uint(vv.y) == __float_as_uint(v0.y) &&
+                              __float_as_uint(vv.z) == __float_as_uint(v0.z) && __float_as_uint(vv.w) == __float_as_uint(v0.w);
+            if (same) { ++j; break; }
+        }
+    }
+    if (j > s + 1) {
+        *reinterpret_cast<float4*>(w) = x;
+        *reinterpret_cast<float4*>(w + gap) = mm;
+        *reinterpret_cast<float4*>(w + 2 * gap) = vv;
+    }
+    return j - (s + 1);
+}
+
+// One deferred record caught up by the 8 lanes of a lane group (mask gm; lane lig takes float4 chunks lig, lig + 8, ...), then
+// stamped: train ? g + 1 : max(stamp, g).  Counters of lane 0 of the group accumulate in cnt.
+struct CatchUpCount { unsigned long long rows = 0, replayed = 0, skipped = 0, gap = 0; };
+__device__ __forceinline__ void catch_up_record(const OptParams& o, const AdamReplay& ar, float* rec, int dim, uint32_t g, bool train,
+                                                unsigned gm, int lig, CatchUpCount& cnt) {
+    uint32_t* stamp = reinterpret_cast<uint32_t*>(rec + 3 * dim);
+    const uint32_t s = *stamp;
+    uint32_t run = 0;
+    if (s < g)
+        for (int q = lig; q * 4 < dim; q += 8) run = max(run, adam_replay4(o, ar, rec + q * 4, dim, s, g));
+    run = __reduce_max_sync(gm, run);                   // (every lane has read the stamp before lane 0 writes it)
+    if (lig == 0) {
+        *stamp = train ? g + 1 : max(s, g);
+        if (s < g) {
+            cnt.rows++; cnt.replayed += run; cnt.skipped += (g - s) - run;
+            cnt.gap = max(cnt.gap, (unsigned long long)(g - s));
+        }
+    }
+}
+__device__ __forceinline__ void catch_up_flush(const AdamReplay& ar, const CatchUpCount& c) {
+    unsigned long long r = c.rows, p = c.replayed, k = c.skipped, gp = c.gap;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        r += __shfl_xor_sync(0xffffffffu, r, d); p += __shfl_xor_sync(0xffffffffu, p, d);
+        k += __shfl_xor_sync(0xffffffffu, k, d); gp = max(gp, __shfl_xor_sync(0xffffffffu, gp, d));
+    }
+    if ((threadIdx.x & 31) == 0 && r) {
+        atomicAdd(&ar.stats[0], r); atomicAdd(&ar.stats[1], p); atomicAdd(&ar.stats[2], k); atomicMax(&ar.stats[3], gp);
+    }
+}
+
+// The staged records of list L's unique host rows (rr.uslot[u], or u), one lane group of 8 per row.  The trip count of a warp's
+// loop is made warp-uniform so that the counters are reduced by the whole warp.
+__global__ void __launch_bounds__(256) adam_catch_up_kernel(const int32_t* __restrict__ d_nuniq, const uint32_t* __restrict__ urow,
+                                                            RowRecords rr, OptParams o, AdamReplay ar, int train) {
+    const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
+    const unsigned gm = 0xFFu << (grp * 8);
+    const int nu = *d_nuniq;
+    const uint32_t g = *ar.now;
+    const int64_t w0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4;
+    const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
+    CatchUpCount cnt;
+    for (int64_t u0 = w0; u0 < nu; u0 += gstep) {
+        const int64_t u = u0 + grp;
+        if (u >= nu) continue;
+        const int64_t row = urow[u];
+        const int t = table_of(rr.row_base, rr.ntab, row);
+        if (rr.stage[t] == 0) continue;                                  // HBM table
+        catch_up_record(o, ar, record(rr, t, urow, u), rr.dim[t], g, train != 0, gm, lig, cnt);
+    }
+    catch_up_flush(ar, cnt);
+}
+
+// Every host record of one deferred table in place (rows records of `stride` floats at data): caught up to g, or only stamped g.
+__global__ void __launch_bounds__(256) adam_settle_kernel(float* data, int64_t rows, int dim, int stride, OptParams o, AdamReplay ar,
+                                                          int stamp_only) {
+    const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
+    const unsigned gm = 0xFFu << (grp * 8);
+    const uint32_t g = *ar.now;
+    const int64_t w0 = (((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 4;
+    const int64_t gstep = (((int64_t)gridDim.x * blockDim.x) >> 5) * 4;
+    CatchUpCount cnt;
+    for (int64_t r0 = w0; r0 < rows; r0 += gstep) {
+        const int64_t r = r0 + grp;
+        if (r >= rows) continue;
+        float* rec = data + r * stride;
+        if (stamp_only) { if (lig == 0) *reinterpret_cast<uint32_t*>(rec + 3 * dim) = g; }
+        else catch_up_record(o, ar, rec, dim, g, false, gm, lig, cnt);
+    }
+    catch_up_flush(ar, cnt);
+}
+
+// lr_t[j] = with_lr_t of step j (beta powers bp[2j], bp[2j + 1]), j = 1 .. n
+__global__ void adam_lr_t_kernel(OptParams o, const float* __restrict__ bp, int64_t n, float* __restrict__ lr_t) {
+    for (int64_t j = 1 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j <= n; j += (int64_t)gridDim.x * blockDim.x) {
+        OptParams p = o;
+        p.bpow = bp + 2 * j;
+        lr_t[j] = with_lr_t(p).lr_t;
+    }
+}
+
+static AdamReplay adam_replay(const WdModel* m) { return AdamReplay{m->d_lr_t, m->lr_t_last, m->d_adam_step, m->d_defer_stats}; }
+
+// The lr_t table of the deferred tables and their counters.  The beta powers are multiplied up on the host in fp32 exactly as
+// adam_tick_kernel and wd_set_opt_step do (beta^1 before the first step), up to the first step at which both 1 - beta^j round to
+// 1; lr_t itself is computed on the device by with_lr_t's expression.
+int deferred_adam_setup(WdModel* m) {
+    const WdOptimizer& o = m->dnn_opt;
+    std::vector<float> bp = {0.f, 0.f, o.beta1, o.beta2};
+    float b1 = o.beta1, b2 = o.beta2;
+    int64_t j = 1;
+    while (!(1.f - b1 == 1.f && 1.f - b2 == 1.f)) {
+        if (j >= kMaxLrT) {
+            set_error("WD_PLACE_DEFER_ADAM: Adam betas (%g, %g) need more than %lld steps before lr_t reaches lr", (double)o.beta1,
+                      (double)o.beta2, (long long)kMaxLrT);
+            return WD_EUNSUPPORTED;
+        }
+        b1 *= o.beta1; b2 *= o.beta2;
+        bp.push_back(b1); bp.push_back(b2);
+        ++j;
+    }
+    m->lr_t_last = j;
+    int rc;
+    float* d_bp = nullptr;
+    if ((rc = dev_alloc(m, &m->d_lr_t, j + 1))) return rc;
+    if ((rc = dev_alloc(m, &m->d_defer_stats, 4))) return rc;
+    if ((rc = upload(m, &d_bp, bp))) return rc;
+    adam_lr_t_kernel<<<grid_for(j, 256), 256, 0, m->stream>>>(make_opt(o), d_bp, j, m->d_lr_t);
+    m->launches++;
+    WD_CUDA(cudaGetLastError());
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    return dev_free(m, d_bp);
+}
+
+static int adam_catch_up(WdModel* m, int L, const RowRecords& rr, bool train) {
+    const RowList& l = m->lists[L];
+    adam_catch_up_kernel<<<grid_for(m->max_nnz * 8, 256), 256, 0, m->stream>>>(l.nuniq, l.urow, rr, make_opt(m->dnn_opt), adam_replay(m),
+                                                                               train ? 1 : 0);
+    m->launches++;
+    mark(m, "adam_catch_up");
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+
+int deferred_adam_settle(WdModel* m, const EmbTable& tb, bool stamp_only) {
+    adam_settle_kernel<<<grid_for(tb.arows * 8, 256), 256, 0, m->stream>>>(tb.data, tb.arows, tb.dim, tb.stride, make_opt(m->dnn_opt),
+                                                                          adam_replay(m), stamp_only ? 1 : 0);
+    m->launches++;
+    WD_CUDA(cudaGetLastError());
+    return WD_OK;
+}
+
 int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, bool train, const CacheMarks& marks) {
     const RowList& l = m->lists[L];
     const int64_t C = c.slots;
@@ -280,7 +458,8 @@ int stage_in_rows(WdModel* m, HostCache& c, int L, const RowRecords& rr, int S, 
     m->launches++;
     if (marks.in) mark(m, marks.in);
     WD_CUDA(cudaGetLastError());
-    return WD_OK;
+    // with Adam every staged table is a deferred one (place_tables): its rows (loads and cache hits alike) catch up here
+    return m->n_defer_tab > 0 ? adam_catch_up(m, L, rr, train) : WD_OK;
 }
 
 int write_back_rows(WdModel* m, const HostCache& c, int L, const RowRecords& rr, int S, const CacheMarks& marks) {
@@ -337,14 +516,14 @@ int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
 int place_tables(WdModel* m, int64_t hbm_reserve) {
     const int nt = (int)m->tables.size();
     auto host_ok = [&](const EmbTable& tb) {
-        if (m->dnn_opt.kind == WD_OPT_ADAM) return false;
+        if (m->dnn_opt.kind == WD_OPT_ADAM && !tb.defer) return false;
         return m->shard.world > 1 ? tb.sharded : m->dense_exchange_max_rows <= 0;
     };
     for (int t = 0; t < nt; ++t)
         if (m->tables[t].place == WD_PLACE_HOST && !host_ok(m->tables[t])) {
             set_error("table %d: host placement is not supported for a replicated table of a row-sharded model, with "
                       "dense_exchange_max_rows > 0 on one GPU or with the Adam dnn optimizer (its sparse update decays the whole table "
-                      "every step)", t);
+                      "every step, unless the table has WD_PLACE_DEFER_ADAM)", t);
             return WD_EUNSUPPORTED;
         }
     auto bytes_of = [&](int t) { return m->tables[t].arows * (int64_t)m->tables[t].stride * 4; };
@@ -382,6 +561,7 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
         WD_CUDA(cudaHostGetDevicePointer(&dp, p, 0));
         tb.data = (float*)dp;                // every element is written by init_sparse_tables before first use
         if (!tb.sharded) m->n_host_tab++;    // (a host shard is staged by its owner, in the shard's own buffer)
+        if (tb.defer) m->n_defer_tab++;
         int& stage_stride = tb.sharded ? m->shard.sp[0].stage_stride : m->stage_stride;
         stage_stride = std::max(stage_stride, tb.stride);
     }
@@ -395,7 +575,7 @@ int place_tables(WdModel* m, int64_t hbm_reserve) {
     // host shards: the owner's staging rows of the step's unique owned rows (+1: see the serve in shard.cu)
     ShardSpace& se = m->shard.sp[0];
     if (se.stage_stride > 0 && (rc = dev_alloc(m, &se.d_stage, (m->max_nnz + 1) * (int64_t)se.stage_stride, false))) return rc;
-    return WD_OK;
+    return m->n_defer_tab > 0 ? deferred_adam_setup(m) : WD_OK;
 }
 
 // dst = per-table values f(table) of the tables `ids`, in that order
@@ -431,7 +611,7 @@ int build_record_sets(WdModel* m) {
         if (m->tables[t].sharded) slots.push_back((int)t);          // slot order = table order (shard_build)
     }
     auto x0_of = [](const EmbTable& tb) { return (int32_t)tb.x0_off; };
-    auto rows_of = [](const EmbTable& tb) { return tb.arows; };
+    auto rows_of = [](const EmbTable& tb) { return deferred(tb) ? (int64_t)0 : tb.arows; };   // (read by the untouched pass only)
     if (!m->tables.empty()) {
         // by table
         if ((rc = upload_records(m, m->tabs.rec, all, m->stage_stride, m->d_stage, m->hcache.d_uslot))) return rc;
@@ -552,6 +732,20 @@ extern "C" int wd_shard_cache_enable(WdModel* m, int64_t bytes) {
     ShardSpace& se = m->shard.sp[0];
     if (se.stage_stride == 0) return WD_OK;                              // no host shard on this rank: capacity 0
     return cache_enable(m, se.cache, bytes, se.stage_stride, m->max_nnz + 1, &se.d_stage, "wd_shard_cache_enable");
+}
+
+extern "C" int wd_deferred_adam_stats(WdModel* m, int64_t* out, int32_t n, int32_t reset) {
+    if (!m || n < 0 || (n > 0 && !out)) { set_error("null argument"); return WD_EINVAL; }
+    WD_CUDA(cudaSetDevice(m->device));
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    unsigned long long h[4] = {0, 0, 0, 0};
+    if (m->d_defer_stats) WD_CUDA(cudaMemcpy(h, m->d_defer_stats, sizeof(h), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n && i < 4; ++i) out[i] = (int64_t)h[i];
+    if (reset && m->d_defer_stats) {
+        WD_CUDA(cudaMemsetAsync(m->d_defer_stats, 0, sizeof(h), m->stream));
+        WD_CUDA(cudaStreamSynchronize(m->stream));
+    }
+    return WD_OK;
 }
 
 extern "C" int wd_host_cache_stats(WdModel* m, int64_t* out, int32_t n, int32_t reset) {

@@ -168,10 +168,11 @@ int metrics_finish(WdModel* m, const double* acc, double* out) {
 
 // ---- Adam's non-slot variables (beta1^t, beta2^t per optimizer) live in device memory so that a replayed CUDA graph advances them
 namespace wd {
-__global__ void adam_tick_kernel(float* bpow, float lb1, float lb2, float db1, float db2, int lin, int dnn) {
+__global__ void adam_tick_kernel(float* bpow, uint32_t* step, float lb1, float lb2, float db1, float db2, int lin, int dnn) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
         if (lin) { bpow[0] *= lb1; bpow[1] *= lb2; }
         if (dnn) { bpow[2] *= db1; bpow[3] *= db2; }
+        *step += 1u;
     }
 }
 __global__ void step_tick_kernel(unsigned int* step) { if (threadIdx.x == 0 && blockIdx.x == 0) *step += 1u; }
@@ -182,7 +183,7 @@ int step_tick(WdModel* m) {
     return WD_OK;
 }
 int adam_tick(WdModel* m) {
-    adam_tick_kernel<<<1, 32, 0, m->stream>>>(m->d_bpow, m->lin_opt.beta1, m->lin_opt.beta2, m->dnn_opt.beta1, m->dnn_opt.beta2,
+    adam_tick_kernel<<<1, 32, 0, m->stream>>>(m->d_bpow, m->d_adam_step, m->lin_opt.beta1, m->lin_opt.beta2, m->dnn_opt.beta1, m->dnn_opt.beta2,
                                              m->lin_opt.kind == WD_OPT_ADAM, m->dnn_opt.kind == WD_OPT_ADAM);
     m->launches++;
     WD_CUDA(cudaGetLastError());
@@ -190,9 +191,11 @@ int adam_tick(WdModel* m) {
 }
 }  // namespace wd
 
-// Restores the optimizers' step count (checkpoint resume): beta^(steps + 1), multiplied up in fp32 exactly as training does.
+// Restores the optimizers' step count (checkpoint resume): beta^(steps + 1), multiplied up in fp32 exactly as training does.  The
+// Adam step count moves too; the stamps of deferred tables' rows stay (the rows then owe the steps in between).
 extern "C" int wd_set_opt_step(WdModel* m, int64_t steps) {
     if (!m || steps < 0) { wd::set_error("wd_set_opt_step: bad arguments"); return WD_EINVAL; }
+    if (m->n_defer_tab > 0 && steps > 0xFFFFFFFFll) { wd::set_error("wd_set_opt_step: deferred Adam tables stamp rows with 32-bit steps"); return WD_EINVAL; }
     WD_CUDA(cudaSetDevice(m->device));
     float bp[4] = {m->lin_opt.beta1, m->lin_opt.beta2, m->dnn_opt.beta1, m->dnn_opt.beta2};
     const float b[4] = {m->lin_opt.beta1, m->lin_opt.beta2, m->dnn_opt.beta1, m->dnn_opt.beta2};
@@ -201,6 +204,7 @@ extern "C" int wd_set_opt_step(WdModel* m, int64_t steps) {
     WD_CUDA(cudaMemcpyAsync(m->d_bpow, bp, sizeof(bp), cudaMemcpyHostToDevice, m->stream));
     const unsigned int st = (unsigned int)steps;                   // dropout counter
     WD_CUDA(cudaMemcpyAsync(m->d_step, &st, sizeof(st), cudaMemcpyHostToDevice, m->stream));
+    WD_CUDA(cudaMemcpyAsync(m->d_adam_step, &st, sizeof(st), cudaMemcpyHostToDevice, m->stream));
     WD_CUDA(cudaStreamSynchronize(m->stream));
     return WD_OK;
 }

@@ -610,7 +610,8 @@ static int shard_owner_reduce_apply(WdModel* m, int s) {
         if ((rc = list_chunk_combine(m, l))) return rc;
         const OptParams o = space_opt(m, 0, sp.d_adam_touched);
         if ((rc = list_apply_emb(m, l, sp.set.rec, o))) return rc;
-        // Adam: the shard's rows no rank touched, after its touched ones (no host-placed shards with Adam: no staged records)
+        // Adam: the shard's rows no rank touched, after its touched ones (host-placed shards with Adam are deferred: their rows
+        // are 0 here, their staged records were caught up by the serve's stage-in)
         if ((rc = adam_untouched_emb(m, sp.set, sp.local_rows, o))) return rc;
         // staged records home (overflow rows only with a cache), on this stream: it joins the main stream before the step ends, so
         // the next stage-in comes after

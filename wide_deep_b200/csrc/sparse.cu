@@ -308,7 +308,7 @@ __global__ void __launch_bounds__(256) chunk_combine_kernel(const int32_t* __res
                         const int64_t row = ra.urow[uu];
                         const int t = table_of(ra.rec.row_base, ra.rec.ntab, row);
                         const int dim = ra.rec.dim[t];
-                        if (lq * 4 < dim) update_record4(ra.o, record(ra.rec, t, ra.urow, uu) + lq * 4, dim, ra.rec.stride[t] / dim - 1, acc);
+                        if (lq * 4 < dim) update_record4(ra.o, record(ra.rec, t, ra.urow, uu) + lq * 4, dim, kind_nslots(ra.o.kind), acc);
                     }
                 } else if (cg == 0) *reinterpret_cast<float4*>(ugrad + uu * width + lq * 4) = acc;
             } else {
@@ -340,7 +340,7 @@ __global__ void __launch_bounds__(256) emb_apply_kernel(const int32_t* __restric
     for (int64_t u = g0; u < nu; u += gstep) {
         const int64_t row = urow[u];
         const int t = table_of(rr.row_base, rr.ntab, row);
-        const int dim = rr.dim[t], nslots = rr.stride[t] / dim - 1;
+        const int dim = rr.dim[t], nslots = kind_nslots(o.kind);
         float* rec = record(rr, t, urow, u);
         for (int q = lig; q * 4 < dim; q += 8)
             update_record4(o, rec + q * 4, dim, nslots, *reinterpret_cast<const float4*>(ugrad + (int64_t)u * width + q * 4));
@@ -675,7 +675,7 @@ __global__ void __launch_bounds__(256) small_apply_emb_kernel(const float* __res
         const int64_t local = i * 4 - rtab_gs_off[t];
         if (touched[rtab_row_base[t] - small_base + local / dim] == 0.f) continue;
         const float4 g = *reinterpret_cast<const float4*>(Gs + i * 4);
-        update_record4(o, rtab_data[t] + (local / dim) * stride + (local % dim), dim, stride / dim - 1, g);
+        update_record4(o, rtab_data[t] + (local / dim) * stride + (local % dim), dim, kind_nslots(o.kind), g);
         if (local % dim == 0) mark_touched(o, rtab_row_base[t] + local / dim);
     }
 }
@@ -729,6 +729,12 @@ int sparse_apply_which(WdModel* m, int which) {
     // the fused updates of host-table rows went to their staged copies: copy those home (the unfused kernels below update host
     // records in place, through their mapped pointers)
     if (done) return (which == 0 && m->n_host_tab > 0) ? host_tables_write_back(m) : WD_OK;
+    // deferred Adam host tables (the only host tables Adam allows): their rows were staged and caught up by this step's stage-in,
+    // so the update goes to the staged records, which then go home as after the fused updates
+    if (which == 0 && m->n_host_tab > 0 && m->dnn_opt.kind == WD_OPT_ADAM) {
+        if ((rc = list_apply_emb(m, l, m->rtabs.rec, space_opt(m, 0, m->d_adam_touched[0])))) return rc;
+        return host_tables_write_back(m);
+    }
     if (which == 0 && m->hcache.slots > 0) {       // the unfused updates below would write host records behind the cache's back
         set_error("embedding rows of a model with a host-table cache are only updated by the fused single-GPU step");
         return WD_EUNSUPPORTED;

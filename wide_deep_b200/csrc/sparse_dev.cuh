@@ -75,7 +75,9 @@ inline float slot1_init(const WdOptimizer& o) {
     if (o.kind == WD_OPT_ADAGRAD || o.kind == WD_OPT_FTRL) return o.init_acc;
     return o.kind == WD_OPT_RMSPROP ? 1.f : 0.f;
 }
-inline int opt_nslots(const WdOptimizer& o) { return o.kind == WD_OPT_SGD ? 0 : (o.kind == WD_OPT_ADAGRAD ? 1 : 2); }
+// optimizer slots of an embedding record (a deferred table's record has a stamp behind them: the count is not stride / dim - 1)
+__host__ __device__ __forceinline__ int kind_nslots(int kind) { return kind == WD_OPT_SGD ? 0 : (kind == WD_OPT_ADAGRAD ? 1 : 2); }
+inline int opt_nslots(const WdOptimizer& o) { return kind_nslots(o.kind); }
 
 // Sparse Adam (tf.train.AdamOptimizer on IndexedSlices, AdamOptimizer._apply_sparse_shared) decays m and v over the WHOLE variable,
 // scatter-adds the summed gradients of the touched rows, then moves EVERY row by lr_t * m / (sqrt(v) + eps).  A touched row does all
@@ -226,7 +228,7 @@ __global__ void __launch_bounds__(256) emb_grad_sum_kernel(const int32_t* __rest
             }
             if (APPLY && direct) {
                 if (q * 4 < dim)
-                    update_record4(ra.o, record(ra.rec, t, ra.urow, it) + q * 4, dim, ra.rec.stride[t] / dim - 1, acc);
+                    update_record4(ra.o, record(ra.rec, t, ra.urow, it) + q * 4, dim, kind_nslots(ra.o.kind), acc);
             } else {
                 *reinterpret_cast<float4*>(out + q * 4) = acc;
             }

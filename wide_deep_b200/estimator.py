@@ -26,7 +26,7 @@ CKPT_PREFIX = "model.ckpt-"
 class WideAndDeepClassifier(object):
     def __init__(self, model_dir, model_type, config=None, device=0, max_batch=None, seed=None, tf_compat_pad=None,
                  gemm_engine="auto", shard_world=1, shard_rank=0, group=None, host_tables=None,
-                 host_cache_bytes=0, shard_cache_bytes=0):
+                 host_cache_bytes=0, shard_cache_bytes=0, defer_adam=False):
         if model_type not in ("wide", "deep", "wide_deep"):
             raise ValueError("Invalid model type: {}, must be one of `wide`, `deep`, `wide_deep`".format(model_type))
         self.config = config or Config()
@@ -53,9 +53,10 @@ class WideAndDeepClassifier(object):
         # names = exactly those.  Checkpoints do not depend on the placement.  With shard_world > 1 only row-sharded tables can go
         # there (each rank keeps its own shard).  host_cache_bytes > 0 (one GPU only): HBM budget of a write-back cache of the host
         # tables' most recently used records (results do not change, PCIe traffic does).  shard_cache_bytes > 0 (shard_world > 1):
-        # the same cache per rank, in front of the rank's own host-placed shards.
+        # the same cache per rank, in front of the rank's own host-placed shards.  defer_adam: host / auto tables also with the
+        # Adam dnn optimizer, whose untouched rows then catch up when they are next read (Plan(defer_adam=...)).
         self.plan = compile_plan(self.config, model_type, mb, tf_compat_pad=tf_compat_pad, gemm_engine=gemm_engine, host_tables=host_tables,
-                                 host_cache_bytes=host_cache_bytes, shard_cache_bytes=shard_cache_bytes,
+                                 host_cache_bytes=host_cache_bytes, shard_cache_bytes=shard_cache_bytes, defer_adam=defer_adam,
                                  shard_world=self.shard_world, shard_rank=self.shard_rank, shard_slack=float(max(2, self.shard_world)),
                                  max_nnz=mb * len(self.config.read_feature_conf()) * 4 * slack + mb * 64,
                                  max_keys=mb * max(1, len(self.config.read_feature_conf())) * slack)

@@ -117,6 +117,14 @@ class WideDeepModel(object):
         check(self._lib.wd_host_cache_stats(self._h, out, 5, 1 if reset else 0))
         return dict(zip(("capacity", "hits", "loads", "overflow", "evictions"), (int(v) for v in out)))
 
+    def deferred_adam_stats(self, reset=False):
+        """Cumulative counters of the catch-up of deferred Adam tables (Plan(defer_adam=True)): dict(rows (rows caught up),
+        replayed (steps replayed), skipped (steps skipped once a row's values had stopped changing), max_gap (most steps one row
+        had missed)).  All 0 without deferred tables."""
+        out = (ctypes.c_int64 * 4)()
+        check(self._lib.wd_deferred_adam_stats(self._h, out, 4, 1 if reset else 0))
+        return dict(zip(("rows", "replayed", "skipped", "max_gap"), (int(v) for v in out)))
+
     def n_slots(self, name):
         o = self.plan.lin_opt if name.startswith("linear/") else self.plan.dnn_opt
         return {"sgd": 0, "adagrad": 1, "ftrl": 2, "adam": 2, "rmsprop": 2}[o["kind"]]

@@ -37,7 +37,9 @@ T_WIDE_COL, T_EMB_TABLE, T_DENSE, T_WIDE_BIAS = range(4)
 D_KERNEL, D_BIAS, D_GAMMA, D_BETA = range(4)
 GEMM = {"auto": 0, "ffma": 1, "tc3x": 2, "tc1x": 3, "bf16x3": 4}
 PLACE_HBM, PLACE_HOST, PLACE_AUTO = range(3)      # WD_PLACE_*
-PLACE_NAMES = {PLACE_HBM: "hbm", PLACE_HOST: "host", PLACE_AUTO: "auto"}
+PLACE_DEFER_ADAM = 4                              # WD_PLACE_DEFER_ADAM, OR'ed into host / auto entries
+PLACE_NAMES = {PLACE_HBM: "hbm", PLACE_HOST: "host", PLACE_AUTO: "auto",
+               PLACE_HOST | PLACE_DEFER_ADAM: "host+defer", PLACE_AUTO | PLACE_DEFER_ADAM: "auto+defer"}
 API_VERSION = 3                                   # WD_API_VERSION
 
 
@@ -149,7 +151,7 @@ class Plan(object):
     def __init__(self, feature_conf, cross_conf, model_conf, model_type="wide_deep", max_batch=8192,
                  embedding_dim_override=None, tf_compat_pad=False, gemm_engine="auto", max_nnz=0, max_keys=0,
                  dense_exchange_max_rows=0, shard_world=1, shard_rank=0, shard_capacity=0, shard_slack=2.0, host_tables=None,
-                 host_cache_bytes=0, shard_cache_bytes=0):
+                 host_cache_bytes=0, shard_cache_bytes=0, defer_adam=False):
         if model_type not in ("wide", "deep", "wide_deep"):
             raise ValueError("Invalid model type: {}, must be one of `wide`, `deep`, `wide_deep`".format(model_type))
         self.model_type, self.max_batch, self.tf_compat_pad = model_type, int(max_batch), bool(tf_compat_pad)
@@ -329,8 +331,14 @@ class Plan(object):
             unknown = sorted(want - set(names))
             if unknown:
                 raise ValueError("host_tables: no embedding table named {} (tables: {})".format(unknown, names))
+        # defer_adam: host and auto tables may be trained with the Adam dnn optimizer.  Sparse Adam moves every row every step; a
+        # deferred table instead replays the steps a row missed when the row is next read (results unchanged, each missed step
+        # costs one replayed step of that row until its values stop changing).  The library ignores it for other optimizers.
+        self.defer_adam = bool(defer_adam)
         for t in self.tables:
             t["placement"] = PLACE_AUTO if want is None else (PLACE_HOST if t["name"] in want else PLACE_HBM)
+            if self.defer_adam and t["placement"] != PLACE_HBM:
+                t["placement"] |= PLACE_DEFER_ADAM
         # HBM budget (bytes) of the write-back cache of host-table records (wd_host_cache_enable); 0 = no cache.  The model has
         # a cache only when some table ended up on the host.
         if isinstance(host_cache_bytes, bool) or not isinstance(host_cache_bytes, (int, np.integer)) or host_cache_bytes < 0:

@@ -107,6 +107,10 @@ class LocalShardGroup(object):
         """Per rank, the counters of its cache of host shard records (WideDeepModel.host_cache_stats)."""
         return [m.host_cache_stats(reset) for m in self.models]
 
+    def deferred_adam_stats(self, reset=False):
+        """Per rank, the catch-up counters of its deferred Adam shards (WideDeepModel.deferred_adam_stats)."""
+        return [m.deferred_adam_stats(reset) for m in self.models]
+
     def get_tensor(self, name, slot=0):
         """Global tensor: row-sharded tensors are interleaved back from the ranks' shards."""
         plan = self.models[0].plan
@@ -192,6 +196,10 @@ class ShardedTrainer(object):
     def host_cache_stats(self, reset=False):
         """Collective: every rank's counters of its cache of host shard records, in rank order."""
         return self.gather(self.model.host_cache_stats(reset))
+
+    def deferred_adam_stats(self, reset=False):
+        """Collective: every rank's catch-up counters of its deferred Adam shards, in rank order."""
+        return self.gather(self.model.deferred_adam_stats(reset))
 
     def gather(self, obj):
         """Collective: every rank's `obj`, in rank order."""
