@@ -189,6 +189,13 @@ int wd_set_opt_step(WdModel *m, int64_t steps);
  * (Adagrad: acc; FTRL: n, z).  Logical (unpadded) shapes; kernels are [in, out] like tf.layers.dense. */
 int wd_tensor_io(WdModel *m, int kind, int index, int sub, int slot, void *host, int64_t count, int to_device);
 int64_t wd_tensor_size(WdModel *m, int kind, int index, int sub);
+/* Copy rows row0 .. row0 + nrows - 1 of an embedding table (WD_T_EMB_TABLE: nrows x dimension floats) or a wide column
+ * (WD_T_WIDE_COL: nrows floats) to/from host, slot as in wd_tensor_io; rows of a row-sharded tensor are this rank's local rows.
+ * WD_EINVAL for any other kind and for a range outside the tensor.  wd_tensor_io's guarantees hold for the range: dirty cached
+ * records of its rows go home before either direction, a write leaves no cached copy of them, and a WD_PLACE_DEFER_ADAM table's
+ * rows are caught up before a read and stamped with the current step after a write.  The cost is that of the range (plus one pass
+ * over an HBM cache's slot tags), not of the table: checkpoints move a table in bounded chunks through this call. */
+int wd_tensor_io_rows(WdModel *m, int kind, int index, int sub, int slot, int64_t row0, int64_t nrows, void *host, int to_device);
 /* Memory the model holds: device_bytes = HBM it allocated, host_bytes = page-locked host memory of its host-placed embedding
  * tables (WdPlanDesc::table_placement; a rank of a row-sharded model counts its own shards).  Either pointer may be NULL.  (The reference's parameters sit in host RAM on the CPU
  * or on the parameter servers, reference python/lib/build_estimator.py:211-214.) */

@@ -43,6 +43,7 @@ SYMBOLS = {
     "wd_model_init": (ctypes.c_int, [_vp, _u64]),
     "wd_set_opt_step": (ctypes.c_int, [_vp, _i64]),
     "wd_tensor_io": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _i64, ctypes.c_int]),
+    "wd_tensor_io_rows": (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _i64, _i64, _vp, ctypes.c_int]),
     "wd_tensor_size": (_i64, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int]),
     "wd_memory_usage": (ctypes.c_int, [_vp, ctypes.POINTER(_i64), ctypes.POINTER(_i64)]),
     "wd_host_cache_enable": (ctypes.c_int, [_vp, _i64]),

@@ -607,14 +607,14 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         }
         // a deferred table's rows are brought up to the current step before a read; a write makes them current
         if (deferred(tb) && !to_device) {
-            const int rc = deferred_adam_settle(m, tb, false);
+            const int rc = deferred_adam_settle(m, tb, 0, tb.arows, false);
             if (rc) return rc;
         }
         const cudaMemcpyKind dir = tb.host ? cudaMemcpyDefault : (to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost);
         if (to_device) WD_CUDA(cudaMemcpy2DAsync(dev, (size_t)tb.stride * 4, host, lw, lw, tb.arows, dir, m->stream));
         else WD_CUDA(cudaMemcpy2DAsync(host, lw, dev, (size_t)tb.stride * 4, lw, tb.arows, dir, m->stream));
         if (deferred(tb) && to_device) {
-            const int rc = deferred_adam_settle(m, tb, true);
+            const int rc = deferred_adam_settle(m, tb, 0, tb.arows, true);
             if (rc) return rc;
         }
         WD_CUDA(cudaStreamSynchronize(m->stream));
@@ -671,6 +671,47 @@ extern "C" int wd_tensor_io(WdModel* m, int kind, int index, int sub, int slot, 
         WD_CUDA(cudaStreamSynchronize(m->stream));
         if (slot == 0 && t.wt_off >= 0) return refresh_weight_copies(m);
     }
+    return WD_OK;
+}
+
+extern "C" int wd_tensor_io_rows(WdModel* m, int kind, int index, int sub, int slot, int64_t row0, int64_t nrows, void* host, int to_device) {
+    if (!m || !host) { set_error("null argument"); return WD_EINVAL; }
+    if (kind != WD_T_EMB_TABLE && kind != WD_T_WIDE_COL) { set_error("wd_tensor_io_rows: tensor kind %d has no rows", kind); return WD_EINVAL; }
+    WD_CUDA(cudaSetDevice(m->device));
+    WD_CUDA(cudaStreamSynchronize(m->stream));
+    const int64_t size = wd_tensor_size(m, kind, index, sub);
+    if (size < 0) { set_error("no tensor (%d,%d,%d)", kind, index, sub); return WD_EINVAL; }
+    const int64_t rows = kind == WD_T_EMB_TABLE ? m->tables[index].arows : size;
+    if (row0 < 0 || nrows < 0 || row0 > rows - nrows) {
+        set_error("tensor (%d,%d,%d): rows [%lld, %lld) outside its %lld rows", kind, index, sub, (long long)row0, (long long)(row0 + nrows),
+                  (long long)rows);
+        return WD_EINVAL;
+    }
+    if (slot < 0 || slot > 2) { set_error("slot out of range"); return WD_EINVAL; }
+    if (nrows == 0) return WD_OK;
+    if (kind == WD_T_WIDE_COL) {
+        const ShardSpace& sw = m->shard.sp[1];
+        float4* base = (sw.on && sw.h_col_slot[index] >= 0) ? sw.d_wide + sw.h_slot_base[sw.h_col_slot[index]] : m->d_wide + m->col_wide_base[index];
+        float* dev = reinterpret_cast<float*>(base + row0) + slot;
+        if (to_device) WD_CUDA(cudaMemcpy2DAsync(dev, 16, host, 4, 4, nrows, cudaMemcpyHostToDevice, m->stream));
+        else WD_CUDA(cudaMemcpy2DAsync(host, 4, dev, 16, 4, nrows, cudaMemcpyDeviceToHost, m->stream));
+        WD_CUDA(cudaStreamSynchronize(m->stream));
+        return WD_OK;
+    }
+    EmbTable& tb = m->tables[index];
+    if (slot * tb.dim >= tb.stride) { set_error("table has no optimizer slot %d", slot); return WD_EINVAL; }
+    float* dev = tb.data + row0 * tb.stride + slot * tb.dim;
+    const size_t lw = (size_t)tb.dim_logical * 4;
+    int rc;
+    // wd_tensor_io's guarantees, for the rows of the range only: their dirty cached records go home before either direction and a
+    // write empties their slots; a deferred table's rows are settled before a read and stamped after a write
+    if (tb.host && (rc = host_cache_sync_rows(m, tb, row0, nrows, to_device != 0))) return rc;
+    if (deferred(tb) && !to_device && (rc = deferred_adam_settle(m, tb, row0, nrows, false))) return rc;
+    const cudaMemcpyKind dir = tb.host ? cudaMemcpyDefault : (to_device ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToHost);
+    if (to_device) WD_CUDA(cudaMemcpy2DAsync(dev, (size_t)tb.stride * 4, host, lw, lw, nrows, dir, m->stream));
+    else WD_CUDA(cudaMemcpy2DAsync(host, lw, dev, (size_t)tb.stride * 4, lw, nrows, dir, m->stream));
+    if (deferred(tb) && to_device && (rc = deferred_adam_settle(m, tb, row0, nrows, true))) return rc;
+    WD_CUDA(cudaStreamSynchronize(m->stream));
     return WD_OK;
 }
 

@@ -566,8 +566,11 @@ int build_record_sets(WdModel* m);                               // host_tables.
 int host_tables_stage_in(WdModel* m, bool train);                // host_tables.cu: cache lookup, host rows -> staging buffer, gather ids
 int host_tables_write_back(WdModel* m);                          // host_tables.cu: overflow rows of the staging buffer -> host rows
 int host_cache_sync(WdModel* m, bool flush, bool invalidate);    // host_tables.cu: dirty cached records -> host; optionally empty the cache
-// host_tables.cu: every host record of deferred table tb caught up to the current Adam step in place (stamp_only: just stamped)
-int deferred_adam_settle(WdModel* m, const EmbTable& tb, bool stamp_only);
+// host_tables.cu: dirty cached records of host table tb's local rows row0 .. row0 + rows - 1 -> host; optionally empty their slots
+int host_cache_sync_rows(WdModel* m, const EmbTable& tb, int64_t row0, int64_t rows, bool invalidate);
+// host_tables.cu: host records row0 .. row0 + rows - 1 of deferred table tb caught up to the current Adam step in place (stamp_only:
+// just stamped)
+int deferred_adam_settle(WdModel* m, const EmbTable& tb, int64_t row0, int64_t rows, bool stamp_only);
 // host_tables.cu, over any record set `rr` whose staged tables (found by row base) keep the records of the unique rows of list L
 // (lists[L].urow[0 .. *lists[L].nuniq)) in rr.stage_base at stride S, behind cache `c` (c.slots = 0: none, staging row u):
 //   stage_in_rows    cache keys -> sort -> assign (train: the used slots turn dirty), then dirty victims home and the records

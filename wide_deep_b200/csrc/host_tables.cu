@@ -48,7 +48,8 @@
 // (adam_catch_up_kernel): steps s+1 .. g (g = WdModel::d_adam_step) in order, with lr_t[j] from the table deferred_adam_setup
 // builds with with_lr_t's own expression, so the values are bit-identical to the untouched passes of the table in HBM.  A train
 // call stamps g + 1 (the list's update follows, on the staged record, then the write-back); a forward-only call stamps g.  Reads
-// of the whole table (wd_tensor_io) settle every host record first; writes stamp every record with g.
+// of the whole table (wd_tensor_io) settle every host record first; writes stamp every record with g.  wd_tensor_io_rows does the
+// same for its rows only.
 #include <algorithm>
 #include <type_traits>
 
@@ -245,25 +246,28 @@ __global__ void __launch_bounds__(256) host_remap_kernel(const int32_t* __restri
     }
 }
 
-// dirty slots of rr.stage_base -> host records (one thread per float4 of a slot)
+// dirty slots of rr.stage_base that hold a row in [row_lo, row_hi) -> host records: one warp per slot reads the slot's tag and dirty
+// byte once, and its lanes copy the record's float4s
 __global__ void __launch_bounds__(256) cache_flush_kernel(int64_t C, int S, const uint32_t* __restrict__ tag, const uint8_t* __restrict__ dirty,
-                                                          RowRecords rr) {
-    const int q4 = S >> 2;
-    const int64_t total = C * q4;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t slot = i / q4;
-        const int q = (int)(i - slot * q4);
-        if (!dirty[slot] || tag[slot] == kInvalidRow) continue;
+                                                          RowRecords rr, int64_t row_lo, int64_t row_hi) {
+    const int lane = threadIdx.x & 31;
+    const int64_t w0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, wstep = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t slot = w0; slot < C; slot += wstep) {
         const int64_t row = tag[slot];
-        const int lo = table_of(rr.row_base, rr.ntab, row);
-        const int stride = rr.stride[lo];
-        if (q * 4 >= stride) continue;
-        *reinterpret_cast<float4*>(rr.data[lo] + (row - rr.row_base[lo]) * stride + q * 4) =
-            *reinterpret_cast<const float4*>(rr.stage_base + slot * S + q * 4);
+        if (!dirty[slot] || row == kInvalidRow || row < row_lo || row >= row_hi) continue;
+        const int t = table_of(rr.row_base, rr.ntab, row);
+        const int stride = rr.stride[t];
+        float* dst = rr.data[t] + (row - rr.row_base[t]) * stride;
+        const float* src = rr.stage_base + slot * S;
+        for (int q = lane; q * 4 < stride; q += 32)
+            *reinterpret_cast<float4*>(dst + q * 4) = *reinterpret_cast<const float4*>(src + q * 4);
     }
 }
-__global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32_t* __restrict__ stamp, uint8_t* __restrict__ dirty, int invalidate) {
+// slots whose tag is in [row_lo, row_hi) (every slot, empty ones included, when the range covers all 32-bit tags)
+__global__ void cache_clear_kernel(int64_t C, uint32_t* __restrict__ tag, uint32_t* __restrict__ stamp, uint8_t* __restrict__ dirty, int invalidate,
+                                   int64_t row_lo, int64_t row_hi) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < C; i += (int64_t)gridDim.x * blockDim.x) {
+        if ((int64_t)tag[i] < row_lo || (int64_t)tag[i] >= row_hi) continue;
         dirty[i] = 0;
         if (invalidate) { tag[i] = kInvalidRow; stamp[i] = 0; }
     }
@@ -358,9 +362,10 @@ __global__ void __launch_bounds__(256) adam_catch_up_kernel(const int32_t* __res
     catch_up_flush(ar, cnt);
 }
 
-// Every host record of one deferred table in place (rows records of `stride` floats at data): caught up to g, or only stamped g.
-__global__ void __launch_bounds__(256) adam_settle_kernel(float* data, int64_t rows, int dim, int stride, OptParams o, AdamReplay ar,
-                                                          int stamp_only) {
+// Host records row0 .. row0 + rows - 1 of one deferred table in place (records of `stride` floats at data): caught up to g, or only
+// stamped g.
+__global__ void __launch_bounds__(256) adam_settle_kernel(float* data, int64_t row0, int64_t rows, int dim, int stride, OptParams o,
+                                                          AdamReplay ar, int stamp_only) {
     const int lane = threadIdx.x & 31, lig = lane & 7, grp = lane >> 3;
     const unsigned gm = 0xFFu << (grp * 8);
     const uint32_t g = *ar.now;
@@ -370,7 +375,7 @@ __global__ void __launch_bounds__(256) adam_settle_kernel(float* data, int64_t r
     for (int64_t r0 = w0; r0 < rows; r0 += gstep) {
         const int64_t r = r0 + grp;
         if (r >= rows) continue;
-        float* rec = data + r * stride;
+        float* rec = data + (row0 + r) * stride;
         if (stamp_only) { if (lig == 0) *reinterpret_cast<uint32_t*>(rec + 3 * dim) = g; }
         else catch_up_record(o, ar, rec, dim, g, false, gm, lig, cnt);
     }
@@ -429,9 +434,10 @@ static int adam_catch_up(WdModel* m, int L, const RowRecords& rr, bool train) {
     return WD_OK;
 }
 
-int deferred_adam_settle(WdModel* m, const EmbTable& tb, bool stamp_only) {
-    adam_settle_kernel<<<grid_for(tb.arows * 8, 256), 256, 0, m->stream>>>(tb.data, tb.arows, tb.dim, tb.stride, make_opt(m->dnn_opt),
-                                                                          adam_replay(m), stamp_only ? 1 : 0);
+int deferred_adam_settle(WdModel* m, const EmbTable& tb, int64_t row0, int64_t rows, bool stamp_only) {
+    if (rows <= 0) return WD_OK;
+    adam_settle_kernel<<<grid_for(rows * 8, 256), 256, 0, m->stream>>>(tb.data, row0, rows, tb.dim, tb.stride, make_opt(m->dnn_opt),
+                                                                      adam_replay(m), stamp_only ? 1 : 0);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
@@ -487,25 +493,36 @@ int host_tables_stage_in(WdModel* m, bool train) {
 
 int host_tables_write_back(WdModel* m) { return write_back_rows(m, m->hcache, 0, m->rtabs.rec, m->stage_stride, kHostMarks); }
 
-// Everything that reads or writes host records outside the step: flush = dirty slots home (they stay cached, now clean),
-// invalidate = empty every slot (after the host records were rewritten).  Enqueued on the model stream.
-static int cache_sync(WdModel* m, HostCache& c, const RowRecords& rr, int S, bool flush, bool invalidate) {
+// Everything that reads or writes host records outside the step, for the slots holding a row of [row_lo, row_hi) in the set's row
+// space: flush = dirty slots home (they stay cached, now clean), invalidate = empty the slots (after the host records were
+// rewritten).  Enqueued on the model stream.  One pass over the slots' metadata either way, whatever the range.
+static int cache_sync(WdModel* m, HostCache& c, const RowRecords& rr, int S, bool flush, bool invalidate, int64_t row_lo, int64_t row_hi) {
     const int64_t C = c.slots;
     if (C == 0) return WD_OK;
     if (flush) {
-        cache_flush_kernel<<<grid_for(C * (S / 4), 256), 256, 0, m->stream>>>(C, S, c.d_tag, c.d_dirty, rr);
+        cache_flush_kernel<<<grid_for(C * 32, 256), 256, 0, m->stream>>>(C, S, c.d_tag, c.d_dirty, rr, row_lo, row_hi);
         m->launches++;
     }
-    cache_clear_kernel<<<grid_for(C, 256), 256, 0, m->stream>>>(C, c.d_tag, c.d_stamp, c.d_dirty, invalidate ? 1 : 0);
+    cache_clear_kernel<<<grid_for(C, 256), 256, 0, m->stream>>>(C, c.d_tag, c.d_stamp, c.d_dirty, invalidate ? 1 : 0, row_lo, row_hi);
     m->launches++;
     WD_CUDA(cudaGetLastError());
     return WD_OK;
 }
+constexpr int64_t kEveryTag = int64_t(1) << 32;       // hi of a range that holds every tag, kInvalidRow (empty slots) included
 // the model's cache, whichever it has (the single-GPU one or the owner's cache of its host shards)
 int host_cache_sync(WdModel* m, bool flush, bool invalidate) {
     ShardSpace& se = m->shard.sp[0];
-    int rc = cache_sync(m, m->hcache, m->rtabs.rec, m->stage_stride, flush, invalidate);
-    return rc ? rc : cache_sync(m, se.cache, se.set.rec, se.stage_stride, flush, invalidate);
+    int rc = cache_sync(m, m->hcache, m->rtabs.rec, m->stage_stride, flush, invalidate, 0, kEveryTag);
+    return rc ? rc : cache_sync(m, se.cache, se.set.rec, se.stage_stride, flush, invalidate, 0, kEveryTag);
+}
+// The cached records of host table tb's rows row0 .. row0 + rows - 1 (local rows; a shard's rows for a sharded table): dirty ones
+// go home, and with invalidate the slots holding them are emptied.  The single-GPU cache tags global rows, an owner's cache its
+// shard rows: tb.row_base counts in that space either way.
+int host_cache_sync_rows(WdModel* m, const EmbTable& tb, int64_t row0, int64_t rows, bool invalidate) {
+    ShardSpace& se = m->shard.sp[0];
+    const int64_t row_lo = tb.row_base + row0;
+    if (tb.sharded) return cache_sync(m, se.cache, se.set.rec, se.stage_stride, true, invalidate, row_lo, row_lo + rows);
+    return cache_sync(m, m->hcache, m->rtabs.rec, m->stage_stride, true, invalidate, row_lo, row_lo + rows);
 }
 
 // Allocates every embedding table — in HBM (WD_PLACE_HBM, and WD_PLACE_AUTO tables while they fit, largest first, with

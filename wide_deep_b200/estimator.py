@@ -16,17 +16,16 @@ import time
 
 import numpy as np
 
+from . import checkpoint
 from .config import Config
 from .model import Batch, WideDeepModel
 from .plan import compile_plan
-
-CKPT_PREFIX = "model.ckpt-"
 
 
 class WideAndDeepClassifier(object):
     def __init__(self, model_dir, model_type, config=None, device=0, max_batch=None, seed=None, tf_compat_pad=None,
                  gemm_engine="auto", shard_world=1, shard_rank=0, group=None, host_tables=None,
-                 host_cache_bytes=0, shard_cache_bytes=0, defer_adam=False):
+                 host_cache_bytes=0, shard_cache_bytes=0, defer_adam=False, checkpoint_layout=None):
         if model_type not in ("wide", "deep", "wide_deep"):
             raise ValueError("Invalid model type: {}, must be one of `wide`, `deep`, `wide_deep`".format(model_type))
         self.config = config or Config()
@@ -34,6 +33,12 @@ class WideAndDeepClassifier(object):
         run = self.config.runconfig or {}
         self.seed = run.get("tf_random_seed", 123) if seed is None else seed
         self.keep_checkpoint_max = run.get("keep_checkpoint_max") or 5
+        # checkpoints save() writes: "npz" = one flat .npz of the whole model, written by rank 0 (the default); "sharded" = every
+        # rank writes its own rows in bounded chunks (wide_deep_b200/checkpoint.py), restorable at any GPU count.  restore() reads
+        # either, whichever the newest checkpoint is.
+        self.checkpoint_layout = checkpoint_layout or run.get("checkpoint_layout") or "npz"
+        if self.checkpoint_layout not in ("npz", "sharded"):
+            raise ValueError("checkpoint_layout must be `npz` or `sharded`, got {!r}".format(self.checkpoint_layout))
         mb = max_batch or self.config.train["batch_size"]
         # quirk Q2 (SURVEY Appendix A): the reference pads multi-valued string fields with '' per batch and the padding takes
         # part in SparseCross.  The file-based entry points reproduce that by default (train.yaml key `tf_compat_pad`, default
@@ -61,15 +66,13 @@ class WideAndDeepClassifier(object):
                                  max_nnz=mb * len(self.config.read_feature_conf()) * 4 * slack + mb * 64,
                                  max_keys=mb * max(1, len(self.config.read_feature_conf())) * slack)
         self._model = None
+        self._saved = None                               # (global step, path) of this process's last sharded-layout save
         self.device = device
 
     # ------------------------------------------------------------------ checkpoints
     def latest_checkpoint(self):
-        if not os.path.isdir(self.model_dir):
-            return None
-        steps = sorted(int(f[len(CKPT_PREFIX):-4]) for f in os.listdir(self.model_dir)
-                       if f.startswith(CKPT_PREFIX) and f.endswith(".npz"))
-        return os.path.join(self.model_dir, "%s%d.npz" % (CKPT_PREFIX, steps[-1])) if steps else None
+        found = checkpoint.list_checkpoints(self.model_dir)
+        return found[-1][1] if found else None
 
     def _ensure_model(self, checkpoint_path=None, need_trained=False):
         if self._model is None:
@@ -90,51 +93,34 @@ class WideAndDeepClassifier(object):
         return self._model
 
     def save(self):
-        """Flat .npz of every variable (TensorFlow variable names) + optimizer slots; keeps the newest
-        keep_checkpoint_max files (reference conf/train.yaml runconfig)."""
+        """Checkpoint of every variable (TensorFlow variable names) + optimizer slots in self.checkpoint_layout; keeps the newest
+        keep_checkpoint_max checkpoints of either layout (reference conf/train.yaml runconfig).  Multi-GPU: a collective."""
         m = self._model
-        # multi-GPU: a collective — row-sharded tensors are gathered from all ranks; rank 0 alone writes
-        get = self._trainer.get_tensor if self._trainer is not None else m.get_tensor
-        blob = {"global_step": np.asarray(m.global_step)}
-        for name in m.tensor_names():
-            blob[name] = get(name)
-            for s in range(m.n_slots(name)):
-                blob["%s/slot%d" % (name, s + 1)] = get(name, slot=s + 1)
-        if self.shard_rank != 0:
-            return None
-        os.makedirs(self.model_dir, exist_ok=True)
-        path = os.path.join(self.model_dir, "%s%d.npz" % (CKPT_PREFIX, m.global_step))
-        tmp = path + ".tmp.%d" % os.getpid()                 # written beside, then renamed: a crash never leaves a truncated
-        with open(tmp, "wb") as fh:                          # checkpoint that latest_checkpoint() would pick up
-            np.savez(fh, **blob)
-            fh.flush()
-            os.fsync(fh.fileno())
-        os.replace(tmp, path)
-        olds = sorted(int(f[len(CKPT_PREFIX):-4]) for f in os.listdir(self.model_dir) if f.startswith(CKPT_PREFIX) and f.endswith(".npz"))
-        for st in olds[:-self.keep_checkpoint_max]:
-            os.remove(os.path.join(self.model_dir, "%s%d.npz" % (CKPT_PREFIX, st)))
+        if self.checkpoint_layout == "sharded":
+            # Nothing has changed since this process's last save at this step (train() on input that yields no batch still ends in
+            # save()): skipping it keeps a fast rank from writing the same .tmp directory that rank 0 is still committing.
+            if self._saved is not None and self._saved[0] == m.global_step:
+                return self._saved[1]
+            if self._trainer is not None:
+                path = self._trainer.save(self.model_dir)
+            else:
+                path = checkpoint.save(self.model_dir, [m])
+            self._saved = (m.global_step, path)
+        else:
+            # multi-GPU: a collective — row-sharded tensors are gathered from all ranks; rank 0 alone writes
+            get = self._trainer.get_tensor if self._trainer is not None else m.get_tensor
+            path = checkpoint.save_npz(self.model_dir, m, get, write=self.shard_rank == 0)
+        if self.shard_rank == 0:
+            checkpoint.rotate(self.model_dir, self.keep_checkpoint_max)
         return path
 
     def restore(self, path):
-        m = self._model
-        with np.load(path) as z:
-            have = set(z.files)
-            want = []
-            for name in m.tensor_names():
-                want.append((name, 0, tuple(self.plan.tensor_names[name][3])))
-                for s in range(m.n_slots(name)):
-                    want.append(("%s/slot%d" % (name, s + 1), s + 1, tuple(self.plan.tensor_names[name][3])))
-            missing = [k for k, _, _ in want if k not in have]
-            if missing or "global_step" not in have:
-                raise ValueError("checkpoint {} does not match this model (feature conf, model_type or optimizers changed?): "
-                                 "missing {} of {} tensors, e.g. {}".format(path, len(missing), len(want), missing[:3]))
-            for key, slot, shape in want:
-                if tuple(z[key].shape) != shape:
-                    raise ValueError("checkpoint {}: tensor {} has shape {}, the model expects {}".format(path, key, tuple(z[key].shape), shape))
-            m.global_step = int(z["global_step"])
-            m.set_opt_step(m.global_step)
-            for key, slot, _ in want:
-                m.set_tensor(key if slot == 0 else key[:key.rindex("/slot")], z[key], slot=slot)
+        """Either layout: a sharded-layout directory (this rank's rows only) or an .npz file."""
+        self._saved = None
+        if os.path.isdir(path):
+            checkpoint.restore(path, [self._model])
+        else:
+            checkpoint.restore_npz(path, self._model)
 
     # ------------------------------------------------------------------ estimator API
     def train(self, input_fn, hooks=None, steps=None, max_steps=None, saving_listeners=None):

@@ -146,6 +146,21 @@ class WideDeepModel(object):
             v = np.ascontiguousarray(v[self.plan.shard_rank::self.plan.shard_world])
         check(self._lib.wd_tensor_io(self._h, kind, index, sub, slot, v.ctypes.data, v.size, 1))
 
+    def get_rows(self, name, row0, nrows, slot=0):
+        """Rows row0 .. row0 + nrows - 1 of an embedding table or wide column (this rank's local rows of a row-sharded one)."""
+        kind, index, sub, shape = self.plan.tensor_names[name]
+        out = np.empty((int(nrows),) + tuple(shape[1:]), dtype=np.float32)
+        check(self._lib.wd_tensor_io_rows(self._h, kind, index, sub, slot, int(row0), int(nrows), out.ctypes.data, 0))
+        return out
+
+    def set_rows(self, name, row0, value, slot=0):
+        """Writes ``value`` (nrows x the tensor's row shape) to local rows row0 .. row0 + nrows - 1 (get_rows' rows)."""
+        kind, index, sub, shape = self.plan.tensor_names[name]
+        v = np.ascontiguousarray(value, dtype=np.float32)
+        if v.shape[1:] != tuple(shape[1:]):
+            raise ValueError("%s: rows of shape %s, the tensor's rows have shape %s" % (name, v.shape[1:], tuple(shape[1:])))
+        check(self._lib.wd_tensor_io_rows(self._h, kind, index, sub, slot, int(row0), int(v.shape[0]), v.ctypes.data, 1))
+
     # ------------------------------------------------------------------ steps
     def train_step(self, batch: Batch):
         """One optimizer step on a host batch; returns the sum-reduced loss (reference joint.py:404-406)."""

@@ -20,7 +20,7 @@ import ctypes
 
 import numpy as np
 
-from . import _native
+from . import _native, checkpoint
 from ._native import check
 from .model import METRIC_KEYS
 
@@ -126,6 +126,14 @@ class LocalShardGroup(object):
         for m in self.models:
             m.set_tensor(name, value, slot)
 
+    def save(self, model_dir):
+        """Sharded-layout checkpoint of every rank (wide_deep_b200/checkpoint.py) -> its directory."""
+        return checkpoint.save(model_dir, self.models)
+
+    def restore(self, path):
+        """Every rank's rows from a sharded-layout checkpoint written at any GPU count -> global step."""
+        return checkpoint.restore(path, self.models)
+
 
 class ShardedTrainer(object):
     """One rank of a torchrun job.  ``group``: a torch.distributed process group (default: WORLD)."""
@@ -207,6 +215,16 @@ class ShardedTrainer(object):
         parts = [None] * self.world
         dist.all_gather_object(parts, obj, group=self.group)
         return parts
+
+    def save(self, model_dir):
+        """Collective: sharded-layout checkpoint (wide_deep_b200/checkpoint.py), this rank's rows written by this rank; one barrier
+        on the group, then rank 0 commits it.  -> its directory on rank 0, None elsewhere."""
+        import torch.distributed as dist
+        return checkpoint.save(model_dir, [self.model], barrier=lambda: dist.barrier(group=self.group))
+
+    def restore(self, path):
+        """This rank's rows from a sharded-layout checkpoint written at any GPU count (no collective) -> global step."""
+        return checkpoint.restore(path, [self.model])
 
     def get_tensor(self, name, slot=0):
         """Global tensor on every rank (row-sharded tensors are all-gathered through the host and interleaved)."""
